@@ -1,9 +1,10 @@
 #!/usr/bin/env python3
 """Headline benchmark: Mvoxels/s of the igneous hot path (downsample 2 mode mips
--> 6-connected CCL -> marching-cubes meshing at mip 2) on a synthetic 2048^3
-uint32 segmentation resident in HBM, one z-slab of the dataset per GPU.
+-> 6-connected CCL -> marching-cubes meshing at mip 2) on a synthetic
+2048x2048x1024 uint32 segmentation resident in HBM, one z-slab of the dataset per GPU.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--size S] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--size S] [--depth D] [--impl reference]
+                  [--dump-outputs DIR]
 
 Contract (see the task brief): W untimed warm-up steps, exactly K timed steps
 bracketed by barrier + device synchronisation, CUDA-event timing on the stream
@@ -26,7 +27,7 @@ if ROOT not in sys.path:
 
 def _baseline_metric():
   """The metric string of BASELINE.json (the bench line must name exactly that metric)."""
-  fallback = "Mvoxels/s on 2048\u00b3 uint32 seg (downsample+CCL+mesh) @1/2/4/8 B200; % HBM roofline"
+  fallback = "Mvoxels/s on 2048x2048x1024 uint32 seg per GPU (downsample+CCL+mesh) @1/2/4/8 H100; % HBM roofline"
   try:
     with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "BASELINE.json")) as f:
       return json.load(f).get("metric", fallback)
@@ -46,7 +47,7 @@ def measured_peaks():
       return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
       pass
-  return 6650.0, "fallback (B200_PROFILING.md)"
+  return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3, 700 W card)"
 
 
 class ClockSampler(threading.Thread):
@@ -60,7 +61,7 @@ class ClockSampler(threading.Thread):
   def run(self):
     q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit,name")
     try:
       self.proc = subprocess.Popen(
         ["nvidia-smi", "-i", str(self.index), "--query-gpu=" + q, "--format=csv,noheader,nounits",
@@ -90,9 +91,11 @@ class ClockSampler(threading.Thread):
             reasons.add(n)
       except Exception:
         continue
+    last = self.samples[-1] if self.samples and len(self.samples[-1]) >= 9 else [None] * 9
     return {"sm_mhz": float(np.median(sm)) if sm else None,
             "sm_max_mhz": float(max(mx)) if mx else None,
-            "reasons": sorted(reasons), "samples": len(sm)}
+            "reasons": sorted(reasons), "samples": len(sm),
+            "gpu": last[8], "power_limit_w": last[7]}
 
 
 # ----------------------------------------------------------------- CPU legs
@@ -142,15 +145,15 @@ def host_cores():
   return n
 
 
-def ref_chunk_offset(index, size):
-  """Chunk `index` of the REF_CHUNK grid over the size^3 bench volume (x fastest, as
+def ref_chunk_offset(index, shape):
+  """Chunk `index` of the REF_CHUNK grid over the bench volume of `shape` (x fastest, as
   FinelyDividedTaskIterator enumerates tasks, igneous/task_creation/common.py:91-98)."""
-  gx, gy, gz = (max(1, size // c) for c in REF_CHUNK)
+  gx, gy, gz = (max(1, s // c) for s, c in zip(shape, REF_CHUNK))
   index %= gx * gy * gz
   return ((index % gx) * REF_CHUNK[0], ((index // gx) % gy) * REF_CHUNK[1], (index // (gx * gy)) * REF_CHUNK[2])
 
 
-def _oracle_worker_init(counter, size):
+def _oracle_worker_init(counter, shape):
   """Each pool worker synthesises its own chunk of the bench volume ONCE (outside any timed region)."""
   from oracle import oracle as O
   with counter.get_lock():
@@ -158,7 +161,7 @@ def _oracle_worker_init(counter, size):
     counter.value += 1
   # spread the workers' chunks over the volume (stride 37 is coprime with the chunk grid)
   _WORKER["seg"] = O.synth_seg(REF_CHUNK, pitch=PITCH, num_ids=NUM_IDS, seed=0,
-                               offset=ref_chunk_offset(wid * 37, size))
+                               offset=ref_chunk_offset(wid * 37, shape))
   O.lib()
 
 
@@ -183,13 +186,14 @@ def run_reference_arm(args):
   O.build()
   cores = host_cores()
   ctx = mp.get_context("spawn")
+  vol = (args.size, args.size, min(args.depth, args.size))
   # one chunk alone on an otherwise idle host: the reference's real per-worker speed
-  _oracle_worker_init(ctx.Value("i", 0), args.size)
+  _oracle_worker_init(ctx.Value("i", 0), vol)
   _oracle_worker(0)
   alone = min(_oracle_worker(0)[1] for _ in range(2))
   counter = ctx.Value("i", 0)
   times, per_chunk = [], []
-  with ctx.Pool(cores, initializer=_oracle_worker_init, initargs=(counter, args.size)) as pool:
+  with ctx.Pool(cores, initializer=_oracle_worker_init, initargs=(counter, vol)) as pool:
     pool.map(_oracle_worker, range(cores), chunksize=1)  # untimed: all workers initialised and warm
     for it in range(args.warmup + args.steps):
       t = time.perf_counter()
@@ -207,10 +211,10 @@ def run_reference_arm(args):
     "steps": args.steps, "warmup": args.warmup, "ms_per_step": 1e3 * sec / max(len(times), 1),
     "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u32",
     "data": "synthetic", "gpu_launches": 0,
-    "config": {"workload": "oracle port of the igneous CPU path on %dx%dx%d uint32 chunks cut from the %d^3 "
+    "config": {"workload": "oracle port of the igneous CPU path on %dx%dx%d uint32 chunks cut from the %dx%dx%d "
                            "jittered-Voronoi bench volume (pitch 64), one chunk per usable host core (%d) per step: "
                            "mode pool 2 mips + 6-connected CCL + marching cubes / weld / quadric simplification "
-                           "x100 at mip 2" % (shape + (args.size, cores)),
+                           "x100 at mip 2" % (shape + vol + (cores,)),
                "chunk": list(shape), "simplification_factor": 100, "cores_used": cores,
                "os_cpu_count": os.cpu_count(),
                "seconds_per_chunk_alone": alone,
@@ -222,21 +226,25 @@ def run_reference_arm(args):
   print(json.dumps(line))
 
 
+def box_to_host(ctx, dptr, shape, size, dtype, origin=(0, 0, 0)):
+  """The sub-box `size` at `origin` of a Fortran-order device volume of `shape`, as a host array."""
+  from igneous_b200 import _shim
+  d = ctx.alloc(int(np.prod(size)) * np.dtype(dtype).itemsize)
+  _shim.check(ctx.lib.ign_copy_box_dev(ctx.handle, _shim.ptr(dptr), c.c_int(_shim.dtype_code(dtype)),
+                                       *[c.c_uint64(v) for v in tuple(shape) + tuple(origin) + tuple(size)],
+                                       _shim.ptr(d)))
+  h = ctx.to_host(d, size, dtype)
+  d.free()
+  return h
+
+
 def cpu_baseline_sample(pipe, ctx, budget_s=20.0):
   """Oracle timed on ONE host core on a bounded sample of the same volume."""
   from oracle import oracle as O
   O.build()
   sx, sy, sz = pipe.shape
-  bz = min(sz, 256)
-  bx, by = min(sx, 256), min(sy, 256)
-  from igneous_b200 import _shim
-  d_box = ctx.alloc(bx * by * bz * 4)
-  _shim.check(ctx.lib.ign_copy_box_dev(ctx.handle, _shim.ptr(pipe.d_in), c.c_int(pipe.code),
-                                       c.c_uint64(sx), c.c_uint64(sy), c.c_uint64(sz), c.c_uint64(0),
-                                       c.c_uint64(0), c.c_uint64(0), c.c_uint64(bx), c.c_uint64(by),
-                                       c.c_uint64(bz), _shim.ptr(d_box)))
-  seg = ctx.to_host(d_box, (bx, by, bz), np.uint32)
-  d_box.free()
+  seg = box_to_host(ctx, pipe.d_in, pipe.shape, (min(sx, 256), min(sy, 256), min(sz, 256)), np.uint32)
+  bx, by, bz = seg.shape
   t = time.perf_counter()
   vox, reps = 0, 0
   while True:
@@ -256,22 +264,13 @@ def parity_check(ctx, pipe):
   CCL labels of the same sub-box (every oracle component carries exactly one label, two
   components share a label only when they hold the same input id, 0 <-> 0) and every fragment
   of one MeshTask body on a 129x129x65 cutout of the mesh mip (bit-exact vertices and faces)."""
-  from igneous_b200 import _shim, zmesh
+  from igneous_b200 import zmesh
   from oracle import oracle as O
   O.build()
   sx, sy, sz = pipe.shape
   bx, by, bz = min(sx, 256), min(sy, 256), min(sz, 64)
 
-  def box(dptr, shape, size, dtype):
-    d = ctx.alloc(int(np.prod(size)) * np.dtype(dtype).itemsize)
-    _shim.check(ctx.lib.ign_copy_box_dev(ctx.handle, _shim.ptr(dptr), c.c_int(_shim.dtype_code(dtype)),
-                                         c.c_uint64(shape[0]), c.c_uint64(shape[1]), c.c_uint64(shape[2]),
-                                         c.c_uint64(0), c.c_uint64(0), c.c_uint64(0), c.c_uint64(size[0]),
-                                         c.c_uint64(size[1]), c.c_uint64(size[2]), _shim.ptr(d)))
-    h = ctx.to_host(d, size, dtype)
-    d.free()
-    return h
-
+  box = lambda dptr, shape, size, dtype: box_to_host(ctx, dptr, shape, size, dtype)
   out = {}
   seg = box(pipe.d_in, pipe.shape, (bx, by, bz), np.uint32)
   want = O.downsample_segmentation(seg, (2, 2, 1), num_mips=pipe.num_mips)
@@ -373,7 +372,7 @@ def run_config(args, ctx, rank, world, dist):
                  "gpu_launches": 2 * chunks * args.steps,
                  "config": {"workload": "C2: 5-level 2x2x1 average pyramid of a 2048x2048x512 uint8 image, one 512^3 chunk "
                                         "per call (16 calls per step; the 128 MiB chunk is re-read from L2/HBM every call)",
-                            "l2": "one 512^3 u8 chunk (134 MB) + outputs exceed the 126 MB L2"},
+                            "l2": "one 512^3 u8 chunk (134 MB) + outputs exceed the 50 MB L2"},
                  "roofline": {"bound": "hbm", "kernel": "k_avg_fused<u8>", "achieved": bytes_alg / 1e9 / (ms * 1e-3),
                               "peak": peak, "unit": "GB/s", "frac": bytes_alg / 1e9 / (ms * 1e-3) / peak,
                               "traffic": None, "peak_source": peak_src, "algorithmic_bytes_per_voxel": 1.333}})
@@ -461,10 +460,16 @@ def main():
   ap.add_argument("--gpus", type=int, default=1)
   ap.add_argument("--steps", type=int, default=5)
   ap.add_argument("--warmup", type=int, default=3)
-  ap.add_argument("--size", type=int, default=2048, help="cube edge of the per-GPU volume (weak scaling) / of the whole volume (strong)")
+  ap.add_argument("--size", type=int, default=2048, help="x / y edge of the per-GPU volume (weak scaling) / edge of the whole cube (strong)")
+  ap.add_argument("--depth", type=int, default=1024,
+                  help="z extent of the per-GPU volume (weak scaling; at most --size): 2048x2048x1024 uint32 with "
+                       "its mips, labels and CCL scratch is ~50 GB, what an 80 GB H100 holds with room for the mesh stage")
+  ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                  help="after the timed steps, write what the last step computed to DIR/<name>.npy (float64; "
+                       "fixed seeded sub-boxes of the mips and CCL labels, per-task mesh counts)")
   ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
   ap.add_argument("--config", default="headline", choices=["headline", "c1", "c2", "c3"],
-                  help="BASELINE.json config: headline = the metric's 2048^3 pipeline; c1 / c2 / c3 print their own line")
+                  help="BASELINE.json config: headline = the metric's 2048x2048x1024 pipeline; c1 / c2 / c3 print their own line")
   ap.add_argument("--scaling", default="weak", choices=["weak", "strong"],
                   help="weak: one size^3 volume per GPU; strong: ONE size^3 volume split into N z-slabs")
   ap.add_argument("--check", action="store_true", help="N>1: also run the N-rank CCL parity check against the oracle")
@@ -505,7 +510,7 @@ def main():
     return
   S = args.size
   strong = args.scaling == "strong" and world > 1
-  sz_local = S // world if strong else S
+  sz_local = S // world if strong else min(args.depth, S)
   shape = (S, S, sz_local)
   simplify = 100 if args.simplify is None else args.simplify
   group = None
@@ -548,6 +553,8 @@ def main():
   pipe.prof_enable(False)
   launches = pipe.launch_count() - launches0
   clocks = sampler.finish() if sampler else None
+  if args.dump_outputs and rank == 0:
+    dump_outputs(ctx, pipe, args.dump_outputs)
 
   if dist is not None:
     import torch
@@ -589,9 +596,7 @@ def main():
   ccl_ms = sum(prof[k][0] for k in ("ccl_local", "ccl_merge", "ccl_label")) / args.steps
   roofline = {
     "bound": "hbm", "kernel": knames[dominant], "achieved": achieved, "peak": peak, "unit": "GB/s",
-    "frac": achieved / peak, "traffic": NCU_TRAFFIC.get(dominant, {}).get("bytes_per_launch"),
-    "traffic_source": NCU_TRAFFIC.get(dominant, {}).get("source"),
-    "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_step[dominant] / dom_launches,
+    "frac": achieved / peak, "traffic": None, "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_step[dominant] / dom_launches,
     "avg_launch_ms": dom_ms / dom_launches, "launches_per_step": dom_launches,
     "share_of_step_kernel_time": prof[dominant][0] / max(sum(v[0] for v in prof.values()), 1e-9),
     "stage_ccl": {"algorithmic_bytes_per_voxel": in_b + out_b, "kernel_ms_per_step": ccl_ms,
@@ -618,7 +623,7 @@ def main():
                   % (S, S, sz_local, PITCH, (" = one %d^3 volume split into %d z-slabs" % (S, world)) if strong else "",
                      (" + quadric simplification x%d" % simplify) if simplify else ""),
       "volume_per_gpu": list(shape), "parallelism": "z-slab per GPU, %d rank(s)" % world,
-      "l2": "inputs larger than L2 (%.1f GB volume vs 126 MB L2)" % (pipe.n * 4 / 1e9),
+      "l2": "inputs larger than L2 (%.1f GB volume vs 50 MB L2)" % (pipe.n * 4 / 1e9),
       "simplification_factor": simplify, "components": pipe.n_components, "mesh": pipe.mesh_stats, "mesh_streams": pipe.mesh_streams,
       "stage_ms_per_step": {k: v / args.steps for k, v in stage.items()},
     },
@@ -640,13 +645,25 @@ def main():
     dist.destroy_process_group()
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from `ncu --set full` captures (profiles/)
-NCU_TRAFFIC = {
-  # dram__bytes_read.sum + dram__bytes_write.sum per launch from ncu --set full captures (profiles/)
-  "simp_labels": {"bytes_per_launch": 3.926e9, "source": "profiles/r02_simp_labels_v8_full_summary.txt (one 257^3 MeshTask at mip 2)"},
-  "ccl_local": {"bytes_per_launch": 6.517e10, "source": "profiles/r02_ccl2048_metrics.csv (2048^3 u32, two CTAs per SM; 1024^3: 5.27e9)"},
-  "ccl_label": {"bytes_per_launch": 3.826e10, "source": "profiles/r02_ccl2048_metrics.csv (2048^3 u32)"},
-}
+DUMP_BOXES, DUMP_BOX = 16, (64, 64, 32)  # float64: 16 * 64*64*32 * 8 B = 16.8 MB per volume, 50 MB in all
+
+
+def dump_outputs(ctx, pipe, out_dir):
+  """Write what the last step left on the device: the mips and CCL labels as DUMP_BOXES sub-boxes at
+  origins drawn from a fixed seed (the whole volumes are tens of GB), and the per-task mesh counts
+  (triangles, vertices, label fragments, triangles and vertices before simplification)."""
+  os.makedirs(out_dir, exist_ok=True)
+  vols = {"mip%d" % (k + 1): (d, s, pipe.dtype) for k, (d, s) in enumerate(zip(pipe.d_mips, pipe.mip_shapes))}
+  vols["ccl_labels"] = (pipe.d_cc, pipe.shape, pipe.ccl_out_dtype)
+  rng = np.random.default_rng(0)
+  for name, (dptr, shape, dtype) in vols.items():
+    size = tuple(min(b, s) for b, s in zip(DUMP_BOX, shape))
+    origins = [tuple(int(rng.integers(0, s - b + 1)) for s, b in zip(shape, size)) for _ in range(DUMP_BOXES)]
+    boxes = [box_to_host(ctx, dptr, shape, size, dtype, o) for o in origins]
+    np.save(os.path.join(out_dir, name + ".npy"), np.stack(boxes).astype(np.float64))
+    np.save(os.path.join(out_dir, name + "_box_origins.npy"), np.array(origins, dtype=np.float64))
+  np.save(os.path.join(out_dir, "mesh_task_counts.npy"), pipe.mesh_task_counts.astype(np.float64))
+  np.save(os.path.join(out_dir, "n_components.npy"), np.array([pipe.n_components], dtype=np.float64))
 
 
 def bind_numa(local_rank):

@@ -1,4 +1,4 @@
-"""igneous_b200 -- B200-native (sm_100a) implementation of the igneous
+"""igneous_b200 -- H100-native (sm_90a) implementation of the igneous
 per-chunk hot path: DownsampleTask pooling, 6-connected CCL, MeshTask
 marching cubes, behind igneous's own task API.
 

@@ -1,5 +1,5 @@
 """Drop-in for the `cc3d` (connected-components-3d) calls on the igneous hot
-path, running on B200.
+path, running on H100.
 
 Reference call sites (seung-lab/igneous):
   igneous/tasks/image/ccl.py:169-172  cc3d.dust(labels, threshold=, connectivity=6, in_place=True)

@@ -1,4 +1,4 @@
-"""Chunk codecs of the Precomputed format on B200 (SURVEY.md 8(f) row 1).
+"""Chunk codecs of the Precomputed format on H100 (SURVEY.md 8(f) row 1).
 
 `compressed_segmentation` is what CloudVolume applies on the host either side of the hot path
 when a segmentation layer asks for it (igneous/task_creation/common.py:215-236 set_encoding,
@@ -7,7 +7,7 @@ decoded where the labels already are.  Byte-identical to the CPU restatement in 
 encoder layout is itself parity-unpinned: no upstream vector exists offline).
 
 crackle and compresso are NOT implemented: both are un-vendored third-party formats whose
-specifications are not in /root/reference.
+specifications are not in the reference checkout.
 """
 import ctypes as c
 

@@ -675,8 +675,8 @@ struct ExpandArgs {
 };
 
 // The expansion is two dependent loads (masks -> run label) followed by a store, so a warp
-// keeps EX_G independent 128-voxel groups in flight (a single group per warp is latency bound:
-// 2.2 TB/s measured).  A lane owns 4 consecutive voxels of each group (one vector store).
+// keeps EX_G independent 128-voxel groups in flight (a single group per warp is latency bound).
+// A lane owns 4 consecutive voxels of each group (one vector store).
 constexpr int EX_G = 4;
 
 template <typename OUT>
@@ -1023,7 +1023,7 @@ static int ccl_structure(ign_ctx* ctx, const R& rd, uint32_t sx, uint32_t sy, ui
   ma.ncols = ma.nby * ma.nbz * 64;
   ma.S = p.S; ma.Z = p.Z; ma.Ey = p.Ey; ma.Ez = p.Ez;
   // whole-sector mask writes pay off where L2 no longer merges the half sectors of x-neighbours: rows of
-  // 16+ tiles (measured at 2048^3: 12.7 vs 16.3 ms; at 1024^3 the unpaired kernel is faster, 1.27 vs 1.60 ms)
+  // 16+ tiles (rows of 2048+ voxels)
   ma.pair = (p.wpr % 8 == 0 && sx % MT_BX == 0 && ma.ntx >= 16) ? 1u : 0u;
   if (const char* e = getenv("IGN_CCL_PAIR")) ma.pair = (atoi(e) != 0 && p.wpr % 8 == 0 && sx % MT_BX == 0) ? 1u : 0u;
   const uint64_t ntiles = (uint64_t)ma.ntx * ma.ncols;
@@ -1570,7 +1570,7 @@ int ign_ccl6_link_dev(ign_ctx* ctx, const uint64_t* values_a, const uint32_t* la
   return IGN_OK;
 }
 
-// Host-side global union-find over provisional ids 1..total (the B200-native
+// Host-side global union-find over provisional ids 1..total (the GPU-native
 // stand-in for create_relabeling, igneous/tasks/image/ccl.py:358-420):
 // smaller id wins (ccl.py:70-73); final ids are the ranks of the component
 // minima, i.e. identical to a whole-volume cc3d numbering.

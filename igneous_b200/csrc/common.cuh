@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device helpers for libigneous_b200 (sm_100a only)
+// common.cuh -- shared host/device helpers for libigneous_b200 (sm_90a only)
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,8 +7,8 @@
 
 #include "../../include/igneous_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libigneous_b200 targets sm_100a (Blackwell B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libigneous_b200 targets sm_90a (Hopper H100) only"
 #endif
 
 namespace ign {

@@ -73,8 +73,7 @@ static int copy_small_launch(ign_ctx* ctx, void* dst, const void* src, size_t by
 
 // Device -> pinned host copy by a kernel (stores to mapped host memory) instead of the D2H copy engine.
 // The engine serves one copy at a time: a MeshTask's fragment export queued behind a multi-gigabyte
-// label download waits for it, and with it the task's stream (measured on the streamed 2048^3 step:
-// +0.38 s).  Stores issued by SMs share the PCIe link with the DMA but are not queued behind it.
+// label download waits for it, and with it the task's stream.  Stores issued by SMs share the PCIe link with the DMA but are not queued behind it.
 __global__ void __launch_bounds__(256) k_copy_to_host(uint4* __restrict__ dst, const uint4* __restrict__ src, uint64_t n16) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n16; i += (uint64_t)gridDim.x * blockDim.x)
     dst[i] = src[i];
@@ -205,8 +204,9 @@ int ign_init(int device, ign_ctx** out) {
   IGN_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   IGN_CUDA(cudaGetDeviceProperties(&prop, device));
-  IGN_REQUIRE(prop.major >= 10, IGN_ERR_UNSUPPORTED,
-              "device %d is sm_%d%d; libigneous_b200 is built for sm_100a only", device,
+  // sm_90a code (TMA, mbarrier expect_tx) runs on compute capability 9.0 only
+  IGN_REQUIRE(prop.major == 9 && prop.minor == 0, IGN_ERR_UNSUPPORTED,
+              "device %d is sm_%d%d; libigneous_b200 is built for sm_90a (H100) only", device,
               prop.major, prop.minor);
   ign_ctx* ctx = new ign_ctx();
   ctx->device = device;

@@ -1300,7 +1300,8 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   // latency bound (barriers, dependent loads), so several CTAs per SM overlap each other's
   // stalls; the shared-memory budget of a label is the SM's divided by the CTAs per SM
   // (IGN_SIMP_THREADS / IGN_SIMP_CTAS override the default for experiments).
-  int sl_threads = 1024, sl_ctas = 1;  // measured on B200: 1024x1 76 ms, 512x2 94 ms, 256x4 91 ms per 257^3 task
+  // measured on an H100 SXM (400 W limit): 1024x1 55 ms, 512x2 93 ms, 256x4 106 ms per 257^3 task
+  int sl_threads = 1024, sl_ctas = 1;
   if (const char* e = getenv("IGN_SIMP_THREADS")) sl_threads = atoi(e);
   if (const char* e = getenv("IGN_SIMP_CTAS")) sl_ctas = atoi(e);
   if (sl_threads != 256 && sl_threads != 512 && sl_threads != 1024) sl_threads = 1024;

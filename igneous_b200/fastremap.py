@@ -1,4 +1,4 @@
-"""Drop-in for the `fastremap` calls on the igneous hot path, running on B200.
+"""Drop-in for the `fastremap` calls on the igneous hot path, running on H100.
 
 Reference call sites (seung-lab/igneous):
   igneous/tasks/mesh/mesh.py:201      fastremap.mask_except(data, object_ids, in_place=True)

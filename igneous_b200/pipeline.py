@@ -60,8 +60,8 @@ class VolumePipeline:
     # of the CCL labels / mips (e2e) overlaps with meshing.
     self.mesh_streams = max(1, int(mesh_streams))
     # Whole-volume passes (pooling, CCL) run on a high-priority stream: their thread blocks are
-    # dispatched first whenever a MeshTask CTA retires (k_simp_labels runs one label per CTA), so a
-    # 46 ms CCL is not stretched over the mesh stage it shares the SMs with.  A second context
+    # dispatched first whenever a MeshTask CTA retires (k_simp_labels runs one label per CTA), so the
+    # CCL is not stretched over the mesh stage it shares the SMs with.  A second context
     # drains finished products to the host while the main stream keeps uploading / computing.
     ctx.set_priority(True)
     self._dl = _shim.Context(ctx.device)
@@ -71,6 +71,7 @@ class VolumePipeline:
       self._workers.append((wctx, wctx.alloc((mx + 1) * (my + 1) * (mz + 1) * es)))
     self.n_components = 0
     self.mesh_stats = {}
+    self.mesh_task_counts = np.zeros((0, 5), dtype=np.int64)
 
   def free(self):
     for b in [self.d_in, self.d_cc, self.d_task] + self.d_mips:
@@ -167,11 +168,12 @@ class VolumePipeline:
     def run(widx):
       wctx, buf = self._workers[widx]
       out = []
-      for t in tasks[widx::self.mesh_streams]:
+      for i in range(widx, len(tasks), self.mesh_streams):
+        t = tasks[i]
         if wait_for is not None:
           mark = wait_for(t)  # the mark the main stream recorded after the last layer this task reads
           _shim.check(self.lib.ign_stream_wait_mark(wctx.handle, self.ctx.handle, c.c_int(mark)))
-        out.append(self._mesh_one(wctx, buf, t, export))
+        out.append((i, self._mesh_one(wctx, buf, t, export)))
       wctx.sync()
       return out
     if self.mesh_streams == 1:
@@ -180,6 +182,9 @@ class VolumePipeline:
       with ThreadPoolExecutor(max_workers=self.mesh_streams) as ex:
         for part in ex.map(run, range(self.mesh_streams)):
           results.extend(part)
+    # per task, in mesh_tasks() order: (triangles, vertices, label fragments, triangles in, vertices in)
+    self.mesh_task_counts = np.array([r for _, r in sorted(results)], dtype=np.int64).reshape(-1, 5)
+    results = [r for _, r in results]
     self.mesh_stats = {"tasks": len(tasks), "triangles": int(sum(r[0] for r in results)),
                        "vertices": int(sum(r[1] for r in results)),
                        "label_fragments": int(sum(r[2] for r in results)),

@@ -1,4 +1,4 @@
-"""Drop-in for the `tinybrain` calls on the igneous hot path, running on B200.
+"""Drop-in for the `tinybrain` calls on the igneous hot path, running on H100.
 
 Reference call sites (seung-lab/igneous):
   igneous/tasks/image/image.py:46-55  downsample_method_to_fn binds

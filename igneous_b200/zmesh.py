@@ -1,4 +1,4 @@
-"""Drop-in for the `zmesh` calls on the igneous hot path, running on B200.
+"""Drop-in for the `zmesh` calls on the igneous hot path, running on H100.
 
 Reference call sites (seung-lab/igneous):
   igneous/tasks/mesh/mesh.py:151      zmesh.Mesher(self._volume.resolution)

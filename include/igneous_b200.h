@@ -1,7 +1,7 @@
 /*
  * igneous_b200.h -- C ABI of libigneous_b200.so
  *
- * B200 (sm_100a) implementation of the igneous per-chunk hot path.  Every
+ * H100 (sm_90a) implementation of the igneous per-chunk hot path.  Every
  * entry point replaces one call the reference (seung-lab/igneous @ 3b6e5b6)
  * makes into a third-party CPU library; the reference call site is cited
  * beside each declaration (paths relative to the igneous repo root).

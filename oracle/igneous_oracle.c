@@ -7,7 +7,7 @@
  *
  * The reference (seung-lab/igneous @ 3b6e5b6) holds no arithmetic of its own
  * for this path; it calls un-vendored third-party wheels that are absent from
- * /root/reference and from this image:
+ * the reference checkout and from this image:
  *   tinybrain >= 1.5.0               (requirements.txt:22)
  *   connected-components-3d >= 3.10.1 (requirements.txt:5)
  *   zmesh >= 1.13.1,<2.0             (requirements.txt:26)

@@ -7,7 +7,7 @@ The product (igneous_b200/) never imports it.
 Heavy loops live in igneous_oracle.c (built by oracle/Makefile); the integer
 glue that the reference takes from `fastremap` is restated here in numpy.
 Every function cites the reference call site it follows
-(paths relative to /root/reference).
+(paths relative to the reference checkout, seung-lab/igneous @ 3b6e5b6).
 
 Parity status: see the header of igneous_oracle.c and DESIGN.md.
 """

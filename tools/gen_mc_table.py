@@ -4,7 +4,7 @@
 The table is the classic published Lorensen/Cline table in P. Bourke's
 corner/edge numbering (see oracle/igneous_oracle.c for the numbering).  It is
 data, not reference code: the reference (zmesh, un-vendored) is absent from
-/root/reference.  `validate()` checks the table structurally so that a typo
+the reference checkout.  `validate()` checks the table structurally so that a typo
 cannot hide: every case uses exactly its active edges, complementary cases
 use the same edges, the triangle count never exceeds 5, and the union of all
 cube-local surfaces is watertight on random volumes (tests/test_oracle.py).
