@@ -95,6 +95,12 @@ def ccl_task(image, shape, threshold_gte=None, threshold_lte=None, dust_threshol
     arr = arr.view(np.uint8)
   if threshold_gte is not None or threshold_lte is not None:
     _shim.require_unsigned(arr.dtype, "thresholded CCL")
+    if arr.dtype == np.uint64:
+      for t in (threshold_gte, threshold_lte):
+        # the kernel receives the threshold as a double and compares integer bounds derived from it
+        if isinstance(t, (int, np.integer)) and float(int(t)) != int(t):
+          raise NotImplementedError("igneous_b200.cc3d.ccl_task: uint64 threshold %d is not exactly "
+                                    "representable as a double" % int(t))
   ctx = ctx or _shim.default_context()
   sx, sy, sz = arr.shape
   out = np.zeros(arr.shape, dtype=np.uint64, order="F")

@@ -45,6 +45,7 @@
 #include <thrust/iterator/transform_iterator.h>
 #include <cuda.h>
 
+#include <cmath>
 #include <stdlib.h>
 #include <string.h>
 
@@ -65,8 +66,9 @@ struct Reader {
   using value_type = T;
   static constexpr bool thresholded = THR;
   const T* in;
-  double gte, lte;
+  double gte, lte;  // float input: compared in float32, as numpy compares a float32 image
   int use_gte, use_lte;
+  uint64_t ilo, ihi;  // integer input: exact bounds ceil(gte) .. floor(lte) (ilo > ihi: nothing passes)
   uint32_t rx, ry, rz;  // rail coordinates (0xFFFFFFFF = none)
   __host__ __device__ __forceinline__ bool has_rails() const { return (rx & ry & rz) != 0xFFFFFFFFu; }
   // label stored back in the staged tile (type T: 0 / 1 when thresholded)
@@ -78,8 +80,7 @@ struct Reader {
         if (use_gte) ok = ok && (raw >= (float)gte);
         if (use_lte) ok = ok && (raw <= (float)lte);
       } else {
-        if (use_gte) ok = ok && ((double)raw >= gte);
-        if (use_lte) ok = ok && ((double)raw <= lte);
+        ok = (uint64_t)raw >= ilo && (uint64_t)raw <= ihi;  // (double)raw is inexact above 2^53
       }
       v = ok ? (T)1 : (T)0;
     }
@@ -1142,6 +1143,8 @@ static Reader<T, false> plain_reader(const void* in) {
   r.in = (const T*)in;
   r.gte = r.lte = 0;
   r.use_gte = r.use_lte = 0;
+  r.ilo = 0;
+  r.ihi = ~0ull;
   r.rx = r.ry = r.rz = 0xFFFFFFFFu;
   return r;
 }
@@ -1263,6 +1266,28 @@ static int ccl_run(ign_ctx* ctx, const R& rd, uint64_t sx, uint64_t sy, uint64_t
   return IGN_ERR_OVERFLOW;
 }
 
+// raw >= gte and raw <= lte for an unsigned integer raw, as exact integer bounds [lo, hi]; an
+// empty range (NaN, gte above 2^64-1, lte below 0, gte > lte) is returned as lo = 1, hi = 0
+static void int_bounds(int use_gte, double gte, int use_lte, double lte, uint64_t* lo, uint64_t* hi) {
+  constexpr double TWO64 = 18446744073709551616.0;
+  uint64_t l = 0, h = ~0ull;
+  bool empty = false;
+  if (use_gte) {
+    if (std::isnan(gte) || std::ceil(gte) >= TWO64) empty = true;
+    else if (gte > 0) l = (uint64_t)std::ceil(gte);
+  }
+  if (use_lte) {
+    if (std::isnan(lte) || lte < 0) empty = true;
+    else if (std::floor(lte) < TWO64) h = (uint64_t)std::floor(lte);
+  }
+  if (empty || l > h) {
+    l = 1;
+    h = 0;
+  }
+  *lo = l;
+  *hi = h;
+}
+
 template <typename T>
 static int ccl_task_typed(ign_ctx* ctx, const void* in, uint64_t sx, uint64_t sy, uint64_t sz,
                           int use_gte, double gte, int use_lte, double lte, uint64_t rx, uint64_t ry,
@@ -1275,6 +1300,7 @@ static int ccl_task_typed(ign_ctx* ctx, const void* in, uint64_t sx, uint64_t sy
     r.lte = lte;
     r.use_gte = use_gte;
     r.use_lte = use_lte;
+    if constexpr (!std::is_same<T, float>::value) int_bounds(use_gte, gte, use_lte, lte, &r.ilo, &r.ihi);
     r.rx = rail(rx, sx);
     r.ry = rail(ry, sy);
     r.rz = rail(rz, sz);

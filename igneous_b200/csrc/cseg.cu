@@ -15,8 +15,11 @@
 // table is emitted by the FIRST block that uses it) is reproduced exactly, so the streams are
 // byte-identical:
 //   1  k_cseg_scan<T, false>  one warp per block: the distinct values are extracted in
-//      ascending order (repeated warp minimum) -> n, bits, 64-bit hash of the table
-//   2  radix sort of (hash, block) -> the first block of every group of identical tables owns it
+//      ascending order (repeated warp minimum) -> n, smallest / largest value, 64-bit hash
+//   2  radix sort of (hash, block) -> the first block of every run of equal hashes is the owner
+//      candidate; k_cseg_verify compares each block's table with its candidate's.  Equal hashes
+//      do not prove equal tables: after a mismatch k_cseg_resolve recomputes every owner by
+//      content, so the owner is always the first block with an identical table
 //   3  exclusive scan of the per-block sizes -> offsets
 //   4  k_cseg_scan<T, true>   the same extraction again, now writing indices, tables, headers
 #include <cub/device/device_radix_sort.cuh>
@@ -45,27 +48,18 @@ __device__ __forceinline__ uint32_t cs_bits(uint32_t n) {
   return b;
 }
 
-// One warp per block.  WRITE = false: info[b] = {n, bits}, hash[b].  WRITE = true: the stream.
-template <typename T, bool WRITE, int CS_PER_LANE>  // CS_PER_LANE * 32 >= voxels per block
-__global__ void __launch_bounds__(128)
-    k_cseg_scan(const T* __restrict__ in, CsegDims d, uint64_t nblock, uint32_t* __restrict__ info_n,
-                unsigned long long* __restrict__ hash, const uint32_t* __restrict__ enc_off,
-                const uint32_t* __restrict__ tab_off, const uint32_t* __restrict__ owner, uint32_t* __restrict__ out) {
-  constexpr int WORDS = sizeof(T) / 4;
-  const uint32_t lane = threadIdx.x & 31u;
-  const uint64_t b = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5;
-  if (b >= nblock) return;
+// lane l of the warp loads positions l, l+32, ... of block b (position p = (z*by + y)*bx + x);
+// returns the mask of slots inside the volume
+template <typename T, int CS_PER_LANE>
+__device__ __forceinline__ uint32_t cs_load(const T* __restrict__ in, const CsegDims& d, uint64_t b, uint32_t lane,
+                                            uint64_t (&val)[CS_PER_LANE]) {
   const uint32_t gxx = (uint32_t)(b % d.gx), gyy = (uint32_t)((b / d.gx) % d.gy), gzz = (uint32_t)(b / ((uint64_t)d.gx * d.gy));
   const uint32_t x0 = gxx * d.bx, y0 = gyy * d.by, z0 = gzz * d.bz;
-  // lane l holds block positions l, l+32, ... (position p = (z*by + y)*bx + x)
-  uint64_t val[CS_PER_LANE];
-  uint32_t idx[CS_PER_LANE];
-  uint32_t have = 0, todo = 0;  // bit k: slot k is inside the volume / not classified yet
+  uint32_t have = 0;
 #pragma unroll
   for (int k = 0; k < CS_PER_LANE; k++) {
     const uint32_t p = lane + 32 * k;
     val[k] = 0;
-    idx[k] = 0;
     if (p < d.bvox) {
       const uint32_t x = p % d.bx, y = (p / d.bx) % d.by, z = p / (d.bx * d.by);
       if (x0 + x < d.sx && y0 + y < d.sy && z0 + z < d.sz) {
@@ -74,21 +68,67 @@ __global__ void __launch_bounds__(128)
       }
     }
   }
-  todo = have;
+  return have;
+}
+
+// smallest value of the warp's slots still in `todo` (the same on every lane)
+template <int CS_PER_LANE>
+__device__ __forceinline__ uint64_t cs_warp_min(const uint64_t (&val)[CS_PER_LANE], uint32_t todo) {
+  uint64_t m = ~0ull;
+#pragma unroll
+  for (int k = 0; k < CS_PER_LANE; k++)
+    if ((todo >> k) & 1u) m = val[k] < m ? val[k] : m;
+#pragma unroll
+  for (int s = 16; s > 0; s >>= 1) {
+    const uint64_t o = cs_shfl_xor(m, s);
+    m = o < m ? o : m;
+  }
+  return m;
+}
+
+// Do blocks a and b, both of n distinct values, hold the same values?  Called by a whole warp;
+// the two sorted tables are extracted side by side and compared value by value.
+template <typename T, int CS_PER_LANE>
+__device__ bool cs_same_table(const T* __restrict__ in, const CsegDims& d, uint64_t a, uint64_t b, uint32_t n,
+                              uint32_t lane) {
+  uint64_t va[CS_PER_LANE], vb[CS_PER_LANE];
+  uint32_t ta = cs_load<T, CS_PER_LANE>(in, d, a, lane, va);
+  uint32_t tb = cs_load<T, CS_PER_LANE>(in, d, b, lane, vb);
+  for (uint32_t i = 0; i < n; i++) {
+    const uint64_t ma = cs_warp_min<CS_PER_LANE>(va, ta), mb = cs_warp_min<CS_PER_LANE>(vb, tb);
+    if (ma != mb) return false;
+#pragma unroll
+    for (int k = 0; k < CS_PER_LANE; k++) {
+      if (va[k] == ma) ta &= ~(1u << k);
+      if (vb[k] == mb) tb &= ~(1u << k);
+    }
+  }
+  return true;
+}
+
+// One warp per block.  WRITE = false: n[b], hash[b] and the smallest / largest value lo[b], hi[b].
+// WRITE = true: the stream.  hash_mask keeps only some bits of the hash (IGN_CSEG_HASH_BITS, a test
+// knob that forces collisions); the hash only groups candidates, k_cseg_verify decides by content.
+template <typename T, bool WRITE, int CS_PER_LANE>  // CS_PER_LANE * 32 >= voxels per block
+__global__ void __launch_bounds__(128)
+    k_cseg_scan(const T* __restrict__ in, CsegDims d, uint64_t nblock, uint32_t* __restrict__ info_n,
+                unsigned long long* __restrict__ hash, unsigned long long hash_mask, unsigned long long* __restrict__ lo,
+                unsigned long long* __restrict__ hi, const uint32_t* __restrict__ enc_off,
+                const uint32_t* __restrict__ tab_off, const uint32_t* __restrict__ owner, uint32_t* __restrict__ out) {
+  constexpr int WORDS = sizeof(T) / 4;
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint64_t b = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5;
+  if (b >= nblock) return;
+  uint64_t val[CS_PER_LANE];
+  uint32_t idx[CS_PER_LANE] = {};
+  const uint32_t have = cs_load<T, CS_PER_LANE>(in, d, b, lane, val);  // bit k: slot k is inside the volume
+  uint32_t todo = have;                                                 // bit k: slot k not classified yet
   uint32_t n = 0;
-  uint64_t h = 0x9E3779B97F4A7C15ull;
+  uint64_t h = 0x9E3779B97F4A7C15ull, first = 0, m = 0;
   const uint32_t toff = WRITE ? tab_off[b] : 0u;
   const bool own = WRITE ? (owner[b] == (uint32_t)b) : false;
   while (__any_sync(CS_FULL, todo != 0)) {
-    uint64_t m = ~0ull;
-#pragma unroll
-    for (int k = 0; k < CS_PER_LANE; k++)
-      if ((todo >> k) & 1u) m = val[k] < m ? val[k] : m;
-#pragma unroll
-    for (int s = 16; s > 0; s >>= 1) {
-      const uint64_t o = cs_shfl_xor(m, s);
-      m = o < m ? o : m;
-    }
+    m = cs_warp_min<CS_PER_LANE>(val, todo);
 #pragma unroll
     for (int k = 0; k < CS_PER_LANE; k++)
       if (((todo >> k) & 1u) && val[k] == m) {
@@ -101,7 +141,8 @@ __global__ void __launch_bounds__(128)
         if (WORDS == 2) out[toff + n * WORDS + 1] = (uint32_t)(m >> 32);
       }
     } else {
-      h ^= m + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2);
+      if (n == 0) first = m;
+      h = mix64(h ^ m);
     }
     n++;
   }
@@ -109,7 +150,9 @@ __global__ void __launch_bounds__(128)
   if (!WRITE) {
     if (lane == 0) {
       info_n[b] = n;
-      hash[b] = (h ^ n) * 0xBF58476D1CE4E5B9ull;
+      hash[b] = mix64(h + n) & hash_mask;
+      lo[b] = first;
+      hi[b] = m;
     }
     return;
   }
@@ -155,6 +198,55 @@ __global__ void __launch_bounds__(256)
                  uint32_t* __restrict__ owner) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) owner[sblock[i]] = sblock[headpos[i]];  // headpos: inclusive max-scan of the head positions
+}
+
+// One warp per block: does the block's table equal the one of the head of its hash run?  Tables
+// of at most two values are fixed by (n, lo, hi); longer ones are compared value by value.  Any
+// mismatch raises *collided and the owners are recomputed by k_cseg_resolve.
+template <typename T, int CS_PER_LANE>
+__global__ void __launch_bounds__(128)
+    k_cseg_verify(const T* __restrict__ in, CsegDims d, uint32_t nblock, const uint32_t* __restrict__ n,
+                  const unsigned long long* __restrict__ lo, const unsigned long long* __restrict__ hi,
+                  const uint32_t* __restrict__ owner, uint32_t* __restrict__ collided) {
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t b = (uint32_t)((blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5);
+  if (b >= nblock) return;
+  const uint32_t o = owner[b];
+  if (o == b) return;
+  bool same = n[o] == n[b] && lo[o] == lo[b] && hi[o] == hi[b];
+  if (same && n[b] > 2) same = cs_same_table<T, CS_PER_LANE>(in, d, o, b, n[b], lane);
+  if (!same && lane == 0) *collided = 1;
+}
+
+// The path taken after a hash collision: one warp per sorted position i.  The owner of block
+// sblock[i] is the first block of its hash run (ascending block order) with an equal table,
+// possibly itself.  Quadratic in the run length; 64-bit hashes of distinct tables rarely meet.
+template <typename T, int CS_PER_LANE>
+__global__ void __launch_bounds__(128)
+    k_cseg_resolve(const T* __restrict__ in, CsegDims d, uint32_t nblock, const uint32_t* __restrict__ n,
+                   const unsigned long long* __restrict__ lo, const unsigned long long* __restrict__ hi,
+                   const uint32_t* __restrict__ sblock, const uint32_t* __restrict__ headpos, uint32_t* __restrict__ owner) {
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t i = (uint32_t)((blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5);
+  if (i >= nblock) return;
+  const uint32_t b = sblock[i];
+  const uint32_t nb = n[b];
+  const unsigned long long lob = lo[b], hib = hi[b];
+  uint32_t own = b;
+  for (uint32_t base = headpos[i]; base < i && own == b; base += 32) {
+    const uint32_t j = base + lane;
+    const uint32_t c = j < i ? sblock[j] : 0u;
+    uint32_t cand = __ballot_sync(CS_FULL, j < i && n[c] == nb && lo[c] == lob && hi[c] == hib);
+    while (cand) {
+      const uint32_t cb = __shfl_sync(CS_FULL, c, __ffs(cand) - 1);
+      if (nb <= 2 || cs_same_table<T, CS_PER_LANE>(in, d, cb, b, nb, lane)) {
+        own = cb;
+        break;
+      }
+      cand &= cand - 1;
+    }
+  }
+  if (lane == 0) owner[b] = own;
 }
 
 template <int WORDS>
@@ -221,14 +313,8 @@ static int cseg_dims(uint64_t sx, uint64_t sy, uint64_t sz, uint32_t bx, uint32_
   return IGN_OK;
 }
 
-// one channel; out_dev may be NULL (size query).  *n_words = words of the channel stream.
-template <typename T>
-static int cseg_encode_channel(ign_ctx* ctx, const T* in, const CsegDims& d, uint32_t* out_dev, uint64_t cap_words,
-                               uint64_t* n_words) {
-  constexpr int WORDS = sizeof(T) / 4;
-  const uint32_t nb = d.gx * d.gy * d.gz;
-  const size_t keep = ctx->scratch_used;
-  const bool own = keep == 0;
+// cub temporary bytes of one channel of nb blocks
+static size_t cseg_tmp_bytes(uint32_t nb) {
   size_t sortb = 0, scanb = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, sortb, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
                                   (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)nb);
@@ -238,14 +324,37 @@ static int cseg_encode_channel(ign_ctx* ctx, const T* in, const CsegDims& d, uin
     cub::DeviceScan::InclusiveScan(nullptr, mb, (const uint32_t*)nullptr, (uint32_t*)nullptr, cub::Max(), (int)nb);
     if (mb > scanb) scanb = mb;
   }
-  const size_t tmpb = (sortb > scanb ? sortb : scanb) + 256;
-  if (own) IGN_TRY(scratch_reserve(ctx, 2 * align_up((size_t)nb * 8, 256) + 8 * align_up(((size_t)nb + 1) * 4, 256) + tmpb + 4096));
+  return (sortb > scanb ? sortb : scanb) + 256;
+}
+
+// scratch bytes cseg_encode_channel takes for nb blocks: 4 u64 and 8 u32 arrays per block, a flag, cub temp
+static size_t cseg_channel_bytes(uint32_t nb) {
+  return 4 * align_up((size_t)nb * 8, 256) + 8 * align_up(((size_t)nb + 1) * 4, 256) + cseg_tmp_bytes(nb) + 4096;
+}
+
+// one channel; out_dev may be NULL (size query).  *n_words = words of the channel stream.
+template <typename T>
+static int cseg_encode_channel(ign_ctx* ctx, const T* in, const CsegDims& d, uint32_t* out_dev, uint64_t cap_words,
+                               uint64_t* n_words) {
+  constexpr int WORDS = sizeof(T) / 4;
+  const uint32_t nb = d.gx * d.gy * d.gz;
+  const size_t keep = ctx->scratch_used;
+  const bool own = keep == 0;
+  const size_t tmpb = cseg_tmp_bytes(nb);
+  if (own) IGN_TRY(scratch_reserve(ctx, cseg_channel_bytes(nb)));
   auto fail = [&](int rc) {
     ctx->scratch_used = keep;
     return rc;
   };
+  unsigned long long hash_mask = ~0ull;
+  if (const char* e = getenv("IGN_CSEG_HASH_BITS")) {
+    const int k = atoi(e);
+    hash_mask = k >= 64 ? ~0ull : k <= 0 ? 0ull : (1ull << k) - 1;
+  }
   unsigned long long* hash = (unsigned long long*)scratch_take(ctx, (size_t)nb * 8);
   unsigned long long* shash = (unsigned long long*)scratch_take(ctx, (size_t)nb * 8);
+  unsigned long long* lo = (unsigned long long*)scratch_take(ctx, (size_t)nb * 8);
+  unsigned long long* hi = (unsigned long long*)scratch_take(ctx, (size_t)nb * 8);
   uint32_t* n = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
   uint32_t* blk = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
   uint32_t* sblk = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
@@ -254,8 +363,10 @@ static int cseg_encode_channel(ign_ctx* ctx, const T* in, const CsegDims& d, uin
   uint32_t* scan = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
   uint32_t* enc_off = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
   uint32_t* tab_off = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
+  uint32_t* collided = (uint32_t*)scratch_take(ctx, 4);
   void* tmp = scratch_take(ctx, tmpb);
-  if (!hash || !shash || !n || !blk || !sblk || !owner || !size || !scan || !enc_off || !tab_off || !tmp) {
+  if (!hash || !shash || !lo || !hi || !n || !blk || !sblk || !owner || !size || !scan || !enc_off || !tab_off ||
+      !collided || !tmp) {
     set_error("scratch arena too small (cseg encode)");
     return fail(IGN_ERR_NOMEM);
   }
@@ -273,13 +384,18 @@ static int cseg_encode_channel(ign_ctx* ctx, const T* in, const CsegDims& d, uin
     ctx->launches++;                                  \
     CS_CUDA(cudaGetLastError());                      \
   } while (0)
+#define CS_LAUNCH_PL(kernel, ...)                                       \
+  do {                                                                  \
+    if (d.bvox <= 512) CS_LAUNCH((kernel<T, 16>), gw, 128, __VA_ARGS__); \
+    else CS_LAUNCH((kernel<T, 32>), gw, 128, __VA_ARGS__);               \
+  } while (0)
   const unsigned gw = blocks_for((uint64_t)nb * 32, 128);
   if (d.bvox <= 512)
-    CS_LAUNCH((k_cseg_scan<T, false, 16>), gw, 128, in, d, (uint64_t)nb, n, hash, (const uint32_t*)nullptr,
-              (const uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr);
+    CS_LAUNCH((k_cseg_scan<T, false, 16>), gw, 128, in, d, (uint64_t)nb, n, hash, hash_mask, lo, hi,
+              (const uint32_t*)nullptr, (const uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr);
   else
-    CS_LAUNCH((k_cseg_scan<T, false, 32>), gw, 128, in, d, (uint64_t)nb, n, hash, (const uint32_t*)nullptr,
-              (const uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr);
+    CS_LAUNCH((k_cseg_scan<T, false, 32>), gw, 128, in, d, (uint64_t)nb, n, hash, hash_mask, lo, hi,
+              (const uint32_t*)nullptr, (const uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr);
   CS_LAUNCH(k_iota32, blocks_for(nb, 256), 256, blk, nb);
   {
     size_t tb = tmpb;
@@ -293,19 +409,26 @@ static int cseg_encode_channel(ign_ctx* ctx, const T* in, const CsegDims& d, uin
     ctx->launches += 2;
   }
   CS_LAUNCH(k_cseg_owner, blocks_for(nb, 256), 256, tab_off, sblk, nb, owner);
-  CS_LAUNCH((k_cseg_sizes<WORDS>), blocks_for(nb, 256), 256, n, owner, nb, d.bvox, size);
-  CS_CUDA(cudaMemsetAsync(size + nb, 0, 4, ctx->stream));
-  {
-    size_t tb = tmpb;
-    CS_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, size, scan, (int)nb + 1, ctx->stream));
-    ctx->launches += 2;
-  }
-  uint32_t total = 0;
-  {
-    const int rc = small_d2h(ctx, &total, scan + nb, 4);
+  CS_CUDA(cudaMemsetAsync(collided, 0, 4, ctx->stream));
+  CS_LAUNCH_PL(k_cseg_verify, in, d, nb, n, (const unsigned long long*)lo, (const unsigned long long*)hi,
+               (const uint32_t*)owner, collided);
+  // the collision flag comes back with `total`; only after a collision is there a second round trip
+  uint32_t total = 0, hcollided = 0;
+  for (int pass = 0;; pass++) {
+    CS_LAUNCH((k_cseg_sizes<WORDS>), blocks_for(nb, 256), 256, n, owner, nb, d.bvox, size);
+    CS_CUDA(cudaMemsetAsync(size + nb, 0, 4, ctx->stream));
+    {
+      size_t tb = tmpb;
+      CS_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, size, scan, (int)nb + 1, ctx->stream));
+      ctx->launches += 2;
+    }
+    int rc = small_d2h(ctx, &total, scan + nb, 4);
+    if (rc == IGN_OK && pass == 0) rc = small_d2h(ctx, &hcollided, collided, 4);
+    if (rc == IGN_OK) rc = small_sync(ctx);
     if (rc != IGN_OK) return fail(rc);
-    const int rc2 = small_sync(ctx);
-    if (rc2 != IGN_OK) return fail(rc2);
+    if (pass > 0 || hcollided == 0) break;
+    CS_LAUNCH_PL(k_cseg_resolve, in, d, nb, n, (const unsigned long long*)lo, (const unsigned long long*)hi,
+                 (const uint32_t*)sblk, (const uint32_t*)tab_off, owner);
   }
   const uint64_t words = 2ull * nb + total;
   *n_words = words;
@@ -317,15 +440,16 @@ static int cseg_encode_channel(ign_ctx* ctx, const T* in, const CsegDims& d, uin
     CS_LAUNCH(k_cseg_offsets, blocks_for(nb, 256), 256, n, owner, scan, nb, d.bvox, enc_off, tab_off);
     if (d.bvox <= 512)
       CS_LAUNCH((k_cseg_scan<T, true, 16>), gw, 128, in, d, (uint64_t)nb, (uint32_t*)nullptr, (unsigned long long*)nullptr,
-                enc_off, tab_off, owner, out_dev);
+                hash_mask, (unsigned long long*)nullptr, (unsigned long long*)nullptr, enc_off, tab_off, owner, out_dev);
     else
       CS_LAUNCH((k_cseg_scan<T, true, 32>), gw, 128, in, d, (uint64_t)nb, (uint32_t*)nullptr, (unsigned long long*)nullptr,
-                enc_off, tab_off, owner, out_dev);
+                hash_mask, (unsigned long long*)nullptr, (unsigned long long*)nullptr, enc_off, tab_off, owner, out_dev);
   }
   ctx->scratch_used = keep;
   return IGN_OK;
 #undef CS_CUDA
 #undef CS_LAUNCH
+#undef CS_LAUNCH_PL
 }
 
 }  // namespace ign
@@ -406,7 +530,10 @@ int ign_cseg_encode(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, ui
   IGN_REQUIRE(dtype == IGN_U32 || dtype == IGN_U64, IGN_ERR_UNSUPPORTED, "compressed_segmentation holds uint32 / uint64 labels");
   const uint64_t n = sx * sy * sz * sc;
   scratch_reset(ctx);
-  IGN_TRY(scratch_reserve(ctx, align_up(n * es, 256) + align_up((out ? cap_words : 0) * 4, 256) + (64ull << 20)));
+  CsegDims d;
+  IGN_TRY(cseg_dims(sx, sy, sz, bx, by, bz, &d));
+  IGN_TRY(scratch_reserve(ctx, align_up(n * es, 256) + align_up((out ? cap_words : 0) * 4, 256) +
+                                   cseg_channel_bytes(d.gx * d.gy * d.gz) + (1 << 20)));
   void* d_in = scratch_take(ctx, n * es);
   uint32_t* d_out = out ? (uint32_t*)scratch_take(ctx, cap_words * 4) : nullptr;
   IGN_REQUIRE(d_in && (!out || d_out), IGN_ERR_NOMEM, "scratch arena too small (cseg)");
