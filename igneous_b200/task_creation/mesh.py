@@ -13,6 +13,7 @@ def create_meshing_tasks(layer_path, mip, shape=(448, 448, 448), simplification=
                          compress="gzip", closed_dataset_edges=True, dust_global=False, fill_holes=0,
                          dry_run=False, exclude_object_ids=[]):
   shape = Vec(*shape)
+  assert 0 <= fill_holes <= 103, "fill_holes must be between 0 to 103 inclusive."
   vol = CloudVolume(layer_path, mip)
   if mesh_dir is None:
     mesh_dir = vol.info.get("mesh", "mesh_mip_{}_err_{}".format(mip, max_simplification_error))

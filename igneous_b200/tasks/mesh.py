@@ -3,12 +3,12 @@
 Mirror of igneous/tasks/mesh/mesh.py:39-464 for the unsharded `precomputed`
 path (MeshTask.__init__ options :98-129, execute :140-265,
 _handle_dataset_boundary :267-303, _remove_dust :313-322, _remap :357-369,
-compute_meshes :371-383, _create_mesh_binary :432-450, uploads :399-464).
-zmesh / fastremap are replaced by igneous_b200.zmesh / igneous_b200.fastremap.
+fill_holes :211-243, compute_meshes :371-383, _create_mesh_binary :432-450, uploads :399-464).
+zmesh / fastremap / fastmorph are replaced by igneous_b200.zmesh / .fastremap / .fastmorph.
 """
 import numpy as np
 
-from .. import fastremap, zmesh
+from .. import fastmorph, fastremap, zmesh
 from .._compat import CloudVolume, CloudFiles, Bbox, Vec, RegisteredTask
 
 _DEFAULTS = {
@@ -37,8 +37,6 @@ class MeshTask(RegisteredTask):
     for k in ("sharded", "dust_global"):
       if self.options[k]:
         raise NotImplementedError("igneous_b200 MeshTask: %s=True is out of scope (DESIGN.md)" % k)
-    if self.options["fill_holes"]:
-      raise NotImplementedError("igneous_b200 MeshTask: fill_holes>0 (fastmorph) is out of scope (DESIGN.md)")
 
   # ------------------------------------------------------------------ execute
   def execute(self):
@@ -71,9 +69,27 @@ class MeshTask(RegisteredTask):
     data, renumbermap = fastremap.renumber(data, in_place=True)
     renumbermap = {v: k for k, v in renumbermap.items()}
 
-    self._mesher.mesh(data[..., 0], preserve_order=False)
-    del data
-    meshes = self.compute_meshes(renumbermap)
+    data = data[..., 0]
+    fill_level = int(opt["fill_holes"])
+    if fill_level > 0:  # mesh.py:211-243: enclosed objects keep their own meshes, their cell is solid
+      if fill_level >= 3:
+        data = fastmorph.dilate(data, mode=fastmorph.Mode.multilabel, background_only=True, parallel=1)
+      filled, holes = fastmorph.fill_holes_v2(
+        data, fix_borders=(fill_level >= 2),
+        merge_threshold=(1.0 if fill_level <= 3 else (1.0 - 0.01 * (fill_level - 3))), parallel=1)
+      del data
+      self._mesher.mesh(filled, preserve_order=False)
+      meshes = self.compute_meshes(renumbermap)
+      del filled
+      self._mesher.mesh(holes)
+      hole_meshes = self.compute_meshes(renumbermap)
+      del holes
+      for segid, mesh in hole_meshes.items():
+        meshes[segid] = zmesh.Mesh.concatenate(meshes[segid], mesh, id=segid) if segid in meshes else mesh
+    else:
+      self._mesher.mesh(data, preserve_order=False)
+      del data
+      meshes = self.compute_meshes(renumbermap)
 
     bounding_boxes = {}
     for segid, mesh in meshes.items():

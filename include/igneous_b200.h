@@ -205,6 +205,30 @@ IGN_API int ign_ccl_task_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64_
                      uint64_t rail_x, uint64_t rail_y, uint64_t rail_z, uint64_t dust_threshold,
                      uint64_t label_offset, uint64_t* out, uint64_t* n_components);
 
+/* ------------------------------------------------------------- hole filling
+ * fastmorph.dilate(data, mode=multilabel, background_only=True)  igneous/tasks/mesh/mesh.py:211-218
+ *   one pass: a 0 voxel with a non-zero voxel among its 26 in-box neighbours takes the most
+ *   frequent non-zero neighbour label, ties to the smaller label; other voxels are copied.
+ * fastmorph.fill_holes_v2(data, fix_borders, merge_threshold)   igneous/tasks/mesh/mesh.py:220-228
+ *   the rule of DESIGN.md "Hole filling" (fastmorph parity unpinned): filled = every region
+ *   replaced by the label of the non-zero region nearest the outside that encloses it; holes =
+ *   input where it differs from filled and is non-zero, else 0.  merge_threshold_pct = 100 *
+ *   merge_threshold (0..100, whole percent).  u8 / u16 / u32 / u64 (label 2^64-1 unsupported);
+ *   out buffers of the input's dtype, not aliasing it.
+ *   Not stream-ordered: the graph solve runs on the host, so ign_fill_holes_dev synchronises the
+ *   ctx stream about four times per pass (one pass per face plane with fix_borders, six at most,
+ *   then one for the volume) and returns with the results written.  ign_dilate_multilabel_dev is
+ *   asynchronous like the other _dev calls.
+ */
+IGN_API int ign_dilate_multilabel(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
+                                  void* out);
+IGN_API int ign_dilate_multilabel_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy,
+                                      uint64_t sz, void* out);
+IGN_API int ign_fill_holes(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
+                           int fix_borders, int merge_threshold_pct, void* filled, void* holes);
+IGN_API int ign_fill_holes_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
+                               int fix_borders, int merge_threshold_pct, void* filled, void* holes);
+
 /* ---------------------------------------------------------------- fastremap
  * fastremap.renumber(data, in_place=True)            igneous/tasks/mesh/mesh.py:206
  *   ids 1..K by first appearance in memory order, 0 kept.  out is u32;

@@ -144,6 +144,30 @@ def probe_cseg(cseg, O, out, report):
   return ok
 
 
+def probe_fastmorph(fm, out, report):
+  """fastmorph.dilate / fill_holes_v2 on the hole-filling test volumes (tests/fillref.py): records
+  the wheel's outputs and whether they follow the rule of DESIGN.md "Hole filling".  That rule
+  is this project's own until the recorded outputs pin it, so a difference is reported, not failed."""
+  sys.path.insert(0, os.path.join(ROOT, "tests"))
+  import fillref as F
+  res, arrays = {}, {}
+  for name, X in sorted(F.kats().items()):
+    for level in (1, 2, 3, 4, 13):
+      X0 = np.asarray(fm.dilate(X, mode=fm.Mode.multilabel, background_only=True, parallel=1)) if level >= 3 else X
+      filled, holes = fm.fill_holes_v2(X0, fix_borders=level >= 2, parallel=1,
+                                       merge_threshold=1.0 if level <= 3 else 1.0 - 0.01 * (level - 3))
+      filled, holes = np.asarray(filled), np.asarray(holes)
+      want_f, want_h = F.fill_level(X, level)
+      res["%s@%d" % (name, level)] = {"dilate_equals_rule": bool(level < 3 or np.array_equal(X0, F.dilate(X))),
+                                      "filled_equals_rule": bool(np.array_equal(filled, want_f)),
+                                      "holes_equals_rule": bool(np.array_equal(holes, want_h))}
+      arrays["%s_l%d_filled" % (name, level)] = filled
+      arrays["%s_l%d_holes" % (name, level)] = holes
+    arrays[name] = X
+  np.savez_compressed(os.path.join(out, "upstream_fastmorph.npz"), **arrays)
+  report["fastmorph"] = res
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument("--out", default=os.path.join(ROOT, "tests", "golden"))
@@ -151,7 +175,8 @@ def main():
   os.makedirs(args.out, exist_ok=True)
   from oracle import oracle as O
   O.build()
-  mods = {n: try_import(n) for n in ("tinybrain", "cc3d", "zmesh", "fastremap", "compressed_segmentation")}
+  mods = {n: try_import(n) for n in ("tinybrain", "cc3d", "zmesh", "fastremap", "compressed_segmentation",
+                                     "fastmorph")}
   report = {"wheels": {n: (getattr(m, "__version__", "present") if m else None) for n, m in mods.items()}}
   verdicts = {}
   if mods["tinybrain"]:
@@ -163,9 +188,12 @@ def main():
     verdicts["zmesh"] = probe_zmesh(mods["zmesh"], O, args.out, report)
   if mods["compressed_segmentation"]:
     verdicts["compressed_segmentation"] = probe_cseg(mods["compressed_segmentation"], O, args.out, report)
+  if mods["fastmorph"]:
+    probe_fastmorph(mods["fastmorph"], args.out, report)
   report["agrees_with_frozen_defaults"] = verdicts
   report["not_run"] = [k for k, n in (("averaging", "tinybrain"), ("mode", "tinybrain"), ("cc3d", "cc3d"),
-                                      ("zmesh", "zmesh"), ("compressed_segmentation", "compressed_segmentation")) if not mods[n]]
+                                      ("zmesh", "zmesh"), ("compressed_segmentation", "compressed_segmentation"),
+                                      ("fastmorph", "fastmorph")) if not mods[n]]
   with open(os.path.join(args.out, "first_contact_report.json"), "w") as f:
     json.dump(report, f, indent=1)
   print(json.dumps(report, indent=1))
