@@ -21,6 +21,7 @@ struct ign_mesher {
   float simp_max_error;
   int simp_rounds;
   uint32_t simp_labels_smem, simp_labels_gmem;  // labels simplified in shared / global memory
+  uint32_t simp_labels_class[3];                // labels simplified in 1024-, 512- and 256-thread CTAs
   std::vector<uint64_t> ids;       // original label of dense id i+1
   std::vector<uint32_t> tri_off;   // [K+2]
   std::vector<uint32_t> vert_off;  // [K+2]

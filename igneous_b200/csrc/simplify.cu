@@ -264,6 +264,35 @@ constexpr uint32_t WF_BAD = 1, WF_OK = 2;  // winner flags: failed validation / 
 constexpr int SL_EQ = 96;      // per-warp queue of faces with half-edges whose cost must be (re)computed
 constexpr int SL_LIST_PER = 16;  // list entries per thread held in registers while a list is compacted in place
 
+// Size classes of k_simp_labels: CTA size and CTAs per SM.  A label runs in the smallest class whose
+// shared-memory budget holds it, so labels that need less than half (a quarter) of an SM's shared
+// memory run two (four) to an SM and overlap each other's barrier and latency phases.
+constexpr int SL_NCLASS = 3;
+constexpr int SL_CLASS_THREADS[SL_NCLASS] = {1024, 512, 256};
+
+// dynamic shared-memory layout of a label at `threads` threads:
+// cost queues | ring lists | key1 | faces SoA | face list | face state | vertex flags | lose marks
+struct SlLayout {
+  size_t wq, o_key, o_f0, o_fl, o_fs, o_vf, o_vl, need;
+};
+__host__ __device__ inline SlLayout sl_layout(uint32_t T, uint32_t U, uint32_t threads) {
+  SlLayout y;
+  y.wq = (size_t)(threads / 32) * SL_EQ * 4;
+  y.o_key = y.wq + (size_t)SL_WCAP * 2 * S_MAXV * 2;  // shared-memory class: 16-bit face ids in the rings
+  y.o_f0 = y.o_key + 4 * (size_t)U;                    // 32-bit keys
+  y.o_fl = y.o_f0 + 6 * (size_t)T;
+  y.o_fs = y.o_fl + 2 * (size_t)T;
+  y.o_vf = (y.o_fs + T + 3) & ~(size_t)3;
+  y.o_vl = (y.o_vf + U + 3) & ~(size_t)3;
+  y.need = y.o_vl + U + 4;
+  return y;
+}
+// the shared-memory class also needs 16-bit keys and lists that a compaction holds in registers
+__host__ __device__ inline bool sl_fits_smem(uint32_t T, uint32_t U, uint32_t threads, size_t smem_bytes) {
+  const uint32_t cap = (uint32_t)SL_LIST_PER * threads;
+  return 3ull * T <= 65536ull && T <= cap && U <= cap && sl_layout(T, U, threads).need <= smem_bytes;
+}
+
 struct SlArgs {
   double* pos;            // 3U
   double* Q;              // 10U
@@ -282,14 +311,18 @@ struct SlArgs {
   const uint32_t* tri_off;   // [K+2]
   const uint32_t* vert_off;  // [K+2]
   const uint32_t* target;    // [K+2]
-  const uint32_t* order;     // [K] dense labels, largest first
+  const uint32_t* order;     // [K] dense labels of this launch's size class, largest first
   uint32_t K;
-  uint32_t* counters;  // [0] next work item  [1] max rounds  [2] labels run in shared memory  [3] in global memory
+  uint32_t base;       // position of order[0] in the task's work order (all classes)
+  uint32_t cls;        // size class of the launch
+  uint32_t* counters;  // [1] max rounds  [2] labels run in shared memory  [3] in global memory
+                       // [4 + class] next work item  [8 + class] labels run in the class
   double max_err2;
   int max_rounds;
   uint32_t smem_bytes;  // dynamic shared memory of the launch
   int persist;          // 1: a CTA keeps taking labels until the list is empty (IGN_SIMP_PERSIST=1)
-  uint32_t* lrec;       // IGN_SIMP_TRACE=1: [work item][4] = faces, rounds, kilocycles, face visits (sum of list lengths)
+  uint32_t* lrec;       // IGN_SIMP_TRACE=1: [base + work item][6] = faces, rounds, kilocycles, face visits
+                        // (sum of list lengths), winners, memory class | size class << 2
   uint32_t* trace;      // IGN_SIMP_TRACE=1: [round][4] = winners, collapses, alive faces, list length of the largest label
 };
 
@@ -964,7 +997,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
       if (total <= (uint32_t)SL_WCAP) break;
     }
     // ---- stop rules of the label
-    if (tid == 0 && A.trace != nullptr && sh.work == 0 && r < 400) {
+    if (tid == 0 && A.trace != nullptr && A.base + sh.work == 0 && r < 400) {
       A.trace[4 * r + 0] = sh.progress;
       A.trace[4 * r + 1] = sh.ncol;
       A.trace[4 * r + 2] = sh.alive;
@@ -1009,24 +1042,27 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
   for (uint32_t v = tid; v < U; v += NT) A.valive[L.vbase + v] = (L.vflag[v] & VF_ALIVE) ? 1 : 0;
   if (tid == 0 && A.trace != nullptr) {
     for (int q = 0; q < 10; q++) atomicAdd((unsigned long long*)(A.trace + 1600) + q, sh.ph[q]);
-    uint32_t* rec = A.lrec + 6 * (size_t)sh.work;
+    uint32_t* rec = A.lrec + 6 * (size_t)(A.base + sh.work);
     rec[0] = T;
     rec[1] = (uint32_t)r;
     rec[2] = (uint32_t)((clock64() - sh.t_label) >> 10);
     rec[3] = (uint32_t)(sh.visits > 0xFFFFFFFFull ? 0xFFFFFFFFull : sh.visits);
     rec[4] = (uint32_t)sh.wins;
-    rec[5] = SM ? 1u : ((const void*)L.key1 == (const void*)(A.key1 + L.vbase) ? 3u : 2u);
+    rec[5] = (SM ? 1u : ((const void*)L.key1 == (const void*)(A.key1 + L.vbase) ? 3u : 2u)) | (A.cls << 2);
   }
   if (tid == 0) {
     atomicMax(&A.counters[1], (uint32_t)r);
     atomicAdd(&A.counters[SM ? 2 : 3], 1u);
+    atomicAdd(&A.counters[8 + A.cls], 1u);
   }
 }
 
 extern __shared__ __align__(16) unsigned char sl_smem[];
 
-// One label per CTA (the launch has one CTA per label; a CTA takes the next label of the size-sorted
-// order from a counter, so big labels start first whatever order the hardware dispatches CTAs in).
+// One label per CTA (the launch has one CTA per label of its size class; a CTA takes the next label of
+// the size-sorted order from a counter, so big labels start first whatever order the hardware dispatches
+// CTAs in).  The block size is the class's (1024, 512 or 256 threads); 64 registers per thread let two
+// 512-thread or four 256-thread CTAs share an SM.
 // CTAs that end after one label keep returning their SM to the block scheduler: kernels of
 // other streams -- the CCL passes of the volume pipeline run on a higher-priority stream while
 // MeshTasks are in flight -- get SMs within a label's run time instead of a whole task's.
@@ -1034,7 +1070,7 @@ __global__ void __launch_bounds__(SL_THREADS, 1) k_simp_labels(SlArgs A) {
   __shared__ SlShared sh;
   do {
     __syncthreads();  // (persistent mode) the previous label is completely written back; sh.work may be reused
-    if (threadIdx.x == 0) sh.work = atomicAdd(&A.counters[0], 1u);
+    if (threadIdx.x == 0) sh.work = atomicAdd(&A.counters[4 + A.cls], 1u);
     __syncthreads();
     const uint32_t wi = sh.work;
     if (wi >= A.K) break;
@@ -1043,42 +1079,32 @@ __global__ void __launch_bounds__(SL_THREADS, 1) k_simp_labels(SlArgs A) {
     const uint32_t vbase = A.vert_off[l], U = A.vert_off[l + 1] - vbase;
     const uint32_t target = A.target[l];
     if (T == 0 || T <= target) continue;  // init left every face / vertex alive
-    // shared-memory layout: cost queues | ring lists | key1 | faces SoA | face list | face state | vertex flags
-    const size_t wq_bytes = (size_t)(SL_THREADS / 32) * SL_EQ * 4;
-    const size_t ring_sm = (size_t)SL_WCAP * 2 * S_MAXV * 2, ring_gl = (size_t)SL_WCAP * 2 * S_MAXV * 4;
-    const size_t o_key = wq_bytes + ring_sm;   // shared-memory class: 16-bit face ids
-    const size_t o_keyg = wq_bytes + ring_gl;  // other classes: 32-bit
-    const size_t o_f0 = o_key + 4 * (size_t)U;  // 32-bit keys
-    const size_t o_fl = o_f0 + 6 * (size_t)T;
-    const size_t o_fs = o_fl + 2 * (size_t)T;
-    const size_t o_vf = (o_fs + T + 3) & ~(size_t)3;
-    const size_t o_vl = (o_vf + U + 3) & ~(size_t)3;
-    const size_t need = o_vl + U + 4;
-    const uint32_t cap = (uint32_t)SL_LIST_PER * blockDim.x;
+    const SlLayout y = sl_layout(T, U, blockDim.x);
+    const size_t o_keyg = y.wq + (size_t)SL_WCAP * 2 * S_MAXV * 4;  // other classes: 32-bit face ids in the rings
     const bool fmt16 = 3ull * T <= 65536ull;
-    if (need <= A.smem_bytes && T <= cap && U <= cap && fmt16) {
+    if (sl_fits_smem(T, U, blockDim.x, A.smem_bytes)) {
       SlLab<true> L;
       L.T = T; L.U = U; L.tbase = tbase; L.vbase = vbase; L.target = target;
       L.wq = (uint32_t*)sl_smem;
-      L.ring = (uint16_t*)(sl_smem + wq_bytes);
-      L.key1 = (uint32_t*)(sl_smem + o_key);
+      L.ring = (uint16_t*)(sl_smem + y.wq);
+      L.key1 = (uint32_t*)(sl_smem + y.o_key);
       L.fmt16 = true;
-      L.fc0 = (uint16_t*)(sl_smem + o_f0);
+      L.fc0 = (uint16_t*)(sl_smem + y.o_f0);
       L.fc1 = L.fc0 + T;
       L.fc2 = L.fc1 + T;
-      L.flist = (uint16_t*)(sl_smem + o_fl);
+      L.flist = (uint16_t*)(sl_smem + y.o_fl);
       L.vlist = nullptr;
       L.flist2 = L.vlist2 = nullptr;
       L.gface = nullptr;
-      L.fstate = sl_smem + o_fs;
-      L.vflag = sl_smem + o_vf;
-      L.vlose = sl_smem + o_vl;
+      L.fstate = sl_smem + y.o_fs;
+      L.vflag = sl_smem + y.o_vf;
+      L.vlose = sl_smem + y.o_vl;
       sl_run<true>(A, L, sh);
     } else {
       SlLab<false> L;
       L.T = T; L.U = U; L.tbase = tbase; L.vbase = vbase; L.target = target;
       L.wq = (uint32_t*)sl_smem;  // the cost queues and the ring lists always fit
-      L.ring = (uint32_t*)(sl_smem + wq_bytes);
+      L.ring = (uint32_t*)(sl_smem + y.wq);
       L.fc0 = L.fc1 = L.fc2 = nullptr;
       L.flist = A.flist + tbase; L.flist2 = A.flist2 + tbase;
       L.vlist = A.vlist + vbase; L.vlist2 = A.vlist2 + vbase;
@@ -1174,6 +1200,8 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   m->simp_factor = reduction_factor;
   m->simp_max_error = max_error;
   m->simp_rounds = 0;
+  m->simp_labels_smem = m->simp_labels_gmem = 0;
+  for (int c = 0; c < SL_NCLASS; c++) m->simp_labels_class[c] = 0;
   const uint64_t U = m->U, T = m->T, K = m->K;
   if (T == 0 || U == 0) {
     m->simplified = true;
@@ -1267,11 +1295,29 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   std::vector<uint32_t> target(K + 2, 0);
   for (uint64_t l = 1; l <= K; l++)
     target[l] = (m->tri_off[l + 1] - m->tri_off[l]) / (uint32_t)reduction_factor;
-  // work order of the label kernel: largest labels first (the tail is made of small ones)
+  // dynamic shared memory of a CTA of each size class: the SM's 227 KB split between its CTAs, less
+  // the static SlShared and the 1 KB the SM reserves per CTA
+  const size_t sl_static = ((sizeof(SlShared) + 255) / 256) * 256 + 1024;
+  size_t sl_dyn[SL_NCLASS];
+  for (int c = 0; c < SL_NCLASS; c++) sl_dyn[c] = (232448 / (size_t)(1024 / SL_CLASS_THREADS[c]) - sl_static) & ~(size_t)255;
+  // size class of every label: the smallest whose shared-memory budget holds the label (labels that fit
+  // no class run in the 1024-thread class on global memory)
+  std::vector<uint32_t> lcls(K + 2, 0);
+  uint32_t ccount[SL_NCLASS] = {0, 0, 0};
+  for (uint64_t l = 1; l <= K; l++) {
+    const uint32_t tl = m->tri_off[l + 1] - m->tri_off[l], ul = m->vert_off[l + 1] - m->vert_off[l];
+    int c = SL_NCLASS - 1;
+    while (c > 0 && !sl_fits_smem(tl, ul, SL_CLASS_THREADS[c], sl_dyn[c])) c--;
+    lcls[l] = (uint32_t)c;
+    ccount[c]++;
+  }
+  // work order of the label kernel: class by class, largest labels first within a class (the tail of
+  // each launch is made of its small labels)
   std::vector<uint32_t> order(K);
   for (uint64_t l = 0; l < K; l++) order[l] = (uint32_t)(l + 1);
   std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
     const uint32_t ta = m->tri_off[a + 1] - m->tri_off[a], tb = m->tri_off[b + 1] - m->tri_off[b];
+    if (lcls[a] != lcls[b]) return lcls[a] < lcls[b];
     return ta != tb ? ta > tb : a < b;
   });
   S_TRY(small_h2d(ctx, d_target, target.data(), (K + 2) * 4));
@@ -1296,25 +1342,16 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   S_LAUNCH(k_simp_quadrics, blocks_for(U, 128), 128, s);
   S_LAUNCH(k_simp_boundary, blocks_for(3 * T, 256), 256, s);
 
-  // ---- all rounds of every label: persistent CTAs pull labels off the order list.  The kernel is
-  // latency bound (barriers, dependent loads), so several CTAs per SM overlap each other's
-  // stalls; the shared-memory budget of a label is the SM's divided by the CTAs per SM
-  // (IGN_SIMP_THREADS / IGN_SIMP_CTAS override the default for experiments).
-  // measured on an H100 SXM (400 W limit): 1024x1 55 ms, 512x2 93 ms, 256x4 106 ms per 257^3 task
-  int sl_threads = 1024, sl_ctas = 1;
-  if (const char* e = getenv("IGN_SIMP_THREADS")) sl_threads = atoi(e);
-  if (const char* e = getenv("IGN_SIMP_CTAS")) sl_ctas = atoi(e);
-  if (sl_threads != 256 && sl_threads != 512 && sl_threads != 1024) sl_threads = 1024;
-  if (sl_ctas < 1 || sl_ctas * sl_threads > 1024) sl_ctas = 1024 / sl_threads;
-  const size_t sl_static = ((sizeof(SlShared) + 255) / 256) * 256 + 1024;
-  const size_t sl_dyn = ((232448 / (size_t)sl_ctas) > sl_static + 16384 ? (232448 / (size_t)sl_ctas) - sl_static : 16384) & ~(size_t)255;
-  S_CUDA(cudaFuncSetAttribute(k_simp_labels, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sl_dyn));
+  // ---- all rounds of every label: one launch per size class, one CTA per label.  The kernel is
+  // latency and barrier bound, so labels that fit half (a quarter) of an SM's shared memory run two
+  // (four) CTAs to an SM, which overlap each other's stalls; larger labels keep the whole SM.
+  S_CUDA(cudaFuncSetAttribute(k_simp_labels, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sl_dyn[0]));
   SlArgs A;
   A.pos = s.pos; A.Q = s.Q; A.face = s.face; A.falive = s.falive; A.valive = s.valive; A.vbound = s.vbound;
   A.ecost = ecost; A.key1 = key1; A.fstate = fstate; A.vflag = vflag; A.vlose = vlose;
   A.flist = gl_f[0]; A.flist2 = gl_f[1]; A.vlist = gl_v[0]; A.vlist2 = gl_v[1];
-  A.tri_off = d_tri_off; A.vert_off = d_vert_off; A.target = d_target; A.order = d_order;
-  A.K = (uint32_t)K; A.counters = flags;
+  A.tri_off = d_tri_off; A.vert_off = d_vert_off; A.target = d_target;
+  A.counters = flags;
   A.max_err2 = (double)max_error * (double)max_error;
   A.max_rounds = 400;
   // IGN_SIMP_GMEM=1 (test knob): run every label on the global-memory arrays, the path of
@@ -1329,20 +1366,51 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
     if (A.trace) S_CUDA(cudaMemsetAsync(A.lrec, 0, (size_t)K * 24 + 64, ctx->stream));
   }
   const char* force_gmem = getenv("IGN_SIMP_GMEM");
-  const uint32_t sl_fixed = (uint32_t)((SL_THREADS / 32) * SL_EQ * 4 + SL_WCAP * 2 * S_MAXV * 4);  // queues + ring lists
-  A.smem_bytes = (force_gmem && force_gmem[0] == '1') ? sl_fixed : (uint32_t)sl_dyn;
+  const bool gmem_only = force_gmem && force_gmem[0] == '1';
   {
     const int slot = prof_begin(ctx, IGN_PROF_SIMP);
     // default: one CTA per label (SMs are handed back to the block scheduler after every label, so
     // higher-priority streams get them quickly); IGN_SIMP_PERSIST=1: one CTA per SM slot loops over labels
     const char* pe = getenv("IGN_SIMP_PERSIST");
     A.persist = (pe && pe[0] == '1') ? 1 : 0;
-    const uint64_t slots = (uint64_t)ctx->sm_count * sl_ctas;
-    const unsigned grid = A.persist ? (unsigned)(K < slots ? K : slots) : (unsigned)K;
-    k_simp_labels<<<grid, sl_threads, sl_dyn, ctx->stream>>>(A);
-    ctx->launches++;
+    // The classes run side by side on streams forked from the task's stream, launched largest class
+    // first: the block scheduler dispatches the CTAs of earlier launches first, so the smaller classes
+    // fill the SMs that the end of a larger class leaves idle instead of waiting for its last label.
+    // (Streams and events are released by the runtime once their work is done.)
+    int prio = 0;
+    S_CUDA(cudaStreamGetPriority(ctx->stream, &prio));
+    cudaStream_t cs[SL_NCLASS] = {ctx->stream, nullptr, nullptr};
+    cudaEvent_t ev[SL_NCLASS] = {nullptr, nullptr, nullptr};
+    cudaError_t err = cudaEventCreateWithFlags(&ev[0], cudaEventDisableTiming);
+    if (err == cudaSuccess) err = cudaEventRecord(ev[0], ctx->stream);
+    uint32_t base = 0;
+    for (int c = 0; c < SL_NCLASS && err == cudaSuccess; c++) {  // largest class first
+      const uint32_t n = ccount[c], nt = (uint32_t)SL_CLASS_THREADS[c];
+      if (n == 0) continue;
+      if (c > 0) {
+        err = cudaStreamCreateWithPriority(&cs[c], cudaStreamNonBlocking, prio);
+        if (err == cudaSuccess) err = cudaStreamWaitEvent(cs[c], ev[0], 0);
+        if (err == cudaSuccess) err = cudaEventCreateWithFlags(&ev[c], cudaEventDisableTiming);
+        if (err != cudaSuccess) break;
+      }
+      A.order = d_order + base; A.K = n; A.base = base; A.cls = (uint32_t)c;
+      // 0: every label takes the global-memory path (only the cost queues and ring lists stay in smem)
+      A.smem_bytes = gmem_only ? 0u : (uint32_t)sl_dyn[c];
+      const uint64_t slots = (uint64_t)ctx->sm_count * (1024 / nt);
+      const unsigned grid = A.persist ? (unsigned)(n < slots ? n : slots) : n;
+      k_simp_labels<<<grid, nt, sl_dyn[c], cs[c]>>>(A);
+      ctx->launches++;
+      err = cudaGetLastError();
+      if (c > 0 && err == cudaSuccess) err = cudaEventRecord(ev[c], cs[c]);
+      if (c > 0 && err == cudaSuccess) err = cudaStreamWaitEvent(ctx->stream, ev[c], 0);
+      base += n;
+    }
+    for (int c = 0; c < SL_NCLASS; c++) {
+      if (ev[c]) cudaEventDestroy(ev[c]);
+      if (c > 0 && cs[c]) cudaStreamDestroy(cs[c]);
+    }
     prof_end(ctx, slot);
-    S_CUDA(cudaGetLastError());
+    S_CUDA(err);
   }
 
   // ---- compaction
@@ -1380,21 +1448,32 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
       // per-label records: where do the cycles go -- per round (fixed latency) or per face visit?
       std::vector<uint32_t> rec(6 * (size_t)K);
       S_CUDA(cudaMemcpy(rec.data(), A.lrec, rec.size() * 4, cudaMemcpyDeviceToHost));
-      static const uint32_t edges[] = {0, 500, 1000, 2000, 4000, 8000, 16000, 32000, 64000, 0xFFFFFFFFu};
-      fprintf(stderr, "%12s %7s %8s %10s %10s %9s %9s  class(sm/hy/gl)\n", "faces<", "labels", "rounds", "Mcycles", "Mvisits", "kwins", "cyc/round");
+      static const uint32_t edges[] = {0, 500, 1000, 2000, 3000, 4000, 6000, 8000, 10000, 12000, 16000, 32000, 64000, 0xFFFFFFFFu};
+      const int nedges = (int)(sizeof(edges) / sizeof(edges[0]));
+      // kilocycles are wall cycles of the label's CTA, which shares its SM with the other CTAs of its class
+      for (int c = 0; c < SL_NCLASS; c++) {
+        int per_sm = 0;
+        S_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_simp_labels, SL_CLASS_THREADS[c], sl_dyn[c]));
+        fprintf(stderr, "size class %d: %4d threads, %6zu B dynamic shared memory, %d CTAs per SM, %u labels\n", c,
+                SL_CLASS_THREADS[c], sl_dyn[c], per_sm, ccount[c]);
+      }
+      fprintf(stderr, "%7s %12s %7s %8s %10s %10s %9s %9s  class(sm/hy/gl)\n", "threads", "faces<", "labels", "rounds", "Mcycles", "Mvisits", "kwins", "cyc/round");
       double sr = 0, sv = 0, sc = 0, srr = 0, svv = 0, srv = 0, src = 0, svc = 0;
-      for (int b = 0; b + 1 < 10; b++) {
-        uint64_t n = 0, rounds = 0, kc = 0, vis = 0, wins = 0, cls[4] = {0, 0, 0, 0};
-        for (uint64_t i = 0; i < K; i++) {
-          const uint32_t* q = &rec[6 * i];
-          if (q[1] == 0 || q[0] < edges[b] || q[0] >= edges[b + 1]) continue;
-          n++; rounds += q[1]; kc += q[2]; vis += q[3]; wins += q[4]; cls[q[5] & 3]++;
-          const double R = q[1], V = q[3], C = q[2] * 1024.0;
-          sr += R; sv += V; sc += C; srr += R * R; svv += V * V; srv += R * V; src += R * C; svc += V * C;
+      for (int szc = 0; szc < SL_NCLASS; szc++) {
+        for (int b = 0; b + 1 < nedges; b++) {
+          uint64_t n = 0, rounds = 0, kc = 0, vis = 0, wins = 0, cls[4] = {0, 0, 0, 0};
+          for (uint64_t i = 0; i < K; i++) {
+            const uint32_t* q = &rec[6 * i];
+            if (q[1] == 0 || (int)(q[5] >> 2) != szc || q[0] < edges[b] || q[0] >= edges[b + 1]) continue;
+            n++; rounds += q[1]; kc += q[2]; vis += q[3]; wins += q[4]; cls[q[5] & 3]++;
+            const double R = q[1], V = q[3], C = q[2] * 1024.0;
+            sr += R; sv += V; sc += C; srr += R * R; svv += V * V; srv += R * V; src += R * C; svc += V * C;
+          }
+          if (n) fprintf(stderr, "%7d %12u %7llu %8.1f %10.2f %10.3f %9.1f %9.0f  %llu/%llu/%llu\n", SL_CLASS_THREADS[szc], edges[b + 1],
+                         (unsigned long long)n, (double)rounds / n, kc * 1024.0 / 1e6, vis / 1e6, wins / 1e3,
+                         rounds ? kc * 1024.0 / rounds : 0.0, (unsigned long long)cls[1], (unsigned long long)cls[2],
+                         (unsigned long long)cls[3]);
         }
-        if (n) fprintf(stderr, "%12u %7llu %8.1f %10.2f %10.3f %9.1f %9.0f  %llu/%llu/%llu\n", edges[b + 1], (unsigned long long)n, (double)rounds / n,
-                       kc * 1024.0 / 1e6, vis / 1e6, wins / 1e3, rounds ? kc * 1024.0 / rounds : 0.0,
-                       (unsigned long long)cls[1], (unsigned long long)cls[2], (unsigned long long)cls[3]);
       }
       // least squares cycles = a * rounds + b * visits (no intercept)
       const double det = srr * svv - srv * srv;
@@ -1407,6 +1486,7 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   m->simp_rounds = (int)hflags[1];
   m->simp_labels_smem = hflags[2];
   m->simp_labels_gmem = hflags[3];
+  for (int c = 0; c < SL_NCLASS; c++) m->simp_labels_class[c] = hflags[8 + c];
   const uint32_t U2 = last[0] + last[1], T2 = last[2] + last[3];
   S_LAUNCH(k_simp_new_offsets, blocks_for(K + 2, 256), 256, d_vert_off, vscan, (uint32_t)(K + 2), U, U2,
            d_new_vert_off);
@@ -1427,4 +1507,14 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   for (uint64_t l = 1; l <= K; l++)
     if (m->tri_off[l + 1] > m->tri_off[l]) m->present.push_back(m->ids[l - 1]);
   return done(IGN_OK);
+}
+
+extern "C" int ign_mesh_simplify_stats(ign_mesher* m, uint32_t stats[6]) {
+  IGN_REQUIRE(m && stats, IGN_ERR_INVALID, "null argument");
+  IGN_REQUIRE(m->simplified, IGN_ERR_INVALID, "mesher is not simplified");
+  stats[0] = (uint32_t)m->simp_rounds;
+  stats[1] = m->simp_labels_smem;
+  stats[2] = m->simp_labels_gmem;
+  for (int c = 0; c < SL_NCLASS; c++) stats[3 + c] = m->simp_labels_class[c];
+  return IGN_OK;
 }

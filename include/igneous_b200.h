@@ -287,6 +287,10 @@ IGN_API int ign_mesh_get(ign_mesher* m, uint64_t id, const float resolution[3], 
  * calls it on first use; ign_mesh_export then returns the simplified meshes. */
 IGN_API int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int reduction_factor,
                               float max_error);
+/* counters of the simplification that ran: [0] most rounds of any label, [1] labels simplified
+ * in shared memory, [2] in global memory, [3..5] labels simplified in the 1024-, 512- and 256-thread
+ * size classes (a label runs in the smallest CTA whose shared-memory budget holds it) */
+IGN_API int ign_mesh_simplify_stats(ign_mesher* m, uint32_t stats[6]);
 /* bulk export of every label's mesh (simplified if ign_mesh_simplify ran) in ign_mesh_ids order:
  * vertices f32 [U,3], faces u32 [T,3] (label-local indices), offsets [n_ids+1] */
 IGN_API int ign_mesh_export(ign_mesher* m, const float resolution[3], int voxel_centered,
