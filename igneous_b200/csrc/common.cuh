@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string>
+#include <vector>
 
 #include "../../include/igneous_b200.h"
 
@@ -52,7 +53,6 @@ static inline int dtype_size(int dt) {
 
 }  // namespace ign
 
-// grow-only device scratch arena, bump allocated per API call
 constexpr int IGN_TIMER_SLOTS = 64;  // CUDA event pairs per context: timers and cross-stream marks
 
 struct ign_ctx {
@@ -60,9 +60,12 @@ struct ign_ctx {
   int sm_count;
   cudaStream_t stream;
   cudaStream_t copy_stream;
-  char* scratch;
-  size_t scratch_bytes;
-  size_t scratch_used;
+  // device scratch arena, bump allocated through ign::ScratchFrame
+  struct ScratchBlock { char* base; size_t bytes, used; };
+  std::vector<ScratchBlock> scratch;  // normally one block
+  size_t scratch_lin;                 // bytes taken, as if the blocks were one
+  size_t scratch_high;                // largest scratch_lin reached: the size a coalesced block needs
+  int scratch_frames;                 // open frames
   char* pinned;  // staging for scalars / small results
   size_t pinned_bytes;
   cudaEvent_t timers[IGN_TIMER_SLOTS][2];
@@ -94,13 +97,35 @@ namespace ign {
 
 // Make `ctx->device` current (one ctx per process is the contract, but be safe).
 int activate(ign_ctx* ctx);
-// Reset the bump pointer; call at the start of every public API function.
-void scratch_reset(ign_ctx* ctx);
-// Bump-allocate `bytes` (256B aligned) from the arena.  The arena never moves
-// while allocations of the current call are alive: scratch_reserve() must be
-// called first with the total the call needs.
-int scratch_reserve(ign_ctx* ctx, size_t total_bytes);
-void* scratch_take(ign_ctx* ctx, size_t bytes);
+// A scope of device scratch.  Opening a frame records the arena's bump offsets and closing
+// it restores them, on every return path, so what a frame takes lives exactly as long
+// as the frame.  Frames nest and close in reverse order: a nested call opens its own frame on
+// top of its caller's.  A take goes to the first device block with room at its end, else to a
+// new block of its own size (rounded up to 1 MiB), so nothing an open frame has taken is ever
+// moved or freed.  When the last frame closes on an arena of several blocks, the stream is synchronised
+// and the blocks are replaced by one block of the high-water size: calls of the same shapes then
+// bump-allocate from one block without cudaMalloc, cudaFree or a synchronisation.
+class ScratchFrame {
+ public:
+  explicit ScratchFrame(ign_ctx* ctx);
+  ~ScratchFrame();
+  ScratchFrame(const ScratchFrame&) = delete;
+  ScratchFrame& operator=(const ScratchFrame&) = delete;
+  // *p = 256-byte aligned room for `bytes` bytes, or for `count` elements of T
+  int take(void** p, size_t bytes);
+  template <typename T>
+  int take(T** p, size_t count) { return take((void**)p, count * sizeof(T)); }
+  // release everything taken in this frame (a data-dependent retry starts over)
+  void rewind();
+  // no frame opened after this one is still open
+  bool innermost() const;
+
+ private:
+  ign_ctx* ctx_;
+  std::vector<size_t> mark_;  // `used` of every block when the frame opened
+  size_t mark_lin_;
+  int depth_;
+};
 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 

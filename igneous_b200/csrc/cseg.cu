@@ -327,105 +327,77 @@ static size_t cseg_tmp_bytes(uint32_t nb) {
   return (sortb > scanb ? sortb : scanb) + 256;
 }
 
-// scratch bytes cseg_encode_channel takes for nb blocks: 4 u64 and 8 u32 arrays per block, a flag, cub temp
-static size_t cseg_channel_bytes(uint32_t nb) {
-  return 4 * align_up((size_t)nb * 8, 256) + 8 * align_up(((size_t)nb + 1) * 4, 256) + cseg_tmp_bytes(nb) + 4096;
-}
-
 // one channel; out_dev may be NULL (size query).  *n_words = words of the channel stream.
 template <typename T>
 static int cseg_encode_channel(ign_ctx* ctx, const T* in, const CsegDims& d, uint32_t* out_dev, uint64_t cap_words,
                                uint64_t* n_words) {
   constexpr int WORDS = sizeof(T) / 4;
   const uint32_t nb = d.gx * d.gy * d.gz;
-  const size_t keep = ctx->scratch_used;
-  const bool own = keep == 0;
   const size_t tmpb = cseg_tmp_bytes(nb);
-  if (own) IGN_TRY(scratch_reserve(ctx, cseg_channel_bytes(nb)));
-  auto fail = [&](int rc) {
-    ctx->scratch_used = keep;
-    return rc;
-  };
   unsigned long long hash_mask = ~0ull;
   if (const char* e = getenv("IGN_CSEG_HASH_BITS")) {
     const int k = atoi(e);
     hash_mask = k >= 64 ? ~0ull : k <= 0 ? 0ull : (1ull << k) - 1;
   }
-  unsigned long long* hash = (unsigned long long*)scratch_take(ctx, (size_t)nb * 8);
-  unsigned long long* shash = (unsigned long long*)scratch_take(ctx, (size_t)nb * 8);
-  unsigned long long* lo = (unsigned long long*)scratch_take(ctx, (size_t)nb * 8);
-  unsigned long long* hi = (unsigned long long*)scratch_take(ctx, (size_t)nb * 8);
-  uint32_t* n = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
-  uint32_t* blk = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
-  uint32_t* sblk = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
-  uint32_t* owner = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
-  uint32_t* size = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
-  uint32_t* scan = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
-  uint32_t* enc_off = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
-  uint32_t* tab_off = (uint32_t*)scratch_take(ctx, ((size_t)nb + 1) * 4);
-  uint32_t* collided = (uint32_t*)scratch_take(ctx, 4);
-  void* tmp = scratch_take(ctx, tmpb);
-  if (!hash || !shash || !lo || !hi || !n || !blk || !sblk || !owner || !size || !scan || !enc_off || !tab_off ||
-      !collided || !tmp) {
-    set_error("scratch arena too small (cseg encode)");
-    return fail(IGN_ERR_NOMEM);
-  }
-#define CS_CUDA(call)                                                                  \
+  ScratchFrame f(ctx);
+  unsigned long long *hash, *shash, *lo, *hi;
+  uint32_t *n, *blk, *sblk, *owner, *size, *scan, *enc_off, *tab_off, *collided;
+  void* tmp;
+  IGN_TRY(f.take(&hash, nb));
+  IGN_TRY(f.take(&shash, nb));
+  IGN_TRY(f.take(&lo, nb));
+  IGN_TRY(f.take(&hi, nb));
+  IGN_TRY(f.take(&n, (size_t)nb + 1));
+  IGN_TRY(f.take(&blk, (size_t)nb + 1));
+  IGN_TRY(f.take(&sblk, (size_t)nb + 1));
+  IGN_TRY(f.take(&owner, (size_t)nb + 1));
+  IGN_TRY(f.take(&size, (size_t)nb + 1));
+  IGN_TRY(f.take(&scan, (size_t)nb + 1));
+  IGN_TRY(f.take(&enc_off, (size_t)nb + 1));
+  IGN_TRY(f.take(&tab_off, (size_t)nb + 1));
+  IGN_TRY(f.take(&collided, 1));
+  IGN_TRY(f.take(&tmp, tmpb));
+#define CS_LAUNCH_PL(kernel, ...)                                                      \
   do {                                                                                 \
-    cudaError_t _e = (call);                                                           \
-    if (_e != cudaSuccess) {                                                           \
-      set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(_e)); \
-      return fail(IGN_ERR_CUDA);                                                       \
-    }                                                                                  \
-  } while (0)
-#define CS_LAUNCH(kernel, g, b, ...)                  \
-  do {                                                \
-    kernel<<<(g), (b), 0, ctx->stream>>>(__VA_ARGS__); \
-    ctx->launches++;                                  \
-    CS_CUDA(cudaGetLastError());                      \
-  } while (0)
-#define CS_LAUNCH_PL(kernel, ...)                                       \
-  do {                                                                  \
-    if (d.bvox <= 512) CS_LAUNCH((kernel<T, 16>), gw, 128, __VA_ARGS__); \
-    else CS_LAUNCH((kernel<T, 32>), gw, 128, __VA_ARGS__);               \
+    if (d.bvox <= 512) IGN_LAUNCH(ctx, (kernel<T, 16>), gw, 128, 0, __VA_ARGS__);     \
+    else IGN_LAUNCH(ctx, (kernel<T, 32>), gw, 128, 0, __VA_ARGS__);                    \
   } while (0)
   const unsigned gw = blocks_for((uint64_t)nb * 32, 128);
   if (d.bvox <= 512)
-    CS_LAUNCH((k_cseg_scan<T, false, 16>), gw, 128, in, d, (uint64_t)nb, n, hash, hash_mask, lo, hi,
-              (const uint32_t*)nullptr, (const uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr);
+    IGN_LAUNCH(ctx, (k_cseg_scan<T, false, 16>), gw, 128, 0, in, d, (uint64_t)nb, n, hash, hash_mask, lo, hi,
+               (const uint32_t*)nullptr, (const uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr);
   else
-    CS_LAUNCH((k_cseg_scan<T, false, 32>), gw, 128, in, d, (uint64_t)nb, n, hash, hash_mask, lo, hi,
-              (const uint32_t*)nullptr, (const uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr);
-  CS_LAUNCH(k_iota32, blocks_for(nb, 256), 256, blk, nb);
+    IGN_LAUNCH(ctx, (k_cseg_scan<T, false, 32>), gw, 128, 0, in, d, (uint64_t)nb, n, hash, hash_mask, lo, hi,
+               (const uint32_t*)nullptr, (const uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr);
+  IGN_LAUNCH(ctx, k_iota32, blocks_for(nb, 256), 256, 0, blk, nb);
   {
     size_t tb = tmpb;
-    CS_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, hash, shash, blk, sblk, (int)nb, 0, 64, ctx->stream));
+    IGN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, hash, shash, blk, sblk, (int)nb, 0, 64, ctx->stream));
     ctx->launches += 9;
   }
-  CS_LAUNCH(k_cseg_heads, blocks_for(nb, 256), 256, shash, nb, enc_off);  // enc_off / tab_off: free until the offsets pass
+  IGN_LAUNCH(ctx, k_cseg_heads, blocks_for(nb, 256), 256, 0, shash, nb, enc_off);  // enc_off / tab_off: free until the offsets pass
   {
     size_t tb = tmpb;
-    CS_CUDA(cub::DeviceScan::InclusiveScan(tmp, tb, enc_off, tab_off, cub::Max(), (int)nb, ctx->stream));
+    IGN_CUDA(cub::DeviceScan::InclusiveScan(tmp, tb, enc_off, tab_off, cub::Max(), (int)nb, ctx->stream));
     ctx->launches += 2;
   }
-  CS_LAUNCH(k_cseg_owner, blocks_for(nb, 256), 256, tab_off, sblk, nb, owner);
-  CS_CUDA(cudaMemsetAsync(collided, 0, 4, ctx->stream));
+  IGN_LAUNCH(ctx, k_cseg_owner, blocks_for(nb, 256), 256, 0, tab_off, sblk, nb, owner);
+  IGN_CUDA(cudaMemsetAsync(collided, 0, 4, ctx->stream));
   CS_LAUNCH_PL(k_cseg_verify, in, d, nb, n, (const unsigned long long*)lo, (const unsigned long long*)hi,
                (const uint32_t*)owner, collided);
   // the collision flag comes back with `total`; only after a collision is there a second round trip
   uint32_t total = 0, hcollided = 0;
   for (int pass = 0;; pass++) {
-    CS_LAUNCH((k_cseg_sizes<WORDS>), blocks_for(nb, 256), 256, n, owner, nb, d.bvox, size);
-    CS_CUDA(cudaMemsetAsync(size + nb, 0, 4, ctx->stream));
+    IGN_LAUNCH(ctx, (k_cseg_sizes<WORDS>), blocks_for(nb, 256), 256, 0, n, owner, nb, d.bvox, size);
+    IGN_CUDA(cudaMemsetAsync(size + nb, 0, 4, ctx->stream));
     {
       size_t tb = tmpb;
-      CS_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, size, scan, (int)nb + 1, ctx->stream));
+      IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, size, scan, (int)nb + 1, ctx->stream));
       ctx->launches += 2;
     }
-    int rc = small_d2h(ctx, &total, scan + nb, 4);
-    if (rc == IGN_OK && pass == 0) rc = small_d2h(ctx, &hcollided, collided, 4);
-    if (rc == IGN_OK) rc = small_sync(ctx);
-    if (rc != IGN_OK) return fail(rc);
+    IGN_TRY(small_d2h(ctx, &total, scan + nb, 4));
+    if (pass == 0) IGN_TRY(small_d2h(ctx, &hcollided, collided, 4));
+    IGN_TRY(small_sync(ctx));
     if (pass > 0 || hcollided == 0) break;
     CS_LAUNCH_PL(k_cseg_resolve, in, d, nb, n, (const unsigned long long*)lo, (const unsigned long long*)hi,
                  (const uint32_t*)sblk, (const uint32_t*)tab_off, owner);
@@ -434,21 +406,18 @@ static int cseg_encode_channel(ign_ctx* ctx, const T* in, const CsegDims& d, uin
   *n_words = words;
   if (words > 0xFFFFFFull + 1024) {
     set_error("cseg: the encoded chunk (%llu words) exceeds the format's 24-bit table offsets", (unsigned long long)words);
-    return fail(IGN_ERR_OVERFLOW);
+    return IGN_ERR_OVERFLOW;
   }
   if (out_dev != nullptr && words <= cap_words) {
-    CS_LAUNCH(k_cseg_offsets, blocks_for(nb, 256), 256, n, owner, scan, nb, d.bvox, enc_off, tab_off);
+    IGN_LAUNCH(ctx, k_cseg_offsets, blocks_for(nb, 256), 256, 0, n, owner, scan, nb, d.bvox, enc_off, tab_off);
     if (d.bvox <= 512)
-      CS_LAUNCH((k_cseg_scan<T, true, 16>), gw, 128, in, d, (uint64_t)nb, (uint32_t*)nullptr, (unsigned long long*)nullptr,
-                hash_mask, (unsigned long long*)nullptr, (unsigned long long*)nullptr, enc_off, tab_off, owner, out_dev);
+      IGN_LAUNCH(ctx, (k_cseg_scan<T, true, 16>), gw, 128, 0, in, d, (uint64_t)nb, (uint32_t*)nullptr, (unsigned long long*)nullptr,
+                 hash_mask, (unsigned long long*)nullptr, (unsigned long long*)nullptr, enc_off, tab_off, owner, out_dev);
     else
-      CS_LAUNCH((k_cseg_scan<T, true, 32>), gw, 128, in, d, (uint64_t)nb, (uint32_t*)nullptr, (unsigned long long*)nullptr,
-                hash_mask, (unsigned long long*)nullptr, (unsigned long long*)nullptr, enc_off, tab_off, owner, out_dev);
+      IGN_LAUNCH(ctx, (k_cseg_scan<T, true, 32>), gw, 128, 0, in, d, (uint64_t)nb, (uint32_t*)nullptr, (unsigned long long*)nullptr,
+                 hash_mask, (unsigned long long*)nullptr, (unsigned long long*)nullptr, enc_off, tab_off, owner, out_dev);
   }
-  ctx->scratch_used = keep;
   return IGN_OK;
-#undef CS_CUDA
-#undef CS_LAUNCH
 #undef CS_LAUNCH_PL
 }
 
@@ -495,18 +464,13 @@ int ign_cseg_decode_dev(ign_ctx* ctx, const uint32_t* in, uint64_t n_words, int 
   std::vector<uint32_t> chan_off(sc, 0);
   IGN_CUDA(cudaMemcpyAsync(chan_off.data(), in, sc * 4, cudaMemcpyDeviceToHost, ctx->stream));
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  const size_t keep = ctx->scratch_used;
-  if (keep == 0) IGN_TRY(scratch_reserve(ctx, 4096));
-  uint32_t* err = (uint32_t*)scratch_take(ctx, 256);
-  IGN_REQUIRE(err != nullptr, IGN_ERR_NOMEM, "scratch arena too small (cseg decode)");
+  ScratchFrame f(ctx);
+  uint32_t* err;
+  IGN_TRY(f.take(&err, 64));
   IGN_CUDA(cudaMemsetAsync(err, 0, 4, ctx->stream));
   for (uint64_t c = 0; c < sc; c++) {
     const uint64_t base = chan_off[c];
-    if (base > n_words) {
-      ctx->scratch_used = keep;
-      set_error("cseg: channel offset outside the stream");
-      return IGN_ERR_INVALID;
-    }
+    IGN_REQUIRE(base <= n_words, IGN_ERR_INVALID, "cseg: channel offset outside the stream");
     if (dtype == IGN_U32)
       IGN_LAUNCH(ctx, (k_cseg_decode<uint32_t>), blocks_for(n, 256), 256, 0, in + base, n_words - base, d, (uint32_t*)out + c * n, err);
     else
@@ -515,7 +479,6 @@ int ign_cseg_decode_dev(ign_ctx* ctx, const uint32_t* in, uint64_t n_words, int 
   uint32_t herr = 0;
   IGN_CUDA(cudaMemcpyAsync(&herr, err, 4, cudaMemcpyDeviceToHost, ctx->stream));
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  ctx->scratch_used = keep;
   IGN_REQUIRE(herr == 0, IGN_ERR_INVALID, "cseg: malformed stream");
   return IGN_OK;
 }
@@ -529,26 +492,20 @@ int ign_cseg_encode(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, ui
   const int es = dtype_size(dtype);
   IGN_REQUIRE(dtype == IGN_U32 || dtype == IGN_U64, IGN_ERR_UNSUPPORTED, "compressed_segmentation holds uint32 / uint64 labels");
   const uint64_t n = sx * sy * sz * sc;
-  scratch_reset(ctx);
   CsegDims d;
   IGN_TRY(cseg_dims(sx, sy, sz, bx, by, bz, &d));
-  IGN_TRY(scratch_reserve(ctx, align_up(n * es, 256) + align_up((out ? cap_words : 0) * 4, 256) +
-                                   cseg_channel_bytes(d.gx * d.gy * d.gz) + (1 << 20)));
-  void* d_in = scratch_take(ctx, n * es);
-  uint32_t* d_out = out ? (uint32_t*)scratch_take(ctx, cap_words * 4) : nullptr;
-  IGN_REQUIRE(d_in && (!out || d_out), IGN_ERR_NOMEM, "scratch arena too small (cseg)");
+  ScratchFrame f(ctx);
+  void* d_in;
+  uint32_t* d_out = nullptr;
+  IGN_TRY(f.take(&d_in, n * es));
+  if (out) IGN_TRY(f.take(&d_out, cap_words));
   IGN_CUDA(cudaMemcpyAsync(d_in, labels, n * es, cudaMemcpyHostToDevice, ctx->stream));
-  int rc = ign_cseg_encode_dev(ctx, d_in, dtype, sx, sy, sz, sc, bx, by, bz, d_out, cap_words, n_words);
-  if (rc == IGN_OK && out && *n_words <= cap_words) {
-    cudaError_t e = cudaMemcpyAsync(out, d_out, *n_words * 4, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) {
-      set_error("cseg D2H: %s", cudaGetErrorString(e));
-      rc = IGN_ERR_CUDA;
-    }
+  IGN_TRY(ign_cseg_encode_dev(ctx, d_in, dtype, sx, sy, sz, sc, bx, by, bz, d_out, cap_words, n_words));
+  if (out && *n_words <= cap_words) {
+    IGN_CUDA(cudaMemcpyAsync(out, d_out, *n_words * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   }
-  scratch_reset(ctx);
-  return rc;
+  return IGN_OK;
 }
 
 int ign_cseg_decode(ign_ctx* ctx, const uint32_t* in, uint64_t n_words, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
@@ -558,23 +515,16 @@ int ign_cseg_decode(ign_ctx* ctx, const uint32_t* in, uint64_t n_words, int dtyp
   const int es = dtype_size(dtype);
   IGN_REQUIRE(dtype == IGN_U32 || dtype == IGN_U64, IGN_ERR_UNSUPPORTED, "compressed_segmentation holds uint32 / uint64 labels");
   const uint64_t n = sx * sy * sz * sc;
-  scratch_reset(ctx);
-  IGN_TRY(scratch_reserve(ctx, align_up(n * es, 256) + align_up(n_words * 4, 256) + (1 << 20)));
-  uint32_t* d_in = (uint32_t*)scratch_take(ctx, n_words * 4);
-  void* d_out = scratch_take(ctx, n * es);
-  IGN_REQUIRE(d_in && d_out, IGN_ERR_NOMEM, "scratch arena too small (cseg)");
+  ScratchFrame f(ctx);
+  uint32_t* d_in;
+  void* d_out;
+  IGN_TRY(f.take(&d_in, n_words));
+  IGN_TRY(f.take(&d_out, n * es));
   IGN_CUDA(cudaMemcpyAsync(d_in, in, n_words * 4, cudaMemcpyHostToDevice, ctx->stream));
-  int rc = ign_cseg_decode_dev(ctx, d_in, n_words, dtype, sx, sy, sz, sc, bx, by, bz, d_out);
-  if (rc == IGN_OK) {
-    cudaError_t e = cudaMemcpyAsync(out, d_out, n * es, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) {
-      set_error("cseg D2H: %s", cudaGetErrorString(e));
-      rc = IGN_ERR_CUDA;
-    }
-  }
-  scratch_reset(ctx);
-  return rc;
+  IGN_TRY(ign_cseg_decode_dev(ctx, d_in, n_words, dtype, sx, sy, sz, sc, bx, by, bz, d_out));
+  IGN_CUDA(cudaMemcpyAsync(out, d_out, n * es, cudaMemcpyDeviceToHost, ctx->stream));
+  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
+  return IGN_OK;
 }
 
 }  // extern "C"

@@ -23,30 +23,58 @@ int activate(ign_ctx* ctx) {
   return IGN_OK;
 }
 
-void scratch_reset(ign_ctx* ctx) { ctx->scratch_used = 0; }
-
-int scratch_reserve(ign_ctx* ctx, size_t total) {
-  total = align_up(total + 4096, 1 << 20);
-  if (total <= ctx->scratch_bytes) return IGN_OK;
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  if (ctx->scratch) IGN_CUDA(cudaFree(ctx->scratch));
-  ctx->scratch = nullptr;
-  ctx->scratch_bytes = 0;
-  cudaError_t e = cudaMalloc((void**)&ctx->scratch, total);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    set_error("scratch arena: cudaMalloc(%zu) failed: %s", total, cudaGetErrorString(e));
-    return IGN_ERR_NOMEM;
-  }
-  ctx->scratch_bytes = total;
-  return IGN_OK;
+ScratchFrame::ScratchFrame(ign_ctx* ctx) : ctx_(ctx), mark_lin_(ctx->scratch_lin), depth_(++ctx->scratch_frames) {
+  for (const auto& b : ctx->scratch) mark_.push_back(b.used);
 }
 
-void* scratch_take(ign_ctx* ctx, size_t bytes) {
-  size_t off = align_up(ctx->scratch_used, 256);
-  if (off + bytes > ctx->scratch_bytes) return nullptr;
-  ctx->scratch_used = off + bytes;
-  return ctx->scratch + off;
+ScratchFrame::~ScratchFrame() {
+  rewind();
+  if (--ctx_->scratch_frames > 0 || ctx_->scratch.size() < 2) return;
+  // the arena is empty: coalesce its blocks into one (queued kernels may still read them)
+  if (cudaStreamSynchronize(ctx_->stream) != cudaSuccess) {
+    cudaGetLastError();
+    return;
+  }
+  for (const auto& b : ctx_->scratch) cudaFree(b.base);
+  ctx_->scratch.clear();
+  const size_t bytes = align_up(ctx_->scratch_high, 1 << 20);
+  char* base = nullptr;
+  if (cudaMalloc((void**)&base, bytes) == cudaSuccess) ctx_->scratch.push_back({base, bytes, 0});
+  else cudaGetLastError();  // the next take allocates what it needs
+}
+
+void ScratchFrame::rewind() {
+  for (size_t b = 0; b < ctx_->scratch.size(); b++) ctx_->scratch[b].used = b < mark_.size() ? mark_[b] : 0;
+  ctx_->scratch_lin = mark_lin_;
+}
+
+bool ScratchFrame::innermost() const { return ctx_->scratch_frames == depth_; }
+
+int ScratchFrame::take(void** p, size_t bytes) {
+  *p = nullptr;
+  std::vector<ign_ctx::ScratchBlock>& blocks = ctx_->scratch;
+  size_t b = 0, off = 0;
+  for (; b < blocks.size(); b++) {  // first fit: a block's free end is never below a live take
+    off = align_up(blocks[b].used, 256);
+    if (off + bytes <= blocks[b].bytes) break;
+  }
+  if (b == blocks.size()) {
+    const size_t want = align_up(bytes ? bytes : 1, 1 << 20);
+    char* base = nullptr;
+    cudaError_t e = cudaMalloc((void**)&base, want);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      set_error("scratch arena: cudaMalloc(%zu) failed: %s", want, cudaGetErrorString(e));
+      return IGN_ERR_NOMEM;
+    }
+    blocks.push_back({base, want, 0});
+    off = 0;
+  }
+  blocks[b].used = off + bytes;
+  ctx_->scratch_lin = align_up(ctx_->scratch_lin, 256) + bytes;
+  if (ctx_->scratch_lin > ctx_->scratch_high) ctx_->scratch_high = ctx_->scratch_lin;
+  *p = blocks[b].base + off;
+  return IGN_OK;
 }
 
 template <typename T>
@@ -211,8 +239,6 @@ int ign_init(int device, ign_ctx** out) {
   ign_ctx* ctx = new ign_ctx();
   ctx->device = device;
   ctx->sm_count = prop.multiProcessorCount;
-  ctx->scratch = nullptr;
-  ctx->scratch_bytes = ctx->scratch_used = 0;
   ctx->launches = 0;
   ctx->prof_on = 0;
   ctx->prof = nullptr;
@@ -247,7 +273,7 @@ int ign_destroy(ign_ctx* ctx) {
   if (!ctx) return IGN_OK;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
-  if (ctx->scratch) cudaFree(ctx->scratch);
+  for (const auto& b : ctx->scratch) cudaFree(b.base);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->win) cudaFreeHost(ctx->win);
   if (ctx->mesh_pool) cudaFree(ctx->mesh_pool);

@@ -23,8 +23,8 @@
 //              region the non-zero separator nearest the outside (its filler).
 //     apply    k_fill_apply: filled = table[component]; holes = input where filled differs.
 //   The host solve makes ign_fill_holes_dev synchronous: each pass waits on the stream four times
-//   (2^64-1 check + component count, contact count, run count, table upload), and its buffers
-//   come from the stream-ordered allocator (cudaMallocAsync), so repeated calls reuse the pool.
+//   (2^64-1 check + component count, contact count, run count, table upload); its buffers are
+//   taken from the context's scratch arena.
 //   A face plane is gathered into an (a, b, 1) volume (6-connectivity there is 4-connectivity),
 //   solved with only its in-plane edges as the outside, and scattered back.
 #include <cub/device/device_radix_sort.cuh>
@@ -38,27 +38,6 @@
 #include "common.cuh"
 
 namespace ign {
-
-// stream-ordered device allocation owned by one call
-struct FillBuf {
-  ign_ctx* ctx = nullptr;
-  void* p = nullptr;
-  ~FillBuf() {
-    if (p) cudaFreeAsync(p, ctx->stream);
-  }
-  int alloc(ign_ctx* c, size_t bytes) {
-    ctx = c;
-    cudaError_t e = cudaMallocAsync(&p, bytes ? bytes : 16, c->stream);
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      p = nullptr;
-      set_error("fill: cudaMallocAsync(%zu) failed: %s", bytes, cudaGetErrorString(e));
-      return IGN_ERR_NOMEM;
-    }
-    return IGN_OK;
-  }
-  template <typename U> U* as() const { return (U*)p; }
-};
 
 // ------------------------------------------------------------------ dilation
 constexpr int DL_BX = 32, DL_BY = 4, DL_BZ = 4;
@@ -373,40 +352,44 @@ static int fill_pass(ign_ctx* ctx, const T* cur, uint64_t sx, uint64_t sy, uint6
                      const T* x0, T* filled, T* holes) {
   using K = typename KeyOf<T>::type;
   const uint64_t n = sx * sy * sz;
-  FillBuf key, comp, flag;
-  IGN_TRY(key.alloc(ctx, n * sizeof(K)));
-  IGN_TRY(comp.alloc(ctx, n * 4));
-  IGN_TRY(flag.alloc(ctx, 16));
-  IGN_CUDA(cudaMemsetAsync(flag.p, 0, 16, ctx->stream));
-  IGN_LAUNCH(ctx, (k_fill_key<T, K>), blocks_for(n, 256), 256, 0, cur, n, key.as<K>(), flag.as<uint32_t>());
+  ScratchFrame f(ctx);
+  K* key;
+  uint32_t *comp, *flag;
+  IGN_TRY(f.take(&key, n));
+  IGN_TRY(f.take(&comp, n));
+  IGN_TRY(f.take(&flag, 4));
+  IGN_CUDA(cudaMemsetAsync(flag, 0, 16, ctx->stream));
+  IGN_LAUNCH(ctx, (k_fill_key<T, K>), blocks_for(n, 256), 256, 0, cur, n, key, flag);
   uint64_t N = 0;
-  scratch_reset(ctx);
-  IGN_TRY(ign_ccl6_dev(ctx, key.p, sizeof(K) == 4 ? IGN_U32 : IGN_U64, sx, sy, sz, comp.p, IGN_U32, &N));
+  IGN_TRY(ign_ccl6_dev(ctx, key, sizeof(K) == 4 ? IGN_U32 : IGN_U64, sx, sy, sz, comp, IGN_U32, &N));
   unsigned long long* hcnt = (unsigned long long*)ctx->pinned;
-  IGN_CUDA(cudaMemcpyAsync(hcnt, flag.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  IGN_CUDA(cudaMemcpyAsync(hcnt, flag, 4, cudaMemcpyDeviceToHost, ctx->stream));
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   IGN_REQUIRE(((uint32_t*)hcnt)[0] == 0, IGN_ERR_UNSUPPORTED, "fill_holes: label 2^64-1 is not supported");
-  FillBuf clabel, counter;
-  IGN_TRY(clabel.alloc(ctx, (N + 1) * 8));
-  IGN_TRY(counter.alloc(ctx, 8));
-  IGN_CUDA(cudaMemsetAsync(clabel.p, 0, 8, ctx->stream));
-  IGN_LAUNCH(ctx, k_fill_comp_label<T>, blocks_for(n, 256), 256, 0, comp.as<uint32_t>(), cur, n, sx, clabel.as<uint64_t>());
-  IGN_CUDA(cudaMemsetAsync(counter.p, 0, 8, ctx->stream));
-  IGN_LAUNCH(ctx, k_fill_contacts<false>, blocks_for(n, 256), 256, 0, comp.as<uint32_t>(), sx, sy, sz, axes,
-             counter.as<unsigned long long>(), (uint64_t*)nullptr);
-  IGN_CUDA(cudaMemcpyAsync(hcnt, counter.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  uint64_t* clabel;
+  unsigned long long* counter;
+  IGN_TRY(f.take(&clabel, N + 1));
+  IGN_TRY(f.take(&counter, 1));
+  IGN_CUDA(cudaMemsetAsync(clabel, 0, 8, ctx->stream));
+  IGN_LAUNCH(ctx, k_fill_comp_label<T>, blocks_for(n, 256), 256, 0, comp, cur, n, sx, clabel);
+  IGN_CUDA(cudaMemsetAsync(counter, 0, 8, ctx->stream));
+  IGN_LAUNCH(ctx, k_fill_contacts<false>, blocks_for(n, 256), 256, 0, comp, sx, sy, sz, axes, counter,
+             (uint64_t*)nullptr);
+  IGN_CUDA(cudaMemcpyAsync(hcnt, counter, 8, cudaMemcpyDeviceToHost, ctx->stream));
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   const uint64_t M = hcnt[0];
   IGN_REQUIRE(M > 0 && M < 0x7FFFFFFFull, IGN_ERR_OVERFLOW, "fill_holes: %llu contacts", (unsigned long long)M);
-  FillBuf keys, sorted, uniq, counts, nruns, tmp;
-  IGN_TRY(keys.alloc(ctx, M * 8));
-  IGN_TRY(sorted.alloc(ctx, M * 8));
-  IGN_TRY(uniq.alloc(ctx, M * 8));
-  IGN_TRY(counts.alloc(ctx, M * 4));
-  IGN_TRY(nruns.alloc(ctx, 8));
-  IGN_CUDA(cudaMemsetAsync(counter.p, 0, 8, ctx->stream));
-  IGN_LAUNCH(ctx, k_fill_contacts<true>, blocks_for(n, 256), 256, 0, comp.as<uint32_t>(), sx, sy, sz, axes,
-             counter.as<unsigned long long>(), keys.as<uint64_t>());
+  uint64_t *keys, *sorted, *uniq;
+  uint32_t* counts;
+  int* nruns;
+  void* tmp;
+  IGN_TRY(f.take(&keys, M));
+  IGN_TRY(f.take(&sorted, M));
+  IGN_TRY(f.take(&uniq, M));
+  IGN_TRY(f.take(&counts, M));
+  IGN_TRY(f.take(&nruns, 2));
+  IGN_CUDA(cudaMemsetAsync(counter, 0, 8, ctx->stream));
+  IGN_LAUNCH(ctx, k_fill_contacts<true>, blocks_for(n, 256), 256, 0, comp, sx, sy, sz, axes, counter, keys);
   int hi_bits = 1;
   while (hi_bits < 32 && (N >> hi_bits)) hi_bits++;
   const int end_bit = 32 + hi_bits;
@@ -414,30 +397,28 @@ static int fill_pass(ign_ctx* ctx, const T* cur, uint64_t sx, uint64_t sy, uint6
   cub::DeviceRadixSort::SortKeys(nullptr, sort_b, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)M, 0, end_bit);
   cub::DeviceRunLengthEncode::Encode(nullptr, rle_b, (const uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr,
                                      (int*)nullptr, (int)M);
-  IGN_TRY(tmp.alloc(ctx, std::max(sort_b, rle_b)));
-  IGN_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, sort_b, keys.as<uint64_t>(), sorted.as<uint64_t>(), (int)M, 0, end_bit,
-                                          ctx->stream));
-  IGN_CUDA(cub::DeviceRunLengthEncode::Encode(tmp.p, rle_b, sorted.as<uint64_t>(), uniq.as<uint64_t>(),
-                                              counts.as<uint32_t>(), nruns.as<int>(), (int)M, ctx->stream));
+  IGN_TRY(f.take(&tmp, std::max(sort_b, rle_b)));
+  IGN_CUDA(cub::DeviceRadixSort::SortKeys(tmp, sort_b, keys, sorted, (int)M, 0, end_bit, ctx->stream));
+  IGN_CUDA(cub::DeviceRunLengthEncode::Encode(tmp, rle_b, sorted, uniq, counts, nruns, (int)M, ctx->stream));
   ctx->launches += 4;
   int* hruns = (int*)ctx->pinned;
-  IGN_CUDA(cudaMemcpyAsync(hruns, nruns.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  IGN_CUDA(cudaMemcpyAsync(hruns, nruns, 4, cudaMemcpyDeviceToHost, ctx->stream));
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   const uint64_t nk = (uint64_t)hruns[0];
   std::vector<uint64_t> hkeys(nk), hlab(N + 1);
   std::vector<uint32_t> hcnts(nk);
-  IGN_CUDA(cudaMemcpyAsync(hkeys.data(), uniq.p, nk * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaMemcpyAsync(hcnts.data(), counts.p, nk * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaMemcpyAsync(hlab.data(), clabel.p, (N + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  IGN_CUDA(cudaMemcpyAsync(hkeys.data(), uniq, nk * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  IGN_CUDA(cudaMemcpyAsync(hcnts.data(), counts, nk * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  IGN_CUDA(cudaMemcpyAsync(hlab.data(), clabel, (N + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   std::vector<uint64_t> table;
   fill_solve((uint32_t)N, hkeys.data(), hcnts.data(), nk, p, hlab.data(), table);
   std::vector<T> lut(N + 1);
   for (uint64_t c = 0; c <= N; c++) lut[c] = (T)table[c];
-  FillBuf dlut;
-  IGN_TRY(dlut.alloc(ctx, (N + 1) * sizeof(T)));
-  IGN_CUDA(cudaMemcpyAsync(dlut.p, lut.data(), (N + 1) * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-  IGN_LAUNCH(ctx, k_fill_apply<T>, blocks_for(n, 256), 256, 0, comp.as<uint32_t>(), dlut.as<T>(), n, x0, filled, holes);
+  T* dlut;
+  IGN_TRY(f.take(&dlut, N + 1));
+  IGN_CUDA(cudaMemcpyAsync(dlut, lut.data(), (N + 1) * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+  IGN_LAUNCH(ctx, k_fill_apply<T>, blocks_for(n, 256), 256, 0, comp, dlut, n, x0, filled, holes);
   // lut is a host vector: the copy must complete before it goes out of scope
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   return IGN_OK;
@@ -450,16 +431,17 @@ static int fill_typed(ign_ctx* ctx, const T* in, uint64_t sx, uint64_t sy, uint6
   if (fix_borders) {
     IGN_CUDA(cudaMemcpyAsync(filled, in, n * sizeof(T), cudaMemcpyDeviceToDevice, ctx->stream));
     const uint64_t ext[3] = {sx, sy, sz};
-    FillBuf plane;
-    IGN_TRY(plane.alloc(ctx, std::max({sx * sy, sx * sz, sy * sz}) * sizeof(T)));
+    ScratchFrame f(ctx);
+    T* plane;
+    IGN_TRY(f.take(&plane, std::max({sx * sy, sx * sz, sy * sz})));
     for (int axis = 0; axis < 3; axis++) {
       const uint64_t na = axis == 0 ? sy : sx, nb = axis == 2 ? sy : sz;
       for (int side = 0; side < 2; side++) {
         const uint64_t idx = side ? ext[axis] - 1 : 0;
         if (side && idx == 0) continue;  // extent 1: the plane was done already
-        IGN_LAUNCH(ctx, (k_fill_plane<T, true>), blocks_for(na * nb, 256), 256, 0, filled, sx, sy, sz, axis, idx, plane.as<T>());
-        IGN_TRY(fill_pass<T>(ctx, plane.as<T>(), na, nb, 1, 3u, p, nullptr, plane.as<T>(), nullptr));
-        IGN_LAUNCH(ctx, (k_fill_plane<T, false>), blocks_for(na * nb, 256), 256, 0, filled, sx, sy, sz, axis, idx, plane.as<T>());
+        IGN_LAUNCH(ctx, (k_fill_plane<T, true>), blocks_for(na * nb, 256), 256, 0, filled, sx, sy, sz, axis, idx, plane);
+        IGN_TRY(fill_pass<T>(ctx, plane, na, nb, 1, 3u, p, nullptr, plane, nullptr));
+        IGN_LAUNCH(ctx, (k_fill_plane<T, false>), blocks_for(na * nb, 256), 256, 0, filled, sx, sy, sz, axis, idx, plane);
       }
     }
     return fill_pass<T>(ctx, filled, sx, sy, sz, 7u, p, in, filled, holes);
@@ -518,12 +500,13 @@ int ign_dilate_multilabel(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, 
   const int es = dtype_size(dtype);
   IGN_REQUIRE(es > 0 && dtype != IGN_F32, IGN_ERR_UNSUPPORTED, "dilate: unsupported dtype %d", dtype);
   const uint64_t bytes = sx * sy * sz * es;
-  FillBuf din, dout;
-  IGN_TRY(din.alloc(ctx, bytes));
-  IGN_TRY(dout.alloc(ctx, bytes));
-  IGN_CUDA(cudaMemcpyAsync(din.p, in, bytes, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_dilate_multilabel_dev(ctx, din.p, dtype, sx, sy, sz, dout.p));
-  IGN_CUDA(cudaMemcpyAsync(out, dout.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  ScratchFrame f(ctx);
+  void *din, *dout;
+  IGN_TRY(f.take(&din, bytes));
+  IGN_TRY(f.take(&dout, bytes));
+  IGN_CUDA(cudaMemcpyAsync(din, in, bytes, cudaMemcpyHostToDevice, ctx->stream));
+  IGN_TRY(ign_dilate_multilabel_dev(ctx, din, dtype, sx, sy, sz, dout));
+  IGN_CUDA(cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, ctx->stream));
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   return IGN_OK;
 }
@@ -534,14 +517,15 @@ int ign_fill_holes(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_
   IGN_REQUIRE(in && filled && holes, IGN_ERR_INVALID, "null buffer");
   IGN_TRY(fill_check(sx, sy, sz, dtype, merge_threshold_pct));
   const uint64_t bytes = sx * sy * sz * dtype_size(dtype);
-  FillBuf din, dfill, dholes;
-  IGN_TRY(din.alloc(ctx, bytes));
-  IGN_TRY(dfill.alloc(ctx, bytes));
-  IGN_TRY(dholes.alloc(ctx, bytes));
-  IGN_CUDA(cudaMemcpyAsync(din.p, in, bytes, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_fill_holes_dev(ctx, din.p, dtype, sx, sy, sz, fix_borders, merge_threshold_pct, dfill.p, dholes.p));
-  IGN_CUDA(cudaMemcpyAsync(filled, dfill.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaMemcpyAsync(holes, dholes.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  ScratchFrame f(ctx);
+  void *din, *dfill, *dholes;
+  IGN_TRY(f.take(&din, bytes));
+  IGN_TRY(f.take(&dfill, bytes));
+  IGN_TRY(f.take(&dholes, bytes));
+  IGN_CUDA(cudaMemcpyAsync(din, in, bytes, cudaMemcpyHostToDevice, ctx->stream));
+  IGN_TRY(ign_fill_holes_dev(ctx, din, dtype, sx, sy, sz, fix_borders, merge_threshold_pct, dfill, dholes));
+  IGN_CUDA(cudaMemcpyAsync(filled, dfill, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  IGN_CUDA(cudaMemcpyAsync(holes, dholes, bytes, cudaMemcpyDeviceToHost, ctx->stream));
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   return IGN_OK;
 }

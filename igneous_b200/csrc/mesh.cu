@@ -291,8 +291,6 @@ int ign_mesh_begin_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx,
               (unsigned long long)sx, (unsigned long long)sy, (unsigned long long)sz);
   IGN_TRY(load_tables(ctx));
   const uint64_t n = sx * sy * sz;
-  const bool own = (ctx->scratch_used == 0);
-  const size_t keep = ctx->scratch_used;
 
   ign_mesher* m = new ign_mesher();
   m->ctx = ctx;
@@ -305,93 +303,58 @@ int ign_mesh_begin_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx,
   m->simp_factor = 0;
   m->simp_max_error = 0;
   m->simp_rounds = 0;
-  int rc = IGN_OK;
-  auto fail = [&](int code) {
-    ctx->scratch_used = keep;
-    ign_mesh_free(m);
-    return code;
-  };
+  // a failed build frees the half-built mesher
+  struct Guard {
+    ign_mesher* m;
+    ~Guard() { ign_mesh_free(m); }
+  } guard{m};
+  ScratchFrame f(ctx);
 
   // ---- dense labels
-  uint64_t cap2 = 1024;
-  while (cap2 < 2 * n + 16 && cap2 < (1ull << 31)) cap2 <<= 1;
-  const size_t renumber_need = cap2 * 40 + (1 << 20);
-  if (own) {
-    rc = scratch_reserve(ctx, align_up(n * 4, 256) + align_up(n * 8, 256) + renumber_need + (64 << 20));
-    if (rc != IGN_OK) return fail(rc);
-  }
-  uint32_t* d_lab = (uint32_t*)scratch_take(ctx, n * 4);
-  uint64_t* d_uniq = (uint64_t*)scratch_take(ctx, n * 8);
-  if (!d_lab || !d_uniq) {
-    set_error("scratch arena too small (mesher labels)");
-    return fail(IGN_ERR_NOMEM);
-  }
+  uint32_t* d_lab;
+  IGN_TRY(f.take(&d_lab, n));
   uint64_t K = 0;
-  rc = ign_renumber_dev(ctx, labels, dtype, n, d_lab, d_uniq, n, &K);
-  if (rc != IGN_OK) return fail(rc);
-  m->K = K;
-  m->ids.resize(K);
-  if (K) {
-    rc = small_d2h(ctx, m->ids.data(), d_uniq, K * 8);
-    if (rc == IGN_OK) rc = small_sync(ctx);
-    if (rc != IGN_OK) return fail(rc);
+  {
+    ScratchFrame fu(ctx);  // only d_lab outlives the renumber
+    uint64_t* d_uniq;
+    IGN_TRY(fu.take(&d_uniq, n));
+    IGN_TRY(ign_renumber_dev(ctx, labels, dtype, n, d_lab, d_uniq, n, &K));
+    m->K = K;
+    m->ids.resize(K);
+    if (K) {
+      IGN_TRY(small_d2h(ctx, m->ids.data(), d_uniq, K * 8));
+      IGN_TRY(small_sync(ctx));
+    }
   }
   m->tri_off.assign(K + 2, 0);
   m->vert_off.assign(K + 2, 0);
   if (K == 0 || sx < 2 || sy < 2 || sz < 2) {
-    ctx->scratch_used = keep;
+    guard.m = nullptr;
     *out = m;
     return IGN_OK;
   }
-  if (K >= (1ull << 31)) {
-    set_error("mesher: too many labels");
-    return fail(IGN_ERR_OVERFLOW);
-  }
-  // the arena below d_uniq is reusable now: only d_lab must survive
-  ctx->scratch_used = keep;
-  d_lab = (uint32_t*)scratch_take(ctx, n * 4);
+  IGN_REQUIRE(K < (1ull << 31), IGN_ERR_OVERFLOW, "mesher: too many labels");
 
   // ---- count
-  unsigned long long* d_total = (unsigned long long*)scratch_take(ctx, 256);
+  unsigned long long* d_total;
+  IGN_TRY(f.take(&d_total, 32));
   const uint64_t ncubes = (sx - 1) * (sy - 1) * (sz - 1);
   const unsigned grid = blocks_for(ncubes, 256);
   unsigned long long T = 0;
-#define MESH_CUDA(call)                                                            \
-  do {                                                                             \
-    cudaError_t _e = (call);                                                       \
-    if (_e != cudaSuccess) {                                                       \
-      set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(_e)); \
-      return fail(IGN_ERR_CUDA);                                                   \
-    }                                                                              \
-  } while (0)
-#define MESH_TRY(call)                    \
-  do {                                    \
-    const int _s = (call);                \
-    if (_s != IGN_OK) return fail(_s);    \
-  } while (0)
-#define MESH_LAUNCH(kernel, g, b, ...)                    \
-  do {                                                    \
-    kernel<<<(g), (b), 0, ctx->stream>>>(__VA_ARGS__);    \
-    ctx->launches++;                                      \
-    MESH_CUDA(cudaGetLastError());                        \
-  } while (0)
-  MESH_CUDA(cudaMemsetAsync(d_total, 0, 8, ctx->stream));
-  MESH_LAUNCH((k_mc<false>), grid, 256, d_lab, (uint32_t)sx, (uint32_t)sy, (uint32_t)sz, d_total,
-              (uint64_t*)nullptr, (uint8_t*)nullptr, 0ull);
-  MESH_TRY(small_d2h(ctx, &T, d_total, 8));
-  MESH_TRY(small_sync(ctx));
+  IGN_CUDA(cudaMemsetAsync(d_total, 0, 8, ctx->stream));
+  IGN_LAUNCH(ctx, (k_mc<false>), grid, 256, 0, d_lab, (uint32_t)sx, (uint32_t)sy, (uint32_t)sz, d_total,
+             (uint64_t*)nullptr, (uint8_t*)nullptr, 0ull);
+  IGN_TRY(small_d2h(ctx, &T, d_total, 8));
+  IGN_TRY(small_sync(ctx));
   m->T = T;
   if (T == 0) {
-    ctx->scratch_used = keep;
+    guard.m = nullptr;
     *out = m;
     return IGN_OK;
   }
-  if (3 * T >= 0xFFFFFFFFull) {
-    set_error("mesher: %llu triangles exceed 32-bit corner indices", T);
-    return fail(IGN_ERR_OVERFLOW);
-  }
+  IGN_REQUIRE(3 * T < 0xFFFFFFFFull, IGN_ERR_OVERFLOW, "mesher: %llu triangles exceed 32-bit corner indices", T);
 
-  // ---- arena plan for emit + sort + weld
+  // ---- emit + sort + weld buffers
   size_t sort1 = 0, sort2 = 0, scanb = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, sort1, (const uint64_t*)nullptr, (uint64_t*)nullptr,
                                   (const uint8_t*)nullptr, (uint8_t*)nullptr, (int)T);
@@ -400,79 +363,61 @@ int ign_mesh_begin_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx,
   cub::DeviceScan::ExclusiveSum(nullptr, scanb, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)(3 * T));
   size_t tmp_bytes = sort1 > sort2 ? sort1 : sort2;
   if (scanb > tmp_bytes) tmp_bytes = scanb;
-  const size_t need = align_up(n * 4, 256) + 2 * align_up(T * 8, 256) + 2 * align_up(T, 256) +
-                      2 * align_up(3 * T * 8, 256) + 4 * align_up(3 * T * 4, 256) +
-                      2 * align_up((K + 2) * 4, 256) + tmp_bytes + (1 << 20);
-  if (own && need > ctx->scratch_bytes) {
-    // growing the arena invalidates d_lab: re-run the (cheap) renumber into the new arena
-    ctx->scratch_used = keep;
-    rc = scratch_reserve(ctx, need + renumber_need + align_up(n * 8, 256));
-    if (rc != IGN_OK) return fail(rc);
-    d_lab = (uint32_t*)scratch_take(ctx, n * 4);
-    uint64_t* d_uniq2 = (uint64_t*)scratch_take(ctx, n * 8);
-    uint64_t K2 = 0;
-    rc = ign_renumber_dev(ctx, labels, dtype, n, d_lab, d_uniq2, n, &K2);
-    if (rc != IGN_OK) return fail(rc);
-    ctx->scratch_used = keep;
-    d_lab = (uint32_t*)scratch_take(ctx, n * 4);
-    d_total = (unsigned long long*)scratch_take(ctx, 256);
-  }
-  uint64_t* keys = (uint64_t*)scratch_take(ctx, T * 8);
-  uint64_t* keys_s = (uint64_t*)scratch_take(ctx, T * 8);
-  uint8_t* cases = (uint8_t*)scratch_take(ctx, T);
-  uint8_t* cases_s = (uint8_t*)scratch_take(ctx, T);
-  uint64_t* vkeys = (uint64_t*)scratch_take(ctx, 3 * T * 8);
-  uint64_t* vkeys_s = (uint64_t*)scratch_take(ctx, 3 * T * 8);
-  uint32_t* corner = (uint32_t*)scratch_take(ctx, 3 * T * 4);
-  uint32_t* corner_s = (uint32_t*)scratch_take(ctx, 3 * T * 4);
-  uint32_t* heads = (uint32_t*)scratch_take(ctx, 3 * T * 4);
-  uint32_t* rank = (uint32_t*)scratch_take(ctx, 3 * T * 4);
-  uint32_t* d_tri_off = (uint32_t*)scratch_take(ctx, (K + 2) * 4);
-  uint32_t* d_vert_off = (uint32_t*)scratch_take(ctx, (K + 2) * 4);
-  void* tmp = scratch_take(ctx, tmp_bytes);
-  if (!keys || !keys_s || !cases || !cases_s || !vkeys || !vkeys_s || !corner || !corner_s || !heads ||
-      !rank || !d_tri_off || !d_vert_off || !tmp) {
-    set_error("scratch arena too small (mesher: %llu triangles)", T);
-    return fail(IGN_ERR_NOMEM);
-  }
+  uint64_t *keys, *keys_s, *vkeys, *vkeys_s;
+  uint8_t *cases, *cases_s;
+  uint32_t *corner, *corner_s, *heads, *rank, *d_tri_off, *d_vert_off;
+  void* tmp;
+  IGN_TRY(f.take(&keys, T));
+  IGN_TRY(f.take(&keys_s, T));
+  IGN_TRY(f.take(&cases, T));
+  IGN_TRY(f.take(&cases_s, T));
+  IGN_TRY(f.take(&vkeys, 3 * T));
+  IGN_TRY(f.take(&vkeys_s, 3 * T));
+  IGN_TRY(f.take(&corner, 3 * T));
+  IGN_TRY(f.take(&corner_s, 3 * T));
+  IGN_TRY(f.take(&heads, 3 * T));
+  IGN_TRY(f.take(&rank, 3 * T));
+  IGN_TRY(f.take(&d_tri_off, K + 2));
+  IGN_TRY(f.take(&d_vert_off, K + 2));
+  IGN_TRY(f.take(&tmp, tmp_bytes));
 
   // ---- emit + sort
-  MESH_CUDA(cudaMemsetAsync(d_total, 0, 8, ctx->stream));
-  MESH_LAUNCH((k_mc<true>), grid, 256, d_lab, (uint32_t)sx, (uint32_t)sy, (uint32_t)sz, d_total, keys,
-              cases, (uint64_t)T);
+  IGN_CUDA(cudaMemsetAsync(d_total, 0, 8, ctx->stream));
+  IGN_LAUNCH(ctx, (k_mc<true>), grid, 256, 0, d_lab, (uint32_t)sx, (uint32_t)sy, (uint32_t)sz, d_total, keys,
+             cases, (uint64_t)T);
   const int label_bits = bits_for(K);
   size_t tb = tmp_bytes;
-  MESH_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, keys, keys_s, cases, cases_s, (int)T, 0,
-                                            TRI_LABEL_SHIFT + label_bits, ctx->stream));
+  IGN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, keys, keys_s, cases, cases_s, (int)T, 0,
+                                           TRI_LABEL_SHIFT + label_bits, ctx->stream));
   ctx->launches += 4;
 
   // ---- weld
-  MESH_LAUNCH(k_tri_vertices, blocks_for(T, 256), 256, keys_s, cases_s, (uint64_t)T, (uint32_t)(sx - 1),
-              (uint32_t)(sy - 1), vkeys, corner);
+  IGN_LAUNCH(ctx, k_tri_vertices, blocks_for(T, 256), 256, 0, keys_s, cases_s, (uint64_t)T, (uint32_t)(sx - 1),
+             (uint32_t)(sy - 1), vkeys, corner);
   tb = tmp_bytes;
-  MESH_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, vkeys, vkeys_s, corner, corner_s, (int)(3 * T), 0,
-                                            V_LABEL_SHIFT + label_bits, ctx->stream));
+  IGN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, vkeys, vkeys_s, corner, corner_s, (int)(3 * T), 0,
+                                           V_LABEL_SHIFT + label_bits, ctx->stream));
   ctx->launches += 4;
-  MESH_LAUNCH(k_vertex_heads, blocks_for(3 * T, 256), 256, vkeys_s, (uint64_t)(3 * T), heads);
+  IGN_LAUNCH(ctx, k_vertex_heads, blocks_for(3 * T, 256), 256, 0, vkeys_s, (uint64_t)(3 * T), heads);
   tb = tmp_bytes;
-  MESH_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, heads, rank, (int)(3 * T), ctx->stream));
+  IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, heads, rank, (int)(3 * T), ctx->stream));
   ctx->launches += 2;
   uint32_t last[2];
-  MESH_TRY(small_d2h(ctx, &last[0], rank + (3 * T - 1), 4));
-  MESH_TRY(small_d2h(ctx, &last[1], heads + (3 * T - 1), 4));
-  MESH_TRY(small_sync(ctx));
+  IGN_TRY(small_d2h(ctx, &last[0], rank + (3 * T - 1), 4));
+  IGN_TRY(small_d2h(ctx, &last[1], heads + (3 * T - 1), 4));
+  IGN_TRY(small_sync(ctx));
   const uint64_t U = (uint64_t)last[0] + last[1];
   m->U = U;
   {
     const size_t fbytes = align_up(3 * T * 4, 256), vbytes = align_up(U * 12, 256);  // 12: float3 after simplify
     if (!ctx->mesh_pool_busy) {
       if (ctx->mesh_pool_bytes < fbytes + vbytes) {
-        MESH_CUDA(cudaStreamSynchronize(ctx->stream));
+        IGN_CUDA(cudaStreamSynchronize(ctx->stream));
         if (ctx->mesh_pool) cudaFree(ctx->mesh_pool);
         ctx->mesh_pool = nullptr;
         ctx->mesh_pool_bytes = 0;
         const size_t want = (fbytes + vbytes) * 5 / 4;
-        MESH_CUDA(cudaMalloc((void**)&ctx->mesh_pool, want));
+        IGN_CUDA(cudaMalloc((void**)&ctx->mesh_pool, want));
         ctx->mesh_pool_bytes = want;
       }
       m->d_faces = (uint32_t*)ctx->mesh_pool;
@@ -480,32 +425,32 @@ int ign_mesh_begin_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx,
       m->pooled = true;
       ctx->mesh_pool_busy = 1;
     } else {
-      MESH_CUDA(cudaMalloc((void**)&m->d_faces, 3 * T * 4));
-      MESH_CUDA(cudaMalloc((void**)&m->d_uniq_vkeys, U * 12));  // 12: float3 positions after simplification
+      IGN_CUDA(cudaMalloc((void**)&m->d_faces, 3 * T * 4));
+      IGN_CUDA(cudaMalloc((void**)&m->d_uniq_vkeys, U * 12));  // 12: float3 positions after simplification
     }
   }
-  MESH_LAUNCH(k_vertex_assign, blocks_for(3 * T, 256), 256, vkeys_s, corner_s, heads, rank,
-              (uint64_t)(3 * T), m->d_uniq_vkeys, m->d_faces);
+  IGN_LAUNCH(ctx, k_vertex_assign, blocks_for(3 * T, 256), 256, 0, vkeys_s, corner_s, heads, rank,
+             (uint64_t)(3 * T), m->d_uniq_vkeys, m->d_faces);
 
   // ---- per-label offsets (labels are 1..K; slot K+1 is the end sentinel)
-  MESH_LAUNCH(k_fill_u32, blocks_for(K + 2, 256), 256, d_tri_off, (uint32_t)T, (uint32_t)(K + 2));
-  MESH_LAUNCH(k_fill_u32, blocks_for(K + 2, 256), 256, d_vert_off, (uint32_t)U, (uint32_t)(K + 2));
-  MESH_LAUNCH(k_label_starts, blocks_for(T, 256), 256, keys_s, (uint64_t)T, TRI_LABEL_SHIFT, d_tri_off);
-  MESH_LAUNCH(k_label_starts, blocks_for(U, 256), 256, m->d_uniq_vkeys, U, V_LABEL_SHIFT, d_vert_off);
-  MESH_TRY(small_d2h(ctx, m->tri_off.data(), d_tri_off, (K + 2) * 4));
-  MESH_TRY(small_d2h(ctx, m->vert_off.data(), d_vert_off, (K + 2) * 4));
-  MESH_TRY(small_sync(ctx));
+  IGN_LAUNCH(ctx, k_fill_u32, blocks_for(K + 2, 256), 256, 0, d_tri_off, (uint32_t)T, (uint32_t)(K + 2));
+  IGN_LAUNCH(ctx, k_fill_u32, blocks_for(K + 2, 256), 256, 0, d_vert_off, (uint32_t)U, (uint32_t)(K + 2));
+  IGN_LAUNCH(ctx, k_label_starts, blocks_for(T, 256), 256, 0, keys_s, (uint64_t)T, TRI_LABEL_SHIFT, d_tri_off);
+  IGN_LAUNCH(ctx, k_label_starts, blocks_for(U, 256), 256, 0, m->d_uniq_vkeys, U, V_LABEL_SHIFT, d_vert_off);
+  IGN_TRY(small_d2h(ctx, m->tri_off.data(), d_tri_off, (K + 2) * 4));
+  IGN_TRY(small_d2h(ctx, m->vert_off.data(), d_vert_off, (K + 2) * 4));
+  IGN_TRY(small_sync(ctx));
   // absent labels hold the end marker: a suffix minimum turns starts into offsets
   for (int64_t l = (int64_t)K; l >= 0; l--) {
     if (m->tri_off[l] > m->tri_off[l + 1]) m->tri_off[l] = m->tri_off[l + 1];
     if (m->vert_off[l] > m->vert_off[l + 1]) m->vert_off[l] = m->vert_off[l + 1];
   }
-  MESH_TRY(small_h2d(ctx, d_vert_off, m->vert_off.data(), (K + 2) * 4));
-  MESH_LAUNCH(k_faces_local, blocks_for(3 * T, 256), 256, keys_s, d_vert_off, (uint64_t)T, m->d_faces);
-  MESH_CUDA(cudaStreamSynchronize(ctx->stream));
+  IGN_TRY(small_h2d(ctx, d_vert_off, m->vert_off.data(), (K + 2) * 4));
+  IGN_LAUNCH(ctx, k_faces_local, blocks_for(3 * T, 256), 256, 0, keys_s, d_vert_off, (uint64_t)T, m->d_faces);
+  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   for (uint64_t l = 1; l <= K; l++)
     if (m->tri_off[l + 1] > m->tri_off[l]) m->present.push_back(m->ids[l - 1]);
-  ctx->scratch_used = keep;
+  guard.m = nullptr;
   *out = m;
   return IGN_OK;
 }
@@ -525,9 +470,7 @@ int ign_mesh_begin(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uin
     set_error("mesher H2D: %s", cudaGetErrorString(e));
     rc = IGN_ERR_CUDA;
   } else {
-    scratch_reset(ctx);
     rc = ign_mesh_begin_dev(ctx, d, dtype, sx, sy, sz, out);
-    scratch_reset(ctx);
   }
   cudaStreamSynchronize(ctx->stream);
   cudaFree(d);
@@ -577,10 +520,7 @@ int ign_mesh_get(ign_mesher* m, uint64_t id, const float resolution[3], int redu
   IGN_REQUIRE(m && resolution && nv && nf, IGN_ERR_INVALID, "null argument");
   ign_ctx* ctx = m->ctx;
   IGN_TRY(activate(ctx));
-  if (reduction_factor > 0 && !m->simplified) {
-    scratch_reset(ctx);
-    IGN_TRY(ign_mesh_simplify(m, resolution, reduction_factor, max_error));
-  }
+  if (reduction_factor > 0 && !m->simplified) IGN_TRY(ign_mesh_simplify(m, resolution, reduction_factor, max_error));
   if (m->simplified) {
     IGN_REQUIRE(reduction_factor == m->simp_factor && max_error == m->simp_max_error, IGN_ERR_INVALID,
                 "mesher was simplified with reduction_factor=%d max_error=%g; call mesh() again to change",
@@ -593,14 +533,13 @@ int ign_mesh_get(ign_mesher* m, uint64_t id, const float resolution[3], int redu
   *nv = v1 - v0;
   *nf = t1 - t0;
   if (*nv == 0 || vertices == nullptr || faces == nullptr) return IGN_OK;
-  scratch_reset(ctx);
-  IGN_TRY(scratch_reserve(ctx, (v1 - v0) * 12 + 4096));
-  float* d_pos = (float*)scratch_take(ctx, (v1 - v0) * 12);
+  ScratchFrame f(ctx);
+  float* d_pos;
+  IGN_TRY(f.take(&d_pos, (v1 - v0) * 3));
   IGN_TRY(mesher_positions(m, v0, v1 - v0, resolution, voxel_centered, d_pos));
   IGN_CUDA(cudaMemcpyAsync(vertices, d_pos, (v1 - v0) * 12, cudaMemcpyDeviceToHost, ctx->stream));
   IGN_CUDA(cudaMemcpyAsync(faces, m->d_faces + 3 * t0, (t1 - t0) * 12, cudaMemcpyDeviceToHost, ctx->stream));
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  scratch_reset(ctx);
   return IGN_OK;
 }
 
@@ -620,14 +559,13 @@ int ign_mesh_export(ign_mesher* m, const float resolution[3], int voxel_centered
   vert_offsets[j] = m->U;
   face_offsets[j] = m->T;
   if (m->U == 0 || vertices == nullptr || faces == nullptr) return IGN_OK;
-  scratch_reset(ctx);
-  IGN_TRY(scratch_reserve(ctx, m->U * 12 + 4096));
-  float* d_pos = (float*)scratch_take(ctx, m->U * 12);
+  ScratchFrame f(ctx);
+  float* d_pos;
+  IGN_TRY(f.take(&d_pos, m->U * 3));
   IGN_TRY(mesher_positions(m, 0, m->U, resolution, voxel_centered, d_pos));
   IGN_TRY(d2h_by_kernel(ctx, vertices, d_pos, m->U * 12));
   IGN_TRY(d2h_by_kernel(ctx, faces, m->d_faces, m->T * 12));
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  scratch_reset(ctx);
   return IGN_OK;
 }
 
