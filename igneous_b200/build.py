@@ -31,8 +31,9 @@ def _stale(target, deps):
   return any(os.path.getmtime(d) > t for d in deps)
 
 
-# simplify.cu must match the CPU oracle bit for bit: no FMA contraction
-PER_FILE_FLAGS = {"simplify.cu": ["-fmad=false"]}
+# simplify.cu must match the CPU oracle bit for bit, and contrast.cu the float32 rules of
+# DESIGN.md §5b (each product rounded on its own): no FMA contraction
+PER_FILE_FLAGS = {"simplify.cu": ["-fmad=false"], "contrast.cu": ["-fmad=false"]}
 
 
 def _compile(src, obj, log):

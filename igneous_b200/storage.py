@@ -326,6 +326,13 @@ class _Meta:
   def key(self, mip):
     return self._cv.key_at(mip)
 
+  def unlock_mips(self, mips):
+    """Clear the write lock of the given mip(s) (in memory, as cloudvolume does until the
+    next commit_info); the stand-in never sets one, so this only drops a `locked` key."""
+    for m in ([mips] if np.isscalar(mips) else mips):
+      if 0 <= int(m) < len(self._cv.info["scales"]):
+        self._cv.info["scales"][int(m)].pop("locked", None)
+
   @property
   def cloudpath(self):
     return self._cv.cloudpath

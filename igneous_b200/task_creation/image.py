@@ -1,5 +1,6 @@
-"""create_downsampling_tasks, create_image_shard_downsample_tasks and the three CCL
-task creators (igneous/task_creation/image.py:170-345, 639-770, 1726-1889): same
+"""create_downsampling_tasks, create_image_shard_downsample_tasks, the contrast / CLAHE /
+quantize creators and the three CCL task creators (igneous/task_creation/image.py:170-345,
+639-770, 1247-1618, 1726-1889): same
 signatures, same info / provenance side effects, tasks from igneous_b200.tasks."""
 import copy
 import math
@@ -9,8 +10,9 @@ from time import strftime
 import numpy as np
 
 from .. import downsample_scales, fastremap, sharding, shards
-from .._compat import CloudVolume, CloudFiles, InfoUnavailableError, Vec
-from ..tasks import DownsampleTask, ImageShardDownsampleTask, CCLFacesTask, CCLEquivalancesTask, RelabelCCLTask
+from .._compat import Bbox, CloudVolume, CloudFiles, InfoUnavailableError, Vec
+from ..tasks import (DownsampleTask, ImageShardDownsampleTask, CCLFacesTask, CCLEquivalancesTask, RelabelCCLTask,
+                     QuantizeTask, CLAHETask, ContrastNormalizationTask, LuminanceLevelsTask)
 from ..types import DownsampleMethods
 from .common import FinelyDividedTaskIterator, get_bounds, operator_contact
 
@@ -223,3 +225,177 @@ def create_ccl_relabel_tasks(src_path, dest_path, mip, shape=(512, 512, 512), ch
            fill_missing=bool(fill_missing), dust_threshold=dust_threshold)
 
   return RelabelCCLTaskIterator(src.meta.bounds(mip).clone(), shape)
+
+
+# ------------------------------------------------------- contrast, CLAHE, quantize
+# task_creation/image.py:1247-1618: same signatures, destination info, scales, task grids and
+# provenance as the reference; the tasks are those of igneous_b200.tasks.
+
+def _new_dest(src_vol, dest_path, mip):
+  """The destination layer, or (when it has no info yet) the source's info cut to scales[:mip+1]."""
+  try:
+    dvol = CloudVolume(dest_path, mip=mip)
+  except InfoUnavailableError:
+    dvol = CloudVolume(dest_path, mip=mip, info=copy.deepcopy(src_vol.info))
+    dvol.info["scales"] = dvol.info["scales"][:mip + 1]
+    dvol.commit_info()
+  dvol.meta.unlock_mips(mip)
+  return dvol
+
+
+def _default_image_task_shape(chunk_size, bounds):
+  """(2048, 2048, chunk_z) shrunk to whole chunks, then clamped to [1, bounds size] per axis
+  (Bbox.shrink_to_chunk_size + Vec.clamp of the reference)."""
+  cs = np.asarray(chunk_size[:3], dtype=int)
+  want = np.asarray([2048, 2048, int(cs[2])], dtype=int)
+  shrunk = (want // cs) * cs
+  return Vec(*np.maximum(np.minimum(shrunk, np.asarray(bounds.size3(), dtype=int)), 1))
+
+
+def create_contrast_normalization_tasks(src_path, dest_path, levels_path=None, shape=None, mip=0, clip_fraction=0.01,
+                                        fill_missing=False, translate=(0, 0, 0), minval=None, maxval=None,
+                                        bounds=None, bounds_mip=0):
+  """Stretch every slice between its LuminanceLevelsTask (lower, upper) levels into dest_path and
+  build its downsamples (task_creation/image.py:1247-1324)."""
+  srcvol = CloudVolume(src_path, mip=mip)
+  dvol = _new_dest(srcvol, dest_path, mip)
+  if bounds is None:
+    bounds = srcvol.meta.bounds(mip).clone()
+  if shape is None:
+    shape = _default_image_task_shape(dvol.meta.chunk_size(mip), bounds)
+  shape = Vec(*shape)
+  downsample_scales.create_downsample_scales(dest_path, mip=mip, ds_shape=shape, preserve_chunk_size=True)
+  dvol.refresh_info()
+  # as in the reference, bounds (default: the source's bounds at `mip`) are read at bounds_mip
+  bounds = get_bounds(srcvol, bounds, mip, bounds_mip=bounds_mip)
+
+  class ContrastNormalizationTaskIterator(FinelyDividedTaskIterator):
+    def task(self, shape, offset):
+      return ContrastNormalizationTask(src_path=src_path, dest_path=dest_path, levels_path=levels_path,
+                                       shape=shape.clone(), offset=offset.clone(), clip_fraction=clip_fraction,
+                                       mip=mip, fill_missing=fill_missing, translate=translate, minval=minval,
+                                       maxval=maxval)
+
+    def on_finish(self):
+      _log(dvol, "ContrastNormalizationTask", src_path=src_path, dest_path=dest_path,
+           shape=[int(v) for v in shape], clip_fraction=clip_fraction, mip=mip,
+           translate=[int(v) for v in translate], minval=minval, maxval=maxval,
+           bounds=[[int(v) for v in bounds.minpt], [int(v) for v in bounds.maxpt]])
+
+  return ContrastNormalizationTaskIterator(bounds, shape)
+
+
+def create_luminance_levels_tasks(layer_path, levels_path=None, coverage_factor=0.01, shape=None, offset=None, mip=0,
+                                  bounds_mip=0, bounds=None):
+  """One LuminanceLevelsTask per slice, writing $levels_path/levels/$mip/$z
+  (task_creation/image.py:1326-1426).  As in the reference the slices run over the inclusive
+  range(minpt.z, maxpt.z + 1): the last task clamps to an empty box and writes nothing, and
+  len() counts the slices without it.  `shape` is ignored: a task covers the whole (x, y) extent
+  of the bounds."""
+  if shape is not None or offset is not None:
+    print("Create Luminance Levels Tasks: Deprecation Notice: "
+          "shape and offset parameters are deprecated in favor of the bounds argument.")
+  vol = CloudVolume(layer_path, mip=mip)
+  if bounds is None:
+    bounds = vol.meta.bounds(mip).clone()
+  bounds = get_bounds(vol, bounds, mip, bounds_mip=bounds_mip)
+  shape = Vec(*bounds.size3())
+  shape.z = 1
+  offset = Vec(*(bounds.minpt if offset is None or len(offset) == 0 else offset))
+  if str(layer_path).startswith("boss://"):
+    raise NotImplementedError("create_luminance_levels_tasks: boss:// layers are not supported")
+
+  class LuminanceLevelsTaskIterator:
+    def __len__(self):
+      return int(bounds.maxpt.z - bounds.minpt.z)
+
+    def __iter__(self):
+      for z in range(int(bounds.minpt.z), int(bounds.maxpt.z) + 1):
+        zoffset = offset.clone()
+        zoffset.z = z
+        yield LuminanceLevelsTask(src_path=layer_path, levels_path=levels_path, shape=shape.clone(),
+                                  offset=zoffset, coverage_factor=coverage_factor, mip=mip)
+      if levels_path:
+        try:
+          pvol = CloudVolume(levels_path)
+        except InfoUnavailableError:
+          pvol = CloudVolume(levels_path, info=vol.info)
+      else:
+        pvol = CloudVolume(layer_path, mip=mip)
+      _log(pvol, "LuminanceLevelsTask", src=layer_path, levels_path=levels_path, shape=[int(v) for v in shape],
+           offset=[int(v) for v in offset], bounds=[[int(v) for v in bounds.minpt], [int(v) for v in bounds.maxpt]],
+           coverage_factor=coverage_factor, mip=mip)
+
+  return LuminanceLevelsTaskIterator()
+
+
+def create_clahe_tasks(src, dest, shape=None, mip=0, fill_missing=False, bounds=None, bounds_mip=0,
+                       clip_limit=40.0, tile_grid_size=(8, 8)):
+  """CLAHE (contrast limited adaptive histogram equalization) of every slice of src into dest
+  (task_creation/image.py:1428-1508).  The tasks write mip `mip` only."""
+  srcvol = CloudVolume(src, mip=mip)
+  dvol = _new_dest(srcvol, dest, mip)
+  if bounds is None:
+    bounds = srcvol.meta.bounds(mip).clone()
+  if shape is None:
+    shape = _default_image_task_shape(dvol.meta.chunk_size(mip), bounds)
+  shape = Vec(*shape)
+  downsample_scales.create_downsample_scales(dest, mip=mip, ds_shape=shape, preserve_chunk_size=True)
+  dvol.refresh_info()
+  bounds = get_bounds(srcvol, bounds, mip, bounds_mip=bounds_mip)
+
+  class CLAHETaskIterator(FinelyDividedTaskIterator):
+    def task(self, shape, offset):
+      return partial(CLAHETask, src=src, dest=dest, shape=shape.clone(), offset=offset.clone(), mip=mip,
+                     fill_missing=fill_missing, clip_limit=clip_limit, tile_grid_size=tile_grid_size)
+
+    def on_finish(self):
+      _log(dvol, "CLAHETask", src=src, dest=dest, shape=[int(v) for v in shape], clip_limit=clip_limit,
+           tile_grid_size=tile_grid_size, mip=mip,
+           bounds=[[int(v) for v in bounds.minpt], [int(v) for v in bounds.maxpt]])
+
+  return CLAHETaskIterator(bounds, shape)
+
+
+def create_quantized_affinity_info(src_layer, dest_layer, shape, mip, chunk_size, encoding):
+  """The source's info as a 1-channel uint8 image, scales[:mip+1], each with `chunk_size` and
+  `encoding` (task_creation/image.py:1546-1560)."""
+  info = copy.deepcopy(CloudVolume(src_layer).info)
+  info["num_channels"] = 1
+  info["data_type"] = "uint8"
+  info["type"] = "image"
+  info["scales"] = info["scales"][:mip + 1]
+  for i in range(mip + 1):
+    info["scales"][i]["encoding"] = encoding
+    info["scales"][i]["chunk_sizes"] = [list(chunk_size)]
+  return info
+
+
+def create_quantize_tasks(src_layer, dest_layer, shape, mip=0, fill_missing=False, chunk_size=(128, 128, 64),
+                          encoding="raw", bounds=None):
+  """Quantize channel 0 of a float32 affinity layer into a uint8 image with downsamples
+  (task_creation/image.py:1562-1618).  `bounds` are given at mip 0."""
+  shape = Vec(*shape)
+  info = create_quantized_affinity_info(src_layer, dest_layer, shape, mip, chunk_size, encoding)
+  destvol = CloudVolume(dest_layer, info=info, mip=mip)
+  destvol.commit_info()
+  downsample_scales.create_downsample_scales(dest_layer, mip=mip, ds_shape=shape, chunk_size=chunk_size,
+                                             encoding=encoding)
+  if bounds is None:
+    bounds = destvol.meta.bounds(mip)
+  else:
+    bounds = destvol.bbox_to_mip(Bbox.create(bounds), mip=0, to_mip=mip)
+    bounds = bounds.expand_to_chunk_size(destvol.meta.chunk_size(mip), destvol.meta.voxel_offset(mip))
+
+  class QuantizeTasksIterator(FinelyDividedTaskIterator):
+    def task(self, shape, offset):
+      return partial(QuantizeTask, source_layer_path=src_layer, dest_layer_path=dest_layer,
+                     shape=[int(v) for v in shape], offset=[int(v) for v in offset], fill_missing=fill_missing,
+                     mip=mip)
+
+    def on_finish(self):
+      destvol.provenance.sources = [src_layer]
+      _log(destvol, "QuantizeTask", source_layer_path=src_layer, dest_layer_path=dest_layer,
+           shape=[int(v) for v in shape], fill_missing=fill_missing, mip=mip)
+
+  return QuantizeTasksIterator(bounds, shape)

@@ -1,5 +1,6 @@
 from .image import (DownsampleTask, TransferTask, ImageShardDownsampleTask, downsample_and_upload,
-                    downsample_method_to_fn)
+                    downsample_method_to_fn, QuantizeTask, CLAHETask, ContrastNormalizationTask,
+                    LuminanceLevelsTask)
 from .ccl import (CCLFacesTask, CCLEquivalancesTask, RelabelCCLTask, create_relabeling,
                   clean_intermediate_files, threshold_image, blackout_non_face_rails, DisjointSet)
 from .mesh import MeshTask

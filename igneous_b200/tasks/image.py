@@ -4,17 +4,23 @@ Same names, arguments and side effects as igneous/tasks/image/image.py:
   downsample_method_to_fn :37-55, downsample_and_upload :57-100,
   TransferTask :434-516, DownsampleTask :518-549.
   ImageShardDownsampleTask :672-843.
+  QuantizeTask :145-162, CLAHETask :164-209, ContrastNormalizationTask :211-343,
+  LuminanceLevelsTask :345-432 (per-voxel work in igneous_b200.contrast).
 Only the library behind `fn(image, factors[0], num_mips=...)` (:91) changes:
 igneous_b200.tinybrain instead of the CPU tinybrain wheel.
 """
+import json
 import math
+import os
+import random
 from collections import defaultdict
+from collections.abc import Sequence
 from functools import partial
 
 import numpy as np
 
-from .. import downsample_scales, fastremap, sharding, shards, tinybrain
-from .._compat import CloudVolume, CloudFiles, Bbox, Vec, min2, queueable
+from .. import contrast, downsample_scales, fastremap, sharding, shards, tinybrain
+from .._compat import CloudVolume, CloudFiles, Bbox, Vec, min2, queueable, RegisteredTask
 from ..types import DownsampleMethods
 
 
@@ -202,3 +208,155 @@ def _shard_chunks(vol, cutout, box, mip):
     cutout = np.pad(cutout, pad, mode="constant", constant_values=vol.background_color)
     box = Bbox(box.minpt, np.asarray(box.minpt) + np.asarray(cutout.shape[:3]))
   return vol.image.make_shard_chunks(cutout, box, mip)
+
+
+# ------------------------------------------------------- contrast, CLAHE, quantize
+# image.py:145-432: the same tasks with the per-voxel work on the GPU (igneous_b200.contrast,
+# rules in DESIGN.md §5b) and the pyramids through downsample_and_upload as above.
+
+@queueable
+def QuantizeTask(source_layer_path, dest_layer_path, shape, offset, mip, fill_missing=False):
+  """Channel 0 of a float32 affinity layer as uint8 trunc(v * 255), then the z pyramid
+  (image.py:145-162).  Out-of-range products saturate and NaN gives 0."""
+  shape, offset = Vec(*shape), Vec(*offset)
+  srcvol = CloudVolume(source_layer_path, mip=mip, fill_missing=fill_missing)
+  bounds = Bbox.clamp(Bbox(offset, shape + offset), srcvol.bounds)
+  image = contrast.quantize(srcvol[bounds][:, :, :, :1])
+  destvol = CloudVolume(dest_layer_path, mip=mip)
+  downsample_and_upload(image, bounds, destvol, shape, mip=mip, axis="z")
+
+
+@queueable
+def CLAHETask(src, dest, mip, fill_missing, shape, offset, clip_limit=40.0, tile_grid_size=(8, 8)):
+  """CLAHE of every z-slice of channel 0 (image.py:164-209).  As in the reference the box is
+  enlarged by tile_grid_size[0] voxels in x and tile_grid_size[1] in y (grid counts, not tile
+  sizes) and clamped to the dataset, each slice is equalised at that size, and only the task's
+  own box is written (no pyramid)."""
+  shape, offset = Vec(*shape), Vec(*offset)
+  src_cv = CloudVolume(src, mip=mip, fill_missing=fill_missing)
+  bounds = Bbox.clamp(Bbox(offset, shape + offset), src_cv.bounds)
+  over = bounds.clone()
+  over.minpt.x -= tile_grid_size[0]
+  over.maxpt.x += tile_grid_size[0]
+  over.minpt.y -= tile_grid_size[1]
+  over.maxpt.y += tile_grid_size[1]
+  over = Bbox.clamp(over, src_cv.bounds)
+  stack = contrast.clahe(src_cv[over][..., 0], clip_limit, tile_grid_size)
+  crop = tuple(slice(int(a - o), int(b - o)) for a, b, o in zip(bounds.minpt, bounds.maxpt, over.minpt))
+  dest_cv = CloudVolume(dest, mip=mip)
+  dest_cv[bounds] = stack[crop]
+
+
+def read_levels(cf, paths):
+  """{path: bytes or None} for the levels files, from CloudFiles.get of a list in either form:
+  the real package's [{'path', 'content', ...}] or a {path: content} mapping."""
+  got = cf.get(list(paths))
+  if isinstance(got, dict):
+    return {p: got.get(p) for p in paths}
+  return {item["path"]: item.get("content") for item in got}
+
+
+class ContrastNormalizationTask(RegisteredTask):
+  """TransferTask + contrast correction from LuminanceLevelsTask's histograms (image.py:211-343).
+  Each z-slice is stretched between the (lower, upper) luminance of its histogram on the GPU,
+  then the pyramid is built by downsample_and_upload at bounds + translate."""
+
+  def __init__(self, src_path, dest_path, levels_path, shape, offset, mip, clip_fraction, fill_missing,
+               translate, minval, maxval):
+    super().__init__(src_path, dest_path, levels_path, shape, offset, mip, clip_fraction, fill_missing,
+                     translate, minval, maxval)
+    self.src_path = src_path
+    self.dest_path = dest_path
+    self.shape = Vec(*shape)
+    self.offset = Vec(*offset)
+    self.fill_missing = fill_missing
+    self.translate = Vec(*translate)
+    self.mip = int(mip)
+    if isinstance(clip_fraction, Sequence):
+      assert len(clip_fraction) == 2
+      self.lower_clip_fraction = float(clip_fraction[0])
+      self.upper_clip_fraction = float(clip_fraction[1])
+    else:
+      self.lower_clip_fraction = self.upper_clip_fraction = float(clip_fraction)
+    self.minval = minval
+    self.maxval = maxval
+    self.levels_path = levels_path if levels_path else self.src_path
+    assert 0 <= self.lower_clip_fraction <= 1
+    assert 0 <= self.upper_clip_fraction <= 1
+    assert self.lower_clip_fraction + self.upper_clip_fraction <= 1
+
+  def execute(self):
+    srccv = CloudVolume(self.src_path, fill_missing=self.fill_missing, mip=self.mip)
+    destcv = CloudVolume(self.dest_path, fill_missing=self.fill_missing, mip=self.mip)
+    bounds = Bbox.clamp(Bbox(self.offset, self.shape[:3] + self.offset), srccv.bounds)
+    image = srccv[bounds]
+    zlevels = self.fetch_z_levels(bounds)
+    image = contrast.stretch(image, zlevels, self.lower_clip_fraction, self.upper_clip_fraction,
+                             minval=self.minval, maxval=self.maxval, out_dtype=destcv.dtype)
+    bounds += self.translate
+    downsample_and_upload(image, bounds, destcv, self.shape, mip=self.mip)
+
+  def find_section_clamping_values(self, zlevel, lowerfract, upperfract):
+    return contrast.find_section_clamping_values(zlevel, lowerfract, upperfract)
+
+  def fetch_z_levels(self, bounds):
+    cf = CloudFiles(self.levels_path)
+    paths = [cf.join("levels", str(self.mip), str(z)) for z in range(int(bounds.minpt.z), int(bounds.maxpt.z))]
+    got = read_levels(cf, paths)
+    missing = [p for p in paths if got[p] is None]
+    if missing:
+      raise Exception(", ".join(missing) + " were not defined. Did you run a LuminanceLevelsTask for these slices?")
+    return [np.array(json.loads(got[p].decode("utf-8"))["levels"], dtype=np.uint64) for p in paths]
+
+
+class LuminanceLevelsTask(RegisteredTask):
+  """Histogram of randomly sampled 2048 x 2048 x 1 patches of one slice, written to
+  $levels_path/levels/$mip/$z (image.py:345-432).  All patches go to the GPU in one call."""
+
+  def __init__(self, src_path, levels_path, shape, offset, coverage_factor, mip):
+    super().__init__(src_path, levels_path, shape, offset, coverage_factor, mip)
+    self.src_path = src_path
+    self.shape = Vec(*shape)
+    self.offset = Vec(*offset)
+    self.coverage_factor = coverage_factor
+    self.mip = int(mip)
+    self.levels_path = levels_path
+    assert 0 < coverage_factor <= 1, "Coverage Factor must be between 0 and 1"
+
+  def execute(self):
+    srccv = CloudVolume(self.src_path, mip=self.mip, fill_missing=True)
+    bounds = Bbox.clamp(Bbox(self.offset, self.shape[:3] + self.offset), srccv.bounds)
+    bboxes = self.select_bounding_boxes(bounds)
+    if len(bboxes) == 0:
+      return
+    patches = [np.asarray(srccv[b]).ravel(order="F") for b in bboxes]
+    levels = contrast.histogram(np.concatenate(patches))
+    covered_area = sum(b.volume() for b in bboxes)
+    sizes = sorted(((b.volume(), b.size3()) for b in bboxes), key=lambda x: x[0])
+    output = {
+      "levels": levels.tolist(),
+      "patch_size": [int(v) for v in sizes[-1][1]],
+      "num_patches": len(bboxes),
+      "coverage_ratio": covered_area / self.shape.rectVolume(),
+    }
+    path = os.path.join(self.levels_path if self.levels_path else self.src_path, "levels")
+    CloudFiles(path).put_json("{}/{}".format(self.mip, self.offset.z), output, cache_control="no-cache")
+
+  def select_bounding_boxes(self, dataset_bounds):
+    """Non-overlapping patches on a 2048 x 2048 grid, drawn with random.randint in the
+    reference's order, so that a seeded `random` picks the same patches."""
+    sample = Vec(2048, 2048, 1)
+    area = self.shape.rectVolume()
+    total_patches = int(math.ceil(area / (2048 * 2048)))
+    n = int(math.ceil(float(total_patches) * self.coverage_factor))
+    patch_indices = set()
+    while len(patch_indices) < n:
+      patch_indices.add(random.randint(0, total_patches - 1))
+    gridx = int(math.ceil(self.shape.x / sample.x))
+    bboxes = []
+    for i in patch_indices:
+      start = Vec(i % gridx, i // gridx, 0) * sample + self.offset
+      bbox = Bbox.clamp(Bbox(start, start + sample), dataset_bounds)
+      if not bbox.subvoxel():
+        bboxes.append(bbox)
+    return bboxes

@@ -229,6 +229,46 @@ IGN_API int ign_fill_holes(ign_ctx* ctx, const void* in, int dtype, uint64_t sx,
 IGN_API int ign_fill_holes_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
                                int fix_borders, int merge_threshold_pct, void* filled, void* holes);
 
+/* ------------------------------------------------- contrast, CLAHE, quantize
+ * The per-voxel rules are stated in DESIGN.md §5b.  u8 / u16 input only (IGN_ERR_UNSUPPORTED
+ * otherwise).  Buffers must be aligned to their element size (IGN_ERR_INVALID otherwise).
+ *
+ * np.bincount(img2d) accumulated into levels   igneous/tasks/image/image.py:373-376
+ *   hist[v] += number of voxels equal to v; hist has 256 (u8) or 65,536 (u16) entries (a DEVICE
+ *   array for _dev, a HOST array otherwise) and is added into, not cleared.  n < 2^40.
+ */
+IGN_API int ign_histogram(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint64_t* hist);
+IGN_API int ign_histogram_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint64_t* hist);
+/* ContrastNormalizationTask.execute                 igneous/tasks/image/image.py:257-280
+ *   (x, y, z, c) volume; slice z with lower[z] != upper[z] becomes
+ *   (f32(v) - f32(lower)) * f32(maxval_t / (upper - lower)), maxval_t = 2^bits - 1 of in_dtype,
+ *   every other slice keeps its values; then rint (half to even), clip to [minval, maxval] (in
+ *   float32) and cast to out_dtype (u8, u16, u32 or f32).  lower / upper are HOST arrays of sz
+ *   entries in both variants.  [f32(minval), f32(maxval)] outside out_dtype's range -> IGN_ERR_INVALID
+ *   (for u32 output maxval may be at most 4294967040, the largest float32 below 2^32). */
+IGN_API int ign_contrast_stretch(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy,
+                                 uint64_t sz, uint64_t sc, const uint32_t* lower, const uint32_t* upper,
+                                 double minval, double maxval, void* out, int out_dtype);
+IGN_API int ign_contrast_stretch_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy,
+                                     uint64_t sz, uint64_t sc, const uint32_t* lower, const uint32_t* upper,
+                                     double minval, double maxval, void* out, int out_dtype);
+/* (image * 255.0).astype(np.uint8)                  igneous/tasks/image/image.py:158-159
+ *   n float32 -> u8: trunc(v * 255) for products in [0, 256); below 0 -> 0, 256 and above -> 255,
+ *   NaN -> 0 (numpy leaves those undefined).  Channel 0 of an F-order (x, y, z, c) array is its
+ *   first sx*sy*sz elements. */
+IGN_API int ign_quantize(ign_ctx* ctx, const float* in, uint64_t n, uint8_t* out);
+IGN_API int ign_quantize_dev(ign_ctx* ctx, const float* in, uint64_t n, uint8_t* out);
+/* cv2.createCLAHE(clipLimit, tileGridSize).apply(slice) on every z-slice
+ *                                                   igneous/tasks/image/image.py:185, :201-202
+ *   OpenCV 4.13 CLAHE::apply for CV_8UC1 / CV_16UC1 on each (sx, sy) slice of an (sx, sy, sz)
+ *   stack, axis 0 (x) being OpenCV's rows: tiles_x tiles across y, tiles_y across x.  out may
+ *   alias in.  The _dev variant takes the LUTs (sz * tiles_x * tiles_y * 256 or 65,536 entries of
+ *   the dtype) from the scratch arena. */
+IGN_API int ign_clahe(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
+                      double clip_limit, uint32_t tiles_x, uint32_t tiles_y, void* out);
+IGN_API int ign_clahe_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
+                          double clip_limit, uint32_t tiles_x, uint32_t tiles_y, void* out);
+
 /* ---------------------------------------------------------------- fastremap
  * fastremap.renumber(data, in_place=True)            igneous/tasks/mesh/mesh.py:206
  *   ids 1..K by first appearance in memory order, 0 kept.  out is u32;
