@@ -106,20 +106,12 @@ def ccl_task(image, shape, threshold_gte=None, threshold_lte=None, dust_threshol
   out = np.zeros(arr.shape, dtype=np.uint64, order="F")
   n = c.c_uint64(0)
   if arr.size:
-    d_in = ctx.to_device(arr)
-    d_out = ctx.alloc(arr.size * 8)
-    try:
-      _shim.check(ctx.lib.ign_ccl_task_dev(
-        ctx.handle, _shim.ptr(d_in), c.c_int(_shim.dtype_code(arr.dtype)), c.c_uint64(sx), c.c_uint64(sy),
-        c.c_uint64(sz), c.c_int(int(threshold_gte is not None)),
-        c.c_double(float(threshold_gte) if threshold_gte is not None else 0.0),
-        c.c_int(int(threshold_lte is not None)),
-        c.c_double(float(threshold_lte) if threshold_lte is not None else 0.0),
-        c.c_uint64(int(shape[0])), c.c_uint64(int(shape[1])), c.c_uint64(int(shape[2])),
-        c.c_uint64(int(dust_threshold or 0)), c.c_uint64(int(label_offset)), _shim.ptr(d_out), c.byref(n)))
-      ctx.d2h(out, d_out)
-      ctx.sync()
-    finally:
-      d_in.free()
-      d_out.free()
+    _shim.check(ctx.lib.ign_ccl_task(
+      ctx.handle, _shim.ptr(arr), c.c_int(_shim.dtype_code(arr.dtype)), c.c_uint64(sx), c.c_uint64(sy),
+      c.c_uint64(sz), c.c_int(int(threshold_gte is not None)),
+      c.c_double(float(threshold_gte) if threshold_gte is not None else 0.0),
+      c.c_int(int(threshold_lte is not None)),
+      c.c_double(float(threshold_lte) if threshold_lte is not None else 0.0),
+      c.c_uint64(int(shape[0])), c.c_uint64(int(shape[1])), c.c_uint64(int(shape[2])),
+      c.c_uint64(int(dust_threshold or 0)), c.c_uint64(int(label_offset)), _shim.ptr(out), c.byref(n)))
   return out, int(n.value)

@@ -1482,40 +1482,33 @@ int ign_ccl_task_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, ui
 // ---- host-buffer wrappers
 int ign_ccl6(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy, uint64_t sz,
              void* out, int out_dtype, uint64_t* n_components) {
-  IGN_TRY(activate(ctx));
-  IGN_REQUIRE(in && out, IGN_ERR_INVALID, "null buffer");
   IGN_TRY(check_ccl_dims(sx, sy, sz));
-  const int es = dtype_size(in_dtype), os = dtype_size(out_dtype);
-  IGN_REQUIRE(es > 0 && os > 0, IGN_ERR_UNSUPPORTED, "unsupported dtype");
+  // sizes the staged output; ign_ccl6_dev checks out_dtype only once it writes labels
+  IGN_REQUIRE(dtype_size(out_dtype) > 0, IGN_ERR_UNSUPPORTED, "CCL: unsupported output dtype %d", out_dtype);
   const uint64_t n = sx * sy * sz;
-  ScratchFrame f(ctx);
-  void *d_in, *d_out;
-  IGN_TRY(f.take(&d_in, n * es));
-  IGN_TRY(f.take(&d_out, n * os));
-  IGN_CUDA(cudaMemcpyAsync(d_in, in, n * es, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_ccl6_dev(ctx, d_in, in_dtype, sx, sy, sz, d_out, out_dtype, n_components));
-  IGN_CUDA(cudaMemcpyAsync(out, d_out, n * os, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  return IGN_OK;
+  return staged(ctx, {{in, nullptr, n * dtype_size(in_dtype)}, {nullptr, out, n * dtype_size(out_dtype)}},
+                [&](void* const* d) {
+                  return ign_ccl6_dev(ctx, d[0], in_dtype, sx, sy, sz, d[1], out_dtype, n_components);
+                });
 }
 
 int ign_dust(ign_ctx* ctx, void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
              uint64_t threshold) {
-  IGN_TRY(activate(ctx));
-  IGN_REQUIRE(labels, IGN_ERR_INVALID, "null buffer");
-  if (threshold == 0) return IGN_OK;
+  if (threshold == 0) return ign_dust_dev(ctx, labels, dtype, sx, sy, sz, 0);  // leaves labels as they are
   IGN_TRY(check_ccl_dims(sx, sy, sz));
-  const int es = dtype_size(dtype);
-  IGN_REQUIRE(es > 0 && dtype != IGN_F32, IGN_ERR_UNSUPPORTED, "unsupported dtype");
+  return staged(ctx, {{labels, labels, sx * sy * sz * dtype_size(dtype)}},
+                [&](void* const* d) { return ign_dust_dev(ctx, d[0], dtype, sx, sy, sz, threshold); });
+}
+
+int ign_ccl_task(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy, uint64_t sz, int use_gte,
+                 double gte, int use_lte, double lte, uint64_t rail_x, uint64_t rail_y, uint64_t rail_z,
+                 uint64_t dust_threshold, uint64_t label_offset, uint64_t* out, uint64_t* n_components) {
+  IGN_TRY(check_ccl_dims(sx, sy, sz));
   const uint64_t n = sx * sy * sz;
-  ScratchFrame f(ctx);
-  void* d;
-  IGN_TRY(f.take(&d, n * es));
-  IGN_CUDA(cudaMemcpyAsync(d, labels, n * es, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_dust_dev(ctx, d, dtype, sx, sy, sz, threshold));
-  IGN_CUDA(cudaMemcpyAsync(labels, d, n * es, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  return IGN_OK;
+  return staged(ctx, {{in, nullptr, n * dtype_size(in_dtype)}, {nullptr, out, n * 8}}, [&](void* const* d) {
+    return ign_ccl_task_dev(ctx, d[0], in_dtype, sx, sy, sz, use_gte, gte, use_lte, lte, rail_x, rail_y, rail_z,
+                            dust_threshold, label_offset, (uint64_t*)d[1], n_components);
+  });
 }
 
 int ign_ccl6_link_dev(ign_ctx* ctx, const uint64_t* values_a, const uint32_t* labels_a,

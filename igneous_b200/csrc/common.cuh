@@ -129,6 +129,40 @@ class ScratchFrame {
 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// One host buffer of a host-buffer entry point.  `from` is copied to the device before the call and
+// the device buffer back to `to` after it; both set = one device buffer used in place, both null = the
+// call gets a null pointer.  The call may lower `bytes` of an output whose size only its result gives.
+struct HostBuf {
+  const void* from;
+  void* to;
+  size_t bytes;
+};
+
+// Runs call(d) on device buffers d[i] for bufs[i], taken from one ScratchFrame, and returns its status.
+// The copies are cudaMemcpyAsync on the ctx stream; after a successful call the outputs are copied
+// back and the stream is synchronised, after a failed one nothing is copied back.
+template <typename F>
+int staged(ign_ctx* ctx, std::vector<HostBuf>& bufs, F&& call) {
+  IGN_TRY(activate(ctx));
+  ScratchFrame f(ctx);
+  std::vector<void*> d(bufs.size(), nullptr);
+  for (size_t i = 0; i < bufs.size(); i++) {
+    if (!bufs[i].from && !bufs[i].to) continue;
+    IGN_TRY(f.take(&d[i], bufs[i].bytes));
+    if (bufs[i].from)
+      IGN_CUDA(cudaMemcpyAsync(d[i], bufs[i].from, bufs[i].bytes, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  IGN_TRY(call(d.data()));
+  for (size_t i = 0; i < bufs.size(); i++)
+    if (bufs[i].to) IGN_CUDA(cudaMemcpyAsync(bufs[i].to, d[i], bufs[i].bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
+  return IGN_OK;
+}
+template <typename F>
+int staged(ign_ctx* ctx, std::vector<HostBuf>&& bufs, F&& call) {
+  return staged(ctx, bufs, call);
+}
+
 // Small control transfers (counters, per-label offset tables) that sit between kernels
 // of one call.  cudaMemcpyAsync would put them on a copy engine, where they queue behind
 // multi-GB transfers issued by other contexts of the same device (the volume upload /

@@ -472,24 +472,9 @@ int ign_histogram_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint6
 }
 
 int ign_histogram(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint64_t* hist) {
-  IGN_TRY(activate(ctx));
-  IGN_REQUIRE(dtype == IGN_U8 || dtype == IGN_U16, IGN_ERR_UNSUPPORTED, "histogram: dtype %d is not uint8 / uint16",
-              dtype);
-  IGN_REQUIRE(hist && (in || !n), IGN_ERR_INVALID, "null buffer");
-  const uint64_t bins = dtype == IGN_U8 ? 256 : 65536;
-  ScratchFrame f(ctx);
-  void* din = nullptr;
-  uint64_t* dh;
-  if (n) IGN_TRY(f.take(&din, n * dtype_size(dtype)));
-  IGN_TRY(f.take(&dh, bins));
-  std::vector<uint64_t> got(bins);
-  IGN_CUDA(cudaMemsetAsync(dh, 0, bins * 8, ctx->stream));
-  if (n) IGN_CUDA(cudaMemcpyAsync(din, in, n * dtype_size(dtype), cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_histogram_dev(ctx, din, dtype, n, dh));
-  IGN_CUDA(cudaMemcpyAsync(got.data(), dh, bins * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  for (uint64_t i = 0; i < bins; ++i) hist[i] += got[i];
-  return IGN_OK;
+  const uint64_t bins = dtype == IGN_U8 ? 256 : dtype == IGN_U16 ? 65536 : 0;
+  return staged(ctx, {{in, nullptr, n * dtype_size(dtype)}, {hist, hist, bins * 8}},
+                [&](void* const* d) { return ign_histogram_dev(ctx, d[0], dtype, n, (uint64_t*)d[1]); });
 }
 
 int ign_contrast_stretch_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy, uint64_t sz,
@@ -523,20 +508,13 @@ int ign_contrast_stretch_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64_
 int ign_contrast_stretch(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy, uint64_t sz,
                          uint64_t sc, const uint32_t* lower, const uint32_t* upper, double minval, double maxval,
                          void* out, int out_dtype) {
-  IGN_TRY(activate(ctx));
-  IGN_REQUIRE(in && out && lower && upper, IGN_ERR_INVALID, "null buffer");
   IGN_TRY(stretch_check(in_dtype, out_dtype, sx, sy, sz, minval, maxval));
-  sc = sc ? sc : 1;
-  const uint64_t n = sx * sy * sz * sc;
-  ScratchFrame f(ctx);
-  void *din, *dout;
-  IGN_TRY(f.take(&din, n * dtype_size(in_dtype)));
-  IGN_TRY(f.take(&dout, n * dtype_size(out_dtype)));
-  IGN_CUDA(cudaMemcpyAsync(din, in, n * dtype_size(in_dtype), cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_contrast_stretch_dev(ctx, din, in_dtype, sx, sy, sz, sc, lower, upper, minval, maxval, dout, out_dtype));
-  IGN_CUDA(cudaMemcpyAsync(out, dout, n * dtype_size(out_dtype), cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  return IGN_OK;
+  const uint64_t n = sx * sy * sz * (sc ? sc : 1);
+  return staged(ctx, {{in, nullptr, n * dtype_size(in_dtype)}, {nullptr, out, n * dtype_size(out_dtype)}},
+                [&](void* const* d) {
+                  return ign_contrast_stretch_dev(ctx, d[0], in_dtype, sx, sy, sz, sc, lower, upper, minval, maxval,
+                                                  d[1], out_dtype);
+                });
 }
 
 int ign_quantize_dev(ign_ctx* ctx, const float* in, uint64_t n, uint8_t* out) {
@@ -550,19 +528,8 @@ int ign_quantize_dev(ign_ctx* ctx, const float* in, uint64_t n, uint8_t* out) {
 }
 
 int ign_quantize(ign_ctx* ctx, const float* in, uint64_t n, uint8_t* out) {
-  IGN_TRY(activate(ctx));
-  IGN_REQUIRE((in && out) || !n, IGN_ERR_INVALID, "null buffer");
-  if (!n) return IGN_OK;
-  ScratchFrame f(ctx);
-  float* din;
-  uint8_t* dout;
-  IGN_TRY(f.take(&din, n));
-  IGN_TRY(f.take(&dout, n));
-  IGN_CUDA(cudaMemcpyAsync(din, in, n * 4, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_quantize_dev(ctx, din, n, dout));
-  IGN_CUDA(cudaMemcpyAsync(out, dout, n, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  return IGN_OK;
+  return staged(ctx, {{in, nullptr, n * 4}, {nullptr, out, n}},
+                [&](void* const* d) { return ign_quantize_dev(ctx, (const float*)d[0], n, (uint8_t*)d[1]); });
 }
 
 int ign_clahe_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz, double clip_limit,
@@ -582,19 +549,13 @@ int ign_clahe_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t
 
 int ign_clahe(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz, double clip_limit,
               uint32_t tiles_x, uint32_t tiles_y, void* out) {
-  IGN_TRY(activate(ctx));
+  // one staged buffer serves as in and out, so a null one of the two would not reach ign_clahe_dev
   IGN_REQUIRE(in && out, IGN_ERR_INVALID, "null buffer");
   ClaheGeom g;
   IGN_TRY(clahe_geometry(dtype, sx, sy, tiles_x, tiles_y, clip_limit, &g));
-  const uint64_t bytes = sx * sy * sz * dtype_size(dtype);
-  ScratchFrame f(ctx);
-  void* dbuf;
-  IGN_TRY(f.take(&dbuf, bytes));
-  IGN_CUDA(cudaMemcpyAsync(dbuf, in, bytes, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_clahe_dev(ctx, dbuf, dtype, sx, sy, sz, clip_limit, tiles_x, tiles_y, dbuf));
-  IGN_CUDA(cudaMemcpyAsync(out, dbuf, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  return IGN_OK;
+  return staged(ctx, {{in, out, sx * sy * sz * dtype_size(dtype)}}, [&](void* const* d) {
+    return ign_clahe_dev(ctx, d[0], dtype, sx, sy, sz, clip_limit, tiles_x, tiles_y, d[0]);
+  });
 }
 
 }  // extern "C"

@@ -487,44 +487,25 @@ int ign_cseg_decode_dev(ign_ctx* ctx, const uint32_t* in, uint64_t n_words, int 
 // with a capacity of sc + 2*blocks + 3*voxels words, the worst case)
 int ign_cseg_encode(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz, uint64_t sc,
                     uint32_t bx, uint32_t by, uint32_t bz, uint32_t* out, uint64_t cap_words, uint64_t* n_words) {
-  IGN_TRY(activate(ctx));
-  IGN_REQUIRE(labels && n_words, IGN_ERR_INVALID, "null argument");
-  const int es = dtype_size(dtype);
-  IGN_REQUIRE(dtype == IGN_U32 || dtype == IGN_U64, IGN_ERR_UNSUPPORTED, "compressed_segmentation holds uint32 / uint64 labels");
-  const uint64_t n = sx * sy * sz * sc;
-  CsegDims d;
-  IGN_TRY(cseg_dims(sx, sy, sz, bx, by, bz, &d));
-  ScratchFrame f(ctx);
-  void* d_in;
-  uint32_t* d_out = nullptr;
-  IGN_TRY(f.take(&d_in, n * es));
-  if (out) IGN_TRY(f.take(&d_out, cap_words));
-  IGN_CUDA(cudaMemcpyAsync(d_in, labels, n * es, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_cseg_encode_dev(ctx, d_in, dtype, sx, sy, sz, sc, bx, by, bz, d_out, cap_words, n_words));
-  if (out && *n_words <= cap_words) {
-    IGN_CUDA(cudaMemcpyAsync(out, d_out, *n_words * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  }
-  return IGN_OK;
+  CsegDims dims;
+  IGN_TRY(cseg_dims(sx, sy, sz, bx, by, bz, &dims));
+  std::vector<HostBuf> bufs = {{labels, nullptr, sx * sy * sz * sc * dtype_size(dtype)}, {nullptr, out, cap_words * 4}};
+  return staged(ctx, bufs, [&](void* const* d) -> int {
+    IGN_TRY(ign_cseg_encode_dev(ctx, d[0], dtype, sx, sy, sz, sc, bx, by, bz, (uint32_t*)d[1], cap_words, n_words));
+    bufs[1].bytes = *n_words <= cap_words ? *n_words * 4 : 0;
+    return IGN_OK;
+  });
 }
 
 int ign_cseg_decode(ign_ctx* ctx, const uint32_t* in, uint64_t n_words, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
                     uint64_t sc, uint32_t bx, uint32_t by, uint32_t bz, void* out) {
-  IGN_TRY(activate(ctx));
-  IGN_REQUIRE(in && out, IGN_ERR_INVALID, "null argument");
-  const int es = dtype_size(dtype);
-  IGN_REQUIRE(dtype == IGN_U32 || dtype == IGN_U64, IGN_ERR_UNSUPPORTED, "compressed_segmentation holds uint32 / uint64 labels");
-  const uint64_t n = sx * sy * sz * sc;
-  ScratchFrame f(ctx);
-  uint32_t* d_in;
-  void* d_out;
-  IGN_TRY(f.take(&d_in, n_words));
-  IGN_TRY(f.take(&d_out, n * es));
-  IGN_CUDA(cudaMemcpyAsync(d_in, in, n_words * 4, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_cseg_decode_dev(ctx, d_in, n_words, dtype, sx, sy, sz, sc, bx, by, bz, d_out));
-  IGN_CUDA(cudaMemcpyAsync(out, d_out, n * es, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  return IGN_OK;
+  CsegDims dims;
+  IGN_TRY(cseg_dims(sx, sy, sz, bx, by, bz, &dims));
+  return staged(ctx, {{in, nullptr, n_words * 4}, {nullptr, out, sx * sy * sz * sc * dtype_size(dtype)}},
+                [&](void* const* d) {
+                  return ign_cseg_decode_dev(ctx, (const uint32_t*)d[0], n_words, dtype, sx, sy, sz, sc, bx, by, bz,
+                                             d[1]);
+                });
 }
 
 }  // extern "C"

@@ -495,39 +495,18 @@ int ign_fill_holes_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uin
 
 // ---- host-buffer wrappers
 int ign_dilate_multilabel(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz, void* out) {
-  IGN_TRY(activate(ctx));
-  IGN_REQUIRE(in && out, IGN_ERR_INVALID, "null buffer");
-  const int es = dtype_size(dtype);
-  IGN_REQUIRE(es > 0 && dtype != IGN_F32, IGN_ERR_UNSUPPORTED, "dilate: unsupported dtype %d", dtype);
-  const uint64_t bytes = sx * sy * sz * es;
-  ScratchFrame f(ctx);
-  void *din, *dout;
-  IGN_TRY(f.take(&din, bytes));
-  IGN_TRY(f.take(&dout, bytes));
-  IGN_CUDA(cudaMemcpyAsync(din, in, bytes, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_dilate_multilabel_dev(ctx, din, dtype, sx, sy, sz, dout));
-  IGN_CUDA(cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  return IGN_OK;
+  const uint64_t bytes = sx * sy * sz * dtype_size(dtype);
+  return staged(ctx, {{in, nullptr, bytes}, {nullptr, out, bytes}},
+                [&](void* const* d) { return ign_dilate_multilabel_dev(ctx, d[0], dtype, sx, sy, sz, d[1]); });
 }
 
 int ign_fill_holes(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz, int fix_borders,
                    int merge_threshold_pct, void* filled, void* holes) {
-  IGN_TRY(activate(ctx));
-  IGN_REQUIRE(in && filled && holes, IGN_ERR_INVALID, "null buffer");
   IGN_TRY(fill_check(sx, sy, sz, dtype, merge_threshold_pct));
   const uint64_t bytes = sx * sy * sz * dtype_size(dtype);
-  ScratchFrame f(ctx);
-  void *din, *dfill, *dholes;
-  IGN_TRY(f.take(&din, bytes));
-  IGN_TRY(f.take(&dfill, bytes));
-  IGN_TRY(f.take(&dholes, bytes));
-  IGN_CUDA(cudaMemcpyAsync(din, in, bytes, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_fill_holes_dev(ctx, din, dtype, sx, sy, sz, fix_borders, merge_threshold_pct, dfill, dholes));
-  IGN_CUDA(cudaMemcpyAsync(filled, dfill, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaMemcpyAsync(holes, dholes, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  return IGN_OK;
+  return staged(ctx, {{in, nullptr, bytes}, {nullptr, filled, bytes}, {nullptr, holes, bytes}}, [&](void* const* d) {
+    return ign_fill_holes_dev(ctx, d[0], dtype, sx, sy, sz, fix_borders, merge_threshold_pct, d[1], d[2]);
+  });
 }
 
 }  // extern "C"

@@ -457,24 +457,9 @@ int ign_mesh_begin_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx,
 
 int ign_mesh_begin(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
                    ign_mesher** out) {
-  IGN_TRY(activate(ctx));
-  IGN_REQUIRE(labels && out, IGN_ERR_INVALID, "null argument");
-  const int es = dtype_size(dtype);
-  IGN_REQUIRE(es > 0 && dtype != IGN_F32, IGN_ERR_UNSUPPORTED, "unsupported dtype %d", dtype);
-  const uint64_t n = sx * sy * sz;
-  void* d = nullptr;
-  IGN_TRY(ign_dev_alloc(ctx, n * es, &d));
-  cudaError_t e = cudaMemcpyAsync(d, labels, n * es, cudaMemcpyHostToDevice, ctx->stream);
-  int rc = IGN_OK;
-  if (e != cudaSuccess) {
-    set_error("mesher H2D: %s", cudaGetErrorString(e));
-    rc = IGN_ERR_CUDA;
-  } else {
-    rc = ign_mesh_begin_dev(ctx, d, dtype, sx, sy, sz, out);
-  }
-  cudaStreamSynchronize(ctx->stream);
-  cudaFree(d);
-  return rc;
+  // the mesher keeps no reference to its labels: they can go when the staging frame closes
+  return staged(ctx, {{labels, nullptr, sx * sy * sz * dtype_size(dtype)}},
+                [&](void* const* d) { return ign_mesh_begin_dev(ctx, d[0], dtype, sx, sy, sz, out); });
 }
 
 int ign_mesh_num_ids(ign_mesher* m, uint64_t* n) {

@@ -555,6 +555,27 @@ static int check_pool_args(const void* in, int dtype, uint64_t sx, uint64_t sy, 
   return IGN_OK;
 }
 
+static int check_factors(uint32_t fx, uint32_t fy, uint32_t fz) {
+  IGN_REQUIRE(fx >= 1 && fx <= 2 && fy >= 1 && fy <= 2 && fz >= 1 && fz <= 2, IGN_ERR_UNSUPPORTED,
+              "pooling factors must be 1 or 2 per axis (got %u,%u,%u)", fx, fy, fz);
+  return IGN_OK;
+}
+
+// stages `in` and the num_mips outputs of a pyramid with factors (fx, fy, fz) around call(d_in, d_outs)
+template <typename F>
+static int pool_staged(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz, uint32_t fx,
+                       uint32_t fy, uint32_t fz, int num_mips, void* const* outs, F&& call) {
+  IGN_TRY(check_pool_args(in, dtype, sx, sy, sz, num_mips, outs));
+  const size_t es = dtype_size(dtype);
+  std::vector<HostBuf> bufs = {{in, nullptr, sx * sy * sz * es}};
+  for (int m = 0; m < num_mips; m++) {
+    IGN_REQUIRE(outs[m], IGN_ERR_INVALID, "null buffer");
+    sx = (sx + fx - 1) / fx; sy = (sy + fy - 1) / fy; sz = (sz + fz - 1) / fz;
+    bufs.push_back({nullptr, outs[m], sx * sy * sz * es});
+  }
+  return staged(ctx, bufs, [&](void* const* d) { return call(d[0], d + 1); });
+}
+
 // accumulator wide enough for eight samples
 template <typename T> struct BlockAcc { using type = uint32_t; };
 template <> struct BlockAcc<uint32_t> { using type = uint64_t; };
@@ -639,8 +660,7 @@ int ign_pool_select_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, ui
                         uint32_t fx, uint32_t fy, uint32_t fz, int num_mips, int op, void* const* outs) {
   IGN_TRY(activate(ctx));
   IGN_TRY(check_pool_args(in, dtype, sx, sy, sz, num_mips, outs));
-  IGN_REQUIRE(fx >= 1 && fx <= 2 && fy >= 1 && fy <= 2 && fz >= 1 && fz <= 2, IGN_ERR_UNSUPPORTED,
-              "pooling factors must be 1 or 2 per axis (got %u,%u,%u)", fx, fy, fz);
+  IGN_TRY(check_factors(fx, fy, fz));
   IGN_REQUIRE(op >= 0 && op <= 10, IGN_ERR_INVALID,
               "op must be 0 min, 1 max, 2 striding, 3 mode, 4 sparse mode, 5-7 average or 8-10 sparse average "
               "(floor / half-up / half-even)");
@@ -657,65 +677,24 @@ int ign_pool_select_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, ui
 
 int ign_pool_select(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
                     uint32_t fx, uint32_t fy, uint32_t fz, int num_mips, int op, void* const* outs) {
-  IGN_TRY(activate(ctx));
-  IGN_TRY(check_pool_args(in, dtype, sx, sy, sz, num_mips, outs));
-  IGN_REQUIRE(fx >= 1 && fx <= 2 && fy >= 1 && fy <= 2 && fz >= 1 && fz <= 2, IGN_ERR_UNSUPPORTED,
-              "pooling factors must be 1 or 2 per axis (got %u,%u,%u)", fx, fy, fz);
-  const size_t es = dtype_size(dtype);
-  size_t ob[32];
-  uint64_t x = sx, y = sy, z = sz;
-  for (int m = 0; m < num_mips; m++) {
-    x = (x + fx - 1) / fx; y = (y + fy - 1) / fy; z = (z + fz - 1) / fz;
-    ob[m] = x * y * z * es;
-  }
-  ScratchFrame f(ctx);
-  void* d_in;
-  void* d_out[32];
-  IGN_TRY(f.take(&d_in, sx * sy * sz * es));
-  for (int m = 0; m < num_mips; m++) IGN_TRY(f.take(&d_out[m], ob[m]));
-  IGN_CUDA(cudaMemcpyAsync(d_in, in, sx * sy * sz * es, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_pool_select_dev(ctx, d_in, dtype, sx, sy, sz, fx, fy, fz, num_mips, op, d_out));
-  for (int m = 0; m < num_mips; m++)
-    IGN_CUDA(cudaMemcpyAsync(outs[m], d_out[m], ob[m], cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  return IGN_OK;
-}
-
-static int pool_host(ign_ctx* ctx, bool mode, const void* in, int dtype, uint64_t sx, uint64_t sy,
-                     uint64_t sz, int num_mips, int flag, void* const* outs) {
-  IGN_TRY(activate(ctx));
-  IGN_TRY(check_pool_args(in, dtype, sx, sy, sz, num_mips, outs));
-  const size_t es = dtype_size(dtype);
-  const size_t in_bytes = sx * sy * sz * es;
-  uint64_t x = sx, y = sy;
-  size_t out_bytes[32];
-  for (int m = 0; m < num_mips; m++) {
-    x = (x + 1) >> 1;
-    y = (y + 1) >> 1;
-    out_bytes[m] = x * y * sz * es;
-  }
-  ScratchFrame f(ctx);
-  void* d_in;
-  void* d_out[32];
-  IGN_TRY(f.take(&d_in, in_bytes));
-  for (int m = 0; m < num_mips; m++) IGN_TRY(f.take(&d_out[m], out_bytes[m]));
-  IGN_CUDA(cudaMemcpyAsync(d_in, in, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(mode ? ign_pool_mode_2x2x1_dev(ctx, d_in, dtype, sx, sy, sz, num_mips, flag, d_out)
-               : ign_pool_avg_2x2x1_dev(ctx, d_in, dtype, sx, sy, sz, num_mips, flag, d_out));
-  for (int m = 0; m < num_mips; m++)
-    IGN_CUDA(cudaMemcpyAsync(outs[m], d_out[m], out_bytes[m], cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  return IGN_OK;
+  IGN_TRY(check_factors(fx, fy, fz));
+  return pool_staged(ctx, in, dtype, sx, sy, sz, fx, fy, fz, num_mips, outs, [&](void* d_in, void* const* d_outs) {
+    return ign_pool_select_dev(ctx, d_in, dtype, sx, sy, sz, fx, fy, fz, num_mips, op, d_outs);
+  });
 }
 
 int ign_pool_mode_2x2x1(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy,
                         uint64_t sz, int num_mips, int sparse, void* const* outs) {
-  return pool_host(ctx, true, in, dtype, sx, sy, sz, num_mips, sparse, outs);
+  return pool_staged(ctx, in, dtype, sx, sy, sz, 2, 2, 1, num_mips, outs, [&](void* d_in, void* const* d_outs) {
+    return ign_pool_mode_2x2x1_dev(ctx, d_in, dtype, sx, sy, sz, num_mips, sparse, d_outs);
+  });
 }
 
 int ign_pool_avg_2x2x1(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy,
                        uint64_t sz, int num_mips, int rounding, void* const* outs) {
-  return pool_host(ctx, false, in, dtype, sx, sy, sz, num_mips, rounding, outs);
+  return pool_staged(ctx, in, dtype, sx, sy, sz, 2, 2, 1, num_mips, outs, [&](void* d_in, void* const* d_outs) {
+    return ign_pool_avg_2x2x1_dev(ctx, d_in, dtype, sx, sy, sz, num_mips, rounding, d_outs);
+  });
 }
 
 }  // extern "C"

@@ -10,6 +10,8 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace ign {
@@ -397,29 +399,13 @@ int ign_renumber_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint32
 
 int ign_renumber(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint32_t* out, uint64_t* uniq,
                  uint64_t uniq_capacity, uint64_t* k) {
-  IGN_TRY(activate(ctx));
-  IGN_REQUIRE(in && out && k, IGN_ERR_INVALID, "null argument");
-  *k = 0;
-  if (n == 0) return IGN_OK;
-  const int es = dtype_size(dtype);
-  IGN_REQUIRE(es > 0 && dtype != IGN_F32, IGN_ERR_UNSUPPORTED, "unsupported dtype %d", dtype);
-  IGN_REQUIRE(n < 0xFFFFFFFFull, IGN_ERR_OVERFLOW, "renumber: more than 2^32 elements");
-  ScratchFrame f(ctx);
-  void* d_in;
-  uint32_t* d_out;
-  uint64_t* d_uniq = nullptr;
-  IGN_TRY(f.take(&d_in, n * es));
-  IGN_TRY(f.take(&d_out, n));
-  if (uniq_capacity) IGN_TRY(f.take(&d_uniq, uniq_capacity));
-  IGN_CUDA(cudaMemcpyAsync(d_in, in, n * es, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_renumber_dev(ctx, d_in, dtype, n, d_out, d_uniq, uniq_capacity, k));
-  IGN_CUDA(cudaMemcpyAsync(out, d_out, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  if (uniq && d_uniq) {
-    const uint64_t m = (*k < uniq_capacity) ? *k : uniq_capacity;
-    IGN_CUDA(cudaMemcpyAsync(uniq, d_uniq, m * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  return IGN_OK;
+  std::vector<HostBuf> bufs = {{in, nullptr, n * dtype_size(dtype)}, {nullptr, out, n * 4},
+                               {nullptr, uniq, uniq_capacity * 8}};
+  return staged(ctx, bufs, [&](void* const* d) -> int {
+    IGN_TRY(ign_renumber_dev(ctx, d[0], dtype, n, (uint32_t*)d[1], (uint64_t*)d[2], uniq_capacity, k));
+    bufs[2].bytes = std::min(*k, uniq_capacity) * 8;
+    return IGN_OK;
+  });
 }
 
 // keys/vals are HOST arrays (the table is small); arr is a DEVICE array
@@ -458,70 +444,49 @@ int ign_remap_dev(ign_ctx* ctx, void* arr, int dtype, uint64_t n, const uint64_t
 
 int ign_remap(ign_ctx* ctx, void* arr, int dtype, uint64_t n, const uint64_t* keys,
               const uint64_t* vals, uint64_t n_keys, int preserve_missing) {
-  IGN_TRY(activate(ctx));
-  IGN_REQUIRE(arr, IGN_ERR_INVALID, "null argument");
-  if (n == 0) return IGN_OK;
-  const int es = dtype_size(dtype);
-  IGN_REQUIRE(es > 0 && dtype != IGN_F32, IGN_ERR_UNSUPPORTED, "unsupported dtype %d", dtype);
-  ScratchFrame f(ctx);
-  void* d;
-  IGN_TRY(f.take(&d, n * es));
-  IGN_CUDA(cudaMemcpyAsync(d, arr, n * es, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_TRY(ign_remap_dev(ctx, d, dtype, n, keys, vals, n_keys, preserve_missing));
-  IGN_CUDA(cudaMemcpyAsync(arr, d, n * es, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  return IGN_OK;
+  return staged(ctx, {{arr, arr, n * dtype_size(dtype)}}, [&](void* const* d) {
+    return ign_remap_dev(ctx, d[0], dtype, n, keys, vals, n_keys, preserve_missing);
+  });
 }
 
-int ign_mask(ign_ctx* ctx, void* arr, int dtype, uint64_t n, const uint64_t* labels,
-             uint64_t n_labels, int except, uint64_t value) {
-  IGN_TRY(activate(ctx));
+}  // extern "C"
+
+// Bodies of the host-only entry points below, on device buffers.
+static int mask_body(ign_ctx* ctx, void* arr, int dtype, uint64_t n, const uint64_t* labels, uint64_t n_labels,
+                     int except, uint64_t value) {
   IGN_REQUIRE(arr && (n_labels == 0 || labels), IGN_ERR_INVALID, "null argument");
   if (n == 0) return IGN_OK;
-  const int es = dtype_size(dtype);
-  IGN_REQUIRE(es > 0 && dtype != IGN_F32, IGN_ERR_UNSUPPORTED, "unsupported dtype %d", dtype);
+  IGN_REQUIRE(dtype_size(dtype) > 0 && dtype != IGN_F32, IGN_ERR_UNSUPPORTED, "unsupported dtype %d", dtype);
   const uint32_t cap = pow2_at_least(2 * n_labels + 16);
   ScratchFrame f(ctx);
-  void* d;
-  IGN_TRY(f.take(&d, n * es));
   HashTable t;
   uint32_t* counters;
   IGN_TRY(table_alloc(ctx, f, cap, 0, t, &counters));
-  uint64_t* dk;
-  IGN_TRY(f.take(&dk, n_labels + 1));
-  IGN_CUDA(cudaMemcpyAsync(d, arr, n * es, cudaMemcpyHostToDevice, ctx->stream));
-  if (n_labels) {
-    IGN_CUDA(cudaMemcpyAsync(dk, labels, n_labels * 8, cudaMemcpyHostToDevice, ctx->stream));
-    IGN_LAUNCH(ctx, k_table_build, blocks_for(n_labels, 256), 256, 0, dk, (const uint64_t*)nullptr, n_labels, t, counters);
-  }
-#define RUN_MASK(T, dummy) IGN_LAUNCH(ctx, (k_mask<T>), blocks_for(n, 256), 256, 0, (T*)d, n, t, except, (T)value)
+  if (n_labels)
+    IGN_LAUNCH(ctx, k_table_build, blocks_for(n_labels, 256), 256, 0, labels, (const uint64_t*)nullptr, n_labels, t,
+               counters);
+#define RUN_MASK(T, dummy) IGN_LAUNCH(ctx, (k_mask<T>), blocks_for(n, 256), 256, 0, (T*)arr, n, t, except, (T)value)
   DISPATCH_UINT(dtype, RUN_MASK, 0)
 #undef RUN_MASK
-  IGN_CUDA(cudaMemcpyAsync(arr, d, n * es, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   return IGN_OK;
 }
 
-int ign_unique(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint64_t* uniq, uint64_t* counts,
-               uint64_t capacity, uint64_t* k) {
-  IGN_TRY(activate(ctx));
+// uniq / counts: `capacity` entries, may be NULL
+static int unique_body(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint64_t* uniq, uint64_t* counts,
+                       uint64_t capacity, uint64_t* k) {
   IGN_REQUIRE(in && k, IGN_ERR_INVALID, "null argument");
   *k = 0;
   if (n == 0) return IGN_OK;
-  const int es = dtype_size(dtype);
-  IGN_REQUIRE(es > 0 && dtype != IGN_F32, IGN_ERR_UNSUPPORTED, "unsupported dtype %d", dtype);
+  IGN_REQUIRE(dtype_size(dtype) > 0 && dtype != IGN_F32, IGN_ERR_UNSUPPORTED, "unsupported dtype %d", dtype);
   IGN_REQUIRE(n < 0xFFFFFFFFull, IGN_ERR_OVERFLOW, "unique: more than 2^32 elements");
   uint32_t cap = pow2_at_least(n < (1u << 19) ? 2 * n + 16 : (1u << 20));
   const uint32_t cap_max = pow2_at_least(2 * n + 16);
   while (true) {
     ScratchFrame f(ctx);
-    void* d_in;
-    IGN_TRY(f.take(&d_in, n * es));
     HashTable t;
     uint32_t* counters;
     IGN_TRY(table_alloc(ctx, f, cap, 0, t, &counters));
-    IGN_CUDA(cudaMemcpyAsync(d_in, in, n * es, cudaMemcpyHostToDevice, ctx->stream));
-#define RUN_COUNT(T, dummy) IGN_LAUNCH(ctx, (k_count<T>), blocks_for(n, 256), 256, 0, (const T*)d_in, n, t, counters)
+#define RUN_COUNT(T, dummy) IGN_LAUNCH(ctx, (k_count<T>), blocks_for(n, 256), 256, 0, (const T*)in, n, t, counters)
     DISPATCH_UINT(dtype, RUN_COUNT, 0)
 #undef RUN_COUNT
     uint32_t h[8];
@@ -546,44 +511,36 @@ int ign_unique(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint64_t* un
       IGN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, ck, sk, cv, sv, (int)total, 0, 64, ctx->stream));
       ctx->launches += 2;
       const uint64_t m = total < capacity ? total : capacity;
-      IGN_CUDA(cudaMemcpyAsync(uniq, sk, m * 8, cudaMemcpyDeviceToHost, ctx->stream));
-      if (counts) IGN_CUDA(cudaMemcpyAsync(counts, sv, m * 8, cudaMemcpyDeviceToHost, ctx->stream));
-      IGN_CUDA(cudaStreamSynchronize(ctx->stream));
+      IGN_CUDA(cudaMemcpyAsync(uniq, sk, m * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+      if (counts) IGN_CUDA(cudaMemcpyAsync(counts, sv, m * 8, cudaMemcpyDeviceToDevice, ctx->stream));
     }
     return IGN_OK;
   }
 }
 
-int ign_inverse_component_map(ign_ctx* ctx, const void* parents, const void* components, int dtype,
-                              uint64_t n, uint64_t* pairs, uint64_t* n_pairs) {
-  IGN_TRY(activate(ctx));
+// pairs: `capacity` (parent, component) pairs, may be NULL; *n_pairs = the number of unique pairs
+static int inverse_component_map_body(ign_ctx* ctx, const void* parents, const void* components, int dtype,
+                                      uint64_t n, uint64_t* pairs, uint64_t capacity, uint64_t* n_pairs) {
   IGN_REQUIRE(parents && components && n_pairs, IGN_ERR_INVALID, "null argument");
-  const uint64_t capacity = *n_pairs;
   *n_pairs = 0;
   if (n == 0) return IGN_OK;
-  const int es = dtype_size(dtype);
-  IGN_REQUIRE(es > 0 && dtype != IGN_F32, IGN_ERR_UNSUPPORTED, "unsupported dtype %d", dtype);
+  IGN_REQUIRE(dtype_size(dtype) > 0 && dtype != IGN_F32, IGN_ERR_UNSUPPORTED, "unsupported dtype %d", dtype);
   IGN_REQUIRE(n < 0x7FFFFFFFull, IGN_ERR_OVERFLOW, "inverse_component_map: too many elements");
   size_t scan_bytes = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)n);
   const size_t tmp_bytes = sort_tmp_bytes_u64((uint32_t)n) + scan_bytes;
   ScratchFrame f(ctx);
-  void *dp, *dc, *tmp;
-  uint64_t *p0, *c0, *p1, *c1, *dout;
+  void* tmp;
+  uint64_t *p0, *c0, *p1, *c1;
   uint32_t *flags, *pos;
-  IGN_TRY(f.take(&dp, n * es));
-  IGN_TRY(f.take(&dc, n * es));
   IGN_TRY(f.take(&p0, n));
   IGN_TRY(f.take(&c0, n));
   IGN_TRY(f.take(&p1, n));
   IGN_TRY(f.take(&c1, n));
   IGN_TRY(f.take(&flags, n));
   IGN_TRY(f.take(&pos, n + 1));
-  IGN_TRY(f.take(&dout, 2 * n));
   IGN_TRY(f.take(&tmp, tmp_bytes));
-  IGN_CUDA(cudaMemcpyAsync(dp, parents, n * es, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_CUDA(cudaMemcpyAsync(dc, components, n * es, cudaMemcpyHostToDevice, ctx->stream));
-#define RUN_WIDEN(T, dummy) IGN_LAUNCH(ctx, (k_widen_pairs<T>), blocks_for(n, 256), 256, 0, (const T*)dp, (const T*)dc, n, p0, c0)
+#define RUN_WIDEN(T, dummy) IGN_LAUNCH(ctx, (k_widen_pairs<T>), blocks_for(n, 256), 256, 0, (const T*)parents, (const T*)components, n, p0, c0)
   DISPATCH_UINT(dtype, RUN_WIDEN, 0)
 #undef RUN_WIDEN
   // LSD: stable sort by component, then by parent
@@ -596,18 +553,46 @@ int ign_inverse_component_map(ign_ctx* ctx, const void* parents, const void* com
   tb = tmp_bytes;
   IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, flags, pos, (int)n, ctx->stream));
   ctx->launches += 1;
-  IGN_LAUNCH(ctx, k_pair_scatter, blocks_for(n, 256), 256, 0, p0, c0, flags, pos, n, dout, capacity);
+  IGN_LAUNCH(ctx, k_pair_scatter, blocks_for(n, 256), 256, 0, p0, c0, flags, pos, n, pairs, pairs ? capacity : 0);
   uint32_t last[2];
   IGN_CUDA(cudaMemcpyAsync(&last[0], pos + (n - 1), 4, cudaMemcpyDeviceToHost, ctx->stream));
   IGN_CUDA(cudaMemcpyAsync(&last[1], flags + (n - 1), 4, cudaMemcpyDeviceToHost, ctx->stream));
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  const uint64_t total = (uint64_t)last[0] + last[1];
-  *n_pairs = total;
-  if (pairs) {
-    const uint64_t m = total < capacity ? total : capacity;
-    IGN_CUDA(cudaMemcpy(pairs, dout, m * 16, cudaMemcpyDeviceToHost));
-  }
+  *n_pairs = (uint64_t)last[0] + last[1];
   return IGN_OK;
+}
+
+extern "C" {
+
+int ign_mask(ign_ctx* ctx, void* arr, int dtype, uint64_t n, const uint64_t* labels,
+             uint64_t n_labels, int except, uint64_t value) {
+  return staged(ctx, {{arr, arr, n * dtype_size(dtype)}, {labels, nullptr, n_labels * 8}}, [&](void* const* d) {
+    return mask_body(ctx, d[0], dtype, n, (const uint64_t*)d[1], n_labels, except, value);
+  });
+}
+
+int ign_unique(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint64_t* uniq, uint64_t* counts,
+               uint64_t capacity, uint64_t* k) {
+  std::vector<HostBuf> bufs = {{in, nullptr, n * dtype_size(dtype)}, {nullptr, uniq, capacity * 8},
+                               {nullptr, uniq ? counts : nullptr, capacity * 8}};  // counts come only with uniq
+  return staged(ctx, bufs, [&](void* const* d) -> int {
+    IGN_TRY(unique_body(ctx, d[0], dtype, n, (uint64_t*)d[1], (uint64_t*)d[2], capacity, k));
+    bufs[1].bytes = bufs[2].bytes = std::min(*k, capacity) * 8;
+    return IGN_OK;
+  });
+}
+
+// capacity in *n_pairs on entry
+int ign_inverse_component_map(ign_ctx* ctx, const void* parents, const void* components, int dtype,
+                              uint64_t n, uint64_t* pairs, uint64_t* n_pairs) {
+  const uint64_t capacity = n_pairs ? *n_pairs : 0;
+  const uint64_t bytes = n * dtype_size(dtype);
+  std::vector<HostBuf> bufs = {{parents, nullptr, bytes}, {components, nullptr, bytes}, {nullptr, pairs, capacity * 16}};
+  return staged(ctx, bufs, [&](void* const* d) -> int {
+    IGN_TRY(inverse_component_map_body(ctx, d[0], d[1], dtype, n, (uint64_t*)d[2], capacity, n_pairs));
+    bufs[2].bytes = std::min(*n_pairs, capacity) * 16;
+    return IGN_OK;
+  });
 }
 
 }  // extern "C"

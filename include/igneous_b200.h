@@ -200,6 +200,10 @@ IGN_API int ign_dust_dev(ign_ctx* ctx, void* labels, int dtype, uint64_t sx, uin
 /* Fused CCLFacesTask body (igneous/tasks/image/ccl.py:166-175): optional
  * threshold (use_lte/use_gte), blackout_non_face_rails(shape), CCL,
  * += label_offset, background re-zeroed; out is u64. */
+IGN_API int ign_ccl_task(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy,
+                         uint64_t sz, int use_gte, double gte, int use_lte, double lte,
+                         uint64_t rail_x, uint64_t rail_y, uint64_t rail_z, uint64_t dust_threshold,
+                         uint64_t label_offset, uint64_t* out, uint64_t* n_components);
 IGN_API int ign_ccl_task_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy,
                      uint64_t sz, int use_gte, double gte, int use_lte, double lte,
                      uint64_t rail_x, uint64_t rail_y, uint64_t rail_z, uint64_t dust_threshold,
