@@ -1142,6 +1142,14 @@ static Reader<T, false> plain_reader(const void* in) {
   return r;
 }
 
+// labels 1..max_label must be representable in out_dtype
+static int check_labels_fit(int out_dtype, uint64_t max_label) {
+  if (out_dtype == IGN_U16)
+    IGN_REQUIRE(max_label <= 0xFFFFull, IGN_ERR_OVERFLOW, "%llu labels do not fit uint16", (unsigned long long)max_label);
+  if (out_dtype == IGN_U32) IGN_REQUIRE(max_label <= 0xFFFFFFFFull, IGN_ERR_OVERFLOW, "labels do not fit uint32");
+  return IGN_OK;
+}
+
 static int launch_expand(ign_ctx* ctx, const CclPlan& p, uint64_t offset, void* out, int out_dtype,
                          uint64_t max_label) {
   const ExpandArgs e = p.expand_args(offset);
@@ -1150,14 +1158,13 @@ static int launch_expand(ign_ctx* ctx, const CclPlan& p, uint64_t offset, void* 
   const uint64_t warps = vec ? e.rows * (((p.wpr + 3) / 4 + EX_G - 1) / EX_G) : (e.rows * p.wpr + EX_G - 1) / EX_G;
   IGN_REQUIRE(warps * 32 / 256 < 0x7FFFFFFFull, IGN_ERR_OVERFLOW, "CCL expand grid too large");
   const unsigned grid = blocks_for(warps * 32, 256);
+  IGN_TRY(check_labels_fit(out_dtype, max_label + offset));
   switch (out_dtype) {
     case IGN_U16:
-      IGN_REQUIRE(max_label + offset <= 0xFFFFull, IGN_ERR_OVERFLOW, "%llu labels do not fit uint16", (unsigned long long)max_label);
       if (vec) IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_LABEL, (k_ccl_expand4<uint16_t>), grid, 256, 0, e, (uint16_t*)out);
       else IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_LABEL, (k_ccl_expand1<uint16_t>), grid, 256, 0, e, (uint16_t*)out);
       break;
     case IGN_U32:
-      IGN_REQUIRE(max_label + offset <= 0xFFFFFFFFull, IGN_ERR_OVERFLOW, "labels do not fit uint32");
       if (vec) IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_LABEL, (k_ccl_expand4<uint32_t>), grid, 256, 0, e, (uint32_t*)out);
       else IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_LABEL, (k_ccl_expand1<uint32_t>), grid, 256, 0, e, (uint32_t*)out);
       break;
@@ -1359,45 +1366,42 @@ static int grow(char** buf, size_t* have, size_t need) {
   return IGN_OK;
 }
 
-// One rank's share of a CCL over a dataset that is split into z-slabs (rank r above rank r-1).
-// Exactly ONE collective: an all-gather of [n_local | first plane | last plane]; linking the
-// N-1 boundaries, the replicated union-find and the relabelling all run on the device.
-template <typename T>
-static int ccl_sharded_typed(ign_group* g, ign_ccl_volume* v, uint64_t sx, uint64_t sy, uint64_t sz, void* out,
-                             int out_dtype, uint64_t* n_global) {
-  ign_ctx* ctx = g->ctx;
-  const int N = g->nranks, me = g->rank;
-  const uint64_t np = sx * sy;
-  const size_t rec = 256 + 2 * np * 8 + 2 * np * 4;
-  IGN_TRY(grow(&g->d_send, &g->send_bytes, rec));
-  IGN_TRY(grow(&g->d_recv, &g->recv_bytes, rec * (size_t)N));
-  uint64_t* first_v = (uint64_t*)(g->d_send + 256);
-  uint64_t* last_v = first_v + np;
-  uint32_t* first_l = (uint32_t*)(last_v + np);
-  uint32_t* last_l = first_l + np;
-  IGN_TRY(volume_begin_typed<T>(ctx, v, sx, sy, sz, first_v, first_l, last_v, last_l));
+// The post-gather half of a CCL over a dataset split into z-slabs (rank r above rank r-1): `rec_base`
+// holds every rank's plane record (multigpu.plane_record_bytes).  Linking the N-1 boundaries, the
+// dataset-wide union-find and the relabelling all run on the device; only the component counts and
+// the global count come back to the host.
+static int volume_finish_gathered(ign_ccl_volume* v, const char* rec_base, int N, int me, void* out, int out_dtype,
+                                  uint64_t* n_global) {
+  ign_ctx* ctx = v->ctx;
   CclPlan& p = v->plan;
-  uint64_t head[32] = {0};
-  head[0] = v->n_local;
-  IGN_TRY(small_h2d(ctx, g->d_send, head, 256));
-  IGN_TRY(ign_group_allgather(g, g->d_send, rec, g->d_recv));
+  IGN_REQUIRE(rec_base && out, IGN_ERR_INVALID, "null argument");
+  IGN_REQUIRE(N >= 1 && me >= 0 && me < N, IGN_ERR_INVALID, "rank %d of %d ranks", me, N);
+  IGN_REQUIRE(out_dtype == IGN_U16 || out_dtype == IGN_U32 || out_dtype == IGN_U64, IGN_ERR_UNSUPPORTED,
+              "CCL out_dtype must be u16/u32/u64 (got %d)", out_dtype);
+  const uint64_t sx = p.sx, sy = p.sy, sz = p.sz, np = sx * sy;
+  const size_t rec = 256 + 2 * np * 8 + 2 * np * 4;
   std::vector<uint64_t> nloc(N, 0);
-  for (int r = 0; r < N; r++) IGN_TRY(small_d2h(ctx, &nloc[r], g->d_recv + (size_t)r * rec, 8));
+  for (int r = 0; r < N; r++) IGN_TRY(small_d2h(ctx, &nloc[r], rec_base + (size_t)r * rec, 8));
   IGN_TRY(small_sync(ctx));
+  IGN_REQUIRE(nloc[me] == v->n_local, IGN_ERR_INVALID,
+              "plane record %d holds %llu components but the volume has %llu (wrong rank?)", me,
+              (unsigned long long)nloc[me], (unsigned long long)v->n_local);
   std::vector<uint64_t> off(N + 1, 0);
   for (int r = 0; r < N; r++) off[r + 1] = off[r] + nloc[r];
   const uint64_t total = off[N];
   IGN_REQUIRE(total < 0x7FFFFFF0ull, IGN_ERR_OVERFLOW, "multi-GPU CCL: too many provisional components");
   const uint32_t items = (uint32_t)total + 2;  // ids 0..total and one sentinel
   const size_t cubb = ccl_cub_bytes(items);
-  IGN_TRY(grow(&g->d_solve, &g->solve_bytes, 2 * align_up((size_t)items * 4, 256) + align_up(cubb, 256)));
-  uint32_t* parent = (uint32_t*)g->d_solve;
-  uint32_t* rank = (uint32_t*)(g->d_solve + align_up((size_t)items * 4, 256));
-  void* tmp = g->d_solve + 2 * align_up((size_t)items * 4, 256);
+  ScratchFrame f(ctx);
+  uint32_t *parent, *rank;
+  void* tmp;
+  IGN_TRY(f.take(&parent, items));
+  IGN_TRY(f.take(&rank, items));
+  IGN_TRY(f.take(&tmp, cubb));
   IGN_LAUNCH(ctx, k_iota_u32, blocks_for(items, 256), 256, 0, parent, items);
   for (int b = 0; b + 1 < N; b++) {
-    const char* ra = g->d_recv + (size_t)b * rec;
-    const char* rb = g->d_recv + (size_t)(b + 1) * rec;
+    const char* ra = rec_base + (size_t)b * rec;
+    const char* rb = rec_base + (size_t)(b + 1) * rec;
     const uint64_t* va = (const uint64_t*)(ra + 256) + np;                     // last plane of rank b
     const uint32_t* la = (const uint32_t*)(ra + 256 + 2 * np * 8) + np;
     const uint64_t* vb = (const uint64_t*)(rb + 256);                          // first plane of rank b+1
@@ -1419,15 +1423,19 @@ static int ccl_sharded_typed(ign_group* g, ign_ccl_volume* v, uint64_t sx, uint6
   uint32_t hN = 0;
   IGN_TRY(small_d2h(ctx, &hN, rank + (items - 1), 4));  // roots incl. id 0
   IGN_LAUNCH(ctx, k_ccl_rank_of_root, blocks_for(items - 1, 256), 256, 0, parent, rank, items - 1);
-  const uint64_t nglob_max = total;
+  // the output type must hold the global count, not the sum of the slabs' counts: a component
+  // that crosses k boundaries is counted k+1 times in `total`
+  IGN_TRY(small_sync(ctx));
+  const uint64_t nglob = hN ? hN - 1 : 0;
+  IGN_TRY(check_labels_fit(out_dtype, nglob));
   if (p.R > 0) {
     IGN_LAUNCH(ctx, k_ccl_relabel_runs, blocks_for(p.R, 256), 256, 0, p.label, p.R, (const uint32_t*)parent + off[me]);
-    IGN_TRY(launch_expand(ctx, p, 0, out, out_dtype, nglob_max));
+    IGN_TRY(launch_expand(ctx, p, 0, out, out_dtype, nglob));
   } else {
     IGN_CUDA(cudaMemsetAsync(out, 0, sx * sy * sz * dtype_size(out_dtype), ctx->stream));
   }
   IGN_TRY(small_sync(ctx));
-  if (n_global) *n_global = hN ? hN - 1 : 0;
+  if (n_global) *n_global = nglob;
   return IGN_OK;
 }
 
@@ -1644,6 +1652,16 @@ int ign_ccl6_volume_finish_dev(ign_ccl_volume* v, const uint32_t* global_lut, ui
   return rc;
 }
 
+int ign_ccl6_volume_finish_gathered_dev(ign_ccl_volume* v, const void* records_dev, int nranks, int rank,
+                                        void* out, int out_dtype, uint64_t* n_global) {
+  IGN_REQUIRE(v, IGN_ERR_INVALID, "null volume");
+  IGN_TRY(activate(v->ctx));
+  IGN_REQUIRE(v->frame.innermost(), IGN_ERR_INVALID, "CCL volumes of one context must end in reverse order of begin");
+  const int rc = volume_finish_gathered(v, (const char*)records_dev, nranks, rank, out, out_dtype, n_global);
+  delete v;
+  return rc;
+}
+
 int ign_ccl6_volume_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy,
                         uint64_t sz, void* out, int out_dtype, uint64_t* n_components) {
   IGN_REQUIRE(in && out, IGN_ERR_INVALID, "null buffer");
@@ -1663,15 +1681,25 @@ int ign_ccl6_sharded_dev(ign_group* g, const void* in, int in_dtype, uint64_t sx
   IGN_TRY(activate(ctx));
   IGN_TRY(check_ccl_dims(sx, sy, sz));
   IGN_REQUIRE(dtype_size(out_dtype) > 0, IGN_ERR_UNSUPPORTED, "unsupported out dtype");
-  ign_ccl_volume v(ctx, in, in_dtype);
-  switch (in_dtype) {
-    case IGN_U8: return ccl_sharded_typed<uint8_t>(g, &v, sx, sy, sz, out, out_dtype, n_global);
-    case IGN_U16: return ccl_sharded_typed<uint16_t>(g, &v, sx, sy, sz, out, out_dtype, n_global);
-    case IGN_U32: return ccl_sharded_typed<uint32_t>(g, &v, sx, sy, sz, out, out_dtype, n_global);
-    case IGN_U64: return ccl_sharded_typed<uint64_t>(g, &v, sx, sy, sz, out, out_dtype, n_global);
+  // exactly ONE collective: an all-gather of every rank's [n_local | first plane | last plane]
+  const uint64_t np = sx * sy;
+  const size_t rec = 256 + 2 * np * 8 + 2 * np * 4;
+  IGN_TRY(grow(&g->d_send, &g->send_bytes, rec));
+  IGN_TRY(grow(&g->d_recv, &g->recv_bytes, rec * (size_t)g->nranks));
+  uint64_t* first_v = (uint64_t*)(g->d_send + 256);
+  uint64_t* last_v = first_v + np;
+  uint32_t* first_l = (uint32_t*)(last_v + np);
+  uint32_t* last_l = first_l + np;
+  ign_ccl_volume* v = nullptr;
+  uint64_t head[32] = {0};
+  IGN_TRY(ign_ccl6_volume_begin_dev(ctx, in, in_dtype, sx, sy, sz, first_v, first_l, last_v, last_l, &v, &head[0]));
+  int rc = small_h2d(ctx, g->d_send, head, 256);
+  if (rc == IGN_OK) rc = ign_group_allgather(g, g->d_send, rec, g->d_recv);
+  if (rc != IGN_OK) {
+    ign_ccl6_volume_abort(v);
+    return rc;
   }
-  set_error("sharded CCL: unsupported input dtype %d", in_dtype);
-  return IGN_ERR_UNSUPPORTED;
+  return ign_ccl6_volume_finish_gathered_dev(v, g->d_recv, g->nranks, g->rank, out, out_dtype, n_global);
 }
 
 }  // extern "C"

@@ -83,8 +83,8 @@ int ign_group_init(ign_ctx* ctx, int rank, int nranks, const void* id128, ign_gr
   g->ctx = ctx;
   g->rank = rank;
   g->nranks = nranks;
-  g->d_send = g->d_recv = g->d_solve = nullptr;
-  g->send_bytes = g->recv_bytes = g->solve_bytes = 0;
+  g->d_send = g->d_recv = nullptr;
+  g->send_bytes = g->recv_bytes = 0;
   const int rc = g_nccl.init_rank((nccl_comm_t*)&g->comm, nranks, uid, rank);
   if (rc != 0) {
     delete g;
@@ -100,7 +100,6 @@ int ign_group_destroy(ign_group* g) {
   cudaSetDevice(g->ctx->device);
   if (g->d_send) cudaFree(g->d_send);
   if (g->d_recv) cudaFree(g->d_recv);
-  if (g->d_solve) cudaFree(g->d_solve);
   delete g;
   return IGN_OK;
 }

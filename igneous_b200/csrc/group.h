@@ -6,7 +6,7 @@ struct ign_group {
   ign_ctx* ctx;
   void* comm;  // ncclComm_t
   int rank, nranks;
-  // grow-only device buffers of ign_ccl6_sharded_dev (boundary plane records, replicated solve)
-  char *d_send, *d_recv, *d_solve;
-  size_t send_bytes, recv_bytes, solve_bytes;
+  // grow-only device buffers of ign_ccl6_sharded_dev: this rank's plane record, every rank's records
+  char *d_send, *d_recv;
+  size_t send_bytes, recv_bytes;
 };

@@ -149,6 +149,8 @@ IGN_API int ign_pool_select_dev(ign_ctx* ctx, const void* in, int dtype, uint64_
  * Output ids 1..N in order of each component's first voxel in Fortran raster
  * order.  in_dtype U8 also serves bool input (threshold_image output).
  * out_dtype: IGN_U16 / IGN_U32 / IGN_U64 (overflow -> IGN_ERR_OVERFLOW).
+ * Rows of up to 131,072 voxels (sx); longer rows -> IGN_ERR_OVERFLOW before any launch.  Rows
+ * past 2048 voxels resolve in flatter tiles (tests/test_ccl_long_rows_gpu.py covers each height).
  */
 IGN_API int ign_ccl6(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy, uint64_t sz,
              void* out, int out_dtype, uint64_t* n_components);
@@ -188,6 +190,25 @@ IGN_API int ign_ccl6_volume_begin_dev(ign_ctx* ctx, const void* in, int in_dtype
 IGN_API int ign_ccl6_volume_finish_dev(ign_ccl_volume* v, const uint32_t* global_lut,
                                        uint64_t max_label, void* out, int out_dtype);
 IGN_API int ign_ccl6_volume_abort(ign_ccl_volume* v);
+/* The device-side finish of ign_ccl6_sharded_dev, for a volume from ign_ccl6_volume_begin_dev
+ * that is slab `rank` of `nranks` z-slabs (slab r above slab r-1).  records_dev holds nranks
+ * plane records of np = sx*sy entries each, back to back (record r at byte
+ * r * (256 + 24*np), igneous_b200.multigpu.plane_record_bytes):
+ *   bytes [0, 256)             header; u64 word 0 = n_local of slab r, the rest unused
+ *   u64  first_values[np]      slab r's first z-plane, as begin writes it
+ *   u64  last_values[np]       slab r's last z-plane
+ *   u32  first_labels[np]
+ *   u32  last_labels[np]
+ * Links the nranks-1 boundaries, solves the dataset-wide union-find on the device (smaller id
+ * wins), relabels the slab and expands it once into out; *n_global (may be NULL) = the
+ * dataset's component count, the same on every rank.  Stitched together, the slabs' outputs are
+ * bit-identical to one whole-volume ign_ccl6 call.  Consumes the volume, also on failure, except
+ * when v is NULL or when volumes of the context are not ended in reverse order of begin.
+ * IGN_ERR_INVALID: nranks < 1, rank outside [0, nranks), NULL records_dev or out, or record
+ * `rank` whose n_local differs from the volume's.  IGN_ERR_OVERFLOW: the global count does not
+ * fit out_dtype. */
+IGN_API int ign_ccl6_volume_finish_gathered_dev(ign_ccl_volume* v, const void* records_dev, int nranks,
+                                                int rank, void* out, int out_dtype, uint64_t* n_global);
 
 /* cc3d.dust(labels, threshold, connectivity=6, in_place=True)
  *   igneous/tasks/image/ccl.py:169-172, :231-234, :335-338
@@ -391,7 +412,9 @@ IGN_API int ign_group_allgather(ign_group* g, const void* send_dev, uint64_t byt
  * then -- on the device, identically on every rank -- the N-1 boundaries are linked, the small
  * dataset-wide union-find is solved (smaller id wins, ccl.py:70-73) and the slab's labels are
  * expanded once with dataset-wide ids.  Bit-identical to one whole-volume ign_ccl6 call on the
- * stacked dataset.  Replaces ccl.py:177-194, :245-294, :358-420, :296-356. */
+ * stacked dataset.  Replaces ccl.py:177-194, :245-294, :358-420, :296-356.
+ * It is ign_ccl6_volume_begin_dev + the all-gather + ign_ccl6_volume_finish_gathered_dev, so the
+ * merge is tested on one device by emulating the ranks (tests/test_ccl_multirank_gpu.py). */
 IGN_API int ign_ccl6_sharded_dev(ign_group* g, const void* in, int in_dtype, uint64_t sx, uint64_t sy,
                                  uint64_t sz, void* out, int out_dtype, uint64_t* n_global);
 

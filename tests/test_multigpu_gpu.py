@@ -1,7 +1,8 @@
 """Sharded CCL through NCCL against a whole-volume oracle CCL: two ranks on two GPUs.  NCCL does
 not put two ranks of one communicator on the same device, so a one-GPU machine runs the same path
 with a single rank (communicator set-up, the all-gather, the replicated union-find and the
-relabelling); the linking of two ranks is also covered by tests/test_multigpu_cpu.py over gloo."""
+relabelling); the linking of two to eight ranks runs on one device in tests/test_ccl_multirank_gpu.py,
+through the same ign_ccl6_volume_finish_gathered_dev, and over gloo in tests/test_multigpu_cpu.py."""
 import os
 import subprocess
 import sys
