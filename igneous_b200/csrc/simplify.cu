@@ -272,10 +272,11 @@ constexpr int SL_CLASS_THREADS[SL_NCLASS] = {1024, 512, 256};
 
 // dynamic shared-memory layout of a label at `threads` threads:
 // cost queues | ring lists | key1 | faces SoA | face list | face state | vertex flags | lose marks
+// [| original face ids | original vertex ids: a label resumed in a smaller class after migrating]
 struct SlLayout {
-  size_t wq, o_key, o_f0, o_fl, o_fs, o_vf, o_vl, need;
+  size_t wq, o_key, o_f0, o_fl, o_fs, o_vf, o_vl, o_fm, o_vm, need;
 };
-__host__ __device__ inline SlLayout sl_layout(uint32_t T, uint32_t U, uint32_t threads) {
+__host__ __device__ inline SlLayout sl_layout(uint32_t T, uint32_t U, uint32_t threads, bool resumed = false) {
   SlLayout y;
   y.wq = (size_t)(threads / 32) * SL_EQ * 4;
   y.o_key = y.wq + (size_t)SL_WCAP * 2 * S_MAXV * 2;  // shared-memory class: 16-bit face ids in the rings
@@ -284,13 +285,16 @@ __host__ __device__ inline SlLayout sl_layout(uint32_t T, uint32_t U, uint32_t t
   y.o_fs = y.o_fl + 2 * (size_t)T;
   y.o_vf = (y.o_fs + T + 3) & ~(size_t)3;
   y.o_vl = (y.o_vf + U + 3) & ~(size_t)3;
-  y.need = y.o_vl + U + 4;
+  y.o_fm = (y.o_vl + U + 3) & ~(size_t)3;
+  y.o_vm = y.o_fm + 2 * (size_t)T;
+  y.need = resumed ? y.o_vm + 2 * (size_t)U + 4 : y.o_vl + U + 4;
   return y;
 }
 // the shared-memory class also needs 16-bit keys and lists that a compaction holds in registers
-__host__ __device__ inline bool sl_fits_smem(uint32_t T, uint32_t U, uint32_t threads, size_t smem_bytes) {
+__host__ __device__ inline bool sl_fits_smem(uint32_t T, uint32_t U, uint32_t threads, size_t smem_bytes,
+                                             bool resumed = false) {
   const uint32_t cap = (uint32_t)SL_LIST_PER * threads;
-  return 3ull * T <= 65536ull && T <= cap && U <= cap && sl_layout(T, U, threads).need <= smem_bytes;
+  return 3ull * T <= 65536ull && T <= cap && U <= cap && sl_layout(T, U, threads, resumed).need <= smem_bytes;
 }
 
 struct SlArgs {
@@ -317,12 +321,23 @@ struct SlArgs {
   uint32_t cls;        // size class of the launch
   uint32_t* counters;  // [1] max rounds  [2] labels run in shared memory  [3] in global memory
                        // [4 + class] next work item  [8 + class] labels run in the class
+                       // [16 + class] labels migrated into the class  [20 + class] next migrated label to resume
   double max_err2;
   int max_rounds;
   uint32_t smem_bytes;  // dynamic shared memory of the launch
+  // migration into the next smaller class (shared-memory labels only).  A migrated label's state goes to
+  // its own slices of the global-memory class's arrays, which shared-memory labels do not use otherwise:
+  // flist[tbase + i] = vertices 0 | 1 << 16 and flist2[tbase + i] = vertex 2 | original face << 16 of
+  // alive face i, fstate[tbase + i] its state; vlist[vbase + j] = original vertex | flags << 16 of alive
+  // vertex j (in vertex order); finv[tbase + original face] = i.  The header goes to a queue of the class.
+  uint32_t* mq_next;     // [labels][SL_MREC] headers of labels migrating out of this launch (null: no migration)
+  uint32_t smem_next;    // dynamic shared memory of the next smaller class
+  const uint32_t* mq;    // resume launches: headers of the labels migrated into the class
+  uint16_t* finv;        // [T] compacted face of an original face (read when a resumed label decodes a key)
   int persist;          // 1: a CTA keeps taking labels until the list is empty (IGN_SIMP_PERSIST=1)
-  uint32_t* lrec;       // IGN_SIMP_TRACE=1: [base + work item][6] = faces, rounds, kilocycles, face visits
-                        // (sum of list lengths), winners, memory class | size class << 2
+  uint32_t* lrec;       // IGN_SIMP_TRACE=1: [base + work item][SL_LREC] = faces, rounds, kilocycles, face visits
+                        // (sum of list lengths), winners, memory class | size class << 2, SM kilocycles
+                        // (kilocycles / CTAs per SM); a migrated label sums its segments
   uint32_t* trace;      // IGN_SIMP_TRACE=1: [round][4] = winners, collapses, alive faces, list length of the largest label
 };
 
@@ -330,8 +345,13 @@ struct SlWin {
   uint32_t u, v, h, cnt[2], keep, flags, pad;
 };
 
+// header of a migrated label: dense label, trace record, next round, slow rounds, alive faces, alive vertices
+constexpr int SL_MREC = 8;
+constexpr int SL_LREC = 7;  // words of a label's IGN_SIMP_TRACE record (SlArgs::lrec)
+
 struct SlShared {
   uint32_t work, alive, progress, ncol, nwin, stop, slow, counter, nbig;
+  uint32_t rec, valive;  // trace record of the label; alive vertices (one dies per collapse)
   unsigned long long visits, wins;  // IGN_SIMP_TRACE
   long long t_label;
   unsigned long long ph[10];  // phase timers (IGN_SIMP_TRACE)
@@ -343,8 +363,9 @@ struct SlShared {
 template <bool SM>
 struct SlLab {
   typedef typename std::conditional<SM, uint16_t, uint32_t>::type idx_t;
-  uint32_t T, U, tbase, vbase, target;
+  uint32_t T, U, tbase, vbase, target, label;
   idx_t *fc0, *fc1, *fc2;  // SM: label-local ids, SoA in shared memory
+  idx_t *fmap, *vmap;      // resumed labels: original label-local face / vertex id of each compacted one
   uint32_t* gface;         // !SM: AoS global ids in place
   uint8_t* fstate;         // bit 7 alive, bits 2c..2c+1 memo of half-edge c
   uint8_t* vflag;
@@ -375,6 +396,16 @@ __device__ __forceinline__ void sl_fset(const SlLab<SM>& L, uint32_t f, int c, u
   } else {
     L.gface[3 * (uint64_t)f + c] = x + L.vbase;
   }
+}
+// task-wide index of a label-local vertex (positions and quadrics) and label-local id of a face (keys,
+// cached costs): a resumed label maps its compacted ids back to the original ones
+template <bool SM, bool R>
+__device__ __forceinline__ uint64_t sl_vg(const SlLab<SM>& L, uint32_t v) {
+  return L.vbase + (uint64_t)(R ? (uint32_t)L.vmap[v] : v);
+}
+template <bool SM, bool R>
+__device__ __forceinline__ uint32_t sl_fo(const SlLab<SM>& L, uint32_t f) {
+  return R ? (uint32_t)L.fmap[f] : f;
 }
 // flag bytes are modified with word atomics whenever two threads may touch the same word
 // (SM: the flags are in shared memory for sure -> shared-space reductions instead of generic atomics)
@@ -423,18 +454,19 @@ __device__ __forceinline__ uint32_t sl_key_edge(const SlLab<SM>& L, typename SlL
 }
 
 // s_cost on label-local ids (same arithmetic, same order)
-template <bool SM>
+template <bool SM, bool R>
 __device__ __forceinline__ void sl_cost(const SlArgs& A, const SlLab<SM>& L, uint32_t u, uint32_t v, SEval* e) {
   e->valid = false;
   const bool bu = L.vflag[u] & VF_BOUND, bv = L.vflag[v] & VF_BOUND;
   if (bu && bv) return;
-  const double* Qu = A.Q + 10 * (uint64_t)(L.vbase + u);
-  const double* Qv = A.Q + 10 * (uint64_t)(L.vbase + v);
+  const uint64_t gu = sl_vg<SM, R>(L, u), gv = sl_vg<SM, R>(L, v);
+  const double* Qu = A.Q + 10 * gu;
+  const double* Qv = A.Q + 10 * gv;
   double q[10];
 #pragma unroll
   for (int i = 0; i < 10; i++) q[i] = Qu[i] + Qv[i];
-  const double* pu = A.pos + 3 * (uint64_t)(L.vbase + u);
-  const double* pv = A.pos + 3 * (uint64_t)(L.vbase + v);
+  const double* pu = A.pos + 3 * gu;
+  const double* pv = A.pos + 3 * gv;
   double best[3], cost;
   if (bu) {
     e->keep = u;
@@ -467,13 +499,13 @@ __device__ __forceinline__ void sl_cost(const SlArgs& A, const SlLab<SM>& L, uin
 }
 
 // does face (a0,a1,a2) flip when vertex w moves to `best`?  (the validation's flip test)
-template <bool SM>
+template <bool SM, bool R>
 __device__ __forceinline__ bool sl_flips(const SlArgs& A, const SlLab<SM>& L, const uint32_t* a, uint32_t w,
                                          const double* best) {
   double P[3][3], N[3][3];
 #pragma unroll
   for (int k = 0; k < 3; k++) {
-    const double* p = A.pos + 3 * (uint64_t)(L.vbase + a[k]);
+    const double* p = A.pos + 3 * sl_vg<SM, R>(L, a[k]);
     P[k][0] = p[0]; P[k][1] = p[1]; P[k][2] = p[2];
   }
 #pragma unroll
@@ -589,7 +621,7 @@ __device__ __forceinline__ uint32_t sl_compact(IDX*& list, IDX*& list2, uint32_t
 // One pass of E2c with groups of W lanes (16: two winners per warp side by side, only winners whose
 // rings fit 16 lanes; 32: the winners left over).  Both halves of a warp run the same instructions;
 // everything that differs between them is predicated and loop counts are made warp uniform.
-template <bool SM, int W>
+template <bool SM, bool R, int W>
 __device__ __forceinline__ void sl_collapse_pass(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, uint32_t nb) {
   const uint32_t FULL = 0xFFFFFFFFu;
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5, NW = blockDim.x >> 5;
@@ -621,8 +653,9 @@ __device__ __forceinline__ void sl_collapse_pass(const SlArgs& A, const SlLab<SM
     const uint32_t rm = (k == u) ? v : u;
     // the quadrics of the two endpoints are needed only if the collapse happens, but the L2 round
     // trip is as long as the whole link test: request them now
-    double* Qk = A.Q + 10 * (uint64_t)(L.vbase + k);
-    const double* Qr = A.Q + 10 * (uint64_t)(L.vbase + rm);
+    const uint64_t gk = sl_vg<SM, R>(L, k), gr = sl_vg<SM, R>(L, rm);
+    double* Qk = A.Q + 10 * gk;
+    const double* Qr = A.Q + 10 * gr;
     double qk = 0.0, qr = 0.0;
     if (ok && gl < 10) { qk = Qk[gl]; qr = Qr[gl]; }
     const bool hu = ok && gl < nfu, hv = ok && gl < nfv;
@@ -691,7 +724,7 @@ __device__ __forceinline__ void sl_collapse_pass(const SlArgs& A, const SlLab<SM
       if (hu && x1 != v && x2 != v) { sl_vor<SM>(L.vflag, x1, VF_RDIRTY); sl_vor<SM>(L.vflag, x2, VF_RDIRTY); }
       if (hv && y1 != u && y2 != u) { sl_vor<SM>(L.vflag, y1, VF_RDIRTY); sl_vor<SM>(L.vflag, y2, VF_RDIRTY); }
       if (gl < 10) Qk[gl] = qk + qr;
-      if (gl >= 10 && gl < 13) A.pos[3 * (uint64_t)(L.vbase + k) + (gl - 10)] = sh.wbest[3 * slot + (gl - 10)];
+      if (gl >= 10 && gl < 13) A.pos[3 * gk + (gl - 10)] = sh.wbest[3 * slot + (gl - 10)];
       if (gl == 0) {
         sl_vor<SM>(L.vflag, k, VF_CDIRTY | VF_RDIRTY);  // k moved: cached costs of its edges are stale
         sl_vclear<SM>(L.vflag, k, VF_END);
@@ -704,8 +737,67 @@ __device__ __forceinline__ void sl_collapse_pass(const SlArgs& A, const SlLab<SM
   }
 }
 
-template <bool SM>
-__device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
+// Hand a shared-memory label over to the next smaller class at the end of round r (right after a face-list
+// compaction: flist[0, nF) are exactly the alive faces).  Alive vertices are renumbered in vertex order, so
+// keep = min(u, v) and the canonical u < v half-edge of every edge stay what they were.
+template <bool R>
+__device__ void sl_migrate(const SlArgs& A, const SlLab<true>& L, SlShared& sh, const uint16_t* flist, uint32_t nF,
+                           int r) {
+  const uint32_t FULL = 0xFFFFFFFFu;
+  const uint32_t tid = threadIdx.x, NT = blockDim.x, lane = tid & 31u, warp = tid >> 5, NW = NT >> 5;
+  // block-wide exclusive scan of the alive vertices over contiguous chunks (the cost queues are free
+  // between rounds and hold the warp totals)
+  const uint32_t per = (L.U + NT - 1) / NT, v0 = min(tid * per, L.U), v1 = min(v0 + per, L.U);
+  uint32_t cnt = 0;
+  for (uint32_t v = v0; v < v1; v++) cnt += L.vflag[v] & VF_ALIVE;
+  uint32_t inc = cnt;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t o = __shfl_up_sync(FULL, inc, d);
+    if ((int)lane >= d) inc += o;
+  }
+  if (lane == 31) L.wq[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    const uint32_t t = lane < NW ? L.wq[lane] : 0u;
+    uint32_t x = t;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const uint32_t o = __shfl_up_sync(FULL, x, d);
+      if ((int)lane >= d) x += o;
+    }
+    if (lane < NW) L.wq[lane] = x - t;
+  }
+  __syncthreads();
+  uint32_t j = L.wq[warp] + inc - cnt;
+  for (uint32_t v = v0; v < v1; v++) {
+    const uint32_t fl = L.vflag[v];
+    if (!(fl & VF_ALIVE)) continue;
+    A.vlist[L.vbase + j] = (uint32_t)(R ? L.vmap[v] : v) | (fl << 16);
+    L.key1[v] = j++;  // key1 is dead until the next round's P1: it holds the new vertex ids
+  }
+  __syncthreads();
+  for (uint32_t i = tid; i < nF; i += NT) {
+    const uint32_t f = flist[i], fo = sl_fo<true, R>(L, f);
+    A.flist[L.tbase + i] = L.key1[L.fc0[f]] | (L.key1[L.fc1[f]] << 16);
+    A.flist2[L.tbase + i] = L.key1[L.fc2[f]] | (fo << 16);
+    A.fstate[L.tbase + i] = L.fstate[f];
+    A.finv[L.tbase + fo] = (uint16_t)i;
+  }
+  if (tid == 0) {
+    uint32_t* h = A.mq_next + SL_MREC * (size_t)atomicAdd(&A.counters[16 + A.cls + 1], 1u);
+    h[0] = L.label;
+    h[1] = sh.rec;
+    h[2] = (uint32_t)r + 1;
+    h[3] = sh.slow;
+    h[4] = nF;
+    h[5] = sh.valive;
+  }
+}
+
+// All rounds of one label (R: a label resumed from the header `hdr` after it migrated from a larger class)
+template <bool SM, bool R>
+__device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const uint32_t* hdr) {
   if (A.trace != nullptr && threadIdx.x == 0) {
     for (int q = 0; q < 10; q++) sh.ph[q] = 0;
     sh.t_prev = clock64();
@@ -720,29 +812,57 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
   const uint32_t T = L.T, U = L.U;
   idx_t *flist = L.flist, *flist2 = L.flist2, *vlist = L.vlist, *vlist2 = L.vlist2;
   // ---- load the label
-  for (uint32_t f = tid; f < T; f += NT) {
-    if (SM) {
-      const uint32_t* g = A.face + 3 * (uint64_t)(L.tbase + f);
-      sl_fset<SM>(L, f, 0, g[0] - L.vbase);
-      sl_fset<SM>(L, f, 1, g[1] - L.vbase);
-      sl_fset<SM>(L, f, 2, g[2] - L.vbase);
+  int r = 0;
+  if (R) {  // the migrated state (see SlArgs::mq_next)
+    for (uint32_t f = tid; f < T; f += NT) {
+      const uint32_t w0 = A.flist[L.tbase + f], w1 = A.flist2[L.tbase + f];
+      sl_fset<SM>(L, f, 0, w0 & 0xFFFFu);
+      sl_fset<SM>(L, f, 1, w0 >> 16);
+      sl_fset<SM>(L, f, 2, w1 & 0xFFFFu);
+      L.fmap[f] = (idx_t)(w1 >> 16);
+      L.fstate[f] = A.fstate[L.tbase + f];
+      flist[f] = (idx_t)f;
     }
-    L.fstate[f] = 0x80;
-    flist[f] = (idx_t)f;
-  }
-  for (uint32_t v = tid; v < U; v += NT) {
-    L.vflag[v] = (uint8_t)(VF_ALIVE | (A.vbound[L.vbase + v] ? VF_BOUND : 0u));
-    if (!SM) vlist[v] = (idx_t)v;  // the shared-memory class scans its vertices directly (no list: 2 B / vertex saved)
+    for (uint32_t v = tid; v < U; v += NT) {
+      const uint32_t w = A.vlist[L.vbase + v];
+      L.vmap[v] = (idx_t)(w & 0xFFFFu);
+      L.vflag[v] = (uint8_t)(w >> 16);
+    }
+    r = (int)hdr[2];
+    if (tid == 0) {
+      sh.rec = hdr[1];
+      sh.slow = hdr[3];
+      sh.alive = hdr[4];
+    }
+  } else {
+    for (uint32_t f = tid; f < T; f += NT) {
+      if (SM) {
+        const uint32_t* g = A.face + 3 * (uint64_t)(L.tbase + f);
+        sl_fset<SM>(L, f, 0, g[0] - L.vbase);
+        sl_fset<SM>(L, f, 1, g[1] - L.vbase);
+        sl_fset<SM>(L, f, 2, g[2] - L.vbase);
+      }
+      L.fstate[f] = 0x80;
+      flist[f] = (idx_t)f;
+    }
+    for (uint32_t v = tid; v < U; v += NT) {
+      L.vflag[v] = (uint8_t)(VF_ALIVE | (A.vbound[L.vbase + v] ? VF_BOUND : 0u));
+      if (!SM) vlist[v] = (idx_t)v;  // the shared-memory class scans its vertices directly (no list: 2 B / vertex saved)
+    }
+    if (tid == 0) {
+      sh.rec = A.base + sh.work;
+      sh.alive = T;
+      sh.slow = 0;
+    }
   }
   if (tid == 0) {
-    sh.alive = T;
-    sh.slow = 0;
+    sh.valive = U;
     sh.stop = 0;
   }
   __syncthreads();
   uint32_t nF = T, nV = U;
+  bool migrated = false;
 
-  int r = 0;
   for (; r < A.max_rounds; r++) {
     if (sh.alive <= L.target) break;  // reached the target before this round
     // per-round salt: equal-cost edges get a fresh pseudo-random priority every round (a fixed
@@ -772,19 +892,21 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
       // software pipeline: the face id and the three cached costs of the NEXT iteration are
       // requested (global loads, L2 latency) before the current face is processed
       const float* ecb = A.ecost + 3 * (uint64_t)L.tbase;
-      uint32_t f_n = 0;
+      uint32_t f_n = 0, fo_n = 0;
       float ec_n[3] = {0.f, 0.f, 0.f};
       if (warp * 32 + lane < nF) {
         f_n = flist[warp * 32 + lane];
-        ec_n[0] = ecb[3 * (uint64_t)f_n]; ec_n[1] = ecb[3 * (uint64_t)f_n + 1]; ec_n[2] = ecb[3 * (uint64_t)f_n + 2];
+        fo_n = sl_fo<SM, R>(L, f_n);
+        ec_n[0] = ecb[3 * (uint64_t)fo_n]; ec_n[1] = ecb[3 * (uint64_t)fo_n + 1]; ec_n[2] = ecb[3 * (uint64_t)fo_n + 2];
       }
       for (uint32_t base = warp * 32; base < nF; base += NT) {
         const uint32_t i = base + lane;
-        const uint32_t f = f_n;
+        const uint32_t f = f_n, fo = fo_n;
         const float ec[3] = {ec_n[0], ec_n[1], ec_n[2]};
         if (i + NT < nF) {
           f_n = flist[i + NT];
-          ec_n[0] = ecb[3 * (uint64_t)f_n]; ec_n[1] = ecb[3 * (uint64_t)f_n + 1]; ec_n[2] = ecb[3 * (uint64_t)f_n + 2];
+          fo_n = sl_fo<SM, R>(L, f_n);
+          ec_n[0] = ecb[3 * (uint64_t)fo_n]; ec_n[1] = ecb[3 * (uint64_t)fo_n + 1]; ec_n[2] = ecb[3 * (uint64_t)fo_n + 2];
         }
         uint32_t st = 0, a[3] = {0, 0, 0}, fl[3] = {0, 0, 0};
         if (i < nF) st = L.fstate[f];
@@ -809,7 +931,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
             if (es == 0) {
               pend |= 1u << c;
             } else if (es == 2) {
-              sl_post(L.key1, u, v, sl_key<SM>(L, ec[c], 3u * f + (uint32_t)c, salt));
+              sl_post(L.key1, u, v, sl_key<SM>(L, ec[c], 3u * fo + (uint32_t)c, salt));
             }
             nst = (nst & ~(3u << (2 * c))) | (es << (2 * c));
           }
@@ -825,20 +947,20 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
         if (qn > (uint32_t)SL_EQ - 32 || (last && qn)) {
           __syncwarp();
           for (uint32_t j = lane; j < qn; j += 32) {
-            const uint32_t e = wq[j], ef = e >> 3, ep = e & 7u;
+            const uint32_t e = wq[j], ef = e >> 3, ep = e & 7u, efo = sl_fo<SM, R>(L, ef);
             uint32_t est = L.fstate[ef];
 #pragma unroll
             for (int c = 0; c < 3; c++) {
               if (!((ep >> c) & 1u)) continue;
               const uint32_t u = sl_fget<SM>(L, ef, c), v = sl_fget<SM>(L, ef, (c + 1) % 3);
               SEval ev;
-              sl_cost<SM>(A, L, u, v, &ev);
+              sl_cost<SM, R>(A, L, u, v, &ev);
               uint32_t es = 3;  // exceeds max_error
               if (ev.valid) {
                 const float cf = __double2float_rn(ev.cost);
-                A.ecost[3 * (uint64_t)(L.tbase + ef) + c] = cf;
+                A.ecost[3 * (uint64_t)(L.tbase + efo) + c] = cf;
                 es = 2;
-                sl_post(L.key1, u, v, sl_key<SM>(L, cf, 3u * ef + (uint32_t)c, salt));
+                sl_post(L.key1, u, v, sl_key<SM>(L, cf, 3u * efo + (uint32_t)c, salt));
               }
               est = (est & ~(3u << (2 * c))) | (es << (2 * c));
             }
@@ -896,7 +1018,8 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
         const key_t key = L.key1[a];
         if (key == (key_t)S_KEYMAX) continue;
         const uint32_t hl = sl_key_edge<SM>(L, key, salt);
-        const uint32_t f = hl / 3, c = hl - 3 * f;
+        const uint32_t fo = hl / 3, c = hl - 3 * fo;
+        const uint32_t f = R ? (uint32_t)A.finv[L.tbase + fo] : fo;
         if (sl_fget<SM>(L, f, (int)c) != a) continue;
         const uint32_t v = sl_fget<SM>(L, f, (int)((c + 1) % 3));
         if (L.key1[v] != key || (L.vflag[v] & VF_DONE) || L.vlose[v]) continue;
@@ -904,7 +1027,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
         if (slot < (uint32_t)SL_WCAP) {
           sh.win[slot].u = a;
           sh.win[slot].v = v;
-          sh.win[slot].h = hl;
+          sh.win[slot].h = 3 * f + c;
           sh.win[slot].cnt[0] = 0;
           sh.win[slot].cnt[1] = 0;
           sh.win[slot].flags = 0;
@@ -934,7 +1057,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
         if (tid < nb) {
           const uint32_t i = tid;
           SEval e;
-          sl_cost<SM>(A, L, sh.win[i].u, sh.win[i].v, &e);
+          sl_cost<SM, R>(A, L, sh.win[i].u, sh.win[i].v, &e);
           sh.win[i].keep = e.valid ? e.keep : sh.win[i].u;
           sh.win[i].flags = e.valid ? 0u : WF_BAD;
           if (e.valid) {
@@ -977,7 +1100,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
         const uint32_t a[3] = {sl_fget<SM>(L, f, 0), sl_fget<SM>(L, f, 1), sl_fget<SM>(L, f, 2)};
         if (a[0] == other || a[1] == other || a[2] == other) continue;  // dies with the edge
         const double best[3] = {sh.wbest[3 * i], sh.wbest[3 * i + 1], sh.wbest[3 * i + 2]};
-        if (sl_flips<SM>(A, L, a, w, best)) atomicOr(&sh.win[i].flags, WF_BAD);
+        if (sl_flips<SM, R>(A, L, a, w, best)) atomicOr(&sh.win[i].flags, WF_BAD);
       }
       __syncthreads();
       SL_MARK(7);
@@ -987,17 +1110,17 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
       // dependent shared-memory accesses per winner, so its duration is the number of winners a warp
       // handles one after the other.  The few winners with larger rings take a second pass with
       // whole warps.
-      sl_collapse_pass<SM, 16>(A, L, sh, nb);
+      sl_collapse_pass<SM, R, 16>(A, L, sh, nb);
       __syncthreads();
       if (sh.nbig) {
-        sl_collapse_pass<SM, 32>(A, L, sh, nb);
+        sl_collapse_pass<SM, R, 32>(A, L, sh, nb);
       }
       __syncthreads();
       SL_MARK(8);
       if (total <= (uint32_t)SL_WCAP) break;
     }
     // ---- stop rules of the label
-    if (tid == 0 && A.trace != nullptr && A.base + sh.work == 0 && r < 400) {
+    if (tid == 0 && A.trace != nullptr && sh.rec == 0 && r < 400) {
       A.trace[4 * r + 0] = sh.progress;
       A.trace[4 * r + 1] = sh.ncol;
       A.trace[4 * r + 2] = sh.alive;
@@ -1005,6 +1128,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
     }
     if (A.trace != nullptr && tid == 0) sh.visits += nF;
     if (tid == 0) {
+      sh.valive -= sh.ncol;
       uint32_t stop = 0;
       if (!sh.progress) {
         stop = 1;  // nothing collapsed or parked: fixed point
@@ -1026,34 +1150,54 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh) {
     if (r & 1) {
       nF = sl_compact<SM>(flist, flist2, nF, &sh.counter, [&](uint32_t f) { return (L.fstate[f] & 0x80u) != 0; });
       if (!SM) nV = sl_compact<SM>(vlist, vlist2, nV, &sh.counter, [&](uint32_t v) { return (L.vflag[v] & VF_ALIVE) != 0; });
+      // a label that has shrunk enough continues in the next smaller class and returns its SM share (the
+      // header's queue is resumed by a later launch); alive counts only fall, so it never moves back up
+      if (SM && A.mq_next != nullptr && sl_fits_smem(nF, sh.valive, NT / 2, A.smem_next, true)) {
+        if constexpr (SM) sl_migrate<R>(A, L, sh, flist, nF, r);
+        migrated = true;
+        r++;
+        break;
+      }
     }
   }
-  // ---- write the label back to the whole-task arrays
+  // ---- write the label back to the whole-task arrays (a migrating label writes its dead faces and
+  // vertices; the class that resumes it writes the others when it finishes)
   for (uint32_t f = tid; f < T; f += NT) {
     const bool al = L.fstate[f] & 0x80u;
-    A.falive[L.tbase + f] = al ? 1 : 0;
+    const uint32_t fo = sl_fo<SM, R>(L, f);
+    if (migrated && al) continue;
+    A.falive[L.tbase + fo] = al ? 1 : 0;
     if (SM && al) {
-      uint32_t* g = A.face + 3 * (uint64_t)(L.tbase + f);
-      g[0] = sl_fget<SM>(L, f, 0) + L.vbase;
-      g[1] = sl_fget<SM>(L, f, 1) + L.vbase;
-      g[2] = sl_fget<SM>(L, f, 2) + L.vbase;
+      uint32_t* g = A.face + 3 * (uint64_t)(L.tbase + fo);
+      g[0] = (uint32_t)sl_vg<SM, R>(L, sl_fget<SM>(L, f, 0));
+      g[1] = (uint32_t)sl_vg<SM, R>(L, sl_fget<SM>(L, f, 1));
+      g[2] = (uint32_t)sl_vg<SM, R>(L, sl_fget<SM>(L, f, 2));
     }
   }
-  for (uint32_t v = tid; v < U; v += NT) A.valive[L.vbase + v] = (L.vflag[v] & VF_ALIVE) ? 1 : 0;
+  for (uint32_t v = tid; v < U; v += NT) {
+    const bool al = L.vflag[v] & VF_ALIVE;
+    if (!(migrated && al)) A.valive[sl_vg<SM, R>(L, v)] = al ? 1 : 0;
+  }
   if (tid == 0 && A.trace != nullptr) {
+    // a migrated label's record sums the cycles, visits and winners of all its segments
     for (int q = 0; q < 10; q++) atomicAdd((unsigned long long*)(A.trace + 1600) + q, sh.ph[q]);
-    uint32_t* rec = A.lrec + 6 * (size_t)(A.base + sh.work);
-    rec[0] = T;
+    uint32_t* rec = A.lrec + SL_LREC * (size_t)sh.rec;
+    const unsigned long long vis = rec[3] + sh.visits;
+    const uint32_t kc = (uint32_t)((clock64() - sh.t_label) >> 10);
+    if (!R) rec[0] = T;
     rec[1] = (uint32_t)r;
-    rec[2] = (uint32_t)((clock64() - sh.t_label) >> 10);
-    rec[3] = (uint32_t)(sh.visits > 0xFFFFFFFFull ? 0xFFFFFFFFull : sh.visits);
-    rec[4] = (uint32_t)sh.wins;
-    rec[5] = (SM ? 1u : ((const void*)L.key1 == (const void*)(A.key1 + L.vbase) ? 3u : 2u)) | (A.cls << 2);
+    rec[2] += kc;
+    rec[6] += kc / (SL_THREADS / NT);
+    rec[3] = (uint32_t)(vis > 0xFFFFFFFFull ? 0xFFFFFFFFull : vis);
+    rec[4] += (uint32_t)sh.wins;
+    if (!R) rec[5] = (SM ? 1u : ((const void*)L.key1 == (const void*)(A.key1 + L.vbase) ? 3u : 2u)) | (A.cls << 2);
   }
   if (tid == 0) {
-    atomicMax(&A.counters[1], (uint32_t)r);
-    atomicAdd(&A.counters[SM ? 2 : 3], 1u);
-    atomicAdd(&A.counters[8 + A.cls], 1u);
+    if (!migrated) atomicMax(&A.counters[1], (uint32_t)r);
+    if (!R) {  // a label counts in the class it started in
+      atomicAdd(&A.counters[SM ? 2 : 3], 1u);
+      atomicAdd(&A.counters[8 + A.cls], 1u);
+    }
   }
 }
 
@@ -1099,10 +1243,14 @@ __global__ void __launch_bounds__(SL_THREADS, 1) k_simp_labels(SlArgs A) {
       L.fstate = sl_smem + y.o_fs;
       L.vflag = sl_smem + y.o_vf;
       L.vlose = sl_smem + y.o_vl;
-      sl_run<true>(A, L, sh);
+      L.label = l;
+      L.fmap = L.vmap = nullptr;
+      sl_run<true, false>(A, L, sh, nullptr);
     } else {
       SlLab<false> L;
       L.T = T; L.U = U; L.tbase = tbase; L.vbase = vbase; L.target = target;
+      L.label = l;
+      L.fmap = L.vmap = nullptr;
       L.wq = (uint32_t*)sl_smem;  // the cost queues and the ring lists always fit
       L.ring = (uint32_t*)(sl_smem + y.wq);
       L.fc0 = L.fc1 = L.fc2 = nullptr;
@@ -1126,8 +1274,49 @@ __global__ void __launch_bounds__(SL_THREADS, 1) k_simp_labels(SlArgs A) {
         L.vflag = A.vflag + vbase;
         L.vlose = A.vlose + vbase;
       }
-      sl_run<false>(A, L, sh);
+      sl_run<false, false>(A, L, sh, nullptr);
     }
+  } while (A.persist);
+}
+
+// Labels that migrated into the launch's class (A.mq), in the order they migrated; the grid is an upper
+// bound on their number and surplus CTAs exit at once.  Its own kernel, so that the maps of the resumed
+// path cost k_simp_labels no registers.
+__global__ void __launch_bounds__(SL_THREADS / 2, 2) k_simp_resume(SlArgs A) {
+  __shared__ SlShared sh;
+  do {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      sh.work = atomicAdd(&A.counters[20 + A.cls], 1u);
+      sh.counter = A.counters[16 + A.cls];  // written by earlier launches only
+    }
+    __syncthreads();
+    const uint32_t wi = sh.work;
+    if (wi >= sh.counter) break;
+    const uint32_t* hdr = A.mq + SL_MREC * (size_t)wi;
+    const uint32_t l = hdr[0];
+    const uint32_t T = hdr[4], U = hdr[5];
+    const SlLayout y = sl_layout(T, U, blockDim.x, true);
+    SlLab<true> L;
+    L.T = T; L.U = U; L.tbase = A.tri_off[l]; L.vbase = A.vert_off[l]; L.target = A.target[l];
+    L.label = l;
+    L.wq = (uint32_t*)sl_smem;
+    L.ring = (uint16_t*)(sl_smem + y.wq);
+    L.key1 = (uint32_t*)(sl_smem + y.o_key);
+    L.fmt16 = true;
+    L.fc0 = (uint16_t*)(sl_smem + y.o_f0);
+    L.fc1 = L.fc0 + T;
+    L.fc2 = L.fc1 + T;
+    L.flist = (uint16_t*)(sl_smem + y.o_fl);
+    L.vlist = nullptr;
+    L.flist2 = L.vlist2 = nullptr;
+    L.gface = nullptr;
+    L.fstate = sl_smem + y.o_fs;
+    L.vflag = sl_smem + y.o_vf;
+    L.vlose = sl_smem + y.o_vl;
+    L.fmap = (uint16_t*)(sl_smem + y.o_fm);
+    L.vmap = (uint16_t*)(sl_smem + y.o_vm);
+    sl_run<true, true>(A, L, sh, hdr);
   } while (A.persist);
 }
 
@@ -1201,7 +1390,7 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   m->simp_max_error = max_error;
   m->simp_rounds = 0;
   m->simp_labels_smem = m->simp_labels_gmem = 0;
-  for (int c = 0; c < SL_NCLASS; c++) m->simp_labels_class[c] = 0;
+  for (int c = 0; c < SL_NCLASS; c++) m->simp_labels_class[c] = m->simp_migrations[c] = 0;
   const uint64_t U = m->U, T = m->T, K = m->K;
   if (T == 0 || U == 0) {
     m->simplified = true;
@@ -1219,7 +1408,8 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   s.U = U;
   s.T = T;
   uint32_t *node_v, *node_h, *vscan, *vflag32, *d_target, *d_tri_off, *d_vert_off, *d_new_tri_off, *d_new_vert_off;
-  uint32_t *d_order, *flags, *gl_f[2], *gl_v[2], *sorted_v, *sorted_h;
+  uint32_t *d_order, *flags, *gl_f[2], *gl_v[2], *sorted_v, *sorted_h, *d_mq;
+  uint16_t* finv;
   uint8_t *fstate, *vflag, *vlose;
   unsigned long long* key1;
   float* ecost;
@@ -1254,6 +1444,10 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   IGN_TRY(f.take(&gl_f[1], T));
   IGN_TRY(f.take(&gl_v[0], U));
   IGN_TRY(f.take(&gl_v[1], U));
+  // labels migrating to a smaller size class: headers (one queue per destination class) and the
+  // original-to-compacted face map
+  IGN_TRY(f.take(&d_mq, (size_t)SL_MREC * K * (SL_NCLASS - 1)));
+  IGN_TRY(f.take(&finv, T));
   IGN_TRY(f.take(&tmp, tmpb));
   IGN_TRY(f.take(&sorted_v, 3 * T));
   IGN_TRY(f.take(&sorted_h, 3 * T));
@@ -1303,7 +1497,7 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
                                              ctx->stream));
     ctx->launches += 3;
   }
-  IGN_CUDA(cudaMemsetAsync(flags, 0, 64, ctx->stream));
+  IGN_CUDA(cudaMemsetAsync(flags, 0, 32 * 4, ctx->stream));
   IGN_LAUNCH(ctx, k_simp_link, blocks_for(3 * T, 256), 256, 0, sorted_v, sorted_h, (uint64_t)(3 * T), s.vf, s.vn,
              flags + 12);
   IGN_LAUNCH(ctx, k_simp_quadrics, blocks_for(U, 128), 128, 0, s);
@@ -1313,9 +1507,10 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   // latency and barrier bound, so labels that fit half (a quarter) of an SM's shared memory run two
   // (four) CTAs to an SM, which overlap each other's stalls; larger labels keep the whole SM.
   IGN_CUDA(cudaFuncSetAttribute(k_simp_labels, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sl_dyn[0]));
+  IGN_CUDA(cudaFuncSetAttribute(k_simp_resume, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sl_dyn[1]));
   SlArgs A;
   A.pos = s.pos; A.Q = s.Q; A.face = s.face; A.falive = s.falive; A.valive = s.valive; A.vbound = s.vbound;
-  A.ecost = ecost; A.key1 = key1; A.fstate = fstate; A.vflag = vflag; A.vlose = vlose;
+  A.ecost = ecost; A.key1 = key1; A.fstate = fstate; A.vflag = vflag; A.vlose = vlose; A.finv = finv;
   A.flist = gl_f[0]; A.flist2 = gl_f[1]; A.vlist = gl_v[0]; A.vlist2 = gl_v[1];
   A.tri_off = d_tri_off; A.vert_off = d_vert_off; A.target = d_target;
   A.counters = flags;
@@ -1327,9 +1522,9 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   A.lrec = nullptr;
   if (getenv("IGN_SIMP_TRACE") != nullptr) {
     IGN_TRY(f.take(&A.trace, 400 * 4 + 64));
-    IGN_TRY(f.take(&A.lrec, (size_t)K * 6 + 16));
+    IGN_TRY(f.take(&A.lrec, (size_t)K * SL_LREC + 16));
     IGN_CUDA(cudaMemsetAsync(A.trace, 0, 400 * 16 + 256, ctx->stream));
-    IGN_CUDA(cudaMemsetAsync(A.lrec, 0, (size_t)K * 24 + 64, ctx->stream));
+    IGN_CUDA(cudaMemsetAsync(A.lrec, 0, ((size_t)K * SL_LREC + 16) * 4, ctx->stream));
   }
   const char* force_gmem = getenv("IGN_SIMP_GMEM");
   const bool gmem_only = force_gmem && force_gmem[0] == '1';
@@ -1343,34 +1538,71 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
     // first: the block scheduler dispatches the CTAs of earlier launches first, so the smaller classes
     // fill the SMs that the end of a larger class leaves idle instead of waiting for its last label.
     // (Streams and events are released by the runtime once their work is done.)
+    //
+    // A shared-memory label whose alive faces and vertices come to fit the next smaller class migrates
+    // there (SlArgs::mq_next).  After the fresh launches, a resume launch of the 512-thread class takes the
+    // labels that left the 1024-thread class once that launch is over, and one of the 256-thread class
+    // those that left the 512-thread class once both of its launches are over: stream and event order
+    // only, no CTA waits for another.
+    // resume[c]: most labels that can migrate into class c (the grid of its resume launch)
+    uint32_t resume[SL_NCLASS] = {0, 0, 0};
+    if (!gmem_only)
+      for (int c = 1; c < SL_NCLASS; c++) resume[c] = resume[c - 1] + ccount[c - 1];
     int prio = 0;
     IGN_CUDA(cudaStreamGetPriority(ctx->stream, &prio));
     cudaStream_t cs[SL_NCLASS] = {ctx->stream, nullptr, nullptr};
-    cudaEvent_t ev[SL_NCLASS] = {nullptr, nullptr, nullptr};
+    cudaEvent_t ev[SL_NCLASS] = {nullptr, nullptr, nullptr};  // [0] fork, [c] end of class c's launches
     cudaError_t err = cudaEventCreateWithFlags(&ev[0], cudaEventDisableTiming);
     if (err == cudaSuccess) err = cudaEventRecord(ev[0], ctx->stream);
+    for (int c = 1; c < SL_NCLASS && err == cudaSuccess; c++) {
+      if (ccount[c] == 0 && resume[c] == 0) continue;
+      err = cudaStreamCreateWithPriority(&cs[c], cudaStreamNonBlocking, prio);
+      if (err == cudaSuccess) err = cudaStreamWaitEvent(cs[c], ev[0], 0);
+      if (err == cudaSuccess) err = cudaEventCreateWithFlags(&ev[c], cudaEventDisableTiming);
+    }
+    cudaEvent_t ev_full = nullptr;  // end of the 1024-thread class
+    if (err == cudaSuccess && resume[1]) err = cudaEventCreateWithFlags(&ev_full, cudaEventDisableTiming);
     uint32_t base = 0;
     for (int c = 0; c < SL_NCLASS && err == cudaSuccess; c++) {  // largest class first
       const uint32_t n = ccount[c], nt = (uint32_t)SL_CLASS_THREADS[c];
-      if (n == 0) continue;
-      if (c > 0) {
-        err = cudaStreamCreateWithPriority(&cs[c], cudaStreamNonBlocking, prio);
-        if (err == cudaSuccess) err = cudaStreamWaitEvent(cs[c], ev[0], 0);
-        if (err == cudaSuccess) err = cudaEventCreateWithFlags(&ev[c], cudaEventDisableTiming);
-        if (err != cudaSuccess) break;
-      }
-      A.order = d_order + base; A.K = n; A.base = base; A.cls = (uint32_t)c;
+      A.cls = (uint32_t)c;
       // 0: every label takes the global-memory path (only the cost queues and ring lists stay in smem)
       A.smem_bytes = gmem_only ? 0u : (uint32_t)sl_dyn[c];
+      A.smem_next = c + 1 < SL_NCLASS ? (uint32_t)sl_dyn[c + 1] : 0u;
+      A.mq_next = (c + 1 < SL_NCLASS && resume[c + 1]) ? d_mq + (size_t)SL_MREC * K * c : nullptr;
+      A.mq = nullptr;
       const uint64_t slots = (uint64_t)ctx->sm_count * (1024 / nt);
-      const unsigned grid = A.persist ? (unsigned)(n < slots ? n : slots) : n;
-      k_simp_labels<<<grid, nt, sl_dyn[c], cs[c]>>>(A);
-      ctx->launches++;
-      err = cudaGetLastError();
-      if (c > 0 && err == cudaSuccess) err = cudaEventRecord(ev[c], cs[c]);
-      if (c > 0 && err == cudaSuccess) err = cudaStreamWaitEvent(ctx->stream, ev[c], 0);
-      base += n;
+      if (n) {
+        A.order = d_order + base; A.K = n; A.base = base;
+        const unsigned grid = A.persist ? (unsigned)(n < slots ? n : slots) : n;
+        k_simp_labels<<<grid, nt, sl_dyn[c], cs[c]>>>(A);
+        ctx->launches++;
+        err = cudaGetLastError();
+        base += n;
+      }
+      if (c == 0 && ev_full && err == cudaSuccess) err = cudaEventRecord(ev_full, cs[0]);
     }
+    for (int c = 1; c < SL_NCLASS && err == cudaSuccess; c++) {
+      if (resume[c]) {
+        const uint32_t nt = (uint32_t)SL_CLASS_THREADS[c];
+        err = cudaStreamWaitEvent(cs[c], c == 1 ? ev_full : ev[c - 1], 0);
+        if (err != cudaSuccess) break;
+        A.cls = (uint32_t)c;
+        A.smem_bytes = (uint32_t)sl_dyn[c];
+        A.smem_next = c + 1 < SL_NCLASS ? (uint32_t)sl_dyn[c + 1] : 0u;
+        A.mq_next = (c + 1 < SL_NCLASS) ? d_mq + (size_t)SL_MREC * K * c : nullptr;
+        A.mq = d_mq + (size_t)SL_MREC * K * (c - 1);
+        const uint64_t slots = (uint64_t)ctx->sm_count * (1024 / nt);
+        const unsigned grid = A.persist ? (unsigned)(resume[c] < slots ? resume[c] : slots) : resume[c];
+        k_simp_resume<<<grid, nt, sl_dyn[c], cs[c]>>>(A);
+        ctx->launches++;
+        err = cudaGetLastError();
+      }
+      if (ev[c] && err == cudaSuccess) err = cudaEventRecord(ev[c], cs[c]);
+    }
+    for (int c = 1; c < SL_NCLASS && err == cudaSuccess; c++)
+      if (ev[c]) err = cudaStreamWaitEvent(ctx->stream, ev[c], 0);
+    if (ev_full) cudaEventDestroy(ev_full);
     for (int c = 0; c < SL_NCLASS; c++) {
       if (ev[c]) cudaEventDestroy(ev[c]);
       if (c > 0 && cs[c]) cudaStreamDestroy(cs[c]);
@@ -1389,12 +1621,12 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   tb = tmpb;
   IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, fflag, fscan, (int)T, ctx->stream));
   ctx->launches += 4;
-  uint32_t last[4], hflags[16];
+  uint32_t last[4], hflags[32];
   IGN_TRY(small_d2h(ctx, &last[0], vscan + (U - 1), 4));
   IGN_TRY(small_d2h(ctx, &last[1], vflag32 + (U - 1), 4));
   IGN_TRY(small_d2h(ctx, &last[2], fscan + (T - 1), 4));
   IGN_TRY(small_d2h(ctx, &last[3], fflag + (T - 1), 4));
-  IGN_TRY(small_d2h(ctx, hflags, flags, 64));
+  IGN_TRY(small_d2h(ctx, hflags, flags, sizeof(hflags)));
   IGN_TRY(small_sync(ctx));
   if (hflags[12] != 0) {
     set_error("simplify: a vertex has more than %d incident faces", S_VCAP);
@@ -1412,35 +1644,42 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
       fprintf(stderr, "phase %-18s %6.2f %%  %10.3f Mcycles\n", names[q], 100.0 * phs[q] / (tot ? tot : 1), phs[q] / 1e6);
     {
       // per-label records: where do the cycles go -- per round (fixed latency) or per face visit?
-      std::vector<uint32_t> rec(6 * (size_t)K);
+      std::vector<uint32_t> rec(SL_LREC * (size_t)K);
       IGN_CUDA(cudaMemcpy(rec.data(), A.lrec, rec.size() * 4, cudaMemcpyDeviceToHost));
       static const uint32_t edges[] = {0, 500, 1000, 2000, 3000, 4000, 6000, 8000, 10000, 12000, 16000, 32000, 64000, 0xFFFFFFFFu};
       const int nedges = (int)(sizeof(edges) / sizeof(edges[0]));
-      // kilocycles are wall cycles of the label's CTA, which shares its SM with the other CTAs of its class
+      // kilocycles are wall cycles of the label's CTA, which shares its SM with the other CTAs of its class;
+      // SM Mcycles divide each segment's wall cycles by the CTAs per SM of the class it ran in.  A label
+      // that migrated sums all its segments and is listed under the class it started in.
       for (int c = 0; c < SL_NCLASS; c++) {
         int per_sm = 0;
         IGN_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_simp_labels, SL_CLASS_THREADS[c], sl_dyn[c]));
         fprintf(stderr, "size class %d: %4d threads, %6zu B dynamic shared memory, %d CTAs per SM, %u labels\n", c,
                 SL_CLASS_THREADS[c], sl_dyn[c], per_sm, ccount[c]);
       }
-      fprintf(stderr, "%7s %12s %7s %8s %10s %10s %9s %9s  class(sm/hy/gl)\n", "threads", "faces<", "labels", "rounds", "Mcycles", "Mvisits", "kwins", "cyc/round");
+      fprintf(stderr, "%7s %12s %7s %8s %10s %10s %10s %9s %9s  class(sm/hy/gl)\n", "threads", "faces<", "labels", "rounds", "Mcycles", "SM Mcyc", "Mvisits", "kwins", "cyc/round");
       double sr = 0, sv = 0, sc = 0, srr = 0, svv = 0, srv = 0, src = 0, svc = 0;
+      uint64_t sm_total[SL_NCLASS] = {0, 0, 0};
       for (int szc = 0; szc < SL_NCLASS; szc++) {
         for (int b = 0; b + 1 < nedges; b++) {
-          uint64_t n = 0, rounds = 0, kc = 0, vis = 0, wins = 0, cls[4] = {0, 0, 0, 0};
+          uint64_t n = 0, rounds = 0, kc = 0, ksm = 0, vis = 0, wins = 0, cls[4] = {0, 0, 0, 0};
           for (uint64_t i = 0; i < K; i++) {
-            const uint32_t* q = &rec[6 * i];
+            const uint32_t* q = &rec[SL_LREC * i];
             if (q[1] == 0 || (int)(q[5] >> 2) != szc || q[0] < edges[b] || q[0] >= edges[b + 1]) continue;
-            n++; rounds += q[1]; kc += q[2]; vis += q[3]; wins += q[4]; cls[q[5] & 3]++;
+            n++; rounds += q[1]; kc += q[2]; ksm += q[6]; vis += q[3]; wins += q[4]; cls[q[5] & 3]++;
             const double R = q[1], V = q[3], C = q[2] * 1024.0;
             sr += R; sv += V; sc += C; srr += R * R; svv += V * V; srv += R * V; src += R * C; svc += V * C;
           }
-          if (n) fprintf(stderr, "%7d %12u %7llu %8.1f %10.2f %10.3f %9.1f %9.0f  %llu/%llu/%llu\n", SL_CLASS_THREADS[szc], edges[b + 1],
-                         (unsigned long long)n, (double)rounds / n, kc * 1024.0 / 1e6, vis / 1e6, wins / 1e3,
+          sm_total[szc] += ksm;
+          if (n) fprintf(stderr, "%7d %12u %7llu %8.1f %10.2f %10.2f %10.3f %9.1f %9.0f  %llu/%llu/%llu\n", SL_CLASS_THREADS[szc], edges[b + 1],
+                         (unsigned long long)n, (double)rounds / n, kc * 1024.0 / 1e6, ksm * 1024.0 / 1e6, vis / 1e6, wins / 1e3,
                          rounds ? kc * 1024.0 / rounds : 0.0, (unsigned long long)cls[1], (unsigned long long)cls[2],
                          (unsigned long long)cls[3]);
         }
       }
+      fprintf(stderr, "SM Mcycles by starting class: %.0f + %.0f + %.0f = %.0f; labels resumed in the 512- / 256-thread class: %u / %u\n",
+              sm_total[0] * 1024.0 / 1e6, sm_total[1] * 1024.0 / 1e6, sm_total[2] * 1024.0 / 1e6,
+              (sm_total[0] + sm_total[1] + sm_total[2]) * 1024.0 / 1e6, hflags[17], hflags[18]);
       // least squares cycles = a * rounds + b * visits (no intercept)
       const double det = srr * svv - srv * srv;
       if (det != 0) fprintf(stderr, "fit: cycles ~= %.0f * rounds + %.2f * face visits   (totals: %.0f rounds, %.3g visits, %.3g cycles)\n",
@@ -1453,6 +1692,7 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   m->simp_labels_smem = hflags[2];
   m->simp_labels_gmem = hflags[3];
   for (int c = 0; c < SL_NCLASS; c++) m->simp_labels_class[c] = hflags[8 + c];
+  for (int c = 0; c < SL_NCLASS; c++) m->simp_migrations[c] = hflags[16 + c];
   const uint32_t U2 = last[0] + last[1], T2 = last[2] + last[3];
   IGN_LAUNCH(ctx, k_simp_new_offsets, blocks_for(K + 2, 256), 256, 0, d_vert_off, vscan, (uint32_t)(K + 2), U, U2,
                    d_new_vert_off);
@@ -1482,5 +1722,12 @@ extern "C" int ign_mesh_simplify_stats(ign_mesher* m, uint32_t stats[6]) {
   stats[1] = m->simp_labels_smem;
   stats[2] = m->simp_labels_gmem;
   for (int c = 0; c < SL_NCLASS; c++) stats[3 + c] = m->simp_labels_class[c];
+  return IGN_OK;
+}
+
+extern "C" int ign_mesh_simplify_migrations(ign_mesher* m, uint32_t resumed[3]) {
+  IGN_REQUIRE(m && resumed, IGN_ERR_INVALID, "null argument");
+  IGN_REQUIRE(m->simplified, IGN_ERR_INVALID, "mesher is not simplified");
+  for (int c = 0; c < SL_NCLASS; c++) resumed[c] = m->simp_migrations[c];
   return IGN_OK;
 }

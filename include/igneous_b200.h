@@ -356,6 +356,10 @@ IGN_API int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int redu
  * in shared memory, [2] in global memory, [3..5] labels simplified in the 1024-, 512- and 256-thread
  * size classes (a label runs in the smallest CTA whose shared-memory budget holds it) */
 IGN_API int ign_mesh_simplify_stats(ign_mesher* m, uint32_t stats[6]);
+/* labels of the simplification that ran which continued in the 1024-, 512- and 256-thread size class
+ * after migrating from the next larger one, once their alive faces and vertices fit it ([0] is always 0;
+ * a label that migrates twice counts in both smaller classes) */
+IGN_API int ign_mesh_simplify_migrations(ign_mesher* m, uint32_t resumed[3]);
 /* bulk export of every label's mesh (simplified if ign_mesh_simplify ran) in ign_mesh_ids order:
  * vertices f32 [U,3], faces u32 [T,3] (label-local indices), offsets [n_ids+1] */
 IGN_API int ign_mesh_export(ign_mesher* m, const float resolution[3], int voxel_centered,
