@@ -6,6 +6,12 @@ igneous/tasks/image/image.py:95-100 uploads, ccl.py:346-356); here the chunk is 
 decoded where the labels already are.  Byte-identical to the CPU restatement in oracle/ (whose
 encoder layout is itself parity-unpinned: no upstream vector exists offline).
 
+`jpeg` is the encoding of uint8 image layers (igneous_cli/cli.py:64, `jpeg_quality` in
+set_encoding).  A chunk [x, y, z(, 1)] is one grayscale JPEG of width sx and height sy*sz; the
+encoder writes libjpeg's default stream byte for byte, the decoder reproduces libjpeg's islow
+decode (oracle_jpeg/ restates both; tests/golden/jpeg_libjpeg.npz pins them to libjpeg-turbo).
+Chunks are encoded / decoded a batch per call.
+
 crackle and compresso are NOT implemented: both are un-vendored third-party formats whose
 specifications are not in the reference checkout.
 """
@@ -15,7 +21,7 @@ import numpy as np
 
 from . import _shim
 
-__all__ = ["cseg_encode", "cseg_decode"]
+__all__ = ["cseg_encode", "cseg_decode", "jpeg_encode", "jpeg_decode", "jpeg_encode_batch", "jpeg_decode_batch"]
 
 
 def _chunk(labels):
@@ -67,3 +73,103 @@ def cseg_decode(data, shape, dtype, block_size=(8, 8, 8), ctx=None):
     c.c_uint64(shape[0]), c.c_uint64(shape[1]), c.c_uint64(shape[2]), c.c_uint64(shape[3]), c.c_uint32(bx),
     c.c_uint32(by), c.c_uint32(bz), _shim.ptr(out)))
   return out
+
+
+JPEG_MAX_SIDE = 65535
+
+
+def _jpeg_shape(shape):
+  shape = tuple(int(v) for v in shape)
+  if len(shape) == 4:
+    if shape[3] != 1:
+      raise NotImplementedError("jpeg chunks hold one channel, got %d" % shape[3])
+    shape = shape[:3]
+  if len(shape) != 3 or min(shape) < 1:
+    raise ValueError("jpeg chunks are non-empty [x, y, z] or [x, y, z, 1] arrays, got shape %r" % (shape,))
+  if shape[0] > JPEG_MAX_SIDE or shape[1] * shape[2] > JPEG_MAX_SIDE:
+    raise ValueError("a jpeg chunk is an image of sx by sy*sz pixels, at most %d per side; got %r"
+                     % (JPEG_MAX_SIDE, shape))
+  return shape
+
+
+def _jpeg_chunk(chunk):
+  arr = np.asarray(chunk)
+  if arr.dtype != np.uint8:
+    raise NotImplementedError("jpeg holds uint8 images, got %s" % arr.dtype)
+  shape = _jpeg_shape(arr.shape)
+  return np.asfortranarray(arr[..., 0] if arr.ndim == 4 else arr), shape
+
+
+def _restart(restart_interval):
+  """None: one block row per chunk (-1 at the C ABI); 0: no restart markers; n: every n blocks."""
+  if restart_interval is None:
+    return -1
+  ri = int(restart_interval)
+  if not 0 <= ri <= 65535:
+    raise ValueError("restart_interval must be in 0..65535 blocks, got %d" % ri)
+  return ri
+
+
+def jpeg_encode_batch(chunks, quality=85, restart_interval=None, ctx=None):
+  """uint8 chunks [x,y,z(,1)] -> list of jpeg files (bytes), one call for the batch.
+  restart_interval: None = a restart marker after every block row (so the GPU decoder can give
+  each row its own thread), 0 = none, n = every n 8x8 blocks."""
+  quality = int(quality)
+  if not 1 <= quality <= 100:
+    raise ValueError("jpeg quality must be in 1..100, got %d" % quality)
+  ri = _restart(restart_interval)
+  arrs, shapes = zip(*[_jpeg_chunk(ch) for ch in chunks]) if len(chunks) else ((), ())
+  n = len(arrs)
+  packed = np.concatenate([a.reshape(-1, order="F") for a in arrs]) if n else np.zeros(1, np.uint8)
+  shp = np.ascontiguousarray(np.array(shapes, dtype=np.uint32).reshape(n, 3)) if n else np.zeros((1, 3), np.uint32)
+  ctx = ctx or _shim.default_context()
+  offsets = np.zeros(n + 1, dtype=np.uint64)
+  need = c.c_uint64(0)
+  args = [ctx.handle, _shim.ptr(packed), c.c_uint64(n), _shim.ptr(shp), c.c_int(quality), c.c_int64(ri)]
+  # a first guess that holds smooth image data; the call reports the size when it does not
+  cap = max(4096, packed.size // 2 + 1024 * n)
+  out = np.empty(cap, dtype=np.uint8)
+  _shim.check(ctx.lib.ign_jpeg_encode(*args, _shim.ptr(out), c.c_uint64(cap), _shim.ptr(offsets), c.byref(need)))
+  if need.value > cap:
+    out = np.empty(int(need.value), dtype=np.uint8)
+    _shim.check(ctx.lib.ign_jpeg_encode(*args, _shim.ptr(out), c.c_uint64(need.value), _shim.ptr(offsets),
+                                        c.byref(need)))
+  return [out[int(offsets[i]):int(offsets[i + 1])].tobytes() for i in range(n)]
+
+
+def jpeg_encode(chunk, quality=85, restart_interval=None, ctx=None):
+  """uint8 chunk [x,y,z(,1)] -> the jpeg file as bytes."""
+  return jpeg_encode_batch([chunk], quality, restart_interval, ctx)[0]
+
+
+def jpeg_decode_batch(datas, shapes, ctx=None):
+  """jpeg files + their chunk shapes [x,y,z] or [x,y,z,1] -> list of uint8 chunks (Fortran order,
+  in the shapes given), one call for the batch."""
+  if len(datas) != len(shapes):
+    raise ValueError("%d streams but %d shapes" % (len(datas), len(shapes)))
+  n = len(datas)
+  if n == 0:
+    return []
+  given = [tuple(int(v) for v in s) for s in shapes]
+  shp = np.ascontiguousarray(np.array([_jpeg_shape(s) for s in given], dtype=np.uint32).reshape(n, 3))
+  lens = np.array([len(d) for d in datas], dtype=np.uint64)
+  offsets = np.zeros(n + 1, dtype=np.uint64)
+  np.cumsum(lens, out=offsets[1:])
+  packed = np.frombuffer(b"".join(bytes(d) for d in datas), dtype=np.uint8)
+  if packed.size == 0:
+    packed = np.zeros(1, np.uint8)
+  vox = shp.astype(np.uint64).prod(axis=1)
+  out = np.empty(max(int(vox.sum()), 1), dtype=np.uint8)
+  ctx = ctx or _shim.default_context()
+  _shim.check(ctx.lib.ign_jpeg_decode(ctx.handle, _shim.ptr(np.ascontiguousarray(packed)), _shim.ptr(offsets),
+                                      c.c_uint64(n), _shim.ptr(shp), _shim.ptr(out)))
+  res, at = [], 0
+  for s, v in zip(given, vox):
+    res.append(out[at:at + int(v)].reshape(s, order="F"))
+    at += int(v)
+  return res
+
+
+def jpeg_decode(data, shape, ctx=None):
+  """jpeg file bytes -> uint8 chunk of `shape` ([x,y,z] or [x,y,z,1], Fortran order)."""
+  return jpeg_decode_batch([data], [shape], ctx)[0]

@@ -363,12 +363,18 @@ class _ImageSource:
     if np.any((np.asarray(bbox.minpt) - np.asarray(off)) % np.asarray(cs)):
       raise ValueError("shard cutout %r is not chunk aligned" % (bbox,))
     out = {}
+    jpeg = {}  # jpeg chunks are encoded in one call
     for c in cv._chunks(mip, Bbox.clamp(bbox, cv.bounds_at(mip))):
       src = tuple(slice(int(a - o), int(b - o)) for a, b, o in zip(c.minpt, c.maxpt, bbox.minpt))
       block = np.asfortranarray(img[src].astype(cv.dtype, copy=False))
       if tuple(block.shape[:3]) != tuple(int(v) for v in c.size3()):
         raise ValueError("image %r does not cover chunk %r of %r" % (img.shape, c, bbox))
+      if cv._encoding(mip) == "jpeg":
+        jpeg[cv._chunk_id(mip, c)] = block
+        continue
       out[cv._chunk_id(mip, c)] = cv._encode_chunk(block, mip)
+    if jpeg:
+      out.update(zip(jpeg.keys(), cv._jpeg_encode(list(jpeg.values()), mip)))
     return out
 
   def make_shard(self, img, bbox, mip, progress=False):
@@ -593,11 +599,26 @@ class CloudVolume:
     blob = shard_cache[name]
     return None if blob is None else spec.read_chunk(blob, cid)
 
-  # chunk codecs: `raw` is the bytes of the Fortran-order array; `compressed_segmentation` goes
-  # through the device codec (igneous_b200.codecs); anything else the Precomputed format knows
-  # (jpeg, compresso, crackle, ...) is outside this stand-in
+  # chunk codecs: `raw` is the bytes of the Fortran-order array; `compressed_segmentation` and
+  # `jpeg` go through the device codecs (igneous_b200.codecs), jpeg a whole read or write per call;
+  # anything else the Precomputed format knows (png, compresso, crackle, ...) is outside this stand-in
   def _encoding(self, mip):
     return self.info["scales"][mip].get("encoding", "raw")
+
+  def _jpeg_check(self, mip):
+    if self.dtype != np.uint8 or self.num_channels != 1:
+      raise NotImplementedError("storage stand-in: jpeg scales hold one uint8 channel (got %s x %d)"
+                                % (self.dtype, self.num_channels))
+
+  def _jpeg_encode(self, blocks, mip):
+    self._jpeg_check(mip)
+    from . import codecs
+    return codecs.jpeg_encode_batch(blocks, quality=int(self.info["scales"][mip].get("jpeg_quality", 85)))
+
+  def _jpeg_decode(self, datas, mip, shapes):
+    self._jpeg_check(mip)
+    from . import codecs
+    return codecs.jpeg_decode_batch(datas, shapes)
 
   def _cseg_block(self, mip):
     return tuple(int(v) for v in self.info["scales"][mip].get("compressed_segmentation_block_size", (8, 8, 8)))
@@ -609,6 +630,8 @@ class CloudVolume:
     if enc == "compressed_segmentation":
       from . import codecs
       return codecs.cseg_encode(block, self._cseg_block(mip))
+    if enc == "jpeg":
+      return self._jpeg_encode([block], mip)[0]
     raise NotImplementedError("storage stand-in: chunk encoding %r is not supported" % enc)
 
   def _decode_chunk(self, data, mip, shape):
@@ -618,6 +641,8 @@ class CloudVolume:
     if enc == "compressed_segmentation":
       from . import codecs
       return codecs.cseg_decode(data, shape, self.dtype, self._cseg_block(mip))
+    if enc == "jpeg":
+      return self._jpeg_decode([data], mip, [shape])[0]
     raise NotImplementedError("storage stand-in: chunk encoding %r is not supported" % enc)
 
   def _to_bbox(self, key):
@@ -648,6 +673,7 @@ class CloudVolume:
       raise OutOfBoundsError("%r is outside %r" % (bbox, self.bounds_at(mip)))
     out = np.zeros(tuple(int(v) for v in bbox.size3()) + (self.num_channels,), dtype=self.dtype, order="F")
     shard_cache = {}
+    jpeg = []  # (chunk, intersection, bytes): jpeg chunks are decoded in one call
     for c in self._chunks(mip, bbox):
       data = self._read_chunk(mip, c, shard_cache)
       inter = Bbox.intersection(c, bbox)
@@ -657,10 +683,19 @@ class CloudVolume:
         if not self.fill_missing:
           raise EmptyVolumeException(self._chunk_name(mip, c))
         continue
+      if self._encoding(mip) == "jpeg":
+        jpeg.append((c, inter, data))
+        continue
       chunk = self._decode_chunk(data, mip, tuple(int(v) for v in c.size3()) + (self.num_channels,))
       src = tuple(slice(int(a - o), int(b - o)) for a, b, o in zip(inter.minpt, inter.maxpt, c.minpt))
       dst = tuple(slice(int(a - o), int(b - o)) for a, b, o in zip(inter.minpt, inter.maxpt, bbox.minpt))
       out[dst] = chunk[src]
+    if jpeg:
+      shapes = [tuple(int(v) for v in c.size3()) + (self.num_channels,) for c, _, _ in jpeg]
+      for (c, inter, _), chunk in zip(jpeg, self._jpeg_decode([d for _, _, d in jpeg], mip, shapes)):
+        src = tuple(slice(int(a - o), int(b - o)) for a, b, o in zip(inter.minpt, inter.maxpt, c.minpt))
+        dst = tuple(slice(int(a - o), int(b - o)) for a, b, o in zip(inter.minpt, inter.maxpt, bbox.minpt))
+        out[dst] = chunk[src]
     return out
 
   def __getitem__(self, key):
@@ -677,6 +712,7 @@ class CloudVolume:
     img = img.astype(self.dtype, copy=False)
     if self._sharding(mip) is not None:
       raise NotImplementedError("writes to a sharded scale go through image.make_shard (whole shards only)")
+    jpeg = []  # (name, block): jpeg chunks are encoded in one call
     for c in self._chunks(mip, bbox):
       inter = Bbox.intersection(c, bbox)
       if inter.subvoxel():
@@ -689,7 +725,13 @@ class CloudVolume:
       if self.delete_black_uploads and not np.any(block != self.background_color):
         self.cf.delete(name)
         continue
+      if self._encoding(mip) == "jpeg":
+        jpeg.append((name, block))
+        continue
       self.cf.put(name, self._encode_chunk(block, mip), compress=self.compress)
+    if jpeg:  # already entropy coded: stored without gzip, as CloudVolume stores jpeg chunks
+      for (name, _), data in zip(jpeg, self._jpeg_encode([b for _, b in jpeg], mip)):
+        self.cf.put(name, data)
 
 
 # --------------------------------------------------------------------- queue

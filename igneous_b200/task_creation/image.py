@@ -91,8 +91,9 @@ def create_downsampling_tasks(layer_path, mip=0, fill_missing=False, axis="z", n
 
 
 def set_encoding(cv, mip, encoding, encoding_level, encoding_effort):
-  """task_creation/common.py:215-236 (the lossy-codec quality keys are recorded but those
-  codecs are outside this implementation)."""
+  """task_creation/common.py:215-236.  `jpeg_quality` is what the device jpeg codec encodes a
+  scale with (85 when absent); the jxl / png / fpzip keys are recorded, but those codecs are
+  outside this implementation."""
   scale = cv.scales[mip]
   if encoding is not None:
     scale["encoding"] = encoding

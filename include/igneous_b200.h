@@ -388,6 +388,36 @@ IGN_API int ign_cseg_decode_dev(ign_ctx* ctx, const uint32_t* in, uint64_t n_wor
                                 uint64_t sy, uint64_t sz, uint64_t sc, uint32_t bx, uint32_t by,
                                 uint32_t bz, void* out);
 
+/* ------------------------------------------------------------------ jpeg codec
+ * The Precomputed `jpeg` chunk encoding of uint8 image layers, which CloudVolume applies on the host
+ * around the image tasks (igneous/tasks/image/image.py:95-100 uploads; the CLI's image encoding,
+ * igneous_cli/cli.py:64; `jpeg_quality` set by igneous/task_creation/common.py:215-236 set_encoding;
+ * the png top mip of a sharded jpeg pyramid, task_creation/image.py:708-709).  A chunk [x,y,z] of
+ * uint8 (one channel) is one grayscale JPEG of width sx and height sy*sz: image row y + sy*z, so the
+ * Fortran-order chunk is the raster.  Each side of the image is at most 65535 pixels.
+ * encode: byte-identical to libjpeg's defaults at the same quality (1..100) and restart interval:
+ * JFIF APP0, the IJG-scaled Annex K table, SOF0, the Annex K Huffman tables, accurate integer DCT.
+ * restart_interval: blocks between RSTn markers; 0 = no markers; < 0 = one block row of each chunk,
+ * which lets ign_jpeg_decode give each row its own thread.
+ * decode: pixel-identical to libjpeg's islow decode of any SOF0 / SOF1 8-bit grayscale stream
+ * (any Huffman tables, APPn / COM, fill bytes, restart markers or none); progressive, arithmetic,
+ * lossless, 12-bit, multi-component and DNL streams fail with IGN_ERR_UNSUPPORTED, malformed or
+ * truncated ones and dimensions other than the chunk's with IGN_ERR_INVALID.
+ * Batches: chunks / outputs are packed back to back; shapes are host arrays of n x {sx, sy, sz}.
+ * encode: *n_bytes = bytes of all streams; nothing is written when out is NULL or cap is too small;
+ * else offsets[0..n] (host) delimit stream c as out[offsets[c] : offsets[c+1]].
+ * decode: stream c is streams[offsets[c] : offsets[c+1]] (offsets on the host). */
+IGN_API int ign_jpeg_encode(ign_ctx* ctx, const uint8_t* chunks, uint64_t n_chunks, const uint32_t* shapes,
+                            int quality, int64_t restart_interval, uint8_t* out, uint64_t cap, uint64_t* offsets,
+                            uint64_t* n_bytes);
+IGN_API int ign_jpeg_encode_dev(ign_ctx* ctx, const uint8_t* chunks, uint64_t n_chunks, const uint32_t* shapes,
+                                int quality, int64_t restart_interval, uint8_t* out, uint64_t cap,
+                                uint64_t* offsets, uint64_t* n_bytes);
+IGN_API int ign_jpeg_decode(ign_ctx* ctx, const uint8_t* streams, const uint64_t* offsets, uint64_t n_streams,
+                            const uint32_t* shapes, uint8_t* out);
+IGN_API int ign_jpeg_decode_dev(ign_ctx* ctx, const uint8_t* streams, const uint64_t* offsets, uint64_t n_streams,
+                                const uint32_t* shapes, uint8_t* out);
+
 /* --------------------------------------------------- synthetic volumes (bench)
  * SURVEY.md 8(d): jittered-grid Voronoi segmentation / hash-byte image,
  * bit-identical to oracle.synth_seg / oracle.synth_image. */
