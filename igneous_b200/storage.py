@@ -403,6 +403,7 @@ class CloudVolume:
     self.cf = CloudFiles(cloudpath)
     self.provenance = _Provenance()
     self.mesh = _MeshMeta()
+    self.skeleton = self.mesh  # cv.skeleton.spatial_index.precision is cv.mesh's
     if info is not None:
       self.info = copy.deepcopy(info)
     else:

@@ -3,10 +3,13 @@
 import copy
 import os
 import subprocess
+from functools import partial
+from time import strftime
 
 import numpy as np
 
-from .._compat import Bbox, Vec
+from .._compat import Bbox, CloudFiles, CloudVolume, Vec
+from ..tasks import SpatialIndexTask
 
 
 def operator_contact():
@@ -64,3 +67,43 @@ class FinelyDividedTaskIterator:
 
   def on_finish(self):
     pass
+
+
+def spatial_index_tasks(cloudpath, shape, mip, fill_missing, compress, subdir, kind):
+  """The body the mesh and skeleton spatial-index creators share (task_creation/mesh.py:363-435,
+  task_creation/skeleton.py:795-867).  kind is "mesh" or "skeletons": the info key naming the
+  directory.  Sets the layer's directory if it has none, records @type / mip / chunk_size /
+  spatial_index in {subdir}/info when they change, and yields one SpatialIndexTask per grid cell."""
+  shape = Vec(*shape)
+  vol = CloudVolume(cloudpath, mip=mip)
+  if subdir is None:
+    subdir = vol.info.get(kind) or ("mesh_mip_%d_err_40" % mip if kind == "mesh" else "skeletons_mip_%d" % mip)
+  if kind not in vol.info:
+    vol.info[kind] = subdir
+    vol.commit_info()
+  cf = CloudFiles(cloudpath)
+  info_filename = cf.join(subdir, "info")
+  info = cf.get_json(info_filename) or {}
+  new_info = copy.deepcopy(info)
+  new_info["@type"] = new_info.get("@type", "neuroglancer_legacy_mesh" if kind == "mesh" else "neuroglancer_skeletons")
+  new_info["mip"] = new_info.get("mip", int(vol.mip))
+  new_info["chunk_size"] = shape.tolist()
+  new_info["spatial_index"] = {"resolution": vol.resolution.tolist(), "chunk_size": (shape * vol.resolution).tolist()}
+  if new_info != info:
+    cf.put_json(info_filename, new_info)
+  vol = CloudVolume(cloudpath, mip=mip)  # reload the spatial index
+  precision = (vol.mesh if kind == "mesh" else vol.skeleton).spatial_index.precision
+
+  class SpatialIndexTaskIterator(FinelyDividedTaskIterator):
+    def task(self, shape, offset):
+      return partial(SpatialIndexTask, cloudpath=cloudpath, shape=shape, offset=offset, subdir=subdir,
+                     precision=precision, mip=int(mip), fill_missing=bool(fill_missing), compress=compress)
+
+    def on_finish(self):
+      vol.provenance.processing.append({
+        "method": {"task": "SpatialIndexTask", "cloudpath": vol.cloudpath, "shape": shape.tolist(), "mip": int(mip),
+                   "subdir": subdir, "fill_missing": fill_missing, "compress": compress},
+        "by": operator_contact(), "date": strftime("%Y-%m-%d %H:%M %Z")})
+      vol.commit_provenance()
+
+  return SpatialIndexTaskIterator(vol.bounds, shape)

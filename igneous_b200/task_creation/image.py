@@ -1,6 +1,6 @@
 """create_downsampling_tasks, create_image_shard_downsample_tasks, the contrast / CLAHE /
-quantize creators and the three CCL task creators (igneous/task_creation/image.py:170-345,
-639-770, 1247-1618, 1726-1889): same
+quantize creators, the three CCL task creators and create_voxel_counting_tasks
+(igneous/task_creation/image.py:170-345, 639-770, 1247-1618, 1726-1936): same
 signatures, same info / provenance side effects, tasks from igneous_b200.tasks."""
 import copy
 import math
@@ -10,9 +10,9 @@ from time import strftime
 import numpy as np
 
 from .. import downsample_scales, fastremap, sharding, shards
-from .._compat import Bbox, CloudVolume, CloudFiles, InfoUnavailableError, Vec
+from .._compat import Bbox, CloudVolume, CloudFiles, InfoUnavailableError, Vec, min2
 from ..tasks import (DownsampleTask, ImageShardDownsampleTask, CCLFacesTask, CCLEquivalancesTask, RelabelCCLTask,
-                     QuantizeTask, CLAHETask, ContrastNormalizationTask, LuminanceLevelsTask)
+                     QuantizeTask, CLAHETask, ContrastNormalizationTask, LuminanceLevelsTask, CountVoxelsTask)
 from ..types import DownsampleMethods
 from .common import FinelyDividedTaskIterator, get_bounds, operator_contact
 
@@ -400,3 +400,23 @@ def create_quantize_tasks(src_layer, dest_layer, shape, mip=0, fill_missing=Fals
            shape=[int(v) for v in shape], fill_missing=fill_missing, mip=mip)
 
   return QuantizeTasksIterator(bounds, shape)
+
+
+def create_voxel_counting_tasks(cloudpath, mip, fill_missing=False, agglomerate=False, timestamp=None):
+  """Count the voxels of every label in 512^3 tasks (clamped at the far edges) and write the JSON
+  files to {key}/stats/voxel_counts/{bbox}.json (task_creation/image.py:1891-1936)."""
+  vol = CloudVolume(cloudpath, max_redirects=0, mip=mip)
+  shape = Vec(512, 512, 512)
+  bounds = vol.bounds.clone()
+
+  class CountVoxelsTaskIterator(FinelyDividedTaskIterator):
+    def task(self, shape, offset):
+      bounded_shape = min2(shape, bounds.maxpt - offset)
+      return partial(CountVoxelsTask, cloudpath=cloudpath, shape=bounded_shape.clone(), offset=offset.clone(), mip=mip,
+                     fill_missing=fill_missing, agglomerate=agglomerate, timestamp=timestamp)
+
+    def on_finish(self):
+      _log(CloudVolume(cloudpath, max_redirects=0), "CountVoxelsTask", cloudpath=cloudpath, mip=mip,
+           shape=shape.tolist(), fill_missing=fill_missing, agglomerate=agglomerate, timestamp=timestamp)
+
+  return CountVoxelsTaskIterator(bounds, shape)

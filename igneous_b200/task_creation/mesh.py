@@ -1,9 +1,10 @@
-"""create_meshing_tasks (igneous/task_creation/mesh.py:158-267)."""
+"""create_meshing_tasks (igneous/task_creation/mesh.py:158-267) and
+create_spatial_index_mesh_tasks (:363-435)."""
 from time import strftime
 
 from .._compat import CloudVolume, CloudFiles, Vec
 from ..tasks import MeshTask
-from .common import FinelyDividedTaskIterator, operator_contact
+from .common import FinelyDividedTaskIterator, operator_contact, spatial_index_tasks
 
 
 def create_meshing_tasks(layer_path, mip, shape=(448, 448, 448), simplification=True,
@@ -48,3 +49,10 @@ def create_meshing_tasks(layer_path, mip, shape=(448, 448, 448), simplification=
       vol.commit_provenance()
 
   return MeshTaskIterator(vol.mip_bounds(mip), shape)
+
+
+def create_spatial_index_mesh_tasks(cloudpath, shape=(448, 448, 448), mip=0, fill_missing=False, compress="gzip",
+                                    mesh_dir=None):
+  """Rebuild the spatial index of a mesh directory (default: the layer's, else mesh_mip_{mip}_err_40),
+  or build one over a different grid than the mesh tasks used."""
+  return spatial_index_tasks(cloudpath, shape, mip, fill_missing, compress, mesh_dir, "mesh")

@@ -3,7 +3,7 @@
 Same names, arguments and side effects as igneous/tasks/image/image.py:
   downsample_method_to_fn :37-55, downsample_and_upload :57-100,
   TransferTask :434-516, DownsampleTask :518-549.
-  ImageShardDownsampleTask :672-843.
+  ImageShardDownsampleTask :672-843, CountVoxelsTask :845-880.
   QuantizeTask :145-162, CLAHETask :164-209, ContrastNormalizationTask :211-343,
   LuminanceLevelsTask :345-432 (per-voxel work in igneous_b200.contrast).
 Only the library behind `fn(image, factors[0], num_mips=...)` (:91) changes:
@@ -193,6 +193,22 @@ def ImageShardDownsampleTask(src_path, shape, offset, mip=0, fill_missing=False,
       filename, blob = src.image.make_shard(chunk_dict, shard_box, m, progress=False)
       CloudFiles(base).put(filename, blob, compress=None)
     pending[i] = None
+
+
+@queueable
+def CountVoxelsTask(cloudpath, shape, offset, mip=0, fill_missing=False, agglomerate=False, timestamp=None):
+  """Voxel count of every label (0 included) in the task's box, clamped to the dataset, written to
+  {key}/stats/voxel_counts/{bbox}.json (image.py:845-880); the counts come from fastremap.unique
+  on the GPU."""
+  shape, offset = Vec(*shape), Vec(*offset)
+  mip = int(mip)
+  cv = CloudVolume(cloudpath, fill_missing=bool(fill_missing), mip=mip, bounded=False, progress=False)
+  bbox = Bbox.clamp(Bbox(offset, offset + shape), cv.meta.bounds(mip))
+  labels = cv.download(bbox, agglomerate=agglomerate, timestamp=timestamp)
+  uniq, cts = fastremap.unique(labels, return_counts=True)
+  voxel_counts = {str(int(segid)): int(ct) for segid, ct in zip(uniq, cts)}
+  cf = CloudFiles(cloudpath)
+  cf.put_json(cf.join(cv.key, "stats", "voxel_counts", "%s.json" % bbox.to_filename()), voxel_counts)
 
 
 def _shard_chunks(vol, cutout, box, mip):

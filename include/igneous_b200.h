@@ -324,6 +324,23 @@ IGN_API int ign_inverse_component_map(ign_ctx* ctx, const void* parents, const v
 /* widen/narrow unsigned integer arrays on the device */
 IGN_API int ign_cast_dev(ign_ctx* ctx, const void* in, int in_dtype, void* out, int out_dtype, uint64_t n);
 
+/* ---------------------------------------------------------- label statistics
+ * scipy.ndimage.find_objects(labels)                 igneous/tasks/spatial_index.py:10-20, :56
+ *   (sx, sy, sz) volume of u8 / u16 / u32 / u64 labels, each side below 2^31.
+ *   *max_label == 0: the largest label is found on the device and written to *max_label
+ *     (0 for an empty or all-zero volume); boxes is not touched.  The _dev variant
+ *     synchronises the ctx stream in this case.
+ *   *max_label == N > 0: boxes[N][6] (a DEVICE array for _dev, a HOST array otherwise)
+ *     receives, for label l = 1..N in row l - 1, (min x, min y, min z, max x, max y, max z),
+ *     maxima inclusive.  A label without voxels has mins 0xFFFFFFFF and maxima 0.  Label 0
+ *     and labels above N are ignored.  The volume is read once.
+ *   A given or found N of 2^32 or more -> IGN_ERR_UNSUPPORTED (renumber the labels first).
+ */
+IGN_API int ign_find_objects(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy,
+                             uint64_t sz, uint64_t* max_label, uint32_t* boxes);
+IGN_API int ign_find_objects_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy,
+                                 uint64_t sz, uint64_t* max_label, uint32_t* boxes);
+
 /* --------------------------------------------------------------------- mesh
  * zmesh.Mesher(resolution).mesh(data, preserve_order=False)  igneous/tasks/mesh/mesh.py:151,245
  * Mesher.ids()                                                igneous/tasks/mesh/mesh.py:374
