@@ -40,6 +40,7 @@
 //              lookup table (dust, multi-GPU relabelling); u16 / u32 / u64.
 // HBM traffic ~ in + 0.625 (A) + ~0.6 (B, R: masks + runs) + 0.25 + out (C)
 // bytes/voxel; algorithmic bytes (cc3d contract) = in + out.
+#include <cub/device/device_reduce.cuh>
 #include <cub/device/device_scan.cuh>
 #include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
@@ -653,6 +654,9 @@ struct PopcOp {
 #endif
   }
 };
+struct Popc64Op {
+  __host__ __device__ __forceinline__ uint64_t operator()(uint32_t w) const { return PopcOp()(w); }
+};
 
 // parent[r] (flattened) -> label of the run: rank of its root + 1
 __global__ void __launch_bounds__(256)
@@ -804,7 +808,8 @@ __global__ void __launch_bounds__(256)
 
 // ------------------------------------------------------------------- dust
 // voxels per component: every x-segment of a run inside a word adds its length once
-__global__ void __launch_bounds__(256) k_ccl_count(const ExpandArgs a, uint32_t* __restrict__ counts) {
+// (64-bit: one component of a 2^32+ voxel volume can hold 2^32 voxels)
+__global__ void __launch_bounds__(256) k_ccl_count(const ExpandArgs a, unsigned long long* __restrict__ counts) {
   const uint64_t wi = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (wi >= a.rows * a.wpr) return;
   const uint32_t S = a.S[wi], Z = a.Z[wi];
@@ -819,12 +824,12 @@ __global__ void __launch_bounds__(256) k_ccl_count(const ExpandArgs a, uint32_t*
     const uint32_t stop = (p == 31) ? 0u : ((S | ~Z) & ~mask_le(p));
     const uint32_t q = stop ? (uint32_t)(__ffs(stop) - 1) : 32u;
     const uint32_t l = a.label[rb + __popc(S & mask_le(p)) - 1];
-    atomicAdd(&counts[l], q - p);
+    atomicAdd(&counts[l], (unsigned long long)(q - p));
   }
 }
 
 __global__ void __launch_bounds__(256)
-    k_dust_flags(const uint32_t* __restrict__ counts, uint32_t n, uint64_t threshold, uint32_t* __restrict__ keep) {
+    k_dust_flags(const unsigned long long* __restrict__ counts, uint32_t n, uint64_t threshold, uint32_t* __restrict__ keep) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i <= n + 1) keep[i] = (i >= 1 && i <= n && (uint64_t)counts[i] >= threshold) ? 1u : 0u;
 }
@@ -1067,17 +1072,35 @@ static int ccl_structure(ign_ctx* ctx, ScratchFrame& f, const R& rd, uint32_t sx
     IGN_CUDA(cub::DeviceScan::ExclusiveSum(p.cub_tmp, tb, it, p.rbase, (int)(W + 1), ctx->stream));
     ctx->launches += 2;
   }
+  // rbase[W] is the run count modulo 2^32; a volume of 2^32+ voxels can hold 2^32+ runs, so there
+  // the count is a 64-bit sum of popc(S) (one more read of S)
   uint32_t hR = 0;
+  uint64_t runs = 0;
   IGN_TRY(small_d2h(ctx, &hR, p.rbase + W, 4));
+  if (p.n >= (1ull << 32)) {
+    auto it = thrust::make_transform_iterator((const uint32_t*)p.S, Popc64Op());
+    uint64_t* d_runs;
+    void* tmp;
+    size_t tb = 0;
+    cub::DeviceReduce::Sum(nullptr, tb, it, (uint64_t*)nullptr, (int)W);
+    IGN_TRY(f.take(&d_runs, 1));
+    IGN_TRY(f.take(&tmp, tb));
+    IGN_CUDA(cub::DeviceReduce::Sum(tmp, tb, it, d_runs, (int)W, ctx->stream));
+    ctx->launches += 2;
+    IGN_TRY(small_d2h(ctx, &runs, d_runs, 8));
+  }
   IGN_TRY(small_sync(ctx));
-  p.R = hR;
-  if ((uint64_t)hR > rcap) {
-    *need_rcap = hR;
+  if (p.n < (1ull << 32)) runs = hR;
+  // refused before the run arrays are sized from the count
+  IGN_REQUIRE(runs < 0x7FFFFFF0ull, IGN_ERR_OVERFLOW, "CCL: %llu runs exceed the 2^31 limit; split the volume into tasks",
+              (unsigned long long)runs);
+  p.R = (uint32_t)runs;
+  if (runs > rcap) {
+    *need_rcap = runs;
     return IGN_OK;
   }
-  if (hR == 0) return IGN_OK;
-  IGN_REQUIRE(hR < 0x7FFFFFF0u, IGN_ERR_OVERFLOW, "CCL: %u runs exceed the 2^31 limit; split the volume into tasks", hR);
-  const uint32_t Rn = hR;
+  if (runs == 0) return IGN_OK;
+  const uint32_t Rn = p.R;
   // ---- pass B: tiles, then the rows on tile faces
   uint32_t TY = 8;
   while (TY > 1 && (uint64_t)p.wpr * TY * TY > (uint64_t)TB_WMAX) TY >>= 1;
@@ -1186,8 +1209,8 @@ static int dust_runs(ign_ctx* ctx, CclPlan& p, uint64_t threshold, uint32_t* kep
   *kept = N;
   if (N == 0 || p.R == 0) return IGN_OK;
   ScratchFrame f(ctx);
-  const size_t bytes = ((size_t)N + 2) * 4;
-  uint32_t *counts, *keep, *scan, *lut;
+  unsigned long long* counts;
+  uint32_t *keep, *scan, *lut;
   IGN_TRY(f.take(&counts, (size_t)N + 2));
   IGN_TRY(f.take(&keep, (size_t)N + 2));
   IGN_TRY(f.take(&scan, (size_t)N + 2));
@@ -1196,7 +1219,7 @@ static int dust_runs(ign_ctx* ctx, CclPlan& p, uint64_t threshold, uint32_t* kep
   cub::DeviceScan::ExclusiveSum(nullptr, tb, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)(N + 2));
   void* tmp;
   IGN_TRY(f.take(&tmp, tb + 256));
-  IGN_CUDA(cudaMemsetAsync(counts, 0, bytes, ctx->stream));
+  IGN_CUDA(cudaMemsetAsync(counts, 0, ((size_t)N + 2) * sizeof(*counts), ctx->stream));
   const ExpandArgs e = p.expand_args(0);
   IGN_LAUNCH(ctx, k_ccl_count, blocks_for(p.W, 256), 256, 0, e, counts);
   IGN_LAUNCH(ctx, k_dust_flags, blocks_for((uint64_t)N + 2, 256), 256, 0, counts, N, threshold, keep);

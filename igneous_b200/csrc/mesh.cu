@@ -23,6 +23,7 @@
 #include <cub/device/device_scan.cuh>
 
 #include <atomic>
+#include <climits>
 #include <vector>
 
 #include "common.cuh"
@@ -352,7 +353,9 @@ int ign_mesh_begin_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx,
     *out = m;
     return IGN_OK;
   }
-  IGN_REQUIRE(3 * T < 0xFFFFFFFFull, IGN_ERR_OVERFLOW, "mesher: %llu triangles exceed 32-bit corner indices", T);
+  // the sorts and the scan below take int item counts: 3T corners must fit an int
+  IGN_REQUIRE(3 * T <= (unsigned long long)INT_MAX, IGN_ERR_OVERFLOW,
+              "mesher: %llu triangles exceed 2^31 - 1 corners; split the volume into tasks", T);
 
   // ---- emit + sort + weld buffers
   size_t sort1 = 0, sort2 = 0, scanb = 0;
