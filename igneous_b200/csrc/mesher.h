@@ -23,6 +23,7 @@ struct ign_mesher {
   uint32_t simp_labels_smem, simp_labels_gmem;  // labels simplified in shared / global memory
   uint32_t simp_labels_class[3];                // labels simplified in 1024-, 512- and 256-thread CTAs
   uint32_t simp_migrations[3];                  // labels resumed in each class after they shrank
+  uint32_t simp_passes[2];                      // multi-pass label-rounds, winners with a ring over 32 faces
   std::vector<uint64_t> ids;       // original label of dense id i+1
   std::vector<uint32_t> tri_off;   // [K+2]
   std::vector<uint32_t> vert_off;  // [K+2]

@@ -243,7 +243,7 @@ __global__ void __launch_bounds__(256) k_simp_boundary(Simp s) {
 //       round formulation: key2[w] == key1[w] <=> !LOSE[w]); plain byte stores
 //                                                               (face parallel)
 //   P4  a vertex a WINs iff its key's half-edge starts at a, both endpoints hold that
-//       key and neither LOSEs; at most SL_WCAP winners per pass  (vertex parallel)
+//       key and neither LOSEs; at most L.wcap winners per pass   (vertex parallel)
 //   E1  the faces that touch a winner's endpoints append themselves to the winner's
 //       two ring lists; the first warps compute the winners' placement and cost (E2a)
 //       at the same time                                         (face parallel)
@@ -259,7 +259,10 @@ __global__ void __launch_bounds__(256) k_simp_boundary(Simp s) {
 // changed (parked edges around it may be valid now)
 constexpr uint32_t VF_ALIVE = 1, VF_BOUND = 2, VF_CDIRTY = 4, VF_DONE = 16, VF_END = 32, VF_RDIRTY = 64;
 constexpr int SL_THREADS = 1024;
-constexpr int SL_WCAP = 128;  // winners validated per selection pass (a round runs as many passes as it needs)
+// winners validated per selection pass (a round runs as many passes as it needs): every label that fits a
+// class has room for SL_WCAP; a shared-memory label takes more where the class's shared memory leaves room
+// (sl_wcap), since each further pass rescans the vertices (P4) and the alive faces (E1)
+constexpr int SL_WCAP = 128;
 constexpr uint32_t WF_BAD = 1, WF_OK = 2;  // winner flags: failed validation / validated
 constexpr int SL_EQ = 96;      // per-warp queue of faces with half-edges whose cost must be (re)computed
 constexpr int SL_LIST_PER = 16;  // list entries per thread held in registers while a list is compacted in place
@@ -270,16 +273,26 @@ constexpr int SL_LIST_PER = 16;  // list entries per thread held in registers wh
 constexpr int SL_NCLASS = 3;
 constexpr int SL_CLASS_THREADS[SL_NCLASS] = {1024, 512, 256};
 
-// dynamic shared-memory layout of a label at `threads` threads:
-// cost queues | ring lists | key1 | faces SoA | face list | face state | vertex flags | lose marks
+// a winner of a selection pass: its edge, ring lengths, flags and placement (dynamic shared memory)
+struct SlWin {
+  double best[3];
+  uint32_t u, v, h, cnt[2], keep, flags, pad;
+};
+// shared memory a shared-memory label needs per winner of a pass: the record and two 16-bit ring lists
+constexpr size_t SL_WIN_BYTES = sizeof(SlWin) + 2 * S_MAXV * 2;
+
+// dynamic shared-memory layout of a label at `threads` threads with `wcap` winners per pass:
+// winners | cost queues | ring lists | key1 | faces SoA | face list | face state | vertex flags | lose marks
 // [| original face ids | original vertex ids: a label resumed in a smaller class after migrating]
 struct SlLayout {
-  size_t wq, o_key, o_f0, o_fl, o_fs, o_vf, o_vl, o_fm, o_vm, need;
+  size_t o_wq, o_ring, o_key, o_f0, o_fl, o_fs, o_vf, o_vl, o_fm, o_vm, need;
 };
-__host__ __device__ inline SlLayout sl_layout(uint32_t T, uint32_t U, uint32_t threads, bool resumed = false) {
+__host__ __device__ inline SlLayout sl_layout(uint32_t T, uint32_t U, uint32_t threads, bool resumed = false,
+                                              uint32_t wcap = SL_WCAP) {
   SlLayout y;
-  y.wq = (size_t)(threads / 32) * SL_EQ * 4;
-  y.o_key = y.wq + (size_t)SL_WCAP * 2 * S_MAXV * 2;  // shared-memory class: 16-bit face ids in the rings
+  y.o_wq = (size_t)wcap * sizeof(SlWin);
+  y.o_ring = y.o_wq + (size_t)(threads / 32) * SL_EQ * 4;
+  y.o_key = y.o_ring + (size_t)wcap * 2 * S_MAXV * 2;  // shared-memory class: 16-bit face ids in the rings
   y.o_f0 = y.o_key + 4 * (size_t)U;                    // 32-bit keys
   y.o_fl = y.o_f0 + 6 * (size_t)T;
   y.o_fs = y.o_fl + 2 * (size_t)T;
@@ -295,6 +308,14 @@ __host__ __device__ inline bool sl_fits_smem(uint32_t T, uint32_t U, uint32_t th
                                              bool resumed = false) {
   const uint32_t cap = (uint32_t)SL_LIST_PER * threads;
   return 3ull * T <= 65536ull && T <= cap && U <= cap && sl_layout(T, U, threads, resumed).need <= smem_bytes;
+}
+// winners per pass of a label that sl_fits_smem accepts: SL_WCAP plus what the rest of the budget holds, at
+// most one per thread (E2a gives each winner a thread) and at most `limit` (IGN_SIMP_WCAP)
+__host__ __device__ inline uint32_t sl_wcap(uint32_t T, uint32_t U, uint32_t threads, size_t smem_bytes,
+                                            bool resumed, uint32_t limit) {
+  const size_t w = SL_WCAP + (smem_bytes - sl_layout(T, U, threads, resumed).need) / SL_WIN_BYTES;
+  const size_t m = threads < limit ? threads : limit;
+  return (uint32_t)(w < m ? w : m);
 }
 
 struct SlArgs {
@@ -339,25 +360,25 @@ struct SlArgs {
                         // (sum of list lengths), winners, memory class | size class << 2, SM kilocycles
                         // (kilocycles / CTAs per SM); a migrated label sums its segments
   uint32_t* trace;      // IGN_SIMP_TRACE=1: [round][4] = winners, collapses, alive faces, list length of the largest label
+                        // [SL_HIST +] per size class: selection passes, winners, ring lengths per round (SL_H*)
+  uint32_t wcap_max;    // most winners per pass (IGN_SIMP_WCAP; default: no limit beyond the budget)
 };
 
-struct SlWin {
-  uint32_t u, v, h, cnt[2], keep, flags, pad;
-};
+// IGN_SIMP_TRACE histograms, per size class the segment runs in: passes per round (1..SL_HP, last bin more),
+// winners per round before capping (bins of 16, last bin more), ring length per winner side (0..S_MAXV, more)
+constexpr int SL_HIST = 1664, SL_HP = 16, SL_HW = 64, SL_HR = S_MAXV + 2, SL_HCLS = SL_HP + SL_HW + SL_HR;
 
 // header of a migrated label: dense label, trace record, next round, slow rounds, alive faces, alive vertices
 constexpr int SL_MREC = 8;
 constexpr int SL_LREC = 7;  // words of a label's IGN_SIMP_TRACE record (SlArgs::lrec)
 
 struct SlShared {
-  uint32_t work, alive, progress, ncol, nwin, stop, slow, counter, nbig;
+  uint32_t work, alive, progress, ncol, nwin, stop, slow, counter, nbig, npass, bigring;
   uint32_t rec, valive;  // trace record of the label; alive vertices (one dies per collapse)
   unsigned long long visits, wins;  // IGN_SIMP_TRACE
   long long t_label;
   unsigned long long ph[10];  // phase timers (IGN_SIMP_TRACE)
   long long t_prev;
-  SlWin win[SL_WCAP];
-  double wbest[SL_WCAP * 3];  // placement of the round's winners
 };
 
 template <bool SM>
@@ -376,8 +397,9 @@ struct SlLab {
   typedef typename std::conditional<SM, uint32_t, unsigned long long>::type key_t;
   key_t* key1;
   bool fmt16;
+  uint32_t wcap;   // winners per selection pass (their records are at the start of the dynamic shared memory)
   uint32_t* wq;    // [warps][SL_EQ] per-warp cost queues of the key pass (shared memory)
-  idx_t* ring;     // [SL_WCAP][2][S_MAXV] face ids of the winners' rings (shared memory)
+  idx_t* ring;     // [wcap][2][S_MAXV] face ids of the winners' rings (shared memory)
   idx_t *flist, *flist2, *vlist, *vlist2;  // alive lists (flist2 / vlist2: global-memory class only)
 };
 
@@ -618,6 +640,11 @@ __device__ __forceinline__ uint32_t sl_compact(IDX*& list, IDX*& list2, uint32_t
     }                                                 \
   } while (0)
 
+extern __shared__ __align__(16) unsigned char sl_smem[];
+
+// the winner records of the pass (SlLayout: first in the dynamic shared memory)
+__device__ __forceinline__ SlWin* sl_win() { return (SlWin*)sl_smem; }
+
 // One pass of E2c with groups of W lanes (16: two winners per warp side by side, only winners whose
 // rings fit 16 lanes; 32: the winners left over).  Both halves of a warp run the same instructions;
 // everything that differs between them is predicated and loop counts are made warp uniform.
@@ -630,25 +657,27 @@ __device__ __forceinline__ void sl_collapse_pass(const SlArgs& A, const SlLab<SM
   const uint32_t wmask = W == 32 ? FULL : 0xFFFFu;
   const uint32_t gmask = wmask << goff;
   const uint32_t gidx = lane / W;
+  SlWin* const win = sl_win();
   for (uint32_t base = warp * G; base < nb; base += NW * G) {  // warp uniform
     const uint32_t slot = base + gidx;
     bool act = slot < nb;
     uint32_t nfu = 0, nfv = 0;
-    if (act) { nfu = sh.win[slot].cnt[0]; nfv = sh.win[slot].cnt[1]; }
+    if (act) { nfu = win[slot].cnt[0]; nfv = win[slot].cnt[1]; }
     const bool big = nfu > 16u || nfv > 16u;
     if (W == 16) {
       if (act && big && gl == 0) atomicAdd(&sh.nbig, 1u);
       act = act && !big;
     } else {
       act = act && big;
+      if (act && gl == 0 && (nfu > (uint32_t)S_MAXV || nfv > (uint32_t)S_MAXV)) atomicAdd(&A.counters[25], 1u);
     }
     uint32_t fu = 0, fv = 0, u = 0, v = 0, hl = 0, k = 0;
     bool ok = false;
     if (act) {
       if (gl < nfu && gl < (uint32_t)S_MAXV) fu = L.ring[(2 * slot) * S_MAXV + gl];
       if (gl < nfv && gl < (uint32_t)S_MAXV) fv = L.ring[(2 * slot + 1) * S_MAXV + gl];
-      u = sh.win[slot].u; v = sh.win[slot].v; hl = sh.win[slot].h; k = sh.win[slot].keep;
-      ok = !(sh.win[slot].flags & WF_BAD) && nfu <= (uint32_t)S_MAXV && nfv <= (uint32_t)S_MAXV;
+      u = win[slot].u; v = win[slot].v; hl = win[slot].h; k = win[slot].keep;
+      ok = !(win[slot].flags & WF_BAD) && nfu <= (uint32_t)S_MAXV && nfv <= (uint32_t)S_MAXV;
     }
     const uint32_t rm = (k == u) ? v : u;
     // the quadrics of the two endpoints are needed only if the collapse happens, but the L2 round
@@ -724,7 +753,7 @@ __device__ __forceinline__ void sl_collapse_pass(const SlArgs& A, const SlLab<SM
       if (hu && x1 != v && x2 != v) { sl_vor<SM>(L.vflag, x1, VF_RDIRTY); sl_vor<SM>(L.vflag, x2, VF_RDIRTY); }
       if (hv && y1 != u && y2 != u) { sl_vor<SM>(L.vflag, y1, VF_RDIRTY); sl_vor<SM>(L.vflag, y2, VF_RDIRTY); }
       if (gl < 10) Qk[gl] = qk + qr;
-      if (gl >= 10 && gl < 13) A.pos[3 * gk + (gl - 10)] = sh.wbest[3 * slot + (gl - 10)];
+      if (gl >= 10 && gl < 13) A.pos[3 * gk + (gl - 10)] = win[slot].best[gl - 10];
       if (gl == 0) {
         sl_vor<SM>(L.vflag, k, VF_CDIRTY | VF_RDIRTY);  // k moved: cached costs of its edges are stale
         sl_vclear<SM>(L.vflag, k, VF_END);
@@ -880,6 +909,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
     if (tid == 0) {
       sh.progress = 0;
       sh.ncol = 0;
+      sh.npass = 0;
     }
     __syncthreads();
     SL_MARK(0);
@@ -1007,9 +1037,10 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
     }
     __syncthreads();
     SL_MARK(2);
-    // ---- P4 + E: the round's winners (marked DONE on both endpoints), SL_WCAP per pass
+    // ---- P4 + E: the round's winners (marked DONE on both endpoints), L.wcap per pass
+    SlWin* const win = sl_win();
     for (;;) {
-      if (tid == 0) { sh.nwin = 0; sh.nbig = 0; }
+      if (tid == 0) { sh.nwin = 0; sh.nbig = 0; sh.bigring = 0; sh.npass++; }
       __syncthreads();
       for (uint32_t i = tid; i < nV; i += NT) {
         const uint32_t a = SM ? i : (uint32_t)vlist[i];
@@ -1024,13 +1055,13 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
         const uint32_t v = sl_fget<SM>(L, f, (int)((c + 1) % 3));
         if (L.key1[v] != key || (L.vflag[v] & VF_DONE) || L.vlose[v]) continue;
         const uint32_t slot = atomicAdd(&sh.nwin, 1u);
-        if (slot < (uint32_t)SL_WCAP) {
-          sh.win[slot].u = a;
-          sh.win[slot].v = v;
-          sh.win[slot].h = 3 * f + c;
-          sh.win[slot].cnt[0] = 0;
-          sh.win[slot].cnt[1] = 0;
-          sh.win[slot].flags = 0;
+        if (slot < L.wcap) {
+          win[slot].u = a;
+          win[slot].v = v;
+          win[slot].h = 3 * f + c;
+          win[slot].cnt[0] = 0;
+          win[slot].cnt[1] = 0;
+          win[slot].flags = 0;
           sl_vor<SM>(L.vflag, a, VF_DONE | VF_END);
           sl_vor<SM>(L.vflag, v, VF_DONE | VF_END);
         }
@@ -1038,13 +1069,17 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
       __syncthreads();
       SL_MARK(3);
       const uint32_t total = sh.nwin;
-      const uint32_t nb = total < (uint32_t)SL_WCAP ? total : (uint32_t)SL_WCAP;
+      const uint32_t nb = total < L.wcap ? total : L.wcap;
+      if (A.trace != nullptr && tid == 0 && sh.npass == 1) {
+        const uint32_t b = total / 16 < (uint32_t)SL_HW - 1 ? total / 16 : (uint32_t)SL_HW - 1;
+        atomicAdd(&A.trace[SL_HIST + SL_HCLS * A.cls + SL_HP + b], 1u);
+      }
       if (nb == 0) break;
       if (A.trace != nullptr && tid == 0) sh.wins += nb;
       // key1 is dead until the next P1: the winners' entries now name their ring lists
       for (uint32_t i = tid; i < nb; i += NT) {
-        L.key1[sh.win[i].u] = (key_t)(2u * i);
-        L.key1[sh.win[i].v] = (key_t)(2u * i + 1u);
+        L.key1[win[i].u] = (key_t)(2u * i);
+        L.key1[win[i].v] = (key_t)(2u * i + 1u);
       }
       __syncthreads();
       SL_MARK(4);
@@ -1057,11 +1092,11 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
         if (tid < nb) {
           const uint32_t i = tid;
           SEval e;
-          sl_cost<SM, R>(A, L, sh.win[i].u, sh.win[i].v, &e);
-          sh.win[i].keep = e.valid ? e.keep : sh.win[i].u;
-          sh.win[i].flags = e.valid ? 0u : WF_BAD;
+          sl_cost<SM, R>(A, L, win[i].u, win[i].v, &e);
+          win[i].keep = e.valid ? e.keep : win[i].u;
+          win[i].flags = e.valid ? 0u : WF_BAD;
           if (e.valid) {
-            sh.wbest[3 * i + 0] = e.p[0]; sh.wbest[3 * i + 1] = e.p[1]; sh.wbest[3 * i + 2] = e.p[2];
+            win[i].best[0] = e.p[0]; win[i].best[1] = e.p[1]; win[i].best[2] = e.p[2];
           }
         }
         if (!split || tid >= nbt) {
@@ -1080,8 +1115,9 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
             for (int c = 0; c < 6; c++) {
               if (!(fl[c] & VF_END)) continue;
               const uint32_t sl = (uint32_t)L.key1[x[c]];
-              const uint32_t p = atomicAdd(&sh.win[sl >> 1].cnt[sl & 1u], 1u);
+              const uint32_t p = atomicAdd(&win[sl >> 1].cnt[sl & 1u], 1u);
               if (p < (uint32_t)S_MAXV) L.ring[sl * S_MAXV + p] = (idx_t)(c < 3 ? fa : fb);
+              if (p == 16u) sh.bigring = 1;  // (every writer stores 1)
             }
           }
         }
@@ -1089,18 +1125,29 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
       __syncthreads();
       SL_MARK(5);
       SL_MARK(6);
-      // E2b: one flip test per (winner, side, ring entry)
-      for (uint32_t item = tid; item < nb * 64; item += NT) {
-        const uint32_t i = item >> 6, side = (item >> 5) & 1u, j = item & 31u;
-        if (sh.win[i].flags & WF_BAD) continue;
-        if (sh.win[i].cnt[0] > (uint32_t)S_MAXV || sh.win[i].cnt[1] > (uint32_t)S_MAXV) continue;  // fails in E2c
-        if (j >= sh.win[i].cnt[side]) continue;
-        const uint32_t w = side ? sh.win[i].v : sh.win[i].u, other = side ? sh.win[i].u : sh.win[i].v;
-        const uint32_t f = L.ring[(2 * i + side) * S_MAXV + j];
-        const uint32_t a[3] = {sl_fget<SM>(L, f, 0), sl_fget<SM>(L, f, 1), sl_fget<SM>(L, f, 2)};
-        if (a[0] == other || a[1] == other || a[2] == other) continue;  // dies with the edge
-        const double best[3] = {sh.wbest[3 * i], sh.wbest[3 * i + 1], sh.wbest[3 * i + 2]};
-        if (sl_flips<SM, R>(A, L, a, w, best)) atomicOr(&sh.win[i].flags, WF_BAD);
+      if (A.trace != nullptr) {
+        for (uint32_t i = tid; i < 2 * nb; i += NT) {
+          const uint32_t n = win[i >> 1].cnt[i & 1u];
+          atomicAdd(&A.trace[SL_HIST + SL_HCLS * A.cls + SL_HP + SL_HW + (n <= (uint32_t)S_MAXV ? n : S_MAXV + 1)], 1u);
+        }
+      }
+      // E2b: one flip test per (winner, side, ring entry).  Rings hold 5-6 faces typically and at most
+      // 16 almost always, so a half warp takes one winner side (entries 0..15); entries 16..31 take a
+      // second sweep, only in passes where some ring has more than 16 faces.
+      for (uint32_t j0 = 0; j0 < (uint32_t)S_MAXV; j0 += 16) {
+        if (j0 != 0 && !sh.bigring) break;
+        for (uint32_t item = tid; item < nb * 32; item += NT) {
+          const uint32_t i = item >> 5, side = (item >> 4) & 1u, j = j0 + (item & 15u);
+          if (win[i].flags & WF_BAD) continue;
+          if (win[i].cnt[0] > (uint32_t)S_MAXV || win[i].cnt[1] > (uint32_t)S_MAXV) continue;  // fails in E2c
+          if (j >= win[i].cnt[side]) continue;
+          const uint32_t w = side ? win[i].v : win[i].u, other = side ? win[i].u : win[i].v;
+          const uint32_t f = L.ring[(2 * i + side) * S_MAXV + j];
+          const uint32_t a[3] = {sl_fget<SM>(L, f, 0), sl_fget<SM>(L, f, 1), sl_fget<SM>(L, f, 2)};
+          if (a[0] == other || a[1] == other || a[2] == other) continue;  // dies with the edge
+          const double best[3] = {win[i].best[0], win[i].best[1], win[i].best[2]};
+          if (sl_flips<SM, R>(A, L, a, w, best)) atomicOr(&win[i].flags, WF_BAD);
+        }
       }
       __syncthreads();
       SL_MARK(7);
@@ -1117,7 +1164,12 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
       }
       __syncthreads();
       SL_MARK(8);
-      if (total <= (uint32_t)SL_WCAP) break;
+      if (total <= L.wcap) break;
+    }
+    if (tid == 0) {
+      const uint32_t passes = sh.npass;
+      if (passes > 1) atomicAdd(&A.counters[24], 1u);
+      if (A.trace != nullptr) atomicAdd(&A.trace[SL_HIST + SL_HCLS * A.cls + (passes < (uint32_t)SL_HP ? passes : SL_HP) - 1], 1u);
     }
     // ---- stop rules of the label
     if (tid == 0 && A.trace != nullptr && sh.rec == 0 && r < 400) {
@@ -1201,8 +1253,6 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
   }
 }
 
-extern __shared__ __align__(16) unsigned char sl_smem[];
-
 // One label per CTA (the launch has one CTA per label of its size class; a CTA takes the next label of
 // the size-sorted order from a counter, so big labels start first whatever order the hardware dispatches
 // CTAs in).  The block size is the class's (1024, 512 or 256 threads); 64 registers per thread let two
@@ -1223,14 +1273,15 @@ __global__ void __launch_bounds__(SL_THREADS, 1) k_simp_labels(SlArgs A) {
     const uint32_t vbase = A.vert_off[l], U = A.vert_off[l + 1] - vbase;
     const uint32_t target = A.target[l];
     if (T == 0 || T <= target) continue;  // init left every face / vertex alive
-    const SlLayout y = sl_layout(T, U, blockDim.x);
-    const size_t o_keyg = y.wq + (size_t)SL_WCAP * 2 * S_MAXV * 4;  // other classes: 32-bit face ids in the rings
     const bool fmt16 = 3ull * T <= 65536ull;
     if (sl_fits_smem(T, U, blockDim.x, A.smem_bytes)) {
+      const uint32_t wcap = sl_wcap(T, U, blockDim.x, A.smem_bytes, false, A.wcap_max);
+      const SlLayout y = sl_layout(T, U, blockDim.x, false, wcap);
       SlLab<true> L;
       L.T = T; L.U = U; L.tbase = tbase; L.vbase = vbase; L.target = target;
-      L.wq = (uint32_t*)sl_smem;
-      L.ring = (uint16_t*)(sl_smem + y.wq);
+      L.wcap = wcap;
+      L.wq = (uint32_t*)(sl_smem + y.o_wq);
+      L.ring = (uint16_t*)(sl_smem + y.o_ring);
       L.key1 = (uint32_t*)(sl_smem + y.o_key);
       L.fmt16 = true;
       L.fc0 = (uint16_t*)(sl_smem + y.o_f0);
@@ -1247,12 +1298,15 @@ __global__ void __launch_bounds__(SL_THREADS, 1) k_simp_labels(SlArgs A) {
       L.fmap = L.vmap = nullptr;
       sl_run<true, false>(A, L, sh, nullptr);
     } else {
+      const SlLayout y = sl_layout(T, U, blockDim.x);
+      const size_t o_keyg = y.o_ring + (size_t)SL_WCAP * 2 * S_MAXV * 4;  // 32-bit face ids in the rings
       SlLab<false> L;
       L.T = T; L.U = U; L.tbase = tbase; L.vbase = vbase; L.target = target;
       L.label = l;
       L.fmap = L.vmap = nullptr;
-      L.wq = (uint32_t*)sl_smem;  // the cost queues and the ring lists always fit
-      L.ring = (uint32_t*)(sl_smem + y.wq);
+      L.wcap = SL_WCAP < A.wcap_max ? SL_WCAP : A.wcap_max;
+      L.wq = (uint32_t*)(sl_smem + y.o_wq);  // the winners, the cost queues and the ring lists always fit
+      L.ring = (uint32_t*)(sl_smem + y.o_ring);
       L.fc0 = L.fc1 = L.fc2 = nullptr;
       L.flist = A.flist + tbase; L.flist2 = A.flist2 + tbase;
       L.vlist = A.vlist + vbase; L.vlist2 = A.vlist2 + vbase;
@@ -1296,12 +1350,14 @@ __global__ void __launch_bounds__(SL_THREADS / 2, 2) k_simp_resume(SlArgs A) {
     const uint32_t* hdr = A.mq + SL_MREC * (size_t)wi;
     const uint32_t l = hdr[0];
     const uint32_t T = hdr[4], U = hdr[5];
-    const SlLayout y = sl_layout(T, U, blockDim.x, true);
+    const uint32_t wcap = sl_wcap(T, U, blockDim.x, A.smem_bytes, true, A.wcap_max);
+    const SlLayout y = sl_layout(T, U, blockDim.x, true, wcap);
     SlLab<true> L;
     L.T = T; L.U = U; L.tbase = A.tri_off[l]; L.vbase = A.vert_off[l]; L.target = A.target[l];
     L.label = l;
-    L.wq = (uint32_t*)sl_smem;
-    L.ring = (uint16_t*)(sl_smem + y.wq);
+    L.wcap = wcap;
+    L.wq = (uint32_t*)(sl_smem + y.o_wq);
+    L.ring = (uint16_t*)(sl_smem + y.o_ring);
     L.key1 = (uint32_t*)(sl_smem + y.o_key);
     L.fmt16 = true;
     L.fc0 = (uint16_t*)(sl_smem + y.o_f0);
@@ -1391,6 +1447,7 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   m->simp_rounds = 0;
   m->simp_labels_smem = m->simp_labels_gmem = 0;
   for (int c = 0; c < SL_NCLASS; c++) m->simp_labels_class[c] = m->simp_migrations[c] = 0;
+  m->simp_passes[0] = m->simp_passes[1] = 0;
   const uint64_t U = m->U, T = m->T, K = m->K;
   if (T == 0 || U == 0) {
     m->simplified = true;
@@ -1521,13 +1578,16 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   A.trace = nullptr;
   A.lrec = nullptr;
   if (getenv("IGN_SIMP_TRACE") != nullptr) {
-    IGN_TRY(f.take(&A.trace, 400 * 4 + 64));
+    IGN_TRY(f.take(&A.trace, SL_HIST + SL_NCLASS * SL_HCLS));
     IGN_TRY(f.take(&A.lrec, (size_t)K * SL_LREC + 16));
-    IGN_CUDA(cudaMemsetAsync(A.trace, 0, 400 * 16 + 256, ctx->stream));
+    IGN_CUDA(cudaMemsetAsync(A.trace, 0, (SL_HIST + SL_NCLASS * SL_HCLS) * 4, ctx->stream));
     IGN_CUDA(cudaMemsetAsync(A.lrec, 0, ((size_t)K * SL_LREC + 16) * 4, ctx->stream));
   }
   const char* force_gmem = getenv("IGN_SIMP_GMEM");
   const bool gmem_only = force_gmem && force_gmem[0] == '1';
+  // IGN_SIMP_WCAP=n (test knob): at most n winners per selection pass, so that rounds take several passes
+  const char* wcap_env = getenv("IGN_SIMP_WCAP");
+  A.wcap_max = wcap_env && atoi(wcap_env) > 0 ? (uint32_t)atoi(wcap_env) : 0xFFFFFFFFu;
   {
     const int slot = prof_begin(ctx, IGN_PROF_SIMP);
     // default: one CTA per label (SMs are handed back to the block scheduler after every label, so
@@ -1680,6 +1740,20 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
       fprintf(stderr, "SM Mcycles by starting class: %.0f + %.0f + %.0f = %.0f; labels resumed in the 512- / 256-thread class: %u / %u\n",
               sm_total[0] * 1024.0 / 1e6, sm_total[1] * 1024.0 / 1e6, sm_total[2] * 1024.0 / 1e6,
               (sm_total[0] + sm_total[1] + sm_total[2]) * 1024.0 / 1e6, hflags[17], hflags[18]);
+      // per class the label-rounds ran in: selection passes per round, winners per round (before capping,
+      // bins of 16), ring length per winner side (the last bin of each: more)
+      std::vector<uint32_t> hist(SL_NCLASS * SL_HCLS);
+      IGN_CUDA(cudaMemcpy(hist.data(), A.trace + SL_HIST, hist.size() * 4, cudaMemcpyDeviceToHost));
+      for (int c = 0; c < SL_NCLASS; c++) {
+        const uint32_t* h = &hist[SL_HCLS * c];
+        fprintf(stderr, "class %d passes/round (1..%d+):", SL_CLASS_THREADS[c], SL_HP);
+        for (int b = 0; b < SL_HP; b++) fprintf(stderr, " %u", h[b]);
+        fprintf(stderr, "\nclass %d winners/round (bins of 16, last %d+):", SL_CLASS_THREADS[c], 16 * (SL_HW - 1));
+        for (int b = 0; b < SL_HW; b++) fprintf(stderr, " %u", h[SL_HP + b]);
+        fprintf(stderr, "\nclass %d ring length per winner side (0..%d, more):", SL_CLASS_THREADS[c], S_MAXV);
+        for (int b = 0; b < SL_HR; b++) fprintf(stderr, " %u", h[SL_HP + SL_HW + b]);
+        fprintf(stderr, "\n");
+      }
       // least squares cycles = a * rounds + b * visits (no intercept)
       const double det = srr * svv - srv * srv;
       if (det != 0) fprintf(stderr, "fit: cycles ~= %.0f * rounds + %.2f * face visits   (totals: %.0f rounds, %.3g visits, %.3g cycles)\n",
@@ -1693,6 +1767,8 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   m->simp_labels_gmem = hflags[3];
   for (int c = 0; c < SL_NCLASS; c++) m->simp_labels_class[c] = hflags[8 + c];
   for (int c = 0; c < SL_NCLASS; c++) m->simp_migrations[c] = hflags[16 + c];
+  m->simp_passes[0] = hflags[24];
+  m->simp_passes[1] = hflags[25];
   const uint32_t U2 = last[0] + last[1], T2 = last[2] + last[3];
   IGN_LAUNCH(ctx, k_simp_new_offsets, blocks_for(K + 2, 256), 256, 0, d_vert_off, vscan, (uint32_t)(K + 2), U, U2,
                    d_new_vert_off);
@@ -1729,5 +1805,13 @@ extern "C" int ign_mesh_simplify_migrations(ign_mesher* m, uint32_t resumed[3]) 
   IGN_REQUIRE(m && resumed, IGN_ERR_INVALID, "null argument");
   IGN_REQUIRE(m->simplified, IGN_ERR_INVALID, "mesher is not simplified");
   for (int c = 0; c < SL_NCLASS; c++) resumed[c] = m->simp_migrations[c];
+  return IGN_OK;
+}
+
+extern "C" int ign_mesh_simplify_passes(ign_mesher* m, uint32_t counts[2]) {
+  IGN_REQUIRE(m && counts, IGN_ERR_INVALID, "null argument");
+  IGN_REQUIRE(m->simplified, IGN_ERR_INVALID, "mesher is not simplified");
+  counts[0] = m->simp_passes[0];
+  counts[1] = m->simp_passes[1];
   return IGN_OK;
 }

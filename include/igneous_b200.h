@@ -377,6 +377,10 @@ IGN_API int ign_mesh_simplify_stats(ign_mesher* m, uint32_t stats[6]);
  * after migrating from the next larger one, once their alive faces and vertices fit it ([0] is always 0;
  * a label that migrates twice counts in both smaller classes) */
 IGN_API int ign_mesh_simplify_migrations(ign_mesher* m, uint32_t resumed[3]);
+/* selection counters of the simplification that ran: [0] label-rounds whose winners took more than one
+ * validation pass (more winners than the label's per-pass capacity), [1] winners rejected because an
+ * endpoint had more than 32 alive incident faces */
+IGN_API int ign_mesh_simplify_passes(ign_mesher* m, uint32_t counts[2]);
 /* bulk export of every label's mesh (simplified if ign_mesh_simplify ran) in ign_mesh_ids order:
  * vertices f32 [U,3], faces u32 [T,3] (label-local indices), offsets [n_ids+1] */
 IGN_API int ign_mesh_export(ign_mesher* m, const float resolution[3], int voxel_centered,
