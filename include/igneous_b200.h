@@ -341,6 +341,23 @@ IGN_API int ign_find_objects(ign_ctx* ctx, const void* labels, int dtype, uint64
 IGN_API int ign_find_objects_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy,
                                  uint64_t sz, uint64_t* max_label, uint32_t* boxes);
 
+/* ------------------------------------------------------- distance transform
+ * edt.edt / edt.edtsq(labels, anisotropy, black_border)  kimimaro.skeletonize's distance-to-boundary
+ *   field (SkeletonTask, igneous/tasks/skeleton.py:54, :312); the rule of DESIGN.md §5d (edt parity
+ *   unpinned): out[p] = 0 where labels[p] == 0, else the least sum_i (anisotropy[i] (p_i - q_i))^2 over
+ *   voxels q whose label differs from labels[p] (labels compared for equality only), the one-voxel shell
+ *   around the volume counting as label 0 when black_border != 0; +inf where there is no such q.
+ *   squared == 0 writes sqrtf of that float32 value.
+ *   (sx, sy, sz) volume of u8 / u16 / u32 / u64 labels, each side below 2^30; out is float32 of the
+ *   same shape, not aliasing labels.  anisotropy[i] > 0 and finite; +inf is accepted on an axis of
+ *   extent 1 and means the caller's array does not have that axis (a 1-D or 2-D input), so the shell
+ *   is not applied along it.  Three separable passes (x, then y, then z); the y and z passes take
+ *   their envelope stacks from the scratch arena (at most 1 GiB, or one line's worth if more). */
+IGN_API int ign_edt(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
+                    const float anisotropy[3], int black_border, int squared, float* out);
+IGN_API int ign_edt_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
+                        const float anisotropy[3], int black_border, int squared, float* out);
+
 /* --------------------------------------------------------------------- mesh
  * zmesh.Mesher(resolution).mesh(data, preserve_order=False)  igneous/tasks/mesh/mesh.py:151,245
  * Mesher.ids()                                                igneous/tasks/mesh/mesh.py:374
