@@ -3,14 +3,21 @@
 This module is the only place Python touches the native library.  There is no
 CPU fallback: if the library is missing, or no CUDA device is visible, every
 compute call raises.
+
+The header is the only statement of the ABI: load() reads its prototypes and sets
+argtypes / restype on every declared function, so callers pass Python ints and
+floats and ctypes converts (and type-checks) them.  Pointers are c_void_p, which
+takes None, ints, c_void_p values (ptr()), ctypes arrays and byref(...).
 """
 import ctypes
 import os
+import re
 import threading
 
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
+HEADER = os.path.join(os.path.dirname(_HERE), "include", "igneous_b200.h")
 _LIB_ENV = "IGNEOUS_B200_LIB"
 _DEV_ENV = "IGNEOUS_B200_DEVICE"
 
@@ -67,12 +74,43 @@ def lib_path():
   return os.environ.get(_LIB_ENV) or os.path.join(_HERE, "csrc", "libigneous_b200.so")
 
 
+_SCALARS = {"int": ctypes.c_int, "uint32_t": ctypes.c_uint32, "uint64_t": ctypes.c_uint64,
+            "int64_t": ctypes.c_int64, "float": ctypes.c_float, "double": ctypes.c_double}
+_RETURNS = {"int": ctypes.c_int, "const char*": ctypes.c_char_p}
+_PROTOTYPE = re.compile(r"IGN_API\s+([\w\s\*]+?)\s*\b(ign_\w+)\s*\(([^)]*)\)")
+
+
+def _param_type(param):
+  if "*" in param or "[" in param:
+    return ctypes.c_void_p
+  ctype = _SCALARS.get(" ".join(w for w in param.split()[:-1] if w != "const"))
+  if ctype is None:
+    raise ValueError("%s: no ctypes mapping for parameter %r" % (HEADER, param))
+  return ctype
+
+
+def prototypes():
+  """{name: (restype, argtypes)} of every IGN_API function the header declares.  Every
+  pointer or array parameter is c_void_p; a C type without a mapping raises ValueError."""
+  with open(HEADER) as f:
+    text = f.read()
+  protos = {}
+  for ret, name, params in _PROTOTYPE.findall(text):
+    ret = " ".join(ret.split())
+    if ret not in _RETURNS:
+      raise ValueError("%s: no ctypes mapping for the return type %r of %s" % (HEADER, ret, name))
+    params = [p.strip() for p in params.split(",")]
+    protos[name] = (_RETURNS[ret], [] if params == ["void"] else [_param_type(p) for p in params])
+  return protos
+
+
 _lib = None
 _lock = threading.Lock()
 
 
 def load():
-  """dlopen the native library (no GPU needed for this step)."""
+  """dlopen the native library and declare every function of the header on it (no GPU needed
+  for this step).  A declared function the library does not export raises AttributeError."""
   global _lib
   if _lib is not None:
     return _lib
@@ -85,7 +123,9 @@ def load():
         "libigneous_b200.so not found at %s -- run `python -m igneous_b200.build` "
         "(there is no CPU fallback)" % path)
     lib = ctypes.CDLL(path)
-    lib.ign_last_error.restype = ctypes.c_char_p
+    for name, (restype, argtypes) in prototypes().items():
+      fn = getattr(lib, name)
+      fn.restype, fn.argtypes = restype, argtypes
     _lib = lib
     return _lib
 
@@ -101,10 +141,6 @@ def check(status):
   if status == -4:
     raise MemoryError("libigneous_b200: " + msg)
   raise IgneousB200Error(status, msg)
-
-
-def _u64(v):
-  return ctypes.c_uint64(int(v))
 
 
 def ptr(a):
@@ -123,12 +159,12 @@ class DeviceBuffer:
     self.ctx = ctx
     self.nbytes = int(nbytes)
     p = ctypes.c_void_p()
-    check(ctx.lib.ign_dev_alloc(ctx.handle, _u64(nbytes), ctypes.byref(p)))
+    check(ctx.lib.ign_dev_alloc(ctx.handle, self.nbytes, ctypes.byref(p)))
     self.ptr = p.value or 0
 
   def free(self):
     if self.ptr and self.ctx.handle:
-      check(self.ctx.lib.ign_dev_free(self.ctx.handle, ctypes.c_void_p(self.ptr)))
+      check(self.ctx.lib.ign_dev_free(self.ctx.handle, self.ptr))
     self.ptr = 0
 
   def offset(self, nbytes):
@@ -149,7 +185,7 @@ class Context:
     if device is None:
       device = int(os.environ.get(_DEV_ENV, os.environ.get("LOCAL_RANK", "0")))
     h = ctypes.c_void_p()
-    check(self.lib.ign_init(ctypes.c_int(device), ctypes.byref(h)))
+    check(self.lib.ign_init(device, ctypes.byref(h)))
     self.handle = h
     self.device = device
 
@@ -162,7 +198,7 @@ class Context:
     dtype = np.dtype(dtype)
     n = int(np.prod(shape)) if len(shape) else 1
     p = ctypes.c_void_p()
-    check(self.lib.ign_host_alloc(self.handle, _u64(max(n * dtype.itemsize, 1)), ctypes.byref(p)))
+    check(self.lib.ign_host_alloc(self.handle, max(n * dtype.itemsize, 1), ctypes.byref(p)))
     buf = (ctypes.c_uint8 * max(n * dtype.itemsize, 1)).from_address(p.value)
     arr = np.frombuffer(buf, dtype=dtype, count=n).reshape(shape, order=order)
     self._pinned = getattr(self, "_pinned", [])
@@ -170,24 +206,23 @@ class Context:
     return arr
 
   def h2d(self, dst, src_arr):
-    check(self.lib.ign_h2d(self.handle, ptr(dst), ptr(src_arr), _u64(src_arr.nbytes)))
+    check(self.lib.ign_h2d(self.handle, ptr(dst), ptr(src_arr), src_arr.nbytes))
 
   def d2h(self, dst_arr, src, nbytes=None):
-    check(self.lib.ign_d2h(self.handle, ptr(dst_arr), ptr(src),
-                           _u64(dst_arr.nbytes if nbytes is None else nbytes)))
+    check(self.lib.ign_d2h(self.handle, ptr(dst_arr), ptr(src), dst_arr.nbytes if nbytes is None else nbytes))
 
   def d2d(self, dst, src, nbytes):
-    check(self.lib.ign_d2d(self.handle, ptr(dst), ptr(src), _u64(nbytes)))
+    check(self.lib.ign_d2d(self.handle, ptr(dst), ptr(src), nbytes))
 
   def memset(self, dst, byte, nbytes):
-    check(self.lib.ign_memset(self.handle, ptr(dst), ctypes.c_int(byte), _u64(nbytes)))
+    check(self.lib.ign_memset(self.handle, ptr(dst), byte, nbytes))
 
   def sync(self):
     check(self.lib.ign_sync(self.handle))
 
   def set_priority(self, high=True):
     """Re-create the context's stream with the device's greatest / least stream priority."""
-    check(self.lib.ign_stream_priority(self.handle, ctypes.c_int(int(bool(high)))))
+    check(self.lib.ign_stream_priority(self.handle, int(bool(high))))
 
   def to_device(self, arr):
     arr = np.asarray(arr)
@@ -206,14 +241,14 @@ class Context:
 
   # -- timers
   def timer_start(self, slot=0):
-    check(self.lib.ign_timer_start(self.handle, ctypes.c_int(slot)))
+    check(self.lib.ign_timer_start(self.handle, slot))
 
   def timer_stop(self, slot=0):
-    check(self.lib.ign_timer_stop(self.handle, ctypes.c_int(slot)))
+    check(self.lib.ign_timer_stop(self.handle, slot))
 
   def timer_ms(self, slot=0):
     ms = ctypes.c_float()
-    check(self.lib.ign_timer_ms(self.handle, ctypes.c_int(slot), ctypes.byref(ms)))
+    check(self.lib.ign_timer_ms(self.handle, slot, ctypes.byref(ms)))
     return float(ms.value)
 
   def launch_count(self):
@@ -229,7 +264,7 @@ class Context:
   def close(self):
     if getattr(self, "handle", None):
       for p in getattr(self, "_pinned", []):
-        self.lib.ign_host_free(self.handle, ctypes.c_void_p(p))
+        self.lib.ign_host_free(self.handle, p)
       self._pinned = []
       self.lib.ign_destroy(self.handle)
       self.handle = None

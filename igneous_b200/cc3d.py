@@ -51,10 +51,8 @@ def connected_components(labels, connectivity=6, out_dtype=None, return_N=False,
   if arr.size:
     ctx = ctx or _shim.default_context()
     sx, sy, sz = arr.shape
-    _shim.check(ctx.lib.ign_ccl6(
-      ctx.handle, _shim.ptr(arr), ctypes.c_int(_shim.dtype_code(arr.dtype)),
-      ctypes.c_uint64(sx), ctypes.c_uint64(sy), ctypes.c_uint64(sz),
-      _shim.ptr(out), ctypes.c_int(_shim.dtype_code(out_dtype)), ctypes.byref(n)))
+    _shim.check(ctx.lib.ign_ccl6(ctx.handle, _shim.ptr(arr), _shim.dtype_code(arr.dtype), sx, sy, sz,
+                                 _shim.ptr(out), _shim.dtype_code(out_dtype), ctypes.byref(n)))
   out = out.reshape(shape_in, order="F")
   return (out, int(n.value)) if return_N else out
 
@@ -71,10 +69,7 @@ def dust(img, threshold, connectivity=6, in_place=False, ctx=None):
     work = work.copy(order="F") if not in_place else work
   ctx = ctx or _shim.default_context()
   sx, sy, sz = work.shape
-  _shim.check(ctx.lib.ign_dust(
-    ctx.handle, _shim.ptr(work), ctypes.c_int(_shim.dtype_code(work.dtype)),
-    ctypes.c_uint64(sx), ctypes.c_uint64(sy), ctypes.c_uint64(sz),
-    ctypes.c_uint64(int(threshold))))
+  _shim.check(ctx.lib.ign_dust(ctx.handle, _shim.ptr(work), _shim.dtype_code(work.dtype), sx, sy, sz, int(threshold)))
   res = work.view(src.dtype).reshape(src.shape, order="F")
   if in_place:
     if not np.shares_memory(res, src):
@@ -89,7 +84,6 @@ def ccl_task(image, shape, threshold_gte=None, threshold_lte=None, dust_threshol
   (igneous/tasks/image/ccl.py:165-175, 228-240, 331-344): threshold_image ->
   blackout_non_face_rails(shape) -> dust -> 6-connected CCL -> += label_offset
   with the background re-zeroed, in one pass over HBM.  Returns (uint64 labels, N)."""
-  import ctypes as c
   arr = _volume(image)
   if arr.dtype == np.bool_:
     arr = arr.view(np.uint8)
@@ -104,14 +98,12 @@ def ccl_task(image, shape, threshold_gte=None, threshold_lte=None, dust_threshol
   ctx = ctx or _shim.default_context()
   sx, sy, sz = arr.shape
   out = np.zeros(arr.shape, dtype=np.uint64, order="F")
-  n = c.c_uint64(0)
+  n = ctypes.c_uint64(0)
   if arr.size:
     _shim.check(ctx.lib.ign_ccl_task(
-      ctx.handle, _shim.ptr(arr), c.c_int(_shim.dtype_code(arr.dtype)), c.c_uint64(sx), c.c_uint64(sy),
-      c.c_uint64(sz), c.c_int(int(threshold_gte is not None)),
-      c.c_double(float(threshold_gte) if threshold_gte is not None else 0.0),
-      c.c_int(int(threshold_lte is not None)),
-      c.c_double(float(threshold_lte) if threshold_lte is not None else 0.0),
-      c.c_uint64(int(shape[0])), c.c_uint64(int(shape[1])), c.c_uint64(int(shape[2])),
-      c.c_uint64(int(dust_threshold or 0)), c.c_uint64(int(label_offset)), _shim.ptr(out), c.byref(n)))
+      ctx.handle, _shim.ptr(arr), _shim.dtype_code(arr.dtype), sx, sy, sz,
+      threshold_gte is not None, float(threshold_gte) if threshold_gte is not None else 0.0,
+      threshold_lte is not None, float(threshold_lte) if threshold_lte is not None else 0.0,
+      int(shape[0]), int(shape[1]), int(shape[2]), int(dust_threshold or 0), int(label_offset),
+      _shim.ptr(out), ctypes.byref(n)))
   return out, int(n.value)

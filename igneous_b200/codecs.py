@@ -41,18 +41,17 @@ def cseg_encode(labels, block_size=(8, 8, 8), ctx=None):
   ctx = ctx or _shim.default_context()
   sx, sy, sz, sc = arr.shape
   bx, by, bz = (int(v) for v in block_size)
-  args = [ctx.handle, _shim.ptr(arr), c.c_int(_shim.dtype_code(arr.dtype)), c.c_uint64(sx), c.c_uint64(sy),
-          c.c_uint64(sz), c.c_uint64(sc), c.c_uint32(bx), c.c_uint32(by), c.c_uint32(bz)]
+  args = [ctx.handle, _shim.ptr(arr), _shim.dtype_code(arr.dtype), sx, sy, sz, sc, bx, by, bz]
   n = c.c_uint64(0)
   gx, gy, gz = -(-sx // bx), -(-sy // by), -(-sz // bz)
   # worst case: every voxel its own table entry
   cap = sc * (1 + 2 * gx * gy * gz + (arr.dtype.itemsize // 4 + 1) * gx * gy * gz * bx * by * bz)
   cap = int(min(cap, 1 << 26))
   out = np.empty(cap, dtype=np.uint32)
-  _shim.check(ctx.lib.ign_cseg_encode(*args, _shim.ptr(out), c.c_uint64(cap), c.byref(n)))
+  _shim.check(ctx.lib.ign_cseg_encode(*args, _shim.ptr(out), cap, c.byref(n)))
   if n.value > cap:  # does not happen for 24-bit addressable chunks; kept for safety
     out = np.empty(int(n.value), dtype=np.uint32)
-    _shim.check(ctx.lib.ign_cseg_encode(*args, _shim.ptr(out), c.c_uint64(n.value), c.byref(n)))
+    _shim.check(ctx.lib.ign_cseg_encode(*args, _shim.ptr(out), n.value, c.byref(n)))
   return out[:int(n.value)].tobytes()
 
 
@@ -68,10 +67,9 @@ def cseg_decode(data, shape, dtype, block_size=(8, 8, 8), ctx=None):
   ctx = ctx or _shim.default_context()
   out = np.empty(shape, dtype=dtype, order="F")
   bx, by, bz = (int(v) for v in block_size)
-  _shim.check(ctx.lib.ign_cseg_decode(
-    ctx.handle, _shim.ptr(np.ascontiguousarray(words)), c.c_uint64(len(words)), c.c_int(_shim.dtype_code(dtype)),
-    c.c_uint64(shape[0]), c.c_uint64(shape[1]), c.c_uint64(shape[2]), c.c_uint64(shape[3]), c.c_uint32(bx),
-    c.c_uint32(by), c.c_uint32(bz), _shim.ptr(out)))
+  _shim.check(ctx.lib.ign_cseg_decode(ctx.handle, _shim.ptr(np.ascontiguousarray(words)), len(words),
+                                      _shim.dtype_code(dtype), shape[0], shape[1], shape[2], shape[3], bx, by, bz,
+                                      _shim.ptr(out)))
   return out
 
 
@@ -125,15 +123,14 @@ def jpeg_encode_batch(chunks, quality=85, restart_interval=None, ctx=None):
   ctx = ctx or _shim.default_context()
   offsets = np.zeros(n + 1, dtype=np.uint64)
   need = c.c_uint64(0)
-  args = [ctx.handle, _shim.ptr(packed), c.c_uint64(n), _shim.ptr(shp), c.c_int(quality), c.c_int64(ri)]
+  args = [ctx.handle, _shim.ptr(packed), n, _shim.ptr(shp), quality, ri]
   # a first guess that holds smooth image data; the call reports the size when it does not
   cap = max(4096, packed.size // 2 + 1024 * n)
   out = np.empty(cap, dtype=np.uint8)
-  _shim.check(ctx.lib.ign_jpeg_encode(*args, _shim.ptr(out), c.c_uint64(cap), _shim.ptr(offsets), c.byref(need)))
+  _shim.check(ctx.lib.ign_jpeg_encode(*args, _shim.ptr(out), cap, _shim.ptr(offsets), c.byref(need)))
   if need.value > cap:
     out = np.empty(int(need.value), dtype=np.uint8)
-    _shim.check(ctx.lib.ign_jpeg_encode(*args, _shim.ptr(out), c.c_uint64(need.value), _shim.ptr(offsets),
-                                        c.byref(need)))
+    _shim.check(ctx.lib.ign_jpeg_encode(*args, _shim.ptr(out), need.value, _shim.ptr(offsets), c.byref(need)))
   return [out[int(offsets[i]):int(offsets[i + 1])].tobytes() for i in range(n)]
 
 
@@ -161,8 +158,8 @@ def jpeg_decode_batch(datas, shapes, ctx=None):
   vox = shp.astype(np.uint64).prod(axis=1)
   out = np.empty(max(int(vox.sum()), 1), dtype=np.uint8)
   ctx = ctx or _shim.default_context()
-  _shim.check(ctx.lib.ign_jpeg_decode(ctx.handle, _shim.ptr(np.ascontiguousarray(packed)), _shim.ptr(offsets),
-                                      c.c_uint64(n), _shim.ptr(shp), _shim.ptr(out)))
+  _shim.check(ctx.lib.ign_jpeg_decode(ctx.handle, _shim.ptr(np.ascontiguousarray(packed)), _shim.ptr(offsets), n,
+                                      _shim.ptr(shp), _shim.ptr(out)))
   res, at = [], 0
   for s, v in zip(given, vox):
     res.append(out[at:at + int(v)].reshape(s, order="F"))

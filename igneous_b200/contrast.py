@@ -11,8 +11,6 @@ The rules are those of DESIGN.md §5b.  Everything but find_section_clamping_val
 host-side scan of one histogram per slice) runs in libigneous_b200; there is no CPU
 fallback.
 """
-import ctypes
-
 import numpy as np
 
 from . import _shim
@@ -38,8 +36,7 @@ def histogram(arr, ctx=None):
   if arr.size:
     flat = np.ascontiguousarray(arr.ravel(order="K"))
     ctx = ctx or _shim.default_context()
-    _shim.check(ctx.lib.ign_histogram(ctx.handle, _shim.ptr(flat), ctypes.c_int(_shim.dtype_code(dt)),
-                                      ctypes.c_uint64(flat.size), _shim.ptr(hist)))
+    _shim.check(ctx.lib.ign_histogram(ctx.handle, _shim.ptr(flat), _shim.dtype_code(dt), flat.size, _shim.ptr(hist)))
   return hist
 
 
@@ -101,11 +98,9 @@ def stretch(image, levels_per_z, lower_clip, upper_clip, minval=None, maxval=Non
   out = np.empty(arr.shape, dtype=out_dtype, order="F")
   if arr.size:
     ctx = ctx or _shim.default_context()
-    u = ctypes.c_uint64
     _shim.check(ctx.lib.ign_contrast_stretch(
-      ctx.handle, _shim.ptr(arr), ctypes.c_int(_shim.dtype_code(dt)), u(sx), u(sy), u(sz), u(sc),
-      _shim.ptr(lower), _shim.ptr(upper), ctypes.c_double(lo), ctypes.c_double(hi), _shim.ptr(out),
-      ctypes.c_int(_shim.dtype_code(out_dtype))))
+      ctx.handle, _shim.ptr(arr), _shim.dtype_code(dt), sx, sy, sz, sc, _shim.ptr(lower), _shim.ptr(upper), lo, hi,
+      _shim.ptr(out), _shim.dtype_code(out_dtype)))
   return out.reshape(image.shape, order="F")
 
 
@@ -123,7 +118,7 @@ def quantize(image, ctx=None):
   out = np.empty(chan.shape + (1,), dtype=np.uint8, order="F")
   if chan.size:
     ctx = ctx or _shim.default_context()
-    _shim.check(ctx.lib.ign_quantize(ctx.handle, _shim.ptr(chan), ctypes.c_uint64(chan.size), _shim.ptr(out)))
+    _shim.check(ctx.lib.ign_quantize(ctx.handle, _shim.ptr(chan), chan.size, _shim.ptr(out)))
   return out
 
 
@@ -143,11 +138,8 @@ def clahe(stack, clip_limit=40.0, tile_grid_size=(8, 8), ctx=None):
   out = np.empty(arr.shape, dtype=arr.dtype, order="F")
   if arr.size:
     ctx = ctx or _shim.default_context()
-    u = ctypes.c_uint64
-    _shim.check(ctx.lib.ign_clahe(ctx.handle, _shim.ptr(arr), ctypes.c_int(_shim.dtype_code(arr.dtype)),
-                                  u(arr.shape[0]), u(arr.shape[1]), u(arr.shape[2]),
-                                  ctypes.c_double(float(clip_limit)), ctypes.c_uint32(gx), ctypes.c_uint32(gy),
-                                  _shim.ptr(out)))
+    _shim.check(ctx.lib.ign_clahe(ctx.handle, _shim.ptr(arr), _shim.dtype_code(arr.dtype), *arr.shape,
+                                  float(clip_limit), gx, gy, _shim.ptr(out)))
   return out.reshape(stack.shape, order="F")
 
 

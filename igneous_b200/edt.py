@@ -61,9 +61,8 @@ def _run(data, anisotropy, black_border, order, voxel_graph, squared, ctx):
   aniso = (ctypes.c_float * 3)(*(a + (float("inf"),) * (3 - vol.ndim)))  # +inf: an axis the array lacks
   out = np.empty(vol.shape, dtype=np.float32, order="F")
   ctx = ctx or _shim.default_context()
-  _shim.check(ctx.lib.ign_edt(ctx.handle, _shim.ptr(vol), ctypes.c_int(_shim.dtype_code(vol.dtype)),
-                              *(ctypes.c_uint64(int(s)) for s in shape), aniso, ctypes.c_int(int(bool(black_border))),
-                              ctypes.c_int(int(squared)), _shim.ptr(out)))
+  _shim.check(ctx.lib.ign_edt(ctx.handle, _shim.ptr(vol), _shim.dtype_code(vol.dtype), *shape, aniso,
+                              bool(black_border), squared, _shim.ptr(out)))
   return out.T if rev else out
 
 

@@ -10,7 +10,6 @@ fastmorph itself is not available offline, so these compute the rule stated in D
 "Hole filling" (parity with fastmorph is unpinned).  fill_holes_v2 returns numpy arrays:
 there is no crackle codec here, so return_crackle=True is refused.
 """
-import ctypes
 import enum
 
 import numpy as np
@@ -51,9 +50,8 @@ def dilate(labels, mode=Mode.multilabel, background_only=True, parallel=1, ctx=N
   if arr.size:
     ctx = ctx or _shim.default_context()
     sx, sy, sz = arr.shape
-    _shim.check(ctx.lib.ign_dilate_multilabel(
-      ctx.handle, _shim.ptr(arr), ctypes.c_int(_shim.dtype_code(arr.dtype)), ctypes.c_uint64(sx),
-      ctypes.c_uint64(sy), ctypes.c_uint64(sz), _shim.ptr(out)))
+    _shim.check(ctx.lib.ign_dilate_multilabel(ctx.handle, _shim.ptr(arr), _shim.dtype_code(arr.dtype), sx, sy, sz,
+                                              _shim.ptr(out)))
   return out.reshape(np.shape(labels)) if np.ndim(labels) == 2 else out
 
 
@@ -79,10 +77,8 @@ def fill_holes_v2(labels, return_crackle=False, fix_borders=False, merge_thresho
   if arr.size:
     ctx = ctx or _shim.default_context()
     sx, sy, sz = arr.shape
-    _shim.check(ctx.lib.ign_fill_holes(
-      ctx.handle, _shim.ptr(arr), ctypes.c_int(_shim.dtype_code(arr.dtype)), ctypes.c_uint64(sx),
-      ctypes.c_uint64(sy), ctypes.c_uint64(sz), ctypes.c_int(int(bool(fix_borders))), ctypes.c_int(pct),
-      _shim.ptr(filled), _shim.ptr(holes)))
+    _shim.check(ctx.lib.ign_fill_holes(ctx.handle, _shim.ptr(arr), _shim.dtype_code(arr.dtype), sx, sy, sz,
+                                       bool(fix_borders), pct, _shim.ptr(filled), _shim.ptr(holes)))
   if np.ndim(labels) == 2:
     return filled.reshape(np.shape(labels)), holes.reshape(np.shape(labels))
   return filled, holes

@@ -62,9 +62,8 @@ def renumber(arr, start=1, preserve_zero=True, in_place=False, ctx=None):
   uniq = np.zeros(max(n, 1), dtype=np.uint64)
   if n:
     ctx = ctx or _shim.default_context()
-    _shim.check(ctx.lib.ign_renumber(
-      ctx.handle, _shim.ptr(a), ctypes.c_int(_shim.dtype_code(a.dtype)), ctypes.c_uint64(n),
-      _shim.ptr(out), _shim.ptr(uniq), ctypes.c_uint64(uniq.size), ctypes.byref(k)))
+    _shim.check(ctx.lib.ign_renumber(ctx.handle, _shim.ptr(a), _shim.dtype_code(a.dtype), n, _shim.ptr(out),
+                                     _shim.ptr(uniq), uniq.size, ctypes.byref(k)))
   K = int(k.value)
   mapping = {int(u): i + 1 for i, u in enumerate(uniq[:K])}
   if n and (out == 0).any():
@@ -83,10 +82,8 @@ def remap(arr, table, preserve_missing_labels=False, in_place=False, ctx=None):
     keys = _u64(table.keys())
     vals = _u64(table.values())
     ctx = ctx or _shim.default_context()
-    _shim.check(ctx.lib.ign_remap(
-      ctx.handle, _shim.ptr(work), ctypes.c_int(_shim.dtype_code(work.dtype)),
-      ctypes.c_uint64(work.size), _shim.ptr(keys), _shim.ptr(vals), ctypes.c_uint64(len(keys)),
-      ctypes.c_int(int(bool(preserve_missing_labels)))))
+    _shim.check(ctx.lib.ign_remap(ctx.handle, _shim.ptr(work), _shim.dtype_code(work.dtype), work.size,
+                                  _shim.ptr(keys), _shim.ptr(vals), len(keys), bool(preserve_missing_labels)))
   if in_place and work is not src:
     src[...] = work.reshape(src.shape, order=order)
     return src
@@ -103,15 +100,14 @@ def unique(arr, return_counts=False, ctx=None):
     e = np.zeros(0, dtype=a.dtype)
     return (e, np.zeros(0, dtype=np.uint64)) if return_counts else e
   ctx = ctx or _shim.default_context()
-  code = ctypes.c_int(_shim.dtype_code(a.dtype))
+  code = _shim.dtype_code(a.dtype)
   k = ctypes.c_uint64(0)
-  _shim.check(ctx.lib.ign_unique(ctx.handle, _shim.ptr(a), code, ctypes.c_uint64(n), None, None,
-                                 ctypes.c_uint64(0), ctypes.byref(k)))
+  _shim.check(ctx.lib.ign_unique(ctx.handle, _shim.ptr(a), code, n, None, None, 0, ctypes.byref(k)))
   K = int(k.value)
   uniq = np.zeros(K, dtype=np.uint64)
   counts = np.zeros(K, dtype=np.uint64)
-  _shim.check(ctx.lib.ign_unique(ctx.handle, _shim.ptr(a), code, ctypes.c_uint64(n), _shim.ptr(uniq),
-                                 _shim.ptr(counts), ctypes.c_uint64(K), ctypes.byref(k)))
+  _shim.check(ctx.lib.ign_unique(ctx.handle, _shim.ptr(a), code, n, _shim.ptr(uniq),
+                                 _shim.ptr(counts), K, ctypes.byref(k)))
   uniq = uniq.astype(a.dtype)
   return (uniq, counts) if return_counts else uniq
 
@@ -123,10 +119,8 @@ def _mask(arr, labels, in_place, value, except_, ctx):
   if work.size:
     lab = _u64(labels)
     ctx = ctx or _shim.default_context()
-    _shim.check(ctx.lib.ign_mask(
-      ctx.handle, _shim.ptr(work), ctypes.c_int(_shim.dtype_code(work.dtype)),
-      ctypes.c_uint64(work.size), _shim.ptr(lab), ctypes.c_uint64(len(lab)),
-      ctypes.c_int(int(except_)), ctypes.c_uint64(int(value))))
+    _shim.check(ctx.lib.ign_mask(ctx.handle, _shim.ptr(work), _shim.dtype_code(work.dtype), work.size,
+                                 _shim.ptr(lab), len(lab), bool(except_), int(value)))
   if in_place and work is not src:
     src[...] = work.reshape(src.shape, order=order)
     return src
@@ -159,9 +153,8 @@ def inverse_component_map(parent_labels, component_labels, ctx=None):
   ctx = ctx or _shim.default_context()
   pairs = np.zeros((p.size, 2), dtype=np.uint64)
   n_pairs = ctypes.c_uint64(p.size)
-  _shim.check(ctx.lib.ign_inverse_component_map(
-    ctx.handle, _shim.ptr(p), _shim.ptr(c), ctypes.c_int(_shim.dtype_code(dt)),
-    ctypes.c_uint64(p.size), _shim.ptr(pairs), ctypes.byref(n_pairs)))
+  _shim.check(ctx.lib.ign_inverse_component_map(ctx.handle, _shim.ptr(p), _shim.ptr(c), _shim.dtype_code(dt), p.size,
+                                                _shim.ptr(pairs), ctypes.byref(n_pairs)))
   out = {}
   for a, b in pairs[:int(n_pairs.value)]:
     out.setdefault(int(a), []).append(int(b))

@@ -50,8 +50,8 @@ def solve_pairs(pairs, total):
   lut = np.zeros(total + 1, dtype=np.uint32)
   n = c.c_uint64(0)
   pairs = np.ascontiguousarray(pairs, dtype=np.uint64)
-  _shim.check(lib.ign_ccl6_solve(_shim.ptr(pairs) if len(pairs) else None, c.c_uint64(len(pairs)),
-                                 c.c_uint64(total), _shim.ptr(lut), c.byref(n)))
+  _shim.check(lib.ign_ccl6_solve(_shim.ptr(pairs) if len(pairs) else None, len(pairs), total, _shim.ptr(lut),
+                                 c.byref(n)))
   return lut, int(n.value)
 
 
@@ -84,7 +84,7 @@ class Group:
       unique_id = box[0]
     buf = (c.c_uint8 * 128).from_buffer_copy(unique_id)
     h = c.c_void_p()
-    _shim.check(self.lib.ign_group_init(ctx.handle, c.c_int(rank), c.c_int(world), buf, c.byref(h)))
+    _shim.check(self.lib.ign_group_init(ctx.handle, rank, world, buf, c.byref(h)))
     self.handle = h
     self._bufs = None
 
@@ -107,6 +107,6 @@ class Group:
     sx, sy, sz = pipe.shape
     n = c.c_uint64(0)
     _shim.check(self.lib.ign_ccl6_sharded_dev(
-      self.handle, _shim.ptr(pipe.d_in), c.c_int(pipe.code), c.c_uint64(sx), c.c_uint64(sy), c.c_uint64(sz),
-      _shim.ptr(pipe.d_cc), c.c_int(_shim.dtype_code(pipe.ccl_out_dtype)), c.byref(n)))
+      self.handle, _shim.ptr(pipe.d_in), pipe.code, sx, sy, sz,
+      _shim.ptr(pipe.d_cc), _shim.dtype_code(pipe.ccl_out_dtype), c.byref(n)))
     return int(n.value)

@@ -17,10 +17,6 @@ from . import _shim
 PROF_CLASSES = {"ccl_local": 0, "ccl_merge": 1, "ccl_label": 2, "pool": 3, "mc": 4, "simp_labels": 5}
 
 
-def _u64(v):
-  return c.c_uint64(int(v))
-
-
 class VolumePipeline:
   def __init__(self, ctx, shape, dtype=np.uint32, num_mips=2, mesh_shape=(256, 256, 256),
                resolution=(16, 16, 40), pitch=64, num_ids=1 << 20, seed=0, offset=(0, 0, 0),
@@ -85,10 +81,8 @@ class VolumePipeline:
   def synth(self):
     sx, sy, sz = self.shape
     ox, oy, oz = self.offset
-    _shim.check(self.lib.ign_synth_seg_dev(
-      self.ctx.handle, _shim.ptr(self.d_in), c.c_int(self.code), _u64(sx), _u64(sy), _u64(sz),
-      c.c_int64(ox), c.c_int64(oy), c.c_int64(oz), c.c_uint32(self.pitch), _u64(self.num_ids),
-      _u64(self.seed), _u64(self.id_base)))
+    _shim.check(self.lib.ign_synth_seg_dev(self.ctx.handle, _shim.ptr(self.d_in), self.code, sx, sy, sz, ox, oy, oz,
+                                           self.pitch, self.num_ids, self.seed, self.id_base))
 
   def load_host(self, arr):
     self.ctx.h2d(self.d_in, arr)
@@ -97,9 +91,8 @@ class VolumePipeline:
   def pool(self):
     sx, sy, sz = self.shape
     if self.num_mips:
-      _shim.check(self.lib.ign_pool_mode_2x2x1_dev(
-        self.ctx.handle, _shim.ptr(self.d_in), c.c_int(self.code), _u64(sx), _u64(sy), _u64(sz),
-        c.c_int(self.num_mips), c.c_int(0), _shim.void_pp([m.ptr for m in self.d_mips])))
+      _shim.check(self.lib.ign_pool_mode_2x2x1_dev(self.ctx.handle, _shim.ptr(self.d_in), self.code, sx, sy, sz,
+                                                   self.num_mips, 0, _shim.void_pp([m.ptr for m in self.d_mips])))
     self.ctx.timer_start(15)  # "mips ready" mark for the mesh streams
 
   def ccl(self):
@@ -109,9 +102,8 @@ class VolumePipeline:
       n_glob = self.group.ccl_sharded(self, n)
       self.n_components = n_glob
       return
-    _shim.check(self.lib.ign_ccl6_volume_dev(
-      self.ctx.handle, _shim.ptr(self.d_in), c.c_int(self.code), _u64(sx), _u64(sy), _u64(sz),
-      _shim.ptr(self.d_cc), c.c_int(_shim.dtype_code(self.ccl_out_dtype)), c.byref(n)))
+    _shim.check(self.lib.ign_ccl6_volume_dev(self.ctx.handle, _shim.ptr(self.d_in), self.code, sx, sy, sz,
+                                             _shim.ptr(self.d_cc), _shim.dtype_code(self.ccl_out_dtype), c.byref(n)))
     self.n_components = int(n.value)
 
   def mesh_tasks(self):
@@ -129,19 +121,16 @@ class VolumePipeline:
     src = self.d_mips[-1] if self.num_mips else self.d_in
     msx, msy, msz = self.mip_shapes[-1] if self.num_mips else self.shape
     x0, y0, z0, bx, by, bz = task
-    _shim.check(lib.ign_copy_box_dev(
-      wctx.handle, _shim.ptr(src), c.c_int(self.code), _u64(msx), _u64(msy), _u64(msz),
-      _u64(x0), _u64(y0), _u64(z0), _u64(bx), _u64(by), _u64(bz), _shim.ptr(d_task)))
+    _shim.check(lib.ign_copy_box_dev(wctx.handle, _shim.ptr(src), self.code, msx, msy, msz, x0, y0, z0, bx, by, bz,
+                                     _shim.ptr(d_task)))
     h = c.c_void_p()
-    _shim.check(lib.ign_mesh_begin_dev(
-      wctx.handle, _shim.ptr(d_task), c.c_int(self.code), _u64(bx), _u64(by), _u64(bz), c.byref(h)))
+    _shim.check(lib.ign_mesh_begin_dev(wctx.handle, _shim.ptr(d_task), self.code, bx, by, bz, c.byref(h)))
     try:
       nv0, nf0 = c.c_uint64(0), c.c_uint64(0)
       _shim.check(lib.ign_mesh_totals(h, c.byref(nv0), c.byref(nf0)))  # marching-cubes output (host counters)
       if self.simplification_factor and self.simplification_factor > 0:
-        _shim.check(lib.ign_mesh_simplify(
-          h, (c.c_float * 3)(*[float(r) for r in self.resolution]),
-          c.c_int(int(self.simplification_factor)), c.c_float(float(self.max_simplification_error))))
+        _shim.check(lib.ign_mesh_simplify(h, (c.c_float * 3)(*[float(r) for r in self.resolution]),
+                                          int(self.simplification_factor), float(self.max_simplification_error)))
       nv, nf, nl = c.c_uint64(0), c.c_uint64(0), c.c_uint64(0)
       _shim.check(lib.ign_mesh_totals(h, c.byref(nv), c.byref(nf)))
       _shim.check(lib.ign_mesh_num_ids(h, c.byref(nl)))
@@ -161,7 +150,7 @@ class VolumePipeline:
     tasks = list(self.mesh_tasks())
     if wait_for is None:
       for wctx, _ in self._workers:  # mesh streams start when the mip pyramid is complete
-        _shim.check(self.lib.ign_stream_wait_mark(wctx.handle, self.ctx.handle, c.c_int(15)))
+        _shim.check(self.lib.ign_stream_wait_mark(wctx.handle, self.ctx.handle, 15))
     results = []
     from concurrent.futures import ThreadPoolExecutor
 
@@ -172,7 +161,7 @@ class VolumePipeline:
         t = tasks[i]
         if wait_for is not None:
           mark = wait_for(t)  # the mark the main stream recorded after the last layer this task reads
-          _shim.check(self.lib.ign_stream_wait_mark(wctx.handle, self.ctx.handle, c.c_int(mark)))
+          _shim.check(self.lib.ign_stream_wait_mark(wctx.handle, self.ctx.handle, mark))
         out.append((i, self._mesh_one(wctx, buf, t, export)))
       wctx.sync()
       return out
@@ -254,8 +243,8 @@ class VolumePipeline:
     # finished products are downloaded on a second context's stream while the main stream keeps
     # uploading / computing (ign_d2h only enqueues)
     def download(mark, dst, srcp, nbytes):
-      _shim.check(self.lib.ign_stream_wait_mark(self._dl.handle, self.ctx.handle, c.c_int(mark)))
-      _shim.check(self.lib.ign_d2h(self._dl.handle, c.c_void_p(dst), c.c_void_p(srcp), _u64(nbytes)))
+      _shim.check(self.lib.ign_stream_wait_mark(self._dl.handle, self.ctx.handle, mark))
+      _shim.check(self.lib.ign_d2h(self._dl.handle, dst, srcp, nbytes))
 
     t_host0 = time.perf_counter()
     th = threading.Thread(target=mesh_thread)
@@ -267,13 +256,11 @@ class VolumePipeline:
       for k in range(n_layers):
         z0, z1 = k * lz, min(sz, (k + 1) * lz)
         off = z0 * sx * sy * es
-        _shim.check(self.lib.ign_h2d(self.ctx.handle, c.c_void_p(self.d_in.ptr + off),
-                                     c.c_void_p(src + off), _u64((z1 - z0) * sx * sy * es)))
+        _shim.check(self.lib.ign_h2d(self.ctx.handle, self.d_in.ptr + off, src + off, (z1 - z0) * sx * sy * es))
         if self.num_mips:
           outs = [m.ptr + z0 * s[0] * s[1] * es for m, s in zip(self.d_mips, self.mip_shapes)]
-          _shim.check(self.lib.ign_pool_mode_2x2x1_dev(
-            self.ctx.handle, c.c_void_p(self.d_in.ptr + off), c.c_int(self.code), _u64(sx), _u64(sy),
-            _u64(z1 - z0), c.c_int(self.num_mips), c.c_int(0), _shim.void_pp(outs)))
+          _shim.check(self.lib.ign_pool_mode_2x2x1_dev(self.ctx.handle, self.d_in.ptr + off, self.code, sx, sy, z1 - z0,
+                                                       self.num_mips, 0, _shim.void_pp(outs)))
         self.ctx.timer_start(layer_mark(k))
         if host_out is not None and self.num_mips:
           # the mip planes of this layer are final: download them now (the D2H engine is idle
@@ -321,7 +308,7 @@ class VolumePipeline:
   # --------------------------------------------------------------- profiling
   def prof_enable(self, on=True):
     for ctx in [self.ctx] + [w[0] for w in self._workers]:
-      _shim.check(self.lib.ign_prof_enable(ctx.handle, c.c_int(int(on))))
+      _shim.check(self.lib.ign_prof_enable(ctx.handle, int(on)))
 
   def prof_read(self):
     """(total ms, launches) per kernel class, summed over the main context and the mesh
@@ -331,7 +318,7 @@ class VolumePipeline:
       tot, n = 0.0, 0
       for ctx in [self.ctx] + [w[0] for w in self._workers]:
         ms, cnt = c.c_float(0), c.c_uint64(0)
-        _shim.check(self.lib.ign_prof_read(ctx.handle, c.c_int(cls), c.byref(ms), c.byref(cnt)))
+        _shim.check(self.lib.ign_prof_read(ctx.handle, cls, c.byref(ms), c.byref(cnt)))
         tot += float(ms.value)
         n += int(cnt.value)
       out[name] = (tot, n)

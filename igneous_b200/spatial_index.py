@@ -46,8 +46,8 @@ def bounding_boxes(labels, max_label=0, ctx=None):
                               "(fastremap.renumber)" % n)
   if vol.size == 0:
     return np.full((n, 6), -1, dtype=np.int64)
-  code = ctypes.c_int(_shim.dtype_code(vol.dtype))
-  sx, sy, sz = (ctypes.c_uint64(int(s)) for s in vol.shape)
+  code = _shim.dtype_code(vol.dtype)
+  sx, sy, sz = vol.shape
   ctx = ctx or _shim.default_context()
   if n == 0:
     found = ctypes.c_uint64(0)

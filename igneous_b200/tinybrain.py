@@ -9,8 +9,6 @@ Same names, argument meaning and return convention (a list of `num_mips`
 Fortran-ordered arrays with the input's number of dimensions).  Everything is
 computed by libigneous_b200 on the GPU; there is no CPU fallback.
 """
-import ctypes
-
 import numpy as np
 
 from . import _shim
@@ -54,9 +52,8 @@ def _pool(img, factor, num_mips, mode, flag, ctx):
   outs = [np.empty(s, dtype=arr.dtype, order="F") for s in shapes]
   if arr.size:
     fn = ctx.lib.ign_pool_mode_2x2x1 if mode else ctx.lib.ign_pool_avg_2x2x1
-    _shim.check(fn(ctx.handle, _shim.ptr(arr), ctypes.c_int(code), ctypes.c_uint64(sx),
-                   ctypes.c_uint64(sy), ctypes.c_uint64(nz), ctypes.c_int(num_mips),
-                   ctypes.c_int(int(flag)), _shim.void_pp([o.ctypes.data for o in outs])))
+    _shim.check(fn(ctx.handle, _shim.ptr(arr), code, sx, sy, nz, num_mips, int(flag),
+                   _shim.void_pp([o.ctypes.data for o in outs])))
   if ndim == 2:
     outs = [o[:, :, 0] for o in outs]
   return outs
@@ -111,11 +108,8 @@ def _select(img, factor, num_mips, op, ctx):
       shp = tuple((s + ff - 1) // ff for s, ff in zip(shp, f[:3]))
       outs.append(np.empty(shp, dtype=ch.dtype, order="F"))
     if ch.size:
-      _shim.check(ctx.lib.ign_pool_select(
-        ctx.handle, _shim.ptr(ch), ctypes.c_int(_shim.dtype_code(ch.dtype)), ctypes.c_uint64(sx),
-        ctypes.c_uint64(sy), ctypes.c_uint64(sz), ctypes.c_uint32(f[0]), ctypes.c_uint32(f[1]),
-        ctypes.c_uint32(f[2]), ctypes.c_int(num_mips), ctypes.c_int(op),
-        _shim.void_pp([o.ctypes.data for o in outs])))
+      _shim.check(ctx.lib.ign_pool_select(ctx.handle, _shim.ptr(ch), _shim.dtype_code(ch.dtype), sx, sy, sz, *f[:3],
+                                          num_mips, op, _shim.void_pp([o.ctypes.data for o in outs])))
     per_chan.append(outs)
   if img.ndim == 4:
     return [np.asfortranarray(np.stack([pc[m] for pc in per_chan], axis=3)) for m in range(num_mips)]

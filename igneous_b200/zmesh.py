@@ -110,9 +110,8 @@ class Mesher:
     self._ctx = ctx
     h = ctypes.c_void_p()
     sx, sy, sz = arr.shape
-    _shim.check(ctx.lib.ign_mesh_begin(
-      ctx.handle, _shim.ptr(arr), ctypes.c_int(_shim.dtype_code(arr.dtype)),
-      ctypes.c_uint64(sx), ctypes.c_uint64(sy), ctypes.c_uint64(sz), ctypes.byref(h)))
+    _shim.check(ctx.lib.ign_mesh_begin(ctx.handle, _shim.ptr(arr), _shim.dtype_code(arr.dtype), sx, sy, sz,
+                                       ctypes.byref(h)))
     self._handle = h
 
   def ids(self):
@@ -123,7 +122,7 @@ class Mesher:
     _shim.check(lib.ign_mesh_num_ids(self._handle, ctypes.byref(n)))
     ids = np.zeros(int(n.value), dtype=np.uint64)
     if n.value:
-      _shim.check(lib.ign_mesh_ids(self._handle, _shim.ptr(ids), ctypes.c_uint64(n.value)))
+      _shim.check(lib.ign_mesh_ids(self._handle, _shim.ptr(ids), n.value))
     return [int(i) for i in ids]
 
   def _simplify(self, reduction_factor, max_error):
@@ -134,8 +133,7 @@ class Mesher:
       raise ValueError("igneous_b200.zmesh: the resident meshes were simplified with %r; call mesh() "
                        "again to extract with %r" % (self._simp, want))
     res = (ctypes.c_float * 3)(*[float(r) for r in self.voxel_res])
-    _shim.check(self._ctx.lib.ign_mesh_simplify(self._handle, res, ctypes.c_int(want[0]),
-                                                ctypes.c_float(want[1])))
+    _shim.check(self._ctx.lib.ign_mesh_simplify(self._handle, res, *want))
     self._simp = want
     self._export = {}
 
@@ -151,7 +149,7 @@ class Mesher:
       voff = np.zeros(len(ids) + 1, dtype=np.uint64)
       foff = np.zeros(len(ids) + 1, dtype=np.uint64)
       res = (ctypes.c_float * 3)(*[float(r) for r in self.voxel_res])
-      _shim.check(lib.ign_mesh_export(self._handle, res, ctypes.c_int(int(key)), _shim.ptr(verts),
+      _shim.check(lib.ign_mesh_export(self._handle, res, int(key), _shim.ptr(verts),
                                       _shim.ptr(faces), _shim.ptr(voff), _shim.ptr(foff)))
       index = {i: j for j, i in enumerate(ids)}
       self._export[key] = (verts, faces, voff, foff, index)

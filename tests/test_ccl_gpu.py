@@ -129,10 +129,8 @@ def test_volume_ccl_equals_whole_volume(ctx, oracle, shape, dtype):
   d_in = ctx.to_device(labels)
   d_out = ctx.alloc(labels.size * 4)
   n = c.c_uint64(0)
-  _shim.check(ctx.lib.ign_ccl6_volume_dev(
-    ctx.handle, _shim.ptr(d_in), c.c_int(_shim.dtype_code(dtype)), c.c_uint64(shape[0]),
-    c.c_uint64(shape[1]), c.c_uint64(shape[2]), _shim.ptr(d_out), c.c_int(_shim.IGN_U32),
-    c.byref(n)))
+  _shim.check(ctx.lib.ign_ccl6_volume_dev(ctx.handle, _shim.ptr(d_in), _shim.dtype_code(dtype), shape[0], shape[1],
+                                          shape[2], _shim.ptr(d_out), _shim.IGN_U32, c.byref(n)))
   got = ctx.to_host(d_out, shape, np.uint32)
   assert n.value == n_want
   assert np.array_equal(got, want.astype(np.uint32))
@@ -150,22 +148,21 @@ def test_ccl_device_resident_properties_1024(ctx):
   d_cc = ctx.alloc(n * 4)
   d_cc2 = ctx.alloc(n * 4)
   try:
-    _shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d_in), c.c_int(_shim.IGN_U64), c.c_uint64(S),
-                                          c.c_uint64(S), c.c_uint64(S), c.c_int64(0), c.c_int64(0), c.c_int64(0),
-                                          c.c_uint32(64), c.c_uint64(4096), c.c_uint64(0), c.c_uint64(1 << 32)))
+    _shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d_in), _shim.IGN_U64, S, S, S, 0, 0, 0, 64, 4096, 0,
+                                          1 << 32))
     n1, n2, n3 = c.c_uint64(0), c.c_uint64(0), c.c_uint64(0)
-    args = (c.c_uint64(S), c.c_uint64(S), c.c_uint64(S))
-    _shim.check(ctx.lib.ign_ccl6_dev(ctx.handle, _shim.ptr(d_in), c.c_int(_shim.IGN_U64), *args, _shim.ptr(d_cc),
-                                     c.c_int(_shim.IGN_U32), c.byref(n1)))
-    _shim.check(ctx.lib.ign_ccl6_dev(ctx.handle, _shim.ptr(d_cc), c.c_int(_shim.IGN_U32), *args, _shim.ptr(d_cc2),
-                                     c.c_int(_shim.IGN_U32), c.byref(n2)))
+    args = (S, S, S)
+    _shim.check(ctx.lib.ign_ccl6_dev(ctx.handle, _shim.ptr(d_in), _shim.IGN_U64, *args, _shim.ptr(d_cc), _shim.IGN_U32,
+                                     c.byref(n1)))
+    _shim.check(ctx.lib.ign_ccl6_dev(ctx.handle, _shim.ptr(d_cc), _shim.IGN_U32, *args, _shim.ptr(d_cc2), _shim.IGN_U32,
+                                     c.byref(n2)))
     assert n1.value == n2.value and 4000 < n1.value < 8000
     a = ctx.to_host(d_cc, (S, S, 64), np.uint32)   # first 64 z-planes
     b = ctx.to_host(d_cc2, (S, S, 64), np.uint32)
     assert np.array_equal(a, b)
     # the begin / finish halves must give the same labelling as the single call
-    _shim.check(ctx.lib.ign_ccl6_volume_dev(ctx.handle, _shim.ptr(d_in), c.c_int(_shim.IGN_U64), *args,
-                                            _shim.ptr(d_cc2), c.c_int(_shim.IGN_U32), c.byref(n3)))
+    _shim.check(ctx.lib.ign_ccl6_volume_dev(ctx.handle, _shim.ptr(d_in), _shim.IGN_U64, *args, _shim.ptr(d_cc2),
+                                            _shim.IGN_U32, c.byref(n3)))
     assert n3.value == n1.value
     assert np.array_equal(ctx.to_host(d_cc2, (S, S, 64), np.uint32), a)
     tail = np.empty((S, S, 8), dtype=np.uint32, order="F")

@@ -151,21 +151,20 @@ def test_rows_past_the_limit_are_rejected_before_any_launch(ctx):
   d_out = ctx.alloc(sx * 8)
   ctx.memset(d_in, 1, sx * 2)
   ctx.sync()
-  dims = (c.c_uint64(sx), c.c_uint64(1), c.c_uint64(1))
+  dims = (sx, 1, 1)
   n = c.c_uint64(0)
   before = ctx.launch_count()
-  assert ctx.lib.ign_ccl6_dev(ctx.handle, _shim.ptr(d_in), c.c_int(_shim.IGN_U16), *dims, _shim.ptr(d_out),
-                              c.c_int(_shim.IGN_U32), c.byref(n)) == IGN_ERR_OVERFLOW
-  assert ctx.lib.ign_dust_dev(ctx.handle, _shim.ptr(d_in), c.c_int(_shim.IGN_U16), *dims,
-                              c.c_uint64(5)) == IGN_ERR_OVERFLOW
+  assert ctx.lib.ign_ccl6_dev(ctx.handle, _shim.ptr(d_in), _shim.IGN_U16, *dims, _shim.ptr(d_out), _shim.IGN_U32,
+                              c.byref(n)) == IGN_ERR_OVERFLOW
+  assert ctx.lib.ign_dust_dev(ctx.handle, _shim.ptr(d_in), _shim.IGN_U16, *dims, 5) == IGN_ERR_OVERFLOW
   v = c.c_void_p()
-  assert ctx.lib.ign_ccl6_volume_begin_dev(ctx.handle, _shim.ptr(d_in), c.c_int(_shim.IGN_U16), *dims, None, None,
-                                           None, None, c.byref(v), c.byref(n)) == IGN_ERR_OVERFLOW
+  assert ctx.lib.ign_ccl6_volume_begin_dev(ctx.handle, _shim.ptr(d_in), _shim.IGN_U16, *dims, None, None, None, None,
+                                           c.byref(v), c.byref(n)) == IGN_ERR_OVERFLOW
   assert not v.value
   assert ctx.launch_count() == before
   # the longest accepted row on the same buffers
-  assert ctx.lib.ign_ccl6_dev(ctx.handle, _shim.ptr(d_in), c.c_int(_shim.IGN_U16), c.c_uint64(MAX_SX),
-                              c.c_uint64(1), c.c_uint64(1), _shim.ptr(d_out), c.c_int(_shim.IGN_U32), c.byref(n)) == 0
+  assert ctx.lib.ign_ccl6_dev(ctx.handle, _shim.ptr(d_in), _shim.IGN_U16, MAX_SX, 1, 1, _shim.ptr(d_out), _shim.IGN_U32,
+                              c.byref(n)) == 0
   assert n.value == 1
   got = np.empty(MAX_SX, dtype=np.uint32)
   ctx.d2h(got, d_out)

@@ -53,9 +53,8 @@ class Ranks:
     for r, h in enumerate(self.heights):
       v, n = c.c_void_p(), c.c_uint64(0)
       src = self.d_in.ptr + self.np * self.z0[r] * self.vol.itemsize
-      _shim.check(self.lib.ign_ccl6_volume_begin_dev(
-        self.ctx.handle, c.c_void_p(src), c.c_int(self.code), c.c_uint64(self.sx), c.c_uint64(self.sy),
-        c.c_uint64(h), *[c.c_void_p(p) for p in self.planes(r)], c.byref(v), c.byref(n)))
+      _shim.check(self.lib.ign_ccl6_volume_begin_dev(self.ctx.handle, src, self.code, self.sx, self.sy, h,
+                                                     *self.planes(r), c.byref(v), c.byref(n)))
       self.vols.append(v)
       self.n_local.append(int(n.value))
       self.ctx.h2d(self.record(r), np.array([n.value], dtype=np.uint64))
@@ -70,10 +69,10 @@ class Ranks:
     from igneous_b200 import _shim
     n = c.c_uint64(0)
     innermost = self.vols[r] is [v for v in self.vols if v is not None][-1]
-    st = self.lib.ign_ccl6_volume_finish_gathered_dev(
-      self.vols[r], c.c_void_p(self.d_rec.ptr if records else None), c.c_int(self.N if nranks is None else nranks),
-      c.c_int(r if rank is None else rank), c.c_void_p(self.out_slab(d_out, r, out_dtype)),
-      c.c_int(_shim.dtype_code(out_dtype)), c.byref(n))
+    st = self.lib.ign_ccl6_volume_finish_gathered_dev(self.vols[r], self.d_rec.ptr if records else None,
+                                                      self.N if nranks is None else nranks, r if rank is None else rank,
+                                                      self.out_slab(d_out, r, out_dtype), _shim.dtype_code(out_dtype),
+                                                      c.byref(n))
     if innermost:  # consumed, also on failure; a volume ended out of order is left open
       self.vols[r] = None
     return st, int(n.value)
@@ -300,9 +299,8 @@ def link_dev(ctx, rk, b, off, capacity):
   vb, lb = rk.planes(b + 1)[:2]
   pairs = np.full((max(capacity, 1) + 4, 2), 0xABABABABABABABAB, dtype=np.uint64)
   n = c.c_uint64(0)
-  _shim.check(ctx.lib.ign_ccl6_link_dev(
-    ctx.handle, c.c_void_p(va), c.c_void_p(la), c.c_uint64(int(off[b])), c.c_void_p(vb), c.c_void_p(lb),
-    c.c_uint64(int(off[b + 1])), c.c_uint64(rk.np), _shim.ptr(pairs), c.c_uint64(capacity), c.byref(n)))
+  _shim.check(ctx.lib.ign_ccl6_link_dev(ctx.handle, va, la, int(off[b]), vb, lb, int(off[b + 1]), rk.np,
+                                        _shim.ptr(pairs), capacity, c.byref(n)))
   return pairs, int(n.value)
 
 
@@ -343,8 +341,8 @@ def test_task_file_path_matches_whole_volume(ctx, oracle, dtype):
     d_out = ctx.alloc(vol.size * 4)
     for r in reversed(range(rk.N)):
       table = np.concatenate([[0], lut[int(off[r]) + 1:int(off[r + 1]) + 1]]).astype(np.uint32)
-      st = ctx.lib.ign_ccl6_volume_finish_dev(rk.vols[r], _shim.ptr(table), c.c_uint64(n_global),
-                                             c.c_void_p(rk.out_slab(d_out, r, np.uint32)), c.c_int(_shim.IGN_U32))
+      st = ctx.lib.ign_ccl6_volume_finish_dev(rk.vols[r], _shim.ptr(table), n_global, rk.out_slab(d_out, r, np.uint32),
+                                              _shim.IGN_U32)
       rk.vols[r] = None
       _shim.check(st)
     got = ctx.to_host(d_out, vol.shape, np.uint32)

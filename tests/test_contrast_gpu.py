@@ -1,6 +1,5 @@
 """GPU histogram, contrast stretch, quantize and CLAHE against numpy, tests/contrastref.py and
 the recorded OpenCV fixtures; the contrast tasks end to end on file:// layers."""
-import ctypes
 import os
 import random
 
@@ -50,8 +49,7 @@ def test_histogram_over_2_32_in_one_bin(C, dt):
   try:
     ctx.memset(buf, 7, n * es)  # every element 7 (u8) or 0x0707 (u16)
     ctx.memset(hist, 0, bins * 8)
-    _shim.check(ctx.lib.ign_histogram_dev(ctx.handle, _shim.ptr(buf), ctypes.c_int(_shim.dtype_code(dt)),
-                                          ctypes.c_uint64(n), _shim.ptr(hist)))
+    _shim.check(ctx.lib.ign_histogram_dev(ctx.handle, _shim.ptr(buf), _shim.dtype_code(dt), n, _shim.ptr(hist)))
     got = ctx.to_host(hist, (bins,), np.uint64)
   finally:
     buf.free()
@@ -148,24 +146,18 @@ def test_dev_entries_refuse_misaligned_buffers(C):
   from igneous_b200 import _shim
   ctx = _shim.default_context()
   buf, hist = ctx.alloc(4096), ctx.alloc(65536 * 8)
-  u = ctypes.c_uint64
   try:
     with pytest.raises(_shim.IgneousB200Error) as e:
-      _shim.check(ctx.lib.ign_histogram_dev(ctx.handle, ctypes.c_void_p(buf.ptr + 1), ctypes.c_int(_shim.IGN_U16),
-                                            u(100), _shim.ptr(hist)))
+      _shim.check(ctx.lib.ign_histogram_dev(ctx.handle, buf.ptr + 1, _shim.IGN_U16, 100, _shim.ptr(hist)))
     assert e.value.status == -2
     with pytest.raises(_shim.IgneousB200Error):
-      _shim.check(ctx.lib.ign_clahe_dev(ctx.handle, ctypes.c_void_p(buf.ptr + 1), ctypes.c_int(_shim.IGN_U16), u(8),
-                                        u(8), u(1), ctypes.c_double(40.0), ctypes.c_uint32(2), ctypes.c_uint32(2),
-                                        _shim.ptr(buf)))
+      _shim.check(ctx.lib.ign_clahe_dev(ctx.handle, buf.ptr + 1, _shim.IGN_U16, 8, 8, 1, 40.0, 2, 2, _shim.ptr(buf)))
     with pytest.raises(_shim.IgneousB200Error):
-      _shim.check(ctx.lib.ign_quantize_dev(ctx.handle, ctypes.c_void_p(buf.ptr + 2), u(16),
-                                           ctypes.c_void_p(buf.ptr + 2048)))
+      _shim.check(ctx.lib.ign_quantize_dev(ctx.handle, buf.ptr + 2, 16, buf.ptr + 2048))
     # an odd uint8 offset is fine: the head before the first 16-byte boundary is counted by scalar loads
     ctx.memset(buf, 5, 4096)
     ctx.memset(hist, 0, 256 * 8)
-    _shim.check(ctx.lib.ign_histogram_dev(ctx.handle, ctypes.c_void_p(buf.ptr + 3), ctypes.c_int(_shim.IGN_U8),
-                                          u(4000), _shim.ptr(hist)))
+    _shim.check(ctx.lib.ign_histogram_dev(ctx.handle, buf.ptr + 3, _shim.IGN_U8, 4000, _shim.ptr(hist)))
     got = ctx.to_host(hist, (256,), np.uint64)
     assert int(got[5]) == 4000 and int(got.sum()) == 4000
   finally:

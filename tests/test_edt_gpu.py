@@ -144,15 +144,14 @@ def test_edt_dev_matches_host_entry(ctx):
   from igneous_b200 import _shim
   labels = np.asfortranarray(voronoi((67, 45, 33), seed=11).astype(np.uint32))
   a = (c.c_float * 3)(4.5, 7.25, 40.3)
-  dims = tuple(c.c_uint64(s) for s in labels.shape)
   for bb, sq in ((0, 1), (1, 0)):
     host = np.empty(labels.shape, np.float32, order="F")
-    _shim.check(ctx.lib.ign_edt(ctx.handle, _shim.ptr(labels), c.c_int(_shim.IGN_U32), *dims, a, c.c_int(bb),
-                                c.c_int(sq), _shim.ptr(host)))
+    _shim.check(ctx.lib.ign_edt(ctx.handle, _shim.ptr(labels), _shim.IGN_U32, *labels.shape, a, bb, sq,
+                                _shim.ptr(host)))
     d_in = ctx.to_device(labels)
     d_out = ctx.alloc(labels.size * 4)
-    _shim.check(ctx.lib.ign_edt_dev(ctx.handle, _shim.ptr(d_in), c.c_int(_shim.IGN_U32), *dims, a, c.c_int(bb),
-                                    c.c_int(sq), _shim.ptr(d_out)))
+    _shim.check(ctx.lib.ign_edt_dev(ctx.handle, _shim.ptr(d_in), _shim.IGN_U32, *labels.shape, a, bb, sq,
+                                    _shim.ptr(d_out)))
     dev = ctx.to_host(d_out, labels.shape, np.float32)
     np.testing.assert_array_equal(dev.view(np.uint32), host.view(np.uint32))
     d_in.free()
@@ -175,8 +174,7 @@ def test_refusals(ctx):
   bad = (c.c_float * 3)(1.0, float("inf"), 1.0)  # +inf only on an axis of extent 1
   out = np.empty(64, np.float32)
   with pytest.raises(_shim.IgneousB200Error):
-    _shim.check(ctx.lib.ign_edt(ctx.handle, _shim.ptr(lab), c.c_int(_shim.IGN_U32), c.c_uint64(4), c.c_uint64(4),
-                                c.c_uint64(4), bad, c.c_int(1), c.c_int(1), _shim.ptr(out)))
+    _shim.check(ctx.lib.ign_edt(ctx.handle, _shim.ptr(lab), _shim.IGN_U32, 4, 4, 4, bad, 1, 1, _shim.ptr(out)))
   assert edt.edt(np.zeros((0, 3), np.uint8), ctx=ctx).shape == (0, 3)
 
 
@@ -232,11 +230,10 @@ def test_block_volume_past_2_32_voxels(big_ctx, black_border):
       planes[key] = lab.offset(z * sx * sy)
   ctx.sync()
   a = (c.c_float * 3)(*BIG_A)
-  dims = tuple(c.c_uint64(s) for s in BIG)
 
   def run(squared):
-    _shim.check(ctx.lib.ign_edt_dev(ctx.handle, _shim.ptr(lab), c.c_int(IGN_U8), *dims, a, c.c_int(int(black_border)),
-                                    c.c_int(squared), _shim.ptr(out)))
+    _shim.check(ctx.lib.ign_edt_dev(ctx.handle, _shim.ptr(lab), IGN_U8, *BIG, a, int(black_border), squared,
+                                    _shim.ptr(out)))
     ctx.sync()
 
   run(1)
@@ -252,8 +249,7 @@ def test_block_volume_past_2_32_voxels(big_ctx, black_border):
   bufs.append(box)
   zs = np.arange(sz)
   for x0, y0 in ((0, 0), (sx - 3, sy - 3), (0, sy - 3), (max(0, xb - 1), max(0, yb - 1))):
-    _shim.check(ctx.lib.ign_copy_box_dev(ctx.handle, _shim.ptr(out), c.c_int(IGN_F32), *dims, c.c_uint64(x0),
-                                         c.c_uint64(y0), c.c_uint64(0), c.c_uint64(3), c.c_uint64(3), c.c_uint64(sz),
+    _shim.check(ctx.lib.ign_copy_box_dev(ctx.handle, _shim.ptr(out), IGN_F32, *BIG, x0, y0, 0, 3, 3, sz,
                                          _shim.ptr(box)))
     got = ctx.to_host(box, (3, 3, sz), np.float32)
     g = np.meshgrid(np.arange(x0, x0 + 3), np.arange(y0, y0 + 3), zs, indexing="ij")

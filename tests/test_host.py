@@ -13,12 +13,12 @@ def test_ccl6_solve_union_rule():
   pairs = np.array([[5, 2], [7, 5], [3, 4], [9, 9]], dtype=np.uint64)
   lut = np.zeros(10, dtype=np.uint32)
   n = c.c_uint64(0)
-  _shim.check(lib.ign_ccl6_solve(_shim.ptr(pairs), c.c_uint64(len(pairs)), c.c_uint64(9), _shim.ptr(lut), c.byref(n)))
+  _shim.check(lib.ign_ccl6_solve(_shim.ptr(pairs), len(pairs), 9, _shim.ptr(lut), c.byref(n)))
   assert n.value == 6
   assert [int(v) for v in lut] == [0, 1, 2, 3, 3, 2, 4, 2, 5, 6]
   # out-of-range pair is rejected
   bad = np.array([[1, 11]], dtype=np.uint64)
-  assert lib.ign_ccl6_solve(_shim.ptr(bad), c.c_uint64(1), c.c_uint64(9), _shim.ptr(lut), c.byref(n)) != 0
+  assert lib.ign_ccl6_solve(_shim.ptr(bad), 1, 9, _shim.ptr(lut), c.byref(n)) != 0
 
 
 def test_num_mips_from_memory_target_reference_kats():

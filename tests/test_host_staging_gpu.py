@@ -12,7 +12,6 @@ pytestmark = pytest.mark.gpu
 
 U8, U16, U32, U64, F32 = _shim.IGN_U8, _shim.IGN_U16, _shim.IGN_U32, _shim.IGN_U64, _shim.IGN_F32
 SHAPES = [(37, 29, 11), (64, 48, 8)]  # odd extents; 37*29*11 bytes is not a multiple of 16
-u64, i32, u32, f64 = c.c_uint64, c.c_int, c.c_uint32, c.c_double
 
 
 def _seg(shape, seed, dtype=np.uint32, ids=40):
@@ -95,9 +94,9 @@ def test_ccl6(ctx, shape):
   seg = _seg(shape, 1)
 
   def call(r, dev, dtype=U32):
-    n = u64(0)
-    _shim.check(_fn(ctx, "ign_ccl6", dev)(ctx.handle, r.inp(seg), i32(dtype), *map(u64, shape),
-                                           r.out(np.zeros(shape, np.uint32)), i32(U32), c.byref(n)))
+    n = c.c_uint64(0)
+    _shim.check(_fn(ctx, "ign_ccl6", dev)(ctx.handle, r.inp(seg), dtype, *shape, r.out(np.zeros(shape, np.uint32)), U32,
+                                          c.byref(n)))
     return [n]
   _both(ctx, call)
   _rejects(ctx, lambda r, dev: call(r, dev, F32))
@@ -108,7 +107,7 @@ def test_dust(ctx, shape):
   seg = _seg(shape, 2)
 
   def call(r, dev, dtype=U32):
-    _shim.check(_fn(ctx, "ign_dust", dev)(ctx.handle, r.out(seg), i32(dtype), *map(u64, shape), u64(20)))
+    _shim.check(_fn(ctx, "ign_dust", dev)(ctx.handle, r.out(seg), dtype, *shape, 20))
     return []
   _both(ctx, call)
   _rejects(ctx, lambda r, dev: call(r, dev, F32))
@@ -120,10 +119,9 @@ def test_ccl_task(ctx, shape):
   rails = [s // 2 for s in shape]
 
   def call(r, dev, dtype=U8):
-    n = u64(0)
-    _shim.check(_fn(ctx, "ign_ccl_task", dev)(ctx.handle, r.inp(img), i32(dtype), *map(u64, shape), i32(1), f64(100.0),
-                                               i32(1), f64(200.0), *map(u64, rails), u64(3), u64(1000),
-                                               r.out(np.zeros(shape, np.uint64)), c.byref(n)))
+    n = c.c_uint64(0)
+    _shim.check(_fn(ctx, "ign_ccl_task", dev)(ctx.handle, r.inp(img), dtype, *shape, 1, 100.0, 1, 200.0, *rails, 3,
+                                              1000, r.out(np.zeros(shape, np.uint64)), c.byref(n)))
     return [n]
   _both(ctx, call)
   _rejects(ctx, lambda r, dev: call(r, dev, 99))
@@ -138,8 +136,8 @@ def test_pool_select(ctx, shape):
     for _ in range(max(mips, 1)):
       ext = [(e + 1) // 2 for e in ext]
       outs.append(r.out(np.zeros(ext, np.uint8)))
-    _shim.check(_fn(ctx, "ign_pool_select", dev)(ctx.handle, r.inp(img), i32(U8), *map(u64, shape), u32(2), u32(2),
-                                                  u32(2), i32(mips), i32(0), _shim.void_pp([p.value for p in outs])))
+    _shim.check(_fn(ctx, "ign_pool_select", dev)(ctx.handle, r.inp(img), U8, *shape, 2, 2, 2, mips, 0,
+                                                 _shim.void_pp([p.value for p in outs])))
     return []
   _both(ctx, call)
   _rejects(ctx, lambda r, dev: call(r, dev, 0))
@@ -157,7 +155,7 @@ def test_pool_2x2x1(ctx, shape, mode):
       x, y = (x + 1) // 2, (y + 1) // 2
       outs.append(r.out(np.zeros((x, y, z), arr.dtype)))
     name = "ign_pool_mode_2x2x1" if mode else "ign_pool_avg_2x2x1"
-    _shim.check(_fn(ctx, name, dev)(ctx.handle, r.inp(arr), i32(dt), *map(u64, shape), i32(mips), i32(0),
+    _shim.check(_fn(ctx, name, dev)(ctx.handle, r.inp(arr), dt, *shape, mips, 0,
                                     _shim.void_pp([p.value for p in outs])))
     return []
   _both(ctx, call)
@@ -169,8 +167,8 @@ def test_dilate_multilabel(ctx, shape):
   seg = _seg(shape, 6)
 
   def call(r, dev, dtype=U32):
-    _shim.check(_fn(ctx, "ign_dilate_multilabel", dev)(ctx.handle, r.inp(seg), i32(dtype), *map(u64, shape),
-                                                        r.out(np.zeros(shape, np.uint32))))
+    _shim.check(_fn(ctx, "ign_dilate_multilabel", dev)(ctx.handle, r.inp(seg), dtype, *shape,
+                                                       r.out(np.zeros(shape, np.uint32))))
     return []
   _both(ctx, call)
   _rejects(ctx, lambda r, dev: call(r, dev, F32))
@@ -182,8 +180,7 @@ def test_fill_holes(ctx, shape):
 
   def call(r, dev, dtype=U32):
     z = np.zeros(shape, np.uint32)
-    _shim.check(_fn(ctx, "ign_fill_holes", dev)(ctx.handle, r.inp(seg), i32(dtype), *map(u64, shape), i32(1), i32(50),
-                                                 r.out(z), r.out(z)))
+    _shim.check(_fn(ctx, "ign_fill_holes", dev)(ctx.handle, r.inp(seg), dtype, *shape, 1, 50, r.out(z), r.out(z)))
     return []
   _both(ctx, call)
   _rejects(ctx, lambda r, dev: call(r, dev, F32))
@@ -195,7 +192,7 @@ def test_histogram(ctx, shape):
   start = np.random.default_rng(9).integers(0, 1000, size=65536).astype(np.uint64)  # added into
 
   def call(r, dev, dtype=U16):
-    _shim.check(_fn(ctx, "ign_histogram", dev)(ctx.handle, r.inp(img), i32(dtype), u64(img.size), r.out(start)))
+    _shim.check(_fn(ctx, "ign_histogram", dev)(ctx.handle, r.inp(img), dtype, img.size, r.out(start)))
     return []
   _both(ctx, call)
   _rejects(ctx, lambda r, dev: call(r, dev, 99))
@@ -209,9 +206,9 @@ def test_contrast_stretch(ctx, shape):
   upper[0] = lower[0]
 
   def call(r, dev, dtype=U8):
-    _shim.check(_fn(ctx, "ign_contrast_stretch", dev)(ctx.handle, r.inp(img), i32(dtype), *map(u64, shape), u64(1),
-                                                       _shim.ptr(lower), _shim.ptr(upper), f64(0.0), f64(65535.0),
-                                                       r.out(np.zeros(shape, np.uint16)), i32(U16)))
+    _shim.check(_fn(ctx, "ign_contrast_stretch", dev)(ctx.handle, r.inp(img), dtype, *shape, 1, _shim.ptr(lower),
+                                                      _shim.ptr(upper), 0.0, 65535.0, r.out(np.zeros(shape, np.uint16)),
+                                                      U16))
     return []
   _both(ctx, call)
   _rejects(ctx, lambda r, dev: call(r, dev, U32))
@@ -223,7 +220,7 @@ def test_quantize(ctx, shape):
 
   def call(r, dev, null_out=False):
     out = c.c_void_p(None) if null_out else r.out(np.zeros(x.size, np.uint8))
-    _shim.check(_fn(ctx, "ign_quantize", dev)(ctx.handle, r.inp(x), u64(x.size), out))
+    _shim.check(_fn(ctx, "ign_quantize", dev)(ctx.handle, r.inp(x), x.size, out))
     return []
   _both(ctx, call)
   _rejects(ctx, lambda r, dev: call(r, dev, True))
@@ -234,8 +231,8 @@ def test_clahe(ctx, shape):
   img = np.asfortranarray(np.random.default_rng(12).integers(0, 256, size=shape).astype(np.uint8))
 
   def call(r, dev, dtype=U8):
-    _shim.check(_fn(ctx, "ign_clahe", dev)(ctx.handle, r.inp(img), i32(dtype), *map(u64, shape), f64(2.0), u32(4),
-                                            u32(3), r.out(np.zeros(shape, np.uint8))))
+    _shim.check(_fn(ctx, "ign_clahe", dev)(ctx.handle, r.inp(img), dtype, *shape, 2.0, 4, 3,
+                                           r.out(np.zeros(shape, np.uint8))))
     return []
   _both(ctx, call)
   _rejects(ctx, lambda r, dev: call(r, dev, U32))
@@ -247,9 +244,9 @@ def test_renumber(ctx, shape):
   n = seg.size
 
   def call(r, dev, dtype=U64):
-    k = u64(0)
-    _shim.check(_fn(ctx, "ign_renumber", dev)(ctx.handle, r.inp(seg), i32(dtype), u64(n), r.out(np.zeros(n, np.uint32)),
-                                               r.out(np.zeros(20, np.uint64)), u64(20), c.byref(k)))
+    k = c.c_uint64(0)
+    _shim.check(_fn(ctx, "ign_renumber", dev)(ctx.handle, r.inp(seg), dtype, n, r.out(np.zeros(n, np.uint32)),
+                                              r.out(np.zeros(20, np.uint64)), 20, c.byref(k)))
     return [k]
   _, (k,) = _both(ctx, call)
   assert k > 20  # the unique list is cut at its capacity
@@ -263,15 +260,15 @@ def test_remap(ctx, shape):
   vals = (keys * 7 + 3) % 41
 
   def call(r, dev, dtype=U32, n_keys=keys.size):
-    _shim.check(_fn(ctx, "ign_remap", dev)(ctx.handle, r.out(seg), i32(dtype), u64(seg.size), _shim.ptr(keys),
-                                            _shim.ptr(vals), u64(n_keys), i32(0)))
+    _shim.check(_fn(ctx, "ign_remap", dev)(ctx.handle, r.out(seg), dtype, seg.size, _shim.ptr(keys), _shim.ptr(vals),
+                                           n_keys, 0))
     return []
   _both(ctx, call)
   _rejects(ctx, lambda r, dev: call(r, dev, F32, 0))
 
 
 def _cseg_args(shape):
-  return [*map(u64, shape), u64(1), u32(8), u32(8), u32(8)]
+  return [*shape, 1, 8, 8, 8]
 
 
 @pytest.mark.parametrize("shape", SHAPES)
@@ -280,17 +277,17 @@ def test_cseg(ctx, shape):
   cap = 1 + 2 * 1024 + 3 * seg.size
 
   def encode(r, dev, dtype=U32):
-    n = u64(0)
-    _shim.check(_fn(ctx, "ign_cseg_encode", dev)(ctx.handle, r.inp(seg), i32(dtype), *_cseg_args(shape),
-                                                  r.out(np.zeros(cap, np.uint32)), u64(cap), c.byref(n)))
+    n = c.c_uint64(0)
+    _shim.check(_fn(ctx, "ign_cseg_encode", dev)(ctx.handle, r.inp(seg), dtype, *_cseg_args(shape),
+                                                 r.out(np.zeros(cap, np.uint32)), cap, c.byref(n)))
     return [n]
   (stream,), (n_words,) = _both(ctx, encode)
   stream = stream[:n_words]
   _rejects(ctx, lambda r, dev: encode(r, dev, U8))
 
   def decode(r, dev, dtype=U32):
-    _shim.check(_fn(ctx, "ign_cseg_decode", dev)(ctx.handle, r.inp(stream), u64(stream.size), i32(dtype),
-                                                  *_cseg_args(shape), r.out(np.zeros(shape, np.uint32))))
+    _shim.check(_fn(ctx, "ign_cseg_decode", dev)(ctx.handle, r.inp(stream), stream.size, dtype, *_cseg_args(shape),
+                                                 r.out(np.zeros(shape, np.uint32))))
     return []
   (back,), _ = _both(ctx, decode)
   assert np.array_equal(back, seg)
@@ -298,15 +295,15 @@ def test_cseg(ctx, shape):
 
 
 def _export(ctx, m):
-  nv, nf, nl = u64(0), u64(0), u64(0)
+  nv, nf, nl = c.c_uint64(0), c.c_uint64(0), c.c_uint64(0)
   _shim.check(ctx.lib.ign_mesh_totals(m, c.byref(nv), c.byref(nf)))
   _shim.check(ctx.lib.ign_mesh_num_ids(m, c.byref(nl)))
   ids = np.zeros(nl.value, np.uint64)
-  _shim.check(ctx.lib.ign_mesh_ids(m, _shim.ptr(ids), u64(ids.size)))
+  _shim.check(ctx.lib.ign_mesh_ids(m, _shim.ptr(ids), ids.size))
   out = [ids, np.zeros((nv.value, 3), np.float32), np.zeros((nf.value, 3), np.uint32),
          np.zeros(nl.value + 1, np.uint64), np.zeros(nl.value + 1, np.uint64)]
   res = (c.c_float * 3)(16.0, 16.0, 40.0)
-  _shim.check(ctx.lib.ign_mesh_export(m, res, i32(1), *[_shim.ptr(a) for a in out[1:]]))
+  _shim.check(ctx.lib.ign_mesh_export(m, res, 1, *[_shim.ptr(a) for a in out[1:]]))
   return out
 
 
@@ -317,8 +314,7 @@ def test_mesh_begin(ctx, shape):
 
   def call(r, dev, sx=shape[0]):
     m = c.c_void_p()
-    _shim.check(_fn(ctx, "ign_mesh_begin", dev)(ctx.handle, r.inp(seg), i32(U32), u64(sx), *map(u64, shape[1:]),
-                                                 c.byref(m)))
+    _shim.check(_fn(ctx, "ign_mesh_begin", dev)(ctx.handle, r.inp(seg), U32, sx, *shape[1:], c.byref(m)))
     try:
       got.append(_export(ctx, m))
     finally:

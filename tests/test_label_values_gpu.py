@@ -251,9 +251,8 @@ def test_ccl_and_dust_label_values(ctx, monkeypatch, dtype, name):
       d_out = ctx.alloc(v.size * 4)
       try:
         nn = c.c_uint64(0)
-        _shim.check(ctx.lib.ign_ccl6_volume_dev(
-          ctx.handle, _shim.ptr(d_in), c.c_int(_shim.dtype_code(dtype)), c.c_uint64(shape[0]), c.c_uint64(shape[1]),
-          c.c_uint64(shape[2]), _shim.ptr(d_out), c.c_int(_shim.IGN_U32), c.byref(nn)))
+        _shim.check(ctx.lib.ign_ccl6_volume_dev(ctx.handle, _shim.ptr(d_in), _shim.dtype_code(dtype), shape[0],
+                                                shape[1], shape[2], _shim.ptr(d_out), _shim.IGN_U32, c.byref(nn)))
         assert nn.value == wn and np.array_equal(ctx.to_host(d_out, shape, np.uint32), want.astype(np.uint32))
       finally:
         d_in.free()

@@ -147,14 +147,6 @@ def _alloc(big, nbytes):
   return b
 
 
-def _p(v):
-  return c.c_void_p(int(v))
-
-
-def _dims(shape):
-  return tuple(c.c_uint64(s) for s in shape)
-
-
 def _z_slabs(shape, itemsize):
   sx, sy, sz = shape
   step = max(1, SLAB_BYTES // (sx * sy * itemsize))
@@ -204,7 +196,7 @@ def _histogram_u8(big, buf, n):
   ctx, _ = big
   hist = _alloc(big, 256 * 8)
   ctx.memset(hist, 0, 256 * 8)
-  assert ctx.lib.ign_histogram_dev(ctx.handle, _p(buf.ptr), c.c_int(IGN_U8), c.c_uint64(n), _p(hist.ptr)) == 0
+  assert ctx.lib.ign_histogram_dev(ctx.handle, buf.ptr, IGN_U8, n, hist.ptr) == 0
   out = np.empty(256, np.uint64)
   ctx.d2h(out, hist)
   ctx.sync()
@@ -213,8 +205,7 @@ def _histogram_u8(big, buf, n):
 
 def _ccl(ctx, d_in, shape, d_out, out_dtype):
   n = c.c_uint64(0)
-  rc = ctx.lib.ign_ccl6_dev(ctx.handle, _p(d_in.ptr), c.c_int(IGN_U8), *_dims(shape), _p(d_out.ptr),
-                            c.c_int(out_dtype), c.byref(n))
+  rc = ctx.lib.ign_ccl6_dev(ctx.handle, d_in.ptr, IGN_U8, *shape, d_out.ptr, out_dtype, c.byref(n))
   return rc, n.value
 
 
@@ -257,12 +248,10 @@ def test_ccl_and_find_objects_of_block_volumes_past_2_32(big, shape):
 
   # the largest label, found on the device, then every component's box
   max_label = c.c_uint64(0)
-  assert ctx.lib.ign_find_objects_dev(ctx.handle, _p(d_out.ptr), c.c_int(IGN_U32), *_dims(shape),
-                                      c.byref(max_label), None) == 0
+  assert ctx.lib.ign_find_objects_dev(ctx.handle, d_out.ptr, IGN_U32, *shape, c.byref(max_label), None) == 0
   assert max_label.value == n_want
   d_boxes = _alloc(big, n_want * 24)
-  assert ctx.lib.ign_find_objects_dev(ctx.handle, _p(d_out.ptr), c.c_int(IGN_U32), *_dims(shape),
-                                      c.byref(max_label), _p(d_boxes.ptr)) == 0
+  assert ctx.lib.ign_find_objects_dev(ctx.handle, d_out.ptr, IGN_U32, *shape, c.byref(max_label), d_boxes.ptr) == 0
   boxes = np.empty((n_want, 6), np.uint32)
   ctx.d2h(boxes, d_boxes)
   ctx.sync()
@@ -300,12 +289,11 @@ def test_ccl_refuses_2_31_runs_or_more(big, shape, pattern, runs):
   ctx.sync()
   assert (head == 0xAB).all()  # nothing written
   # the same refusal for dust, the task body and the multi-volume begin
-  assert ctx.lib.ign_dust_dev(ctx.handle, _p(d_in.ptr), c.c_int(IGN_U8), *_dims(shape), c.c_uint64(2)) == \
-      IGN_ERR_OVERFLOW
+  assert ctx.lib.ign_dust_dev(ctx.handle, d_in.ptr, IGN_U8, *shape, 2) == IGN_ERR_OVERFLOW
   v = c.c_void_p()
   k = c.c_uint64(0)
-  assert ctx.lib.ign_ccl6_volume_begin_dev(ctx.handle, _p(d_in.ptr), c.c_int(IGN_U8), *_dims(shape), None, None,
-                                           None, None, c.byref(v), c.byref(k)) == IGN_ERR_OVERFLOW
+  assert ctx.lib.ign_ccl6_volume_begin_dev(ctx.handle, d_in.ptr, IGN_U8, *shape, None, None, None, None, c.byref(v),
+                                           c.byref(k)) == IGN_ERR_OVERFLOW
   assert not v.value
 
 
@@ -318,7 +306,7 @@ def test_dust_keeps_a_component_of_2_32_voxels(big):
   d = _alloc(big, n)
   ctx.memset(d, 1, n)
   ctx.sync()
-  assert ctx.lib.ign_dust_dev(ctx.handle, _p(d.ptr), c.c_int(IGN_U8), *_dims(HEADLINE), c.c_uint64(1)) == 0
+  assert ctx.lib.ign_dust_dev(ctx.handle, d.ptr, IGN_U8, *HEADLINE, 1) == 0
   hist = _histogram_u8(big, d, n)
   assert hist[1] == n and hist.sum() == n
 
@@ -346,7 +334,7 @@ def test_dust_between_a_huge_component_and_small_ones(big):
   _fill_planes(ctx, d, shape, lambda z: with_keep if keep_box[2].start <= z < keep_box[2].stop else ones)
   ctx.h2d(d.offset(tail_z * sx * sy), want_tail)
   ctx.sync()
-  assert ctx.lib.ign_dust_dev(ctx.handle, _p(d.ptr), c.c_int(IGN_U8), *_dims(shape), c.c_uint64(2**21)) == 0
+  assert ctx.lib.ign_dust_dev(ctx.handle, d.ptr, IGN_U8, *shape, 2**21) == 0
 
   hist = _histogram_u8(big, d, n)
   want = np.zeros(256, np.uint64)
@@ -375,14 +363,12 @@ def test_ccl_task_dust_threshold_2_32(big):
   ctx.memset(d_in, 1, n)
   ctx.sync()
   k = c.c_uint64(0)
-  rails = _dims(shape)  # rail coordinates outside the volume: none
-  assert ctx.lib.ign_ccl_task_dev(ctx.handle, _p(d_in.ptr), c.c_int(IGN_U8), *_dims(shape), c.c_int(0),
-                                  c.c_double(0), c.c_int(0), c.c_double(0), *rails, c.c_uint64(2**32),
-                                  c.c_uint64(0), _p(d_out.ptr), c.byref(k)) == 0
+  rails = shape  # rail coordinates outside the volume: none
+  assert ctx.lib.ign_ccl_task_dev(ctx.handle, d_in.ptr, IGN_U8, *shape, 0, 0, 0, 0, *rails, 2**32, 0, d_out.ptr,
+                                  c.byref(k)) == 0
   assert k.value == 1
   # labels narrowed onto the input buffer, then counted
-  assert ctx.lib.ign_cast_dev(ctx.handle, _p(d_out.ptr), c.c_int(IGN_U64), _p(d_in.ptr), c.c_int(IGN_U8),
-                              c.c_uint64(n)) == 0
+  assert ctx.lib.ign_cast_dev(ctx.handle, d_out.ptr, IGN_U64, d_in.ptr, IGN_U8, n) == 0
   hist = _histogram_u8(big, d_in, n)
   assert hist[1] == n and hist.sum() == n
   for z0, z1 in ((0, 1), (shape[2] - 1, shape[2])):  # the u64 labels themselves at both ends
@@ -400,7 +386,7 @@ def test_mesher_refuses_more_than_2_31_corners(big):
   x = np.arange(shape[0])
   _fill_repeated(ctx, d, shape, np.broadcast_to((1 + (x // 4) % 2).astype(np.uint8)[:, None], shape[:2]))
   m = c.c_void_p()
-  rc = ctx.lib.ign_mesh_begin_dev(ctx.handle, _p(d.ptr), c.c_int(IGN_U8), *_dims(shape), c.byref(m))
+  rc = ctx.lib.ign_mesh_begin_dev(ctx.handle, d.ptr, IGN_U8, *shape, c.byref(m))
   assert rc == IGN_ERR_OVERFLOW, ctx.lib.ign_last_error()
   assert not m.value
   assert str(mesher_triangles(shape, 4)).encode() in ctx.lib.ign_last_error()
@@ -414,8 +400,7 @@ BOUNDARY_Z = (0, 511, 512, 1023, 1024)
 def _synth_image(big, shape, seed):
   ctx, _ = big
   d = _alloc(big, shape[0] * shape[1] * shape[2])
-  assert ctx.lib.ign_synth_image_dev(ctx.handle, _p(d.ptr), *_dims(shape), c.c_int64(0), c.c_int64(0),
-                                     c.c_int64(0), c.c_uint64(seed)) == 0
+  assert ctx.lib.ign_synth_image_dev(ctx.handle, d.ptr, *shape, 0, 0, 0, seed) == 0
   return d
 
 
@@ -449,8 +434,7 @@ def test_pool_2x2x1_past_2_32_matches_oracle_on_boundary_planes(big, oracle, kin
     fn, flag = ctx.lib.ign_pool_mode_2x2x1_dev, int(kind == "sparse_mode")
   else:
     fn, flag = ctx.lib.ign_pool_avg_2x2x1_dev, int(kind[-1])
-  assert fn(ctx.handle, _p(d_in.ptr), c.c_int(IGN_U8), *_dims(shape), c.c_int(num_mips), c.c_int(flag),
-            _shim.void_pp([o.ptr for o in outs])) == 0
+  assert fn(ctx.handle, d_in.ptr, IGN_U8, *shape, num_mips, flag, _shim.void_pp([o.ptr for o in outs])) == 0
   ctx.sync()
   k = 2**31 // (sx * sy)  # the plane that holds element 2^31
   zs = sorted({0, k - 1, k, k + 1, min(2**32 // (sx * sy), sz - 1), sz - 1})
@@ -486,8 +470,8 @@ def test_pool_2x2x1_mode_of_a_block_volume_past_2_32(big):
   shapes = _mip_shapes(shape, (2, 2, 1), num_mips)
   outs = [_alloc(big, int(np.prod(s))) for s in shapes]
   from igneous_b200 import _shim
-  assert ctx.lib.ign_pool_mode_2x2x1_dev(ctx.handle, _p(d_in.ptr), c.c_int(IGN_U8), *_dims(shape), c.c_int(num_mips),
-                                         c.c_int(0), _shim.void_pp([o.ptr for o in outs])) == 0
+  assert ctx.lib.ign_pool_mode_2x2x1_dev(ctx.handle, d_in.ptr, IGN_U8, *shape, num_mips, 0,
+                                         _shim.void_pp([o.ptr for o in outs])) == 0
   ctx.sync()
   for m, (s, o) in enumerate(zip(shapes, outs)):
     mblock = (block[0] >> (m + 1), block[1] >> (m + 1), block[2])
@@ -510,8 +494,7 @@ def test_pool_select_2x2x2_past_2_32_matches_oracle(big, oracle, op):
   outs = [_alloc(big, int(np.prod(s))) for s in shapes]
   from igneous_b200 import _shim
   code = {"min": 0, "max": 1, "stride": 2, "mode": 3}[op]
-  assert ctx.lib.ign_pool_select_dev(ctx.handle, _p(d_in.ptr), c.c_int(IGN_U8), *_dims(shape), c.c_uint32(2),
-                                     c.c_uint32(2), c.c_uint32(2), c.c_int(num_mips), c.c_int(code),
+  assert ctx.lib.ign_pool_select_dev(ctx.handle, d_in.ptr, IGN_U8, *shape, 2, 2, 2, num_mips, code,
                                      _shim.void_pp([o.ptr for o in outs])) == 0
   ctx.sync()
   for z0 in (0, 508, 512, 1020, 1024):  # slabs aligned to 2^num_mips; z 1024 is a partial block
@@ -564,8 +547,7 @@ def test_renumber_and_remap_u16_at_2_32_minus_2(big):
   d_uniq = _alloc(big, 65536 * 8)
   _fill_periodic(ctx, d_in, n, pattern)
   k = c.c_uint64(0)
-  assert ctx.lib.ign_renumber_dev(ctx.handle, _p(d_in.ptr), c.c_int(IGN_U16), c.c_uint64(n), _p(d_out.ptr),
-                                  _p(d_uniq.ptr), c.c_uint64(65536), c.byref(k)) == 0
+  assert ctx.lib.ign_renumber_dev(ctx.handle, d_in.ptr, IGN_U16, n, d_out.ptr, d_uniq.ptr, 65536, c.byref(k)) == 0
   assert k.value == nz.size
   uniq = np.empty(k.value, np.uint64)
   ctx.d2h(uniq, d_uniq)
@@ -579,8 +561,8 @@ def test_renumber_and_remap_u16_at_2_32_minus_2(big):
 
   # n = 2^32 - 1 is refused before any launch
   before = ctx.launch_count()
-  assert ctx.lib.ign_renumber_dev(ctx.handle, _p(d_in.ptr), c.c_int(IGN_U16), c.c_uint64(n + 1), _p(d_out.ptr),
-                                  _p(d_uniq.ptr), c.c_uint64(65536), c.byref(k)) == IGN_ERR_OVERFLOW
+  assert ctx.lib.ign_renumber_dev(ctx.handle, d_in.ptr, IGN_U16, n + 1, d_out.ptr, d_uniq.ptr, 65536,
+                                  c.byref(k)) == IGN_ERR_OVERFLOW
   assert ctx.launch_count() == before
 
   # remap every value in place (no value is missing)
@@ -588,8 +570,8 @@ def test_renumber_and_remap_u16_at_2_32_minus_2(big):
   vals = (keys * np.uint64(40503) + np.uint64(7)) % np.uint64(65536)
   table = np.zeros(65536, np.uint16)
   table[keys.astype(np.int64)] = vals.astype(np.uint16)
-  assert ctx.lib.ign_remap_dev(ctx.handle, _p(d_in.ptr), c.c_int(IGN_U16), c.c_uint64(n), keys.ctypes.data_as(c.c_void_p),
-                               vals.ctypes.data_as(c.c_void_p), c.c_uint64(keys.size), c.c_int(0)) == 0
+  assert ctx.lib.ign_remap_dev(ctx.handle, d_in.ptr, IGN_U16, n, keys.ctypes.data_as(c.c_void_p),
+                               vals.ctypes.data_as(c.c_void_p), keys.size, 0) == 0
   for a, b in _index_slabs(n):
     got = np.empty(b - a, np.uint16)
     ctx.d2h(got, d_in.offset(a * 2))
@@ -610,21 +592,19 @@ def test_unique_and_mask_u8_at_2_32_minus_2(big):
   uniq = np.zeros(256, np.uint64)
   counts = np.zeros(256, np.uint64)
   k = c.c_uint64(0)
-  assert ctx.lib.ign_unique(ctx.handle, host.ctypes.data_as(c.c_void_p), c.c_int(IGN_U8), c.c_uint64(n),
-                            uniq.ctypes.data_as(c.c_void_p), counts.ctypes.data_as(c.c_void_p), c.c_uint64(256),
-                            c.byref(k)) == 0
+  assert ctx.lib.ign_unique(ctx.handle, host.ctypes.data_as(c.c_void_p), IGN_U8, n, uniq.ctypes.data_as(c.c_void_p),
+                            counts.ctypes.data_as(c.c_void_p), 256, c.byref(k)) == 0
   assert k.value == p
   assert np.array_equal(uniq[:p], pattern[order].astype(np.uint64))
   assert np.array_equal(counts[:p], counts_of[order])
   before = ctx.launch_count()
-  assert ctx.lib.ign_unique(ctx.handle, host.ctypes.data_as(c.c_void_p), c.c_int(IGN_U8), c.c_uint64(n + 1),
-                            uniq.ctypes.data_as(c.c_void_p), counts.ctypes.data_as(c.c_void_p), c.c_uint64(256),
-                            c.byref(k)) == IGN_ERR_OVERFLOW
+  assert ctx.lib.ign_unique(ctx.handle, host.ctypes.data_as(c.c_void_p), IGN_U8, n + 1, uniq.ctypes.data_as(c.c_void_p),
+                            counts.ctypes.data_as(c.c_void_p), 256, c.byref(k)) == IGN_ERR_OVERFLOW
   assert ctx.launch_count() == before
 
   labels = pattern[::3].astype(np.uint64)
-  assert ctx.lib.ign_mask(ctx.handle, host.ctypes.data_as(c.c_void_p), c.c_int(IGN_U8), c.c_uint64(n),
-                          labels.ctypes.data_as(c.c_void_p), c.c_uint64(labels.size), c.c_int(0), c.c_uint64(255)) == 0
+  assert ctx.lib.ign_mask(ctx.handle, host.ctypes.data_as(c.c_void_p), IGN_U8, n, labels.ctypes.data_as(c.c_void_p),
+                          labels.size, 0, 255) == 0
   masked = np.where(np.isin(pattern, pattern[::3]), np.uint8(255), pattern)
   step = p * (1 << 20)
   tile = np.tile(masked, step // p)
@@ -647,9 +627,8 @@ def test_contrast_stretch_u8_past_2_32_matches_contrastref(big):
   upper[z % 97 == 0] = lower[z % 97 == 0]  # slices left as they are
   d_in = _synth_image(big, shape, seed)
   d_out = _alloc(big, sx * sy * sz)
-  assert ctx.lib.ign_contrast_stretch_dev(ctx.handle, _p(d_in.ptr), c.c_int(IGN_U8), *_dims(shape), c.c_uint64(1),
-                                          lower.ctypes.data_as(c.c_void_p), upper.ctypes.data_as(c.c_void_p),
-                                          c.c_double(3), c.c_double(250), _p(d_out.ptr), c.c_int(IGN_U8)) == 0
+  assert ctx.lib.ign_contrast_stretch_dev(ctx.handle, d_in.ptr, IGN_U8, *shape, 1, lower.ctypes.data_as(c.c_void_p),
+                                          upper.ctypes.data_as(c.c_void_p), 3, 250, d_out.ptr, IGN_U8) == 0
   ctx.sync()
   for zz in BOUNDARY_Z + (970,):  # 970 = 97 * 10: a slice left as it is
     plane = oracle_image(shape, seed, zz)
@@ -677,7 +656,7 @@ def test_quantize_past_2_32_matches_contrastref(big):
   d_in = _alloc(big, n * 4)
   d_out = _alloc(big, n)
   _fill_planes(ctx, d_in, shape, plane_of, dtype=np.float32)
-  assert ctx.lib.ign_quantize_dev(ctx.handle, _p(d_in.ptr), c.c_uint64(n), _p(d_out.ptr)) == 0
+  assert ctx.lib.ign_quantize_dev(ctx.handle, d_in.ptr, n, d_out.ptr) == 0
   ctx.sync()
   for z in BOUNDARY_Z:
     want = contrastref.quantize(plane_of(z)[:, :, None])[:, :, :, 0]
@@ -690,8 +669,8 @@ def _box(ctx, dptr, dtype, shape, origin, size):
   from igneous_b200 import _shim
   d = ctx.alloc(int(np.prod(size)) * np.dtype(dtype).itemsize)
   try:
-    assert ctx.lib.ign_copy_box_dev(ctx.handle, _p(dptr.ptr), c.c_int(_shim.dtype_code(dtype)),
-                                    *_dims(tuple(shape) + tuple(origin) + tuple(size)), _p(d.ptr)) == 0
+    assert ctx.lib.ign_copy_box_dev(ctx.handle, dptr.ptr, _shim.dtype_code(dtype), *shape, *origin, *size,
+                                    d.ptr) == 0
     return ctx.to_host(d, size, dtype)
   finally:
     d.free()

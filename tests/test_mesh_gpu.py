@@ -84,10 +84,9 @@ def test_mc_properties_at_task_size(ctx):
   """257^3 task (BASELINE config C4 task shape + overlap): every label's mesh
   has only valid indices, no degenerate faces, and interior labels are closed."""
   from igneous_b200 import zmesh, _shim
-  import ctypes as c
   n = 257
   d = ctx.alloc(n ** 3 * 4)
-  _shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d), c.c_int(_shim.IGN_U32), c.c_uint64(n), c.c_uint64(n), c.c_uint64(n), c.c_int64(0), c.c_int64(0), c.c_int64(0), c.c_uint32(64), c.c_uint64(1 << 20), c.c_uint64(0), c.c_uint64(0)))
+  _shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d), _shim.IGN_U32, n, n, n, 0, 0, 0, 64, 1 << 20, 0, 0))
   seg = ctx.to_host(d, (n, n, n), np.uint32)
   d.free()
   m = zmesh.Mesher((16, 16, 40))

@@ -132,17 +132,14 @@ def test_synth_matches_oracle(ctx, oracle):
   shape, off = (70, 45, 33), (-7, 11, 2048)
   for dtype, pitch, ids, base in ((np.uint32, 16, 1 << 20, 0), (np.uint64, 24, 5, 1 << 32)):
     d = ctx.alloc(int(np.prod(shape)) * np.dtype(dtype).itemsize)
-    _shim.check(ctx.lib.ign_synth_seg_dev(
-      ctx.handle, _shim.ptr(d), c.c_int(_shim.dtype_code(dtype)), c.c_uint64(shape[0]),
-      c.c_uint64(shape[1]), c.c_uint64(shape[2]), c.c_int64(off[0]), c.c_int64(off[1]), c.c_int64(off[2]),
-      c.c_uint32(pitch), c.c_uint64(ids), c.c_uint64(3), c.c_uint64(base)))
+    _shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d), _shim.dtype_code(dtype), shape[0], shape[1],
+                                          shape[2], off[0], off[1], off[2], pitch, ids, 3, base))
     got = ctx.to_host(d, shape, dtype)
     want = oracle.synth_seg(shape, pitch=pitch, num_ids=ids, seed=3, offset=off, dtype=dtype, id_base=base)
     assert np.array_equal(got, want)
     d.free()
   d = ctx.alloc(int(np.prod(shape)))
-  _shim.check(ctx.lib.ign_synth_image_dev(ctx.handle, _shim.ptr(d), c.c_uint64(shape[0]), c.c_uint64(shape[1]),
-                                          c.c_uint64(shape[2]), c.c_int64(1), c.c_int64(2), c.c_int64(3), c.c_uint64(9)))
+  _shim.check(ctx.lib.ign_synth_image_dev(ctx.handle, _shim.ptr(d), shape[0], shape[1], shape[2], 1, 2, 3, 9))
   assert np.array_equal(ctx.to_host(d, shape, np.uint8), oracle.synth_image(shape, seed=9, offset=(1, 2, 3)))
 
 

@@ -21,9 +21,8 @@ def _ccl_dev(ctx, labels, out_dtype):
   d_out = ctx.alloc(labels.size * np.dtype(out_dtype).itemsize)
   n = c.c_uint64(0)
   try:
-    _shim.check(ctx.lib.ign_ccl6_dev(ctx.handle, _shim.ptr(d_in), c.c_int(_shim.dtype_code(labels.dtype)),
-                                     *[c.c_uint64(s) for s in labels.shape], _shim.ptr(d_out),
-                                     c.c_int(_shim.dtype_code(out_dtype)), c.byref(n)))
+    _shim.check(ctx.lib.ign_ccl6_dev(ctx.handle, _shim.ptr(d_in), _shim.dtype_code(labels.dtype), *labels.shape,
+                                     _shim.ptr(d_out), _shim.dtype_code(out_dtype), c.byref(n)))
     return ctx.to_host(d_out, labels.shape, out_dtype), n.value
   finally:
     d_in.free()
@@ -62,12 +61,10 @@ def test_ccl_nests_on_held_volume(oracle):
   n_local = c.c_uint64(0)
   null = c.c_void_p(None)
   try:
-    _shim.check(ctx.lib.ign_ccl6_volume_begin_dev(ctx.handle, _shim.ptr(d_a), c.c_int(_shim.IGN_U32),
-                                                  *[c.c_uint64(s) for s in a.shape], null, null, null, null,
-                                                  c.byref(vol), c.byref(n_local)))
+    _shim.check(ctx.lib.ign_ccl6_volume_begin_dev(ctx.handle, _shim.ptr(d_a), _shim.IGN_U32, *a.shape, null, null, null,
+                                                  null, c.byref(vol), c.byref(n_local)))
     got_b, got_n_b = _ccl_dev(ctx, b, np.uint32)
-    _shim.check(ctx.lib.ign_ccl6_volume_finish_dev(vol, null, c.c_uint64(n_local.value), _shim.ptr(d_out),
-                                                   c.c_int(_shim.IGN_U32)))
+    _shim.check(ctx.lib.ign_ccl6_volume_finish_dev(vol, null, n_local.value, _shim.ptr(d_out), _shim.IGN_U32))
     got_a = ctx.to_host(d_out, a.shape, np.uint32)
   finally:
     d_a.free()
@@ -103,8 +100,8 @@ def test_error_exits_release_the_arena(oracle):
   d_arr = ctx.to_device(arr)
   try:
     with pytest.raises(KeyError):
-      _shim.check(ctx.lib.ign_remap_dev(ctx.handle, _shim.ptr(d_arr), c.c_int(_shim.IGN_U32), c.c_uint64(arr.size),
-                                        _shim.ptr(keys), _shim.ptr(keys), c.c_uint64(keys.size), c.c_int(0)))
+      _shim.check(ctx.lib.ign_remap_dev(ctx.handle, _shim.ptr(d_arr), _shim.IGN_U32, arr.size, _shim.ptr(keys),
+                                        _shim.ptr(keys), keys.size, 0))
   finally:
     d_arr.free()
   noise = np.asfortranarray(rng.integers(0, 256, size=(96, 96, 96)).astype(np.uint8))  # > 65,535 components

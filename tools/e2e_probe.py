@@ -26,7 +26,7 @@ def export(task, h, nv, nf, nl, wctx):
     bufs[id(wctx)] = (wctx.pinned_empty((1 << 22, 3), np.float32, order="C"), wctx.pinned_empty((1 << 23, 3), np.uint32, order="C"))
   bv, bf = bufs[id(wctx)]
   voff = np.zeros(nl + 1, dtype=np.uint64); foff = np.zeros(nl + 1, dtype=np.uint64)
-  _shim.check(wctx.lib.ign_mesh_export(h, res, c.c_int(1), _shim.ptr(bv), _shim.ptr(bf), _shim.ptr(voff), _shim.ptr(foff)))
+  _shim.check(wctx.lib.ign_mesh_export(h, res, 1, _shim.ptr(bv), _shim.ptr(bf), _shim.ptr(voff), _shim.ptr(foff)))
 os.environ["IGN_PIPE_TRACE"] = "1"
 for name, ho, ex in (("full", host, export), ("full", host, export), ("upload only", None, None), ("upload+download", host, None),
                      ("upload+export", None, export)):

@@ -10,9 +10,9 @@ def run(ctx, dtype, shape, pitch, num_ids, out_dtype=np.uint64, reps=5):
   d_in = ctx.alloc(n * es); d_out = ctx.alloc(n * osz)
   code = _shim.dtype_code(dtype)
   c = ctypes
-  _shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d_in), c.c_int(code), c.c_uint64(sx), c.c_uint64(sy), c.c_uint64(sz), c.c_int64(0), c.c_int64(0), c.c_int64(0), c.c_uint32(pitch), c.c_uint64(num_ids), c.c_uint64(0), c.c_uint64(0)))
+  _shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d_in), code, sx, sy, sz, 0, 0, 0, pitch, num_ids, 0, 0))
   N = c.c_uint64(0)
-  args = (ctx.handle, _shim.ptr(d_in), c.c_int(code), c.c_uint64(sx), c.c_uint64(sy), c.c_uint64(sz), _shim.ptr(d_out), c.c_int(_shim.dtype_code(out_dtype)), c.byref(N))
+  args = (ctx.handle, _shim.ptr(d_in), code, sx, sy, sz, _shim.ptr(d_out), _shim.dtype_code(out_dtype), c.byref(N))
   for _ in range(2): _shim.check(ctx.lib.ign_ccl6_dev(*args))
   ctx.sync(); ts = []
   for _ in range(reps):
@@ -26,11 +26,11 @@ if __name__ == "__main__":
   if len(sys.argv) > 1 and sys.argv[1] == "2048":
     from igneous_b200 import pipeline
     c = ctypes
-    _shim.check(ctx.lib.ign_prof_enable(ctx.handle, c.c_int(1)))
+    _shim.check(ctx.lib.ign_prof_enable(ctx.handle, 1))
     run(ctx, np.uint32, (2048, 2048, 2048), 64, 1 << 20, out_dtype=np.uint32, reps=3)
     for name, cls in pipeline.PROF_CLASSES.items():
       ms, cnt = c.c_float(0), c.c_uint64(0)
-      _shim.check(ctx.lib.ign_prof_read(ctx.handle, c.c_int(cls), c.byref(ms), c.byref(cnt)))
+      _shim.check(ctx.lib.ign_prof_read(ctx.handle, cls, c.byref(ms), c.byref(cnt)))
       if cnt.value:
         print(name, "ms total", round(ms.value, 3), "launches", cnt.value, "ms/launch", round(ms.value / cnt.value, 4))
     sys.exit(0)
@@ -44,10 +44,10 @@ if __name__ == "__main__":
   # per-kernel-class times of the last configuration (CUDA events recorded by the library)
   from igneous_b200 import pipeline
   c = ctypes
-  _shim.check(ctx.lib.ign_prof_enable(ctx.handle, c.c_int(1)))
+  _shim.check(ctx.lib.ign_prof_enable(ctx.handle, 1))
   run(ctx, np.uint32, (1024, 1024, 1024), 64, 1 << 20, out_dtype=np.uint32, reps=3)
   for name, cls in pipeline.PROF_CLASSES.items():
     ms, cnt = c.c_float(0), c.c_uint64(0)
-    _shim.check(ctx.lib.ign_prof_read(ctx.handle, c.c_int(cls), c.byref(ms), c.byref(cnt)))
+    _shim.check(ctx.lib.ign_prof_read(ctx.handle, cls, c.byref(ms), c.byref(cnt)))
     if cnt.value:
       print(name, "ms total", round(ms.value, 3), "launches", cnt.value, "ms/launch", round(ms.value / cnt.value, 4))

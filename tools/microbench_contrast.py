@@ -6,7 +6,6 @@ ign_clahe_dev (clip 40, 8 x 8 tiles).  Per kernel: ms, GB/s of algorithmic bytes
 the input; the others: input + output; CLAHE's LUT writes and reads are reported
 separately) and the fraction of 3.35 TB/s; beside it the host numpy / cv2 call on the same
 slab.  Prints one JSON line per measurement, with the card's name and power limit."""
-import ctypes as c
 import json
 import os
 import subprocess
@@ -55,7 +54,6 @@ def main(reps=10, host=True):
   gpu = card()
   sx, sy, sz = 2048, 2048, 64
   n = sx * sy * sz
-  u = c.c_uint64
   rng = np.random.default_rng(0)
   for dt, code, hs in ((np.uint8, _shim.IGN_U8, 256), (np.uint16, _shim.IGN_U16, 65536)):
     es = np.dtype(dt).itemsize
@@ -74,7 +72,7 @@ def main(reps=10, host=True):
       print(json.dumps(rec), flush=True)
 
     def hist():
-      _shim.check(lib.ign_histogram_dev(ctx.handle, _shim.ptr(d_in), c.c_int(code), u(n), _shim.ptr(d_hist)))
+      _shim.check(lib.ign_histogram_dev(ctx.handle, _shim.ptr(d_in), code, n, _shim.ptr(d_hist)))
     ms, mn = timed(ctx, hist, reps)
     report("ign_histogram_dev", ms, mn, n * es,
            host_ms(lambda: np.bincount(img.ravel(order="F"), minlength=hs)) if host else None)
@@ -83,9 +81,8 @@ def main(reps=10, host=True):
     upper = np.full(sz, hs - hs // 5, np.uint32)
 
     def stretch():
-      _shim.check(lib.ign_contrast_stretch_dev(ctx.handle, _shim.ptr(d_in), c.c_int(code), u(sx), u(sy), u(sz), u(1),
-                                               _shim.ptr(lower), _shim.ptr(upper), c.c_double(0.0),
-                                               c.c_double(hs - 1.0), _shim.ptr(d_out), c.c_int(code)))
+      _shim.check(lib.ign_contrast_stretch_dev(ctx.handle, _shim.ptr(d_in), code, sx, sy, sz, 1, _shim.ptr(lower),
+                                               _shim.ptr(upper), 0.0, hs - 1.0, _shim.ptr(d_out), code))
     ms, mn = timed(ctx, stretch, reps)
 
     def np_stretch():
@@ -95,8 +92,7 @@ def main(reps=10, host=True):
     report("ign_contrast_stretch_dev", ms, mn, 2 * n * es, host_ms(np_stretch, 1) if host else None)
 
     def clahe():
-      _shim.check(lib.ign_clahe_dev(ctx.handle, _shim.ptr(d_in), c.c_int(code), u(sx), u(sy), u(sz), c.c_double(40.0),
-                                    c.c_uint32(8), c.c_uint32(8), _shim.ptr(d_out)))
+      _shim.check(lib.ign_clahe_dev(ctx.handle, _shim.ptr(d_in), code, sx, sy, sz, 40.0, 8, 8, _shim.ptr(d_out)))
     ms, mn = timed(ctx, clahe, reps)
     lut_bytes = sz * 64 * hs * es
     cv_ms = None
@@ -117,7 +113,7 @@ def main(reps=10, host=True):
   ctx.sync()
 
   def quant():
-    _shim.check(lib.ign_quantize_dev(ctx.handle, _shim.ptr(d_f), u(n), _shim.ptr(d_q)))
+    _shim.check(lib.ign_quantize_dev(ctx.handle, _shim.ptr(d_f), n, _shim.ptr(d_q)))
   ms, mn = timed(ctx, quant, reps)
   hq = host_ms(lambda: (f * 255.0).astype(np.uint8), 1) if host else None
   print(json.dumps({"shape": [sx, sy, sz], "dtype": "float32", "gpu": gpu, "reps": reps, "op": "ign_quantize_dev",

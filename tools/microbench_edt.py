@@ -56,10 +56,8 @@ def timed(ctx, fn, reps):
 def synth(ctx, shape, pitch=16):
   n = int(np.prod(shape))
   d = ctx.alloc(n * 4)
-  u = c.c_uint64
-  _shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d), c.c_int(U32), u(shape[0]), u(shape[1]),
-                                        u(shape[2]), c.c_int64(0), c.c_int64(0), c.c_int64(0), c.c_uint32(pitch),
-                                        u(1 << 20), u(0), u(0)))
+  _shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d), U32, shape[0], shape[1], shape[2], 0, 0, 0, pitch,
+                                        1 << 20, 0, 0))
   ctx.sync()
   return d
 
@@ -92,7 +90,6 @@ def stack_entries(ctx, d, shape):
 def main(reps=10, host=True):
   ctx = _shim.default_context()
   gpu = card()
-  u = c.c_uint64
   for name, shape in (("seg512", (512, 512, 512)), ("seg2k", (2048, 2048, 256)), ("seg449", (449, 449, 449))):
     n = int(np.prod(shape))
     d = synth(ctx, shape)
@@ -104,8 +101,8 @@ def main(reps=10, host=True):
       an = (c.c_float * 3)(*a)
 
       def run():
-        _shim.check(ctx.lib.ign_edt_dev(ctx.handle, _shim.ptr(d), c.c_int(U32), u(shape[0]), u(shape[1]),
-                                        u(shape[2]), an, c.c_int(0), c.c_int(1), _shim.ptr(out)))
+        _shim.check(ctx.lib.ign_edt_dev(ctx.handle, _shim.ptr(d), U32, shape[0], shape[1], shape[2], an, 0, 1,
+                                        _shim.ptr(out)))
       ms, mn = timed(ctx, run, reps)
       rec = {"op": "ign_edt_dev", "workload": name, "shape": list(shape), "dtype": "uint32", "anisotropy": list(a),
              "gpu": gpu, "reps": reps, "ms": round(ms, 3), "min_ms": round(mn, 3),

@@ -46,21 +46,18 @@ def main(reps=10, blocks=2):
   mips = [ctx.alloc(2 * S * 2 * S * S * 4), ctx.alloc(S * S * S * 4)]
   vol = ctx.alloc(S ** 3 * 4)
   filled, holes, dil = ctx.alloc(S ** 3 * 4), ctx.alloc(S ** 3 * 4), ctx.alloc(S ** 3 * 4)
-  u = c.c_uint64
   res = (c.c_float * 3)(16.0, 16.0, 40.0)
   for b in range(blocks):
-    _shim.check(lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d_big), c.c_int(U32), u(big[0]), u(big[1]), u(big[2]),
-                                      c.c_int64(0), c.c_int64(0), c.c_int64(b * S), c.c_uint32(64), u(1 << 20),
-                                      u(0), u(0)))
-    _shim.check(lib.ign_pool_mode_2x2x1_dev(ctx.handle, _shim.ptr(d_big), c.c_int(U32), u(big[0]), u(big[1]),
-                                            u(big[2]), c.c_int(2), c.c_int(0), _shim.void_pp([m.ptr for m in mips])))
+    _shim.check(lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d_big), U32, big[0], big[1], big[2], 0, 0, b * S, 64,
+                                      1 << 20, 0, 0))
+    _shim.check(lib.ign_pool_mode_2x2x1_dev(ctx.handle, _shim.ptr(d_big), U32, big[0], big[1], big[2], 2, 0,
+                                            _shim.void_pp([m.ptr for m in mips])))
     ctx.d2d(vol, mips[1], S ** 3 * 4)
     ctx.sync()
     common = {"block": b, "shape": [S, S, S], "dtype": "uint32", "gpu": gpu, "reps": reps}
 
     def dilate():
-      _shim.check(lib.ign_dilate_multilabel_dev(ctx.handle, _shim.ptr(vol), c.c_int(U32), u(S), u(S), u(S),
-                                                _shim.ptr(dil)))
+      _shim.check(lib.ign_dilate_multilabel_dev(ctx.handle, _shim.ptr(vol), U32, S, S, S, _shim.ptr(dil)))
     ms, mn = timed(ctx, dilate, reps)
     print(json.dumps(dict(common, op="ign_dilate_multilabel_dev", ms=round(ms, 3), min_ms=round(mn, 3))), flush=True)
     for level in (1, 2, 4):
@@ -68,17 +65,16 @@ def main(reps=10, blocks=2):
       pct = 100 if level <= 3 else 103 - level
 
       def fill():
-        _shim.check(lib.ign_fill_holes_dev(ctx.handle, _shim.ptr(src), c.c_int(U32), u(S), u(S), u(S),
-                                           c.c_int(int(level >= 2)), c.c_int(pct), _shim.ptr(filled),
-                                           _shim.ptr(holes)))
+        _shim.check(lib.ign_fill_holes_dev(ctx.handle, _shim.ptr(src), U32, S, S, S, int(level >= 2), pct,
+                                           _shim.ptr(filled), _shim.ptr(holes)))
       ms, mn = timed(ctx, fill, reps)
       print(json.dumps(dict(common, op="ign_fill_holes_dev", level=level, ms=round(ms, 3), min_ms=round(mn, 3))),
             flush=True)
 
     def mesh():
       h = c.c_void_p()
-      _shim.check(lib.ign_mesh_begin_dev(ctx.handle, _shim.ptr(vol), c.c_int(U32), u(S), u(S), u(S), c.byref(h)))
-      _shim.check(lib.ign_mesh_simplify(h, res, c.c_int(100), c.c_float(40.0)))
+      _shim.check(lib.ign_mesh_begin_dev(ctx.handle, _shim.ptr(vol), U32, S, S, S, c.byref(h)))
+      _shim.check(lib.ign_mesh_simplify(h, res, 100, 40.0))
       _shim.check(lib.ign_mesh_free(h))
     ms, mn = timed(ctx, mesh, max(3, reps // 2))
     print(json.dumps(dict(common, op="marching cubes + simplify (100, 40)", ms=round(ms, 3), min_ms=round(mn, 3))),

@@ -48,15 +48,13 @@ def synth_renumbered(ctx, shape, pitch):
   """Synthetic segmentation made and renumbered on the device -> (device u32 labels, N)."""
   n = int(np.prod(shape))
   raw, out = ctx.alloc(n * 4), ctx.alloc(n * 4)
-  u = c.c_uint64
-  _shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(raw), c.c_int(U32), u(shape[0]), u(shape[1]),
-                                        u(shape[2]), c.c_int64(0), c.c_int64(0), c.c_int64(0), c.c_uint32(pitch),
-                                        u(1 << 20), u(0), u(0)))
+  _shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(raw), U32, shape[0], shape[1], shape[2], 0, 0, 0, pitch,
+                                        1 << 20, 0, 0))
   cap = 1 << 22
   uniq = ctx.alloc(cap * 8)
   k = c.c_uint64(0)
-  _shim.check(ctx.lib.ign_renumber_dev(ctx.handle, _shim.ptr(raw), c.c_int(U32), u(n), _shim.ptr(out),
-                                       _shim.ptr(uniq), u(cap), c.byref(k)))
+  _shim.check(ctx.lib.ign_renumber_dev(ctx.handle, _shim.ptr(raw), U32, n, _shim.ptr(out), _shim.ptr(uniq), cap,
+                                       c.byref(k)))
   ctx.sync()
   raw.free()
   uniq.free()
@@ -66,7 +64,6 @@ def synth_renumbered(ctx, shape, pitch):
 def main(reps=10, host=True):
   ctx = _shim.default_context()
   gpu = card()
-  u = c.c_uint64
   work = []
   for name, shape, pitch in (("seg449", (449, 449, 449), 16), ("seg2k", (2048, 2048, 256), 16)):
     d, N = synth_renumbered(ctx, shape, pitch)
@@ -82,8 +79,8 @@ def main(reps=10, host=True):
     nn = c.c_uint64(N)
 
     def run():
-      _shim.check(ctx.lib.ign_find_objects_dev(ctx.handle, _shim.ptr(d), c.c_int(U32), u(shape[0]), u(shape[1]),
-                                               u(shape[2]), c.byref(nn), _shim.ptr(boxes)))
+      _shim.check(ctx.lib.ign_find_objects_dev(ctx.handle, _shim.ptr(d), U32, shape[0], shape[1], shape[2], c.byref(nn),
+                                               _shim.ptr(boxes)))
     ms, mn = timed(ctx, run, reps)
     rec = {"op": "ign_find_objects_dev", "workload": name, "what": what, "shape": list(shape), "dtype": "uint32",
            "labels": N, "gpu": gpu, "reps": reps, "ms": round(ms, 3), "min_ms": round(mn, 3),

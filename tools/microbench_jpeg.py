@@ -58,7 +58,6 @@ def main(reps=5, host=True):
   lib = ctx.lib
   gpu = card()
   base = em_volume((512, 512, 64))
-  u = c.c_uint64
   for cs, n in (((64, 64, 64), 512), ((128, 128, 64), 128), ((512, 512, 64), 8)):
     gx, gy = 512 // cs[0], 512 // cs[1]
     tiles = [np.asfortranarray(base[i * cs[0]:(i + 1) * cs[0], j * cs[1]:(j + 1) * cs[1], :cs[2]])
@@ -74,9 +73,8 @@ def main(reps=5, host=True):
     need = c.c_uint64(0)
 
     def enc(ri):
-      _shim.check(lib.ign_jpeg_encode_dev(ctx.handle, _shim.ptr(d_in), u(n), _shim.ptr(shapes), c.c_int(85),
-                                          c.c_int64(ri), _shim.ptr(d_out), u(2 * vox), _shim.ptr(offs[ri]),
-                                          c.byref(need)))
+      _shim.check(lib.ign_jpeg_encode_dev(ctx.handle, _shim.ptr(d_in), n, _shim.ptr(shapes), 85, ri, _shim.ptr(d_out),
+                                          2 * vox, _shim.ptr(offs[ri]), c.byref(need)))
     rec = {"chunk": list(cs), "chunks": n, "voxels": vox, "quality": 85, "gpu": gpu, "reps": reps}
     sizes = {}
     for ri in (0, -1):  # the row-marker streams stay in d_out for the decode
@@ -91,7 +89,7 @@ def main(reps=5, host=True):
                restart_marker_overhead=round(sizes[-1] / sizes[0] - 1, 4))
 
     def dec(ri):
-      _shim.check(lib.ign_jpeg_decode_dev(ctx.handle, _shim.ptr(d_out), _shim.ptr(offs[ri]), u(n), _shim.ptr(shapes),
+      _shim.check(lib.ign_jpeg_decode_dev(ctx.handle, _shim.ptr(d_out), _shim.ptr(offs[ri]), n, _shim.ptr(shapes),
                                           _shim.ptr(d_dec)))
     ms, mn = timed(ctx, lambda: dec(-1), reps)
     dec_bytes = sizes[-1] + vox

@@ -1,5 +1,5 @@
 """Device-resident pooling micro-benchmark (CUDA events on the ctx stream)."""
-import ctypes, json, sys, os
+import json, sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 from igneous_b200 import _shim
@@ -11,9 +11,9 @@ def run(ctx, mode, dtype, shape, num_mips, reps=10):
   d_in = ctx.alloc(n * es)
   code = _shim.dtype_code(dtype)
   if mode:
-    _shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d_in), ctypes.c_int(code), ctypes.c_uint64(sx), ctypes.c_uint64(sy), ctypes.c_uint64(sz), ctypes.c_int64(0), ctypes.c_int64(0), ctypes.c_int64(0), ctypes.c_uint32(64), ctypes.c_uint64(1 << 20), ctypes.c_uint64(0), ctypes.c_uint64(0)))
+    _shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d_in), code, sx, sy, sz, 0, 0, 0, 64, 1 << 20, 0, 0))
   else:
-    _shim.check(ctx.lib.ign_synth_image_dev(ctx.handle, _shim.ptr(d_in), ctypes.c_uint64(sx), ctypes.c_uint64(sy), ctypes.c_uint64(sz), ctypes.c_int64(0), ctypes.c_int64(0), ctypes.c_int64(0), ctypes.c_uint64(0)))
+    _shim.check(ctx.lib.ign_synth_image_dev(ctx.handle, _shim.ptr(d_in), sx, sy, sz, 0, 0, 0, 0))
   outs, ob = [], 0
   x, y = sx, sy
   for m in range(num_mips):
@@ -21,7 +21,7 @@ def run(ctx, mode, dtype, shape, num_mips, reps=10):
     outs.append(ctx.alloc(x * y * sz * es)); ob += x * y * sz * es
   pp = _shim.void_pp([o.ptr for o in outs])
   fn = ctx.lib.ign_pool_mode_2x2x1_dev if mode else ctx.lib.ign_pool_avg_2x2x1_dev
-  args = (ctx.handle, _shim.ptr(d_in), ctypes.c_int(code), ctypes.c_uint64(sx), ctypes.c_uint64(sy), ctypes.c_uint64(sz), ctypes.c_int(num_mips), ctypes.c_int(0), pp)
+  args = (ctx.handle, _shim.ptr(d_in), code, sx, sy, sz, num_mips, 0, pp)
   for _ in range(3): _shim.check(fn(*args))
   ctx.sync()
   ts = []

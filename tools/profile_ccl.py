@@ -12,13 +12,11 @@ ctx = _shim.default_context()
 n = size ** 3
 d_in = ctx.alloc(n * dt_in.itemsize)
 d_out = ctx.alloc(n * dt_out.itemsize)
-_shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d_in), c.c_int(_shim.dtype_code(dt_in)), c.c_uint64(size),
-                                      c.c_uint64(size), c.c_uint64(size), c.c_int64(0), c.c_int64(0), c.c_int64(0),
-                                      c.c_uint32(64), c.c_uint64(1 << 20), c.c_uint64(0), c.c_uint64(0)))
+_shim.check(ctx.lib.ign_synth_seg_dev(ctx.handle, _shim.ptr(d_in), _shim.dtype_code(dt_in), size, size, size, 0, 0, 0,
+                                      64, 1 << 20, 0, 0))
 N = c.c_uint64(0)
 for _ in range(reps):
-  _shim.check(ctx.lib.ign_ccl6_dev(ctx.handle, _shim.ptr(d_in), c.c_int(_shim.dtype_code(dt_in)), c.c_uint64(size),
-                                   c.c_uint64(size), c.c_uint64(size), _shim.ptr(d_out),
-                                   c.c_int(_shim.dtype_code(dt_out)), c.byref(N)))
+  _shim.check(ctx.lib.ign_ccl6_dev(ctx.handle, _shim.ptr(d_in), _shim.dtype_code(dt_in), size, size, size,
+                                   _shim.ptr(d_out), _shim.dtype_code(dt_out), c.byref(N)))
 ctx.sync()
 print("components", N.value)
