@@ -152,11 +152,8 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
 // side, +16 bytes of halo on the low x side: TMA boxes are multiples of 16 bytes)
 constexpr int MT_BX = 128, MT_BY = 8;
 constexpr int MT_THREADS = 512;
-#ifndef MT_BZ_OVERRIDE
-#define MT_BZ_OVERRIDE 0
-#endif
 template <typename T> struct MaskTile {
-  static constexpr int BZ = MT_BZ_OVERRIDE ? MT_BZ_OVERRIDE : (sizeof(T) == 8 ? 4 : 8);
+  static constexpr int BZ = sizeof(T) == 8 ? 4 : 8;
   static constexpr int HX = 16 / (int)sizeof(T);
   static constexpr int PITCH = MT_BX + HX;             // elements per tile row
   static constexpr int ROWS = (MT_BY + 1) * (BZ + 1);  // rows incl. halo
@@ -984,6 +981,21 @@ static size_t ccl_cub_bytes(uint64_t items) {
 }
 static uint64_t default_rcap(uint64_t n) { return n / 8 + 4096; }
 
+// Flattens the union-find forest parent[0..n) and ranks its roots in ascending id order:
+// rank[i] = roots below i.  parent[n] is set to a sentinel that is not a root, so rank[n] = roots;
+// that count is delivered to *roots by the caller's small_sync.  `parent` and `rank` hold n+1 ids.
+static int rank_roots(ign_ctx* ctx, uint32_t* parent, uint32_t* rank, uint32_t n, void* cub_tmp, size_t cub_bytes,
+                      uint32_t* roots) {
+  IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_MERGE, k_ccl_flatten, blocks_for(n, 256), 256, 0, parent, n);
+  IGN_CUDA(cudaMemsetAsync(parent + n, 0xFF, 4, ctx->stream));
+  IsRootOp op;
+  op.parent = parent;
+  auto it = thrust::make_transform_iterator(thrust::counting_iterator<uint32_t>(0), op);
+  IGN_CUDA(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, it, rank, (int)(n + 1), ctx->stream));
+  ctx->launches += 2;
+  return small_d2h(ctx, roots, rank + n, 4);
+}
+
 // Pass A .. run labels.  On success plan.label[r] = component id (1..ncomp, cc3d numbering)
 // of every run and plan.ncomp is on the host.  `rcap` = run capacity taken from the frame;
 // *need_rcap > rcap on return means the volume has more runs (nothing else is valid).
@@ -1037,17 +1049,14 @@ static int ccl_structure(ign_ctx* ctx, ScratchFrame& f, const R& rd, uint32_t sx
     const cuuint64_t gstr[2] = {(cuuint64_t)sx * es, (cuuint64_t)sx * sy * es};
     const cuuint32_t box[3] = {(cuuint32_t)MT::PITCH, MT_BY + 1, (cuuint32_t)MT::BZ + 1};
     const cuuint32_t estr[3] = {1, 1, 1};
-    CUtensorMapL2promotion promo = CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
-    if (const char* e = getenv("IGN_CCL_L2PROMO")) promo = atoi(e) == 256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : (atoi(e) == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B : (atoi(e) == 0 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : promo));
     const CUresult r = enc(&tmap, tmap_dtype<T>(), 3, (void*)rd.in, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                           CU_TENSOR_MAP_SWIZZLE_NONE, promo,
+                           CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     IGN_REQUIRE(r == CUDA_SUCCESS, IGN_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) for %ux%ux%u", (int)r, sx, sy, sz);
   }
   {
     const size_t smem = (use_tma ? 2 : 1) * MT::BYTES;
-    unsigned per_sm = (unsigned)(200 * 1024 / (smem + 1024)) < 8u ? (unsigned)(200 * 1024 / (smem + 1024)) : 8u;
-    if (const char* e = getenv("IGN_CCL_MASK_CTAS")) per_sm = (unsigned)atoi(e) ? (unsigned)atoi(e) : per_sm;
+    const unsigned per_sm = (unsigned)(200 * 1024 / (smem + 1024)) < 8u ? (unsigned)(200 * 1024 / (smem + 1024)) : 8u;
     const uint64_t cap = (uint64_t)ctx->sm_count * (per_sm ? per_sm : 1);
     const uint64_t units = ma.pair ? ntiles / 2 : ntiles;  // tile pairs when the CTAs write whole mask sectors
     const unsigned grid = (unsigned)(units < cap ? units : cap);
@@ -1134,28 +1143,33 @@ static int ccl_structure(ign_ctx* ctx, ScratchFrame& f, const R& rd, uint32_t sx
     IGN_REQUIRE(mitems / 256 < 0x7FFFFFFFull, IGN_ERR_OVERFLOW, "too many CCL face words");
     IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_MERGE, k_ccl_merge, blocks_for(mitems, 256), 256, 0, me);
   }
-  // ---- roots: flatten, rank = exclusive scan over (parent[r] == r), labels
-  IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_MERGE, k_ccl_flatten, blocks_for(Rn, 256), 256, 0, p.label, Rn);
-  IGN_CUDA(cudaMemsetAsync(p.label + Rn, 0xFF, 4, ctx->stream));  // sentinel: not a root
-  {
-    IsRootOp op;
-    op.parent = p.label;
-    auto it = thrust::make_transform_iterator(thrust::counting_iterator<uint32_t>(0), op);
-    size_t tb = p.cub_bytes;
-    IGN_CUDA(cub::DeviceScan::ExclusiveSum(p.cub_tmp, tb, it, p.rank, (int)(Rn + 1), ctx->stream));
-    ctx->launches += 2;
-  }
+  // ---- roots, then the label of every run
   uint32_t hN = 0;
-  IGN_TRY(small_d2h(ctx, &hN, p.rank + Rn, 4));
+  IGN_TRY(rank_roots(ctx, p.label, p.rank, Rn, p.cub_tmp, p.cub_bytes, &hN));
   IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_MERGE, k_ccl_runlabel, blocks_for(Rn, 256), 256, 0, p.label, p.rank, Rn);
   IGN_TRY(small_sync(ctx));
   p.ncomp = hN;
   return IGN_OK;
 }
 
-template <typename T>
-static Reader<T, false> plain_reader(const void* in) {
-  Reader<T, false> r;
+// ccl_structure with the run capacity the volume needs: a volume with more runs than the
+// default capacity is resolved again after rewinding f.
+template <typename R>
+static int ccl_resolve(ign_ctx* ctx, ScratchFrame& f, const R& rd, uint64_t sx, uint64_t sy, uint64_t sz, CclPlan& p) {
+  uint64_t rcap = default_rcap(sx * sy * sz);
+  for (int attempt = 0;; attempt++) {
+    f.rewind();
+    uint64_t need = 0;
+    IGN_TRY(ccl_structure(ctx, f, rd, (uint32_t)sx, (uint32_t)sy, (uint32_t)sz, rcap, p, &need));
+    if (need <= rcap) return IGN_OK;
+    IGN_REQUIRE(attempt == 0, IGN_ERR_NOMEM, "CCL: %llu runs after a retry sized for them", (unsigned long long)need);
+    rcap = need + 16;
+  }
+}
+
+template <typename T, bool THR = false>
+static Reader<T, THR> plain_reader(const void* in) {
+  Reader<T, THR> r;
   r.in = (const T*)in;
   r.gte = r.lte = 0;
   r.use_gte = r.use_lte = 0;
@@ -1173,8 +1187,20 @@ static int check_labels_fit(int out_dtype, uint64_t max_label) {
   return IGN_OK;
 }
 
-static int launch_expand(ign_ctx* ctx, const CclPlan& p, uint64_t offset, void* out, int out_dtype,
-                         uint64_t max_label) {
+// every CCL entry that writes labels calls this before it takes scratch or launches anything
+static int check_out_dtype(int out_dtype) {
+  IGN_REQUIRE(out_dtype == IGN_U16 || out_dtype == IGN_U32 || out_dtype == IGN_U64, IGN_ERR_UNSUPPORTED,
+              "CCL out_dtype must be u16/u32/u64 (got %d)", out_dtype);
+  return IGN_OK;
+}
+
+// the labels of p (+ offset) into out; out_dtype passed check_out_dtype
+static int write_labels(ign_ctx* ctx, const CclPlan& p, uint64_t offset, void* out, int out_dtype,
+                        uint64_t max_label) {
+  if (p.R == 0) {
+    IGN_CUDA(cudaMemsetAsync(out, 0, p.n * dtype_size(out_dtype), ctx->stream));
+    return IGN_OK;
+  }
   const ExpandArgs e = p.expand_args(offset);
   const bool vec = (p.sx % 4 == 0) && ((uintptr_t)out % 16 == 0);
   // vector path: a warp owns EX_G 128-voxel groups of one row; scalar path: EX_G consecutive words
@@ -1182,24 +1208,15 @@ static int launch_expand(ign_ctx* ctx, const CclPlan& p, uint64_t offset, void* 
   IGN_REQUIRE(warps * 32 / 256 < 0x7FFFFFFFull, IGN_ERR_OVERFLOW, "CCL expand grid too large");
   const unsigned grid = blocks_for(warps * 32, 256);
   IGN_TRY(check_labels_fit(out_dtype, max_label + offset));
-  switch (out_dtype) {
-    case IGN_U16:
-      if (vec) IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_LABEL, (k_ccl_expand4<uint16_t>), grid, 256, 0, e, (uint16_t*)out);
-      else IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_LABEL, (k_ccl_expand1<uint16_t>), grid, 256, 0, e, (uint16_t*)out);
-      break;
-    case IGN_U32:
-      if (vec) IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_LABEL, (k_ccl_expand4<uint32_t>), grid, 256, 0, e, (uint32_t*)out);
-      else IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_LABEL, (k_ccl_expand1<uint32_t>), grid, 256, 0, e, (uint32_t*)out);
-      break;
-    case IGN_U64:
-      if (vec) IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_LABEL, (k_ccl_expand4<uint64_t>), grid, 256, 0, e, (uint64_t*)out);
-      else IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_LABEL, (k_ccl_expand1<uint64_t>), grid, 256, 0, e, (uint64_t*)out);
-      break;
-    default:
-      set_error("CCL out_dtype must be u16/u32/u64 (got %d)", out_dtype);
-      return IGN_ERR_UNSUPPORTED;
-  }
-  return IGN_OK;
+  auto expand = [&](auto* o) -> int {
+    using O = std::remove_pointer_t<decltype(o)>;
+    if (vec) IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_LABEL, (k_ccl_expand4<O>), grid, 256, 0, e, o);
+    else IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_LABEL, (k_ccl_expand1<O>), grid, 256, 0, e, o);
+    return IGN_OK;
+  };
+  if (out_dtype == IGN_U16) return expand((uint16_t*)out);
+  if (out_dtype == IGN_U32) return expand((uint32_t*)out);
+  return expand((uint64_t*)out);
 }
 
 // dust on the run labels of p: components with fewer than `threshold` voxels get label 0,
@@ -1234,38 +1251,24 @@ static int dust_runs(ign_ctx* ctx, CclPlan& p, uint64_t threshold, uint32_t* kep
   return IGN_OK;
 }
 
-// full pipeline for one reader type; out may be null when only dust-in-place is wanted
+// CCL, dust and u64 labels (+ offset) for one reader type; out may be null when only dust-in-place
+// is wanted
 template <typename R, typename TL>
-static int ccl_run(ign_ctx* ctx, const R& rd, uint64_t sx, uint64_t sy, uint64_t sz,
-                   uint64_t dust_threshold, uint64_t offset, void* out, int out_dtype,
-                   TL* dust_labels_inplace, uint64_t* n_components) {
+static int ccl_run(ign_ctx* ctx, const R& rd, uint64_t sx, uint64_t sy, uint64_t sz, uint64_t dust_threshold,
+                   uint64_t offset, uint64_t* out, TL* dust_labels_inplace, uint64_t* n_components) {
   IGN_TRY(check_ccl_dims(sx, sy, sz));
-  const uint64_t n = sx * sy * sz;
-  uint64_t rcap = default_rcap(n);
-  for (int attempt = 0; attempt < 2; attempt++) {
-    ScratchFrame f(ctx);
-    CclPlan p;
-    uint64_t need = 0;
-    IGN_TRY(ccl_structure(ctx, f, rd, (uint32_t)sx, (uint32_t)sy, (uint32_t)sz, rcap, p, &need));
-    if (need > rcap) {
-      IGN_REQUIRE(attempt == 0, IGN_ERR_NOMEM, "CCL: %llu runs after a retry sized for them", (unsigned long long)need);
-      rcap = need + 16;
-      continue;
-    }
-    uint32_t kept = p.ncomp;
-    if (dust_threshold > 0 && p.ncomp > 0) IGN_TRY(dust_runs(ctx, p, dust_threshold, &kept));
-    if (dust_labels_inplace != nullptr && dust_threshold > 0 && p.R > 0) {
-      const ExpandArgs e = p.expand_args(0);
-      IGN_LAUNCH(ctx, (k_dust_apply<TL>), blocks_for(p.W * 32, 256), 256, 0, e, dust_labels_inplace);
-    }
-    if (out != nullptr) {
-      if (p.R == 0) IGN_CUDA(cudaMemsetAsync(out, 0, n * dtype_size(out_dtype), ctx->stream));
-      else IGN_TRY(launch_expand(ctx, p, offset, out, out_dtype, kept));
-    }
-    if (n_components) *n_components = kept;
-    return IGN_OK;
+  ScratchFrame f(ctx);
+  CclPlan p;
+  IGN_TRY(ccl_resolve(ctx, f, rd, sx, sy, sz, p));
+  uint32_t kept = p.ncomp;
+  if (dust_threshold > 0 && p.ncomp > 0) IGN_TRY(dust_runs(ctx, p, dust_threshold, &kept));
+  if (dust_labels_inplace != nullptr && dust_threshold > 0 && p.R > 0) {
+    const ExpandArgs e = p.expand_args(0);
+    IGN_LAUNCH(ctx, (k_dust_apply<TL>), blocks_for(p.W * 32, 256), 256, 0, e, dust_labels_inplace);
   }
-  return IGN_ERR_OVERFLOW;
+  if (out != nullptr) IGN_TRY(write_labels(ctx, p, offset, out, IGN_U64, kept));
+  if (n_components) *n_components = kept;
+  return IGN_OK;
 }
 
 // raw >= gte and raw <= lte for an unsigned integer raw, as exact integer bounds [lo, hi]; an
@@ -1294,29 +1297,24 @@ template <typename T>
 static int ccl_task_typed(ign_ctx* ctx, const void* in, uint64_t sx, uint64_t sy, uint64_t sz,
                           int use_gte, double gte, int use_lte, double lte, uint64_t rx, uint64_t ry,
                           uint64_t rz, uint64_t dust, uint64_t offset, uint64_t* out, uint64_t* n) {
-  auto rail = [](uint64_t r, uint64_t s) { return (r < s) ? (uint32_t)r : 0xFFFFFFFFu; };
-  if (use_gte || use_lte) {
-    Reader<T, true> r;
-    r.in = (const T*)in;
+  auto run = [&](auto r) -> int {
     r.gte = gte;
     r.lte = lte;
     r.use_gte = use_gte;
     r.use_lte = use_lte;
     if constexpr (!std::is_same<T, float>::value) int_bounds(use_gte, gte, use_lte, lte, &r.ilo, &r.ihi);
+    auto rail = [](uint64_t c, uint64_t s) { return (c < s) ? (uint32_t)c : 0xFFFFFFFFu; };
     r.rx = rail(rx, sx);
     r.ry = rail(ry, sy);
     r.rz = rail(rz, sz);
-    return ccl_run(ctx, r, sx, sy, sz, dust, offset, out, IGN_U64, (uint8_t*)nullptr, n);
-  }
+    return ccl_run(ctx, r, sx, sy, sz, dust, offset, out, (uint8_t*)nullptr, n);
+  };
+  if (use_gte || use_lte) return run(plain_reader<T, true>(in));
   if constexpr (std::is_same<T, float>::value) {
     set_error("CCL on float input requires a threshold");
     return IGN_ERR_UNSUPPORTED;
   } else {
-    Reader<T, false> r = plain_reader<T>(in);
-    r.rx = rail(rx, sx);
-    r.ry = rail(ry, sy);
-    r.rz = rail(rz, sz);
-    return ccl_run(ctx, r, sx, sy, sz, dust, offset, out, IGN_U64, (uint8_t*)nullptr, n);
+    return run(plain_reader<T>(in));
   }
 }
 
@@ -1329,48 +1327,44 @@ using namespace ign;
 // every rank's volume in between (ONE all-gather) and fold the global relabelling into
 // the run labels before the single expansion pass.
 struct ign_ccl_volume {
-  ign_ccl_volume(ign_ctx* c, const void* i, int dt) : ctx(c), frame(c), in(i), in_dtype(dt) {}
+  ign_ccl_volume(ign_ctx* c) : ctx(c), frame(c) {}
   ign_ctx* ctx;
   ScratchFrame frame;  // holds the masks and run labels from begin to finish / abort
-  const void* in;
-  int in_dtype;
   CclPlan plan;
   uint64_t n_local;
 };
 
-template <typename T>
-static int volume_begin_typed(ign_ctx* ctx, ign_ccl_volume* v, uint64_t sx, uint64_t sy, uint64_t sz,
-                              uint64_t* first_values, uint32_t* first_labels, uint64_t* last_values,
-                              uint32_t* last_labels) {
-  const uint64_t n = sx * sy * sz;
-  uint64_t rcap = default_rcap(n);
-  for (int attempt = 0; attempt < 2; attempt++) {
-    v->frame.rewind();
-    uint64_t need = 0;
-    IGN_TRY(ccl_structure(ctx, v->frame, plain_reader<T>(v->in), (uint32_t)sx, (uint32_t)sy, (uint32_t)sz, rcap, v->plan, &need));
-    if (need > rcap) {
-      IGN_REQUIRE(attempt == 0, IGN_ERR_NOMEM, "CCL: %llu runs after a retry sized for them", (unsigned long long)need);
-      rcap = need + 16;
-      continue;
+// The plane record of one slab (multigpu.plane_record_bytes): a 256-byte header whose first u64
+// is the slab's component count, then its first and last z-planes of voxel values (u64) and of
+// volume-local labels (u32), np = sx*sy entries each.  Byte offsets.
+struct PlaneRecord {
+  size_t bytes, first_values, last_values, first_labels, last_labels;
+};
+static PlaneRecord plane_record(uint64_t np) { return {256 + 24 * np, 256, 256 + 8 * np, 256 + 16 * np, 256 + 20 * np}; }
+
+static int volume_begin(ign_ccl_volume* v, const void* in, int in_dtype, uint64_t sx, uint64_t sy, uint64_t sz,
+                        uint64_t* first_values, uint32_t* first_labels, uint64_t* last_values, uint32_t* last_labels) {
+  ign_ctx* ctx = v->ctx;
+  return dispatch_label(in_dtype, "volume CCL", [&](auto t) -> int {
+    using T = decltype(t);
+    IGN_TRY(ccl_resolve(ctx, v->frame, plain_reader<T>(in), sx, sy, sz, v->plan));
+    v->n_local = v->plan.ncomp;
+    if (first_values && first_labels && last_values && last_labels) {
+      const uint64_t np = sx * sy;
+      const ExpandArgs e = v->plan.expand_args(0);
+      if (v->plan.R == 0) {
+        IGN_CUDA(cudaMemsetAsync(first_labels, 0, np * 4, ctx->stream));
+        IGN_CUDA(cudaMemsetAsync(last_labels, 0, np * 4, ctx->stream));
+        IGN_CUDA(cudaMemsetAsync(first_values, 0, np * 8, ctx->stream));
+        IGN_CUDA(cudaMemsetAsync(last_values, 0, np * 8, ctx->stream));
+      } else {
+        IGN_LAUNCH(ctx, (k_ccl_plane<T>), blocks_for(np, 256), 256, 0, (const T*)in, e, (uint64_t)0, (uint32_t)sy, first_values, first_labels);
+        IGN_LAUNCH(ctx, (k_ccl_plane<T>), blocks_for(np, 256), 256, 0, (const T*)in, e, (uint64_t)(sz - 1), (uint32_t)sy, last_values, last_labels);
+      }
+      IGN_CUDA(cudaStreamSynchronize(ctx->stream));
     }
-    break;
-  }
-  v->n_local = v->plan.ncomp;
-  if (first_values && first_labels && last_values && last_labels) {
-    const uint64_t np = sx * sy;
-    const ExpandArgs e = v->plan.expand_args(0);
-    if (v->plan.R == 0) {
-      IGN_CUDA(cudaMemsetAsync(first_labels, 0, np * 4, ctx->stream));
-      IGN_CUDA(cudaMemsetAsync(last_labels, 0, np * 4, ctx->stream));
-      IGN_CUDA(cudaMemsetAsync(first_values, 0, np * 8, ctx->stream));
-      IGN_CUDA(cudaMemsetAsync(last_values, 0, np * 8, ctx->stream));
-    } else {
-      IGN_LAUNCH(ctx, (k_ccl_plane<T>), blocks_for(np, 256), 256, 0, (const T*)v->in, e, (uint64_t)0, (uint32_t)sy, first_values, first_labels);
-      IGN_LAUNCH(ctx, (k_ccl_plane<T>), blocks_for(np, 256), 256, 0, (const T*)v->in, e, (uint64_t)(sz - 1), (uint32_t)sy, last_values, last_labels);
-    }
-    IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  }
-  return IGN_OK;
+    return IGN_OK;
+  });
 }
 
 static int grow(char** buf, size_t* have, size_t need) {
@@ -1399,12 +1393,11 @@ static int volume_finish_gathered(ign_ccl_volume* v, const char* rec_base, int N
   CclPlan& p = v->plan;
   IGN_REQUIRE(rec_base && out, IGN_ERR_INVALID, "null argument");
   IGN_REQUIRE(N >= 1 && me >= 0 && me < N, IGN_ERR_INVALID, "rank %d of %d ranks", me, N);
-  IGN_REQUIRE(out_dtype == IGN_U16 || out_dtype == IGN_U32 || out_dtype == IGN_U64, IGN_ERR_UNSUPPORTED,
-              "CCL out_dtype must be u16/u32/u64 (got %d)", out_dtype);
-  const uint64_t sx = p.sx, sy = p.sy, sz = p.sz, np = sx * sy;
-  const size_t rec = 256 + 2 * np * 8 + 2 * np * 4;
+  IGN_TRY(check_out_dtype(out_dtype));
+  const uint64_t np = (uint64_t)p.sx * p.sy;
+  const PlaneRecord L = plane_record(np);
   std::vector<uint64_t> nloc(N, 0);
-  for (int r = 0; r < N; r++) IGN_TRY(small_d2h(ctx, &nloc[r], rec_base + (size_t)r * rec, 8));
+  for (int r = 0; r < N; r++) IGN_TRY(small_d2h(ctx, &nloc[r], rec_base + (size_t)r * L.bytes, 8));
   IGN_TRY(small_sync(ctx));
   IGN_REQUIRE(nloc[me] == v->n_local, IGN_ERR_INVALID,
               "plane record %d holds %llu components but the volume has %llu (wrong rank?)", me,
@@ -1423,40 +1416,25 @@ static int volume_finish_gathered(ign_ccl_volume* v, const char* rec_base, int N
   IGN_TRY(f.take(&tmp, cubb));
   IGN_LAUNCH(ctx, k_iota_u32, blocks_for(items, 256), 256, 0, parent, items);
   for (int b = 0; b + 1 < N; b++) {
-    const char* ra = rec_base + (size_t)b * rec;
-    const char* rb = rec_base + (size_t)(b + 1) * rec;
-    const uint64_t* va = (const uint64_t*)(ra + 256) + np;                     // last plane of rank b
-    const uint32_t* la = (const uint32_t*)(ra + 256 + 2 * np * 8) + np;
-    const uint64_t* vb = (const uint64_t*)(rb + 256);                          // first plane of rank b+1
-    const uint32_t* lb = (const uint32_t*)(rb + 256 + 2 * np * 8);
-    IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_MERGE, k_ccl_link_union, blocks_for(np, 256), 256, 0, va, la, (uint32_t)off[b], vb, lb,
-                    (uint32_t)off[b + 1], np, parent);
+    const char* ra = rec_base + (size_t)b * L.bytes;        // last planes of rank b
+    const char* rb = rec_base + (size_t)(b + 1) * L.bytes;  // first planes of rank b+1
+    IGN_LAUNCH_PROF(ctx, IGN_PROF_CCL_MERGE, k_ccl_link_union, blocks_for(np, 256), 256, 0,
+                    (const uint64_t*)(ra + L.last_values), (const uint32_t*)(ra + L.last_labels), (uint32_t)off[b],
+                    (const uint64_t*)(rb + L.first_values), (const uint32_t*)(rb + L.first_labels), (uint32_t)off[b + 1],
+                    np, parent);
   }
-  // roots in ascending id order: the exclusive scan is the dataset-wide cc3d numbering
-  IGN_LAUNCH(ctx, k_ccl_flatten, blocks_for(items - 1, 256), 256, 0, parent, items - 1);
-  IGN_CUDA(cudaMemsetAsync(parent + (items - 1), 0xFF, 4, ctx->stream));  // sentinel: not a root
-  {
-    IsRootOp op;
-    op.parent = parent;
-    auto it = thrust::make_transform_iterator(thrust::counting_iterator<uint32_t>(0), op);
-    size_t tb = cubb;
-    IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, it, rank, (int)items, ctx->stream));
-    ctx->launches += 2;
-  }
-  uint32_t hN = 0;
-  IGN_TRY(small_d2h(ctx, &hN, rank + (items - 1), 4));  // roots incl. id 0
+  // roots in ascending id order: their ranks are the dataset-wide cc3d numbering
+  uint32_t hN = 0;  // roots incl. id 0
+  IGN_TRY(rank_roots(ctx, parent, rank, items - 1, tmp, cubb, &hN));
   IGN_LAUNCH(ctx, k_ccl_rank_of_root, blocks_for(items - 1, 256), 256, 0, parent, rank, items - 1);
   // the output type must hold the global count, not the sum of the slabs' counts: a component
   // that crosses k boundaries is counted k+1 times in `total`
   IGN_TRY(small_sync(ctx));
   const uint64_t nglob = hN ? hN - 1 : 0;
   IGN_TRY(check_labels_fit(out_dtype, nglob));
-  if (p.R > 0) {
+  if (p.R > 0)
     IGN_LAUNCH(ctx, k_ccl_relabel_runs, blocks_for(p.R, 256), 256, 0, p.label, p.R, (const uint32_t*)parent + off[me]);
-    IGN_TRY(launch_expand(ctx, p, 0, out, out_dtype, nglob));
-  } else {
-    IGN_CUDA(cudaMemsetAsync(out, 0, sx * sy * sz * dtype_size(out_dtype), ctx->stream));
-  }
+  IGN_TRY(write_labels(ctx, p, 0, out, out_dtype, nglob));
   IGN_TRY(small_sync(ctx));
   if (n_global) *n_global = nglob;
   return IGN_OK;
@@ -1466,16 +1444,7 @@ extern "C" {
 
 int ign_ccl6_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy, uint64_t sz,
                  void* out, int out_dtype, uint64_t* n_components) {
-  IGN_TRY(activate(ctx));
-  IGN_REQUIRE(in && out, IGN_ERR_INVALID, "null buffer");
-  switch (in_dtype) {
-    case IGN_U8: return ccl_run(ctx, plain_reader<uint8_t>(in), sx, sy, sz, 0, 0, out, out_dtype, (uint8_t*)nullptr, n_components);
-    case IGN_U16: return ccl_run(ctx, plain_reader<uint16_t>(in), sx, sy, sz, 0, 0, out, out_dtype, (uint16_t*)nullptr, n_components);
-    case IGN_U32: return ccl_run(ctx, plain_reader<uint32_t>(in), sx, sy, sz, 0, 0, out, out_dtype, (uint32_t*)nullptr, n_components);
-    case IGN_U64: return ccl_run(ctx, plain_reader<uint64_t>(in), sx, sy, sz, 0, 0, out, out_dtype, (uint64_t*)nullptr, n_components);
-  }
-  set_error("CCL: unsupported input dtype %d", in_dtype);
-  return IGN_ERR_UNSUPPORTED;
+  return ign_ccl6_volume_dev(ctx, in, in_dtype, sx, sy, sz, out, out_dtype, n_components);
 }
 
 int ign_dust_dev(ign_ctx* ctx, void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
@@ -1483,14 +1452,10 @@ int ign_dust_dev(ign_ctx* ctx, void* labels, int dtype, uint64_t sx, uint64_t sy
   IGN_TRY(activate(ctx));
   IGN_REQUIRE(labels, IGN_ERR_INVALID, "null buffer");
   if (threshold == 0) return IGN_OK;
-  switch (dtype) {
-    case IGN_U8: return ccl_run(ctx, plain_reader<uint8_t>(labels), sx, sy, sz, threshold, 0, nullptr, IGN_U64, (uint8_t*)labels, nullptr);
-    case IGN_U16: return ccl_run(ctx, plain_reader<uint16_t>(labels), sx, sy, sz, threshold, 0, nullptr, IGN_U64, (uint16_t*)labels, nullptr);
-    case IGN_U32: return ccl_run(ctx, plain_reader<uint32_t>(labels), sx, sy, sz, threshold, 0, nullptr, IGN_U64, (uint32_t*)labels, nullptr);
-    case IGN_U64: return ccl_run(ctx, plain_reader<uint64_t>(labels), sx, sy, sz, threshold, 0, nullptr, IGN_U64, (uint64_t*)labels, nullptr);
-  }
-  set_error("dust: unsupported dtype %d", dtype);
-  return IGN_ERR_UNSUPPORTED;
+  return dispatch_label(dtype, "dust", [&](auto t) {
+    using T = decltype(t);
+    return ccl_run(ctx, plain_reader<T>(labels), sx, sy, sz, threshold, 0, nullptr, (T*)labels, nullptr);
+  });
 }
 
 int ign_ccl_task_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy,
@@ -1499,23 +1464,19 @@ int ign_ccl_task_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, ui
                      uint64_t label_offset, uint64_t* out, uint64_t* n_components) {
   IGN_TRY(activate(ctx));
   IGN_REQUIRE(in && out, IGN_ERR_INVALID, "null buffer");
-  switch (in_dtype) {
-    case IGN_U8: return ccl_task_typed<uint8_t>(ctx, in, sx, sy, sz, use_gte, gte, use_lte, lte, rail_x, rail_y, rail_z, dust_threshold, label_offset, out, n_components);
-    case IGN_U16: return ccl_task_typed<uint16_t>(ctx, in, sx, sy, sz, use_gte, gte, use_lte, lte, rail_x, rail_y, rail_z, dust_threshold, label_offset, out, n_components);
-    case IGN_U32: return ccl_task_typed<uint32_t>(ctx, in, sx, sy, sz, use_gte, gte, use_lte, lte, rail_x, rail_y, rail_z, dust_threshold, label_offset, out, n_components);
-    case IGN_U64: return ccl_task_typed<uint64_t>(ctx, in, sx, sy, sz, use_gte, gte, use_lte, lte, rail_x, rail_y, rail_z, dust_threshold, label_offset, out, n_components);
-    case IGN_F32: return ccl_task_typed<float>(ctx, in, sx, sy, sz, use_gte, gte, use_lte, lte, rail_x, rail_y, rail_z, dust_threshold, label_offset, out, n_components);
-  }
-  set_error("CCL task: unsupported input dtype %d", in_dtype);
-  return IGN_ERR_UNSUPPORTED;
+  auto run = [&](auto t) {
+    return ccl_task_typed<decltype(t)>(ctx, in, sx, sy, sz, use_gte, gte, use_lte, lte, rail_x, rail_y, rail_z,
+                                       dust_threshold, label_offset, out, n_components);
+  };
+  if (in_dtype == IGN_F32) return run(float{});
+  return dispatch_label(in_dtype, "CCL task", run);
 }
 
 // ---- host-buffer wrappers
 int ign_ccl6(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy, uint64_t sz,
              void* out, int out_dtype, uint64_t* n_components) {
   IGN_TRY(check_ccl_dims(sx, sy, sz));
-  // sizes the staged output; ign_ccl6_dev checks out_dtype only once it writes labels
-  IGN_REQUIRE(dtype_size(out_dtype) > 0, IGN_ERR_UNSUPPORTED, "CCL: unsupported output dtype %d", out_dtype);
+  IGN_TRY(check_out_dtype(out_dtype));
   const uint64_t n = sx * sy * sz;
   return staged(ctx, {{in, nullptr, n * dtype_size(in_dtype)}, {nullptr, out, n * dtype_size(out_dtype)}},
                 [&](void* const* d) {
@@ -1623,15 +1584,8 @@ int ign_ccl6_volume_begin_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64
   IGN_REQUIRE(in && out && n_local, IGN_ERR_INVALID, "null argument");
   *out = nullptr;
   IGN_TRY(check_ccl_dims(sx, sy, sz));
-  ign_ccl_volume* v = new ign_ccl_volume(ctx, in, in_dtype);
-  int rc;
-  switch (in_dtype) {
-    case IGN_U8: rc = volume_begin_typed<uint8_t>(ctx, v, sx, sy, sz, first_values, first_labels, last_values, last_labels); break;
-    case IGN_U16: rc = volume_begin_typed<uint16_t>(ctx, v, sx, sy, sz, first_values, first_labels, last_values, last_labels); break;
-    case IGN_U32: rc = volume_begin_typed<uint32_t>(ctx, v, sx, sy, sz, first_values, first_labels, last_values, last_labels); break;
-    case IGN_U64: rc = volume_begin_typed<uint64_t>(ctx, v, sx, sy, sz, first_values, first_labels, last_values, last_labels); break;
-    default: set_error("volume CCL: unsupported input dtype %d", in_dtype); rc = IGN_ERR_UNSUPPORTED;
-  }
+  ign_ccl_volume* v = new ign_ccl_volume(ctx);
+  const int rc = volume_begin(v, in, in_dtype, sx, sy, sz, first_values, first_labels, last_values, last_labels);
   if (rc != IGN_OK) {
     ign_ccl6_volume_abort(v);
     return rc;
@@ -1645,13 +1599,9 @@ static int volume_finish(ign_ccl_volume* v, const uint32_t* global_lut, uint64_t
                          int out_dtype) {
   ign_ctx* ctx = v->ctx;
   CclPlan& p = v->plan;
+  IGN_TRY(check_out_dtype(out_dtype));
   if (!global_lut) max_label = v->n_local;
-  if (p.R == 0) {
-    IGN_REQUIRE(dtype_size(out_dtype) > 0, IGN_ERR_UNSUPPORTED, "unsupported out dtype");
-    IGN_CUDA(cudaMemsetAsync(out, 0, (uint64_t)p.sx * p.sy * p.sz * dtype_size(out_dtype), ctx->stream));
-    return IGN_OK;
-  }
-  if (global_lut) {
+  if (global_lut && p.R > 0) {
     ScratchFrame f(ctx);
     uint32_t* d_lut;
     IGN_TRY(f.take(&d_lut, v->n_local + 1));
@@ -1660,7 +1610,7 @@ static int volume_finish(ign_ccl_volume* v, const uint32_t* global_lut, uint64_t
     // the host table may be a temporary of the caller
     IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   }
-  return launch_expand(ctx, p, 0, out, out_dtype, max_label);
+  return write_labels(ctx, p, 0, out, out_dtype, max_label);
 }
 
 // global_lut: NULL, or HOST table [n_local+1] volume-local id -> final id (from the caller's
@@ -1685,9 +1635,11 @@ int ign_ccl6_volume_finish_gathered_dev(ign_ccl_volume* v, const void* records_d
   return rc;
 }
 
+// begin + finish with nothing in between: the one implementation of ign_ccl6[_dev]
 int ign_ccl6_volume_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx, uint64_t sy,
                         uint64_t sz, void* out, int out_dtype, uint64_t* n_components) {
   IGN_REQUIRE(in && out, IGN_ERR_INVALID, "null buffer");
+  IGN_TRY(check_out_dtype(out_dtype));
   ign_ccl_volume* v = nullptr;
   uint64_t n = 0;
   IGN_TRY(ign_ccl6_volume_begin_dev(ctx, in, in_dtype, sx, sy, sz, nullptr, nullptr, nullptr, nullptr, &v, &n));
@@ -1696,28 +1648,25 @@ int ign_ccl6_volume_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx,
   return IGN_OK;
 }
 
-
 int ign_ccl6_sharded_dev(ign_group* g, const void* in, int in_dtype, uint64_t sx, uint64_t sy, uint64_t sz,
                          void* out, int out_dtype, uint64_t* n_global) {
   IGN_REQUIRE(g && in && out, IGN_ERR_INVALID, "null argument");
   ign_ctx* ctx = g->ctx;
   IGN_TRY(activate(ctx));
   IGN_TRY(check_ccl_dims(sx, sy, sz));
-  IGN_REQUIRE(dtype_size(out_dtype) > 0, IGN_ERR_UNSUPPORTED, "unsupported out dtype");
+  IGN_TRY(check_out_dtype(out_dtype));
   // exactly ONE collective: an all-gather of every rank's [n_local | first plane | last plane]
-  const uint64_t np = sx * sy;
-  const size_t rec = 256 + 2 * np * 8 + 2 * np * 4;
-  IGN_TRY(grow(&g->d_send, &g->send_bytes, rec));
-  IGN_TRY(grow(&g->d_recv, &g->recv_bytes, rec * (size_t)g->nranks));
-  uint64_t* first_v = (uint64_t*)(g->d_send + 256);
-  uint64_t* last_v = first_v + np;
-  uint32_t* first_l = (uint32_t*)(last_v + np);
-  uint32_t* last_l = first_l + np;
+  const PlaneRecord L = plane_record(sx * sy);
+  IGN_TRY(grow(&g->d_send, &g->send_bytes, L.bytes));
+  IGN_TRY(grow(&g->d_recv, &g->recv_bytes, L.bytes * (size_t)g->nranks));
+  char* const rec = g->d_send;
   ign_ccl_volume* v = nullptr;
   uint64_t head[32] = {0};
-  IGN_TRY(ign_ccl6_volume_begin_dev(ctx, in, in_dtype, sx, sy, sz, first_v, first_l, last_v, last_l, &v, &head[0]));
+  IGN_TRY(ign_ccl6_volume_begin_dev(ctx, in, in_dtype, sx, sy, sz, (uint64_t*)(rec + L.first_values),
+                                    (uint32_t*)(rec + L.first_labels), (uint64_t*)(rec + L.last_values),
+                                    (uint32_t*)(rec + L.last_labels), &v, &head[0]));
   int rc = small_h2d(ctx, g->d_send, head, 256);
-  if (rc == IGN_OK) rc = ign_group_allgather(g, g->d_send, rec, g->d_recv);
+  if (rc == IGN_OK) rc = ign_group_allgather(g, g->d_send, L.bytes, g->d_recv);
   if (rc != IGN_OK) {
     ign_ccl6_volume_abort(v);
     return rc;

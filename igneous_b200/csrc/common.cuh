@@ -51,6 +51,20 @@ static inline int dtype_size(int dt) {
   }
 }
 
+// Calls f(T{}) with T the unsigned type of label dtype IGN_U8 / U16 / U32 / U64 and returns what f
+// returns; any other code is IGN_ERR_UNSUPPORTED, reported as `who`'s.
+template <typename F>
+int dispatch_label(int dtype, const char* who, F&& f) {
+  switch (dtype) {
+    case IGN_U8: return f(uint8_t{});
+    case IGN_U16: return f(uint16_t{});
+    case IGN_U32: return f(uint32_t{});
+    case IGN_U64: return f(uint64_t{});
+  }
+  set_error("%s: unsupported label dtype %d", who, dtype);
+  return IGN_ERR_UNSUPPORTED;
+}
+
 }  // namespace ign
 
 constexpr int IGN_TIMER_SLOTS = 64;  // CUDA event pairs per context: timers and cross-stream marks

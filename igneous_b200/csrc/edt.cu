@@ -287,12 +287,9 @@ int ign_edt_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64
               "edt: labels not aligned to their element size");
   IGN_REQUIRE((uintptr_t)out % 4 == 0, IGN_ERR_INVALID, "edt: out not aligned to 4 bytes");
   const int bb = black_border ? 1 : 0;
-  switch (dtype) {
-    case IGN_U8: return edt_run<uint8_t>(ctx, labels, sx, sy, sz, anisotropy, bb, squared, out);
-    case IGN_U16: return edt_run<uint16_t>(ctx, labels, sx, sy, sz, anisotropy, bb, squared, out);
-    case IGN_U32: return edt_run<uint32_t>(ctx, labels, sx, sy, sz, anisotropy, bb, squared, out);
-    default: return edt_run<uint64_t>(ctx, labels, sx, sy, sz, anisotropy, bb, squared, out);
-  }
+  return dispatch_label(dtype, "edt", [&](auto v) {
+    return edt_run<decltype(v)>(ctx, labels, sx, sy, sz, anisotropy, bb, squared, out);
+  });
 }
 
 int ign_edt(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,

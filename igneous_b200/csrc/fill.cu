@@ -468,14 +468,8 @@ int ign_dilate_multilabel_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t 
   IGN_REQUIRE(in && out && in != out, IGN_ERR_INVALID, "null or aliased buffer");
   IGN_REQUIRE(sx > 0 && sy > 0 && sz > 0, IGN_ERR_INVALID, "empty volume");
   IGN_REQUIRE(sx < (1ull << 31) && sy < (1ull << 31) && sz < (1ull << 31), IGN_ERR_OVERFLOW, "extent too large");
-  switch (dtype) {
-    case IGN_U8: return dilate_typed<uint8_t>(ctx, in, sx, sy, sz, out);
-    case IGN_U16: return dilate_typed<uint16_t>(ctx, in, sx, sy, sz, out);
-    case IGN_U32: return dilate_typed<uint32_t>(ctx, in, sx, sy, sz, out);
-    case IGN_U64: return dilate_typed<uint64_t>(ctx, in, sx, sy, sz, out);
-  }
-  set_error("dilate: unsupported dtype %d", dtype);
-  return IGN_ERR_UNSUPPORTED;
+  return dispatch_label(dtype, "dilate",
+                        [&](auto v) { return dilate_typed<decltype(v)>(ctx, in, sx, sy, sz, out); });
 }
 
 int ign_fill_holes_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
@@ -485,12 +479,10 @@ int ign_fill_holes_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uin
               "null or aliased buffer");
   IGN_TRY(fill_check(sx, sy, sz, dtype, merge_threshold_pct));
   const int p = 100 - merge_threshold_pct;
-  switch (dtype) {
-    case IGN_U8: return fill_typed(ctx, (const uint8_t*)in, sx, sy, sz, fix_borders, p, (uint8_t*)filled, (uint8_t*)holes);
-    case IGN_U16: return fill_typed(ctx, (const uint16_t*)in, sx, sy, sz, fix_borders, p, (uint16_t*)filled, (uint16_t*)holes);
-    case IGN_U32: return fill_typed(ctx, (const uint32_t*)in, sx, sy, sz, fix_borders, p, (uint32_t*)filled, (uint32_t*)holes);
-    default: return fill_typed(ctx, (const uint64_t*)in, sx, sy, sz, fix_borders, p, (uint64_t*)filled, (uint64_t*)holes);
-  }
+  return dispatch_label(dtype, "fill_holes", [&](auto v) {
+    using T = decltype(v);
+    return fill_typed(ctx, (const T*)in, sx, sy, sz, fix_borders, p, (T*)filled, (T*)holes);
+  });
 }
 
 // ---- host-buffer wrappers

@@ -630,15 +630,11 @@ int ign_pool_mode_2x2x1_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx
                             uint64_t sz, int num_mips, int sparse, void* const* outs) {
   IGN_TRY(activate(ctx));
   IGN_TRY(check_pool_args(in, dtype, sx, sy, sz, num_mips, outs));
-  switch (dtype) {
-    case IGN_U8: return mode_pyramid<uint8_t>(ctx, (const uint8_t*)in, sx, sy, sz, num_mips, sparse, outs);
-    case IGN_U16: return mode_pyramid<uint16_t>(ctx, (const uint16_t*)in, sx, sy, sz, num_mips, sparse, outs);
-    case IGN_U32:
-    case IGN_F32: return mode_pyramid<uint32_t>(ctx, (const uint32_t*)in, sx, sy, sz, num_mips, sparse, outs);
-    case IGN_U64: return mode_pyramid<uint64_t>(ctx, (const uint64_t*)in, sx, sy, sz, num_mips, sparse, outs);
-  }
-  set_error("unsupported dtype %d", dtype);
-  return IGN_ERR_UNSUPPORTED;
+  // f32 voxels are pooled as their u32 bit patterns
+  return dispatch_label(dtype == IGN_F32 ? IGN_U32 : dtype, "pool_mode", [&](auto v) {
+    using T = decltype(v);
+    return mode_pyramid<T>(ctx, (const T*)in, sx, sy, sz, num_mips, sparse, outs);
+  });
 }
 
 int ign_pool_avg_2x2x1_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy,
@@ -664,15 +660,9 @@ int ign_pool_select_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, ui
   IGN_REQUIRE(op >= 0 && op <= 10, IGN_ERR_INVALID,
               "op must be 0 min, 1 max, 2 striding, 3 mode, 4 sparse mode, 5-7 average or 8-10 sparse average "
               "(floor / half-up / half-even)");
-  switch (dtype) {
-    case IGN_U8: return select_pyramid<uint8_t>(ctx, in, sx, sy, sz, fx, fy, fz, num_mips, op, outs);
-    case IGN_U16: return select_pyramid<uint16_t>(ctx, in, sx, sy, sz, fx, fy, fz, num_mips, op, outs);
-    case IGN_U32: return select_pyramid<uint32_t>(ctx, in, sx, sy, sz, fx, fy, fz, num_mips, op, outs);
-    case IGN_U64: return select_pyramid<uint64_t>(ctx, in, sx, sy, sz, fx, fy, fz, num_mips, op, outs);
-    case IGN_F32: return select_pyramid<float>(ctx, in, sx, sy, sz, fx, fy, fz, num_mips, op, outs);
-  }
-  set_error("unsupported dtype %d", dtype);
-  return IGN_ERR_UNSUPPORTED;
+  auto run = [&](auto v) { return select_pyramid<decltype(v)>(ctx, in, sx, sy, sz, fx, fy, fz, num_mips, op, outs); };
+  if (dtype == IGN_F32) return run(float{});
+  return dispatch_label(dtype, "pool_select", run);
 }
 
 int ign_pool_select(ign_ctx* ctx, const void* in, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,

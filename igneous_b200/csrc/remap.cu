@@ -286,15 +286,6 @@ static int read_counters(ign_ctx* ctx, const uint32_t* counters, uint32_t* h8) {
   return small_sync(ctx);
 }
 
-#define DISPATCH_UINT(dtype, FN, ...)                                      \
-  switch (dtype) {                                                         \
-    case IGN_U8: FN(uint8_t, __VA_ARGS__); break;                          \
-    case IGN_U16: FN(uint16_t, __VA_ARGS__); break;                        \
-    case IGN_U32: FN(uint32_t, __VA_ARGS__); break;                        \
-    case IGN_U64: FN(uint64_t, __VA_ARGS__); break;                        \
-    default: set_error("unsupported label dtype %d", dtype); return IGN_ERR_UNSUPPORTED; \
-  }
-
 static size_t sort_tmp_bytes_u64(uint32_t n) {
   size_t a = 0, b = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, a, (const uint64_t*)nullptr, (uint64_t*)nullptr,
@@ -316,9 +307,11 @@ static int renumber_table(ign_ctx* ctx, ScratchFrame& f, const void* in, int dty
     f.rewind();
     uint32_t* counters;
     IGN_TRY(table_alloc(ctx, f, cap, 0xFF, t, &counters));
-#define RUN_FIRST(T, dummy) IGN_LAUNCH(ctx, (k_first_index<T>), blocks_for(n, 256), 256, 0, (const T*)in, n, t, counters)
-    DISPATCH_UINT(dtype, RUN_FIRST, 0)
-#undef RUN_FIRST
+    IGN_TRY(dispatch_label(dtype, "renumber", [&](auto v) -> int {
+      using T = decltype(v);
+      IGN_LAUNCH(ctx, (k_first_index<T>), blocks_for(n, 256), 256, 0, (const T*)in, n, t, counters);
+      return IGN_OK;
+    }));
     uint32_t h[8];
     IGN_TRY(read_counters(ctx, counters, h));
     if (h[1] != 0 || h[0] > cap / 2) {
@@ -365,20 +358,14 @@ int ign_cast_dev(ign_ctx* ctx, const void* in, int in_dtype, void* out, int out_
   IGN_TRY(activate(ctx));
   IGN_REQUIRE(in && out, IGN_ERR_INVALID, "null buffer");
   if (n == 0) return IGN_OK;
-  const unsigned g = blocks_for(n, 256);
-#define CAST2(A, B) IGN_LAUNCH(ctx, (k_cast<A, B>), g, 256, 0, (const A*)in, (B*)out, n)
-#define CAST1(A, dummy)                                  \
-  switch (out_dtype) {                                   \
-    case IGN_U8: CAST2(A, uint8_t); break;               \
-    case IGN_U16: CAST2(A, uint16_t); break;             \
-    case IGN_U32: CAST2(A, uint32_t); break;             \
-    case IGN_U64: CAST2(A, uint64_t); break;             \
-    default: set_error("cast: unsupported out dtype %d", out_dtype); return IGN_ERR_UNSUPPORTED; \
-  }
-  DISPATCH_UINT(in_dtype, CAST1, 0)
-#undef CAST1
-#undef CAST2
-  return IGN_OK;
+  return dispatch_label(in_dtype, "cast", [&](auto a) {
+    return dispatch_label(out_dtype, "cast", [&](auto b) -> int {
+      using A = decltype(a);
+      using B = decltype(b);
+      IGN_LAUNCH(ctx, (k_cast<A, B>), blocks_for(n, 256), 256, 0, (const A*)in, (B*)out, n);
+      return IGN_OK;
+    });
+  });
 }
 
 int ign_renumber_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint32_t* out,
@@ -391,10 +378,11 @@ int ign_renumber_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint32
   HashTable t;
   uint32_t* counters;
   IGN_TRY(renumber_table(ctx, f, in, dtype, n, t, &counters, uniq_dev, uniq_capacity, k));
-#define RUN_GATHER(T, dummy) IGN_LAUNCH(ctx, (k_gather<T, uint32_t>), blocks_for(n, 256), 256, 0, (const T*)in, n, t, out)
-  DISPATCH_UINT(dtype, RUN_GATHER, 0)
-#undef RUN_GATHER
-  return IGN_OK;
+  return dispatch_label(dtype, "renumber", [&](auto v) -> int {
+    using T = decltype(v);
+    IGN_LAUNCH(ctx, (k_gather<T, uint32_t>), blocks_for(n, 256), 256, 0, (const T*)in, n, t, out);
+    return IGN_OK;
+  });
 }
 
 int ign_renumber(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint32_t* out, uint64_t* uniq,
@@ -414,32 +402,33 @@ int ign_remap_dev(ign_ctx* ctx, void* arr, int dtype, uint64_t n, const uint64_t
   IGN_TRY(activate(ctx));
   IGN_REQUIRE(arr && (n_keys == 0 || (keys_host && vals_host)), IGN_ERR_INVALID, "null argument");
   if (n == 0) return IGN_OK;
-  const uint32_t cap = pow2_at_least(2 * n_keys + 16);
-  ScratchFrame f(ctx);
-  HashTable t;
-  uint32_t* counters;
-  IGN_TRY(table_alloc(ctx, f, cap, 0, t, &counters));
-  uint64_t *dk, *dv, *dmiss;
-  IGN_TRY(f.take(&dk, n_keys + 1));
-  IGN_TRY(f.take(&dv, n_keys + 1));
-  IGN_TRY(f.take(&dmiss, 1));
-  if (n_keys) {
-    IGN_CUDA(cudaMemcpyAsync(dk, keys_host, n_keys * 8, cudaMemcpyHostToDevice, ctx->stream));
-    IGN_CUDA(cudaMemcpyAsync(dv, vals_host, n_keys * 8, cudaMemcpyHostToDevice, ctx->stream));
-    IGN_LAUNCH(ctx, k_table_build, blocks_for(n_keys, 256), 256, 0, dk, dv, n_keys, t, counters);
-  }
-#define RUN_REMAP(T, dummy) IGN_LAUNCH(ctx, (k_remap<T>), blocks_for(n, 256), 256, 0, (T*)arr, n, t, preserve_missing, counters, dmiss)
-  DISPATCH_UINT(dtype, RUN_REMAP, 0)
-#undef RUN_REMAP
-  uint32_t h[8];
-  IGN_TRY(read_counters(ctx, counters, h));
-  if (h[5] != 0) {
-    uint64_t miss = 0;
-    IGN_CUDA(cudaMemcpy(&miss, dmiss, 8, cudaMemcpyDeviceToHost));
-    set_error("%llu", (unsigned long long)miss);  // KeyError(label), as fastremap.remap
-    return IGN_ERR_KEY;
-  }
-  return IGN_OK;
+  return dispatch_label(dtype, "remap", [&](auto v) -> int {
+    using T = decltype(v);
+    const uint32_t cap = pow2_at_least(2 * n_keys + 16);
+    ScratchFrame f(ctx);
+    HashTable t;
+    uint32_t* counters;
+    IGN_TRY(table_alloc(ctx, f, cap, 0, t, &counters));
+    uint64_t *dk, *dv, *dmiss;
+    IGN_TRY(f.take(&dk, n_keys + 1));
+    IGN_TRY(f.take(&dv, n_keys + 1));
+    IGN_TRY(f.take(&dmiss, 1));
+    if (n_keys) {
+      IGN_CUDA(cudaMemcpyAsync(dk, keys_host, n_keys * 8, cudaMemcpyHostToDevice, ctx->stream));
+      IGN_CUDA(cudaMemcpyAsync(dv, vals_host, n_keys * 8, cudaMemcpyHostToDevice, ctx->stream));
+      IGN_LAUNCH(ctx, k_table_build, blocks_for(n_keys, 256), 256, 0, dk, dv, n_keys, t, counters);
+    }
+    IGN_LAUNCH(ctx, (k_remap<T>), blocks_for(n, 256), 256, 0, (T*)arr, n, t, preserve_missing, counters, dmiss);
+    uint32_t h[8];
+    IGN_TRY(read_counters(ctx, counters, h));
+    if (h[5] != 0) {
+      uint64_t miss = 0;
+      IGN_CUDA(cudaMemcpy(&miss, dmiss, 8, cudaMemcpyDeviceToHost));
+      set_error("%llu", (unsigned long long)miss);  // KeyError(label), as fastremap.remap
+      return IGN_ERR_KEY;
+    }
+    return IGN_OK;
+  });
 }
 
 int ign_remap(ign_ctx* ctx, void* arr, int dtype, uint64_t n, const uint64_t* keys,
@@ -465,10 +454,11 @@ static int mask_body(ign_ctx* ctx, void* arr, int dtype, uint64_t n, const uint6
   if (n_labels)
     IGN_LAUNCH(ctx, k_table_build, blocks_for(n_labels, 256), 256, 0, labels, (const uint64_t*)nullptr, n_labels, t,
                counters);
-#define RUN_MASK(T, dummy) IGN_LAUNCH(ctx, (k_mask<T>), blocks_for(n, 256), 256, 0, (T*)arr, n, t, except, (T)value)
-  DISPATCH_UINT(dtype, RUN_MASK, 0)
-#undef RUN_MASK
-  return IGN_OK;
+  return dispatch_label(dtype, "mask", [&](auto v) -> int {
+    using T = decltype(v);
+    IGN_LAUNCH(ctx, (k_mask<T>), blocks_for(n, 256), 256, 0, (T*)arr, n, t, except, (T)value);
+    return IGN_OK;
+  });
 }
 
 // uniq / counts: `capacity` entries, may be NULL
@@ -486,9 +476,11 @@ static int unique_body(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint
     HashTable t;
     uint32_t* counters;
     IGN_TRY(table_alloc(ctx, f, cap, 0, t, &counters));
-#define RUN_COUNT(T, dummy) IGN_LAUNCH(ctx, (k_count<T>), blocks_for(n, 256), 256, 0, (const T*)in, n, t, counters)
-    DISPATCH_UINT(dtype, RUN_COUNT, 0)
-#undef RUN_COUNT
+    IGN_TRY(dispatch_label(dtype, "unique", [&](auto v) -> int {
+      using T = decltype(v);
+      IGN_LAUNCH(ctx, (k_count<T>), blocks_for(n, 256), 256, 0, (const T*)in, n, t, counters);
+      return IGN_OK;
+    }));
     uint32_t h[8];
     IGN_TRY(read_counters(ctx, counters, h));
     if (h[1] != 0 || h[0] > cap / 2) {
@@ -540,9 +532,11 @@ static int inverse_component_map_body(ign_ctx* ctx, const void* parents, const v
   IGN_TRY(f.take(&flags, n));
   IGN_TRY(f.take(&pos, n + 1));
   IGN_TRY(f.take(&tmp, tmp_bytes));
-#define RUN_WIDEN(T, dummy) IGN_LAUNCH(ctx, (k_widen_pairs<T>), blocks_for(n, 256), 256, 0, (const T*)parents, (const T*)components, n, p0, c0)
-  DISPATCH_UINT(dtype, RUN_WIDEN, 0)
-#undef RUN_WIDEN
+  IGN_TRY(dispatch_label(dtype, "inverse_component_map", [&](auto v) -> int {
+    using T = decltype(v);
+    IGN_LAUNCH(ctx, (k_widen_pairs<T>), blocks_for(n, 256), 256, 0, (const T*)parents, (const T*)components, n, p0, c0);
+    return IGN_OK;
+  }));
   // LSD: stable sort by component, then by parent
   size_t tb = tmp_bytes;
   IGN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, c0, c1, p0, p1, (int)n, 0, 64, ctx->stream));

@@ -197,23 +197,15 @@ int ign_find_objects_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t s
               "find_objects: labels not aligned to their element size");
   if (*max_label == 0) {
     if (!n) return IGN_OK;
-    switch (dtype) {
-      case IGN_U8: IGN_TRY(find_max<uint8_t>(ctx, labels, n, max_label)); break;
-      case IGN_U16: IGN_TRY(find_max<uint16_t>(ctx, labels, n, max_label)); break;
-      case IGN_U32: IGN_TRY(find_max<uint32_t>(ctx, labels, n, max_label)); break;
-      default: IGN_TRY(find_max<uint64_t>(ctx, labels, n, max_label));
-    }
+    IGN_TRY(dispatch_label(dtype, "find_objects",
+                           [&](auto v) { return find_max<decltype(v)>(ctx, labels, n, max_label); }));
     return fo_check(dtype, sx, sy, sz, max_label);
   }
   IGN_REQUIRE(boxes, IGN_ERR_INVALID, "null buffer");
   IGN_REQUIRE((uintptr_t)boxes % 4 == 0, IGN_ERR_INVALID, "find_objects: boxes not aligned to 4 bytes");
   const uint64_t N = *max_label;
-  switch (dtype) {
-    case IGN_U8: return find_boxes<uint8_t>(ctx, labels, sx, sy, sz, N, boxes);
-    case IGN_U16: return find_boxes<uint16_t>(ctx, labels, sx, sy, sz, N, boxes);
-    case IGN_U32: return find_boxes<uint32_t>(ctx, labels, sx, sy, sz, N, boxes);
-    default: return find_boxes<uint64_t>(ctx, labels, sx, sy, sz, N, boxes);
-  }
+  return dispatch_label(dtype, "find_objects",
+                        [&](auto v) { return find_boxes<decltype(v)>(ctx, labels, sx, sy, sz, N, boxes); });
 }
 
 int ign_find_objects(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,

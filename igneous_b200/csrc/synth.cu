@@ -77,14 +77,11 @@ int ign_synth_seg_dev(ign_ctx* ctx, void* out, int dtype, uint64_t sx, uint64_t 
   if (total == 0) return IGN_OK;
   IGN_REQUIRE(total / 256 < 0x7FFFFFFFull, IGN_ERR_OVERFLOW, "volume too large for one launch");
   const unsigned grid = blocks_for(total, 256);
-  switch (dtype) {
-    case IGN_U8: IGN_LAUNCH(ctx, (k_synth_seg<uint8_t>), grid, 256, 0, (uint8_t*)out, sx, sy, sz, ox, oy, oz, (int)pitch, num_ids, seed, id_base); break;
-    case IGN_U16: IGN_LAUNCH(ctx, (k_synth_seg<uint16_t>), grid, 256, 0, (uint16_t*)out, sx, sy, sz, ox, oy, oz, (int)pitch, num_ids, seed, id_base); break;
-    case IGN_U32: IGN_LAUNCH(ctx, (k_synth_seg<uint32_t>), grid, 256, 0, (uint32_t*)out, sx, sy, sz, ox, oy, oz, (int)pitch, num_ids, seed, id_base); break;
-    case IGN_U64: IGN_LAUNCH(ctx, (k_synth_seg<uint64_t>), grid, 256, 0, (uint64_t*)out, sx, sy, sz, ox, oy, oz, (int)pitch, num_ids, seed, id_base); break;
-    default: set_error("synth_seg: unsupported dtype %d", dtype); return IGN_ERR_UNSUPPORTED;
-  }
-  return IGN_OK;
+  return dispatch_label(dtype, "synth_seg", [&](auto v) -> int {
+    using T = decltype(v);
+    IGN_LAUNCH(ctx, (k_synth_seg<T>), grid, 256, 0, (T*)out, sx, sy, sz, ox, oy, oz, (int)pitch, num_ids, seed, id_base);
+    return IGN_OK;
+  });
 }
 
 int ign_synth_image_dev(ign_ctx* ctx, uint8_t* out, uint64_t sx, uint64_t sy, uint64_t sz,

@@ -148,7 +148,8 @@ IGN_API int ign_pool_select_dev(ign_ctx* ctx, const void* in, int dtype, uint64_
  * 6-connected, multi-label (equal non-zero values connect), 0 = background.
  * Output ids 1..N in order of each component's first voxel in Fortran raster
  * order.  in_dtype U8 also serves bool input (threshold_image output).
- * out_dtype: IGN_U16 / IGN_U32 / IGN_U64 (overflow -> IGN_ERR_OVERFLOW).
+ * out_dtype: IGN_U16 / IGN_U32 / IGN_U64 (overflow -> IGN_ERR_OVERFLOW); any other code ->
+ * IGN_ERR_UNSUPPORTED before any launch, in every CCL call that writes labels.
  * Rows of up to 131,072 voxels (sx); longer rows -> IGN_ERR_OVERFLOW before any launch.  Rows
  * past 2048 voxels resolve in flatter tiles (tests/test_ccl_long_rows_gpu.py covers each height).
  */
@@ -167,7 +168,7 @@ IGN_API int ign_ccl6_dev(ign_ctx* ctx, const void* in, int in_dtype, uint64_t sx
  * The result is bit-identical to one whole-volume ign_ccl6 call.
  *
  * ign_ccl6_volume_dev: one volume of up to 2^36 voxels in one call (no slabs: the
- * union-find runs over x-runs, not voxels). */
+ * union-find runs over x-runs, not voxels).  ign_ccl6_dev is the same call. */
 IGN_API int ign_ccl6_link_dev(ign_ctx* ctx, const uint64_t* values_a, const uint32_t* labels_a,
                               uint64_t offset_a, const uint64_t* values_b, const uint32_t* labels_b,
                               uint64_t offset_b, uint64_t n_plane, uint64_t* pairs_host,

@@ -20,7 +20,7 @@ IGN_ERR_OVERFLOW = -6
 
 
 def dispatch(sx, itemsize):
-  """What ccl_structure / launch_expand select for rows of sx voxels (16-byte aligned buffers)."""
+  """What ccl_structure / write_labels select for rows of sx voxels (16-byte aligned buffers)."""
   wpr = (sx + 31) // 32
   ty = 8
   while ty > 1 and wpr * ty * ty > TB_WMAX:
