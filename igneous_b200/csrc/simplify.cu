@@ -122,6 +122,51 @@ struct SEval {
   double p[3];
 };
 
+// collapse cost of the edge (u, v) (min over {u, v, midpoint} of p^T (Qu+Qv) p, boundary endpoints stay
+// put): u / v are vertex ids of any one numbering (they pick the kept vertex), gu / gv their rows of Q and
+// pos.  Invalid when both endpoints are on the boundary or the cost exceeds max_err2.
+__device__ __forceinline__ void s_cost(const double* Q, const double* pos, double max_err2, uint32_t u, uint32_t v,
+                                       uint64_t gu, uint64_t gv, bool bu, bool bv, SEval* e) {
+  e->valid = false;
+  if (bu && bv) return;
+  const double* Qu = Q + 10 * gu;
+  const double* Qv = Q + 10 * gv;
+  double q[10];
+#pragma unroll
+  for (int i = 0; i < 10; i++) q[i] = Qu[i] + Qv[i];
+  const double* pu = pos + 3 * gu;
+  const double* pv = pos + 3 * gv;
+  double best[3], cost;
+  if (bu) {
+    e->keep = u;
+    e->remove = v;
+    best[0] = pu[0]; best[1] = pu[1]; best[2] = pu[2];
+    cost = s_qeval(q, best);
+  } else if (bv) {
+    e->keep = v;
+    e->remove = u;
+    best[0] = pv[0]; best[1] = pv[1]; best[2] = pv[2];
+    cost = s_qeval(q, best);
+  } else {
+    e->keep = u < v ? u : v;
+    e->remove = u < v ? v : u;
+    const double* pk = u < v ? pu : pv;
+    const double* pr = u < v ? pv : pu;
+    const double kk[3] = {pk[0], pk[1], pk[2]}, rr[3] = {pr[0], pr[1], pr[2]};
+    const double mid[3] = {(kk[0] + rr[0]) * 0.5, (kk[1] + rr[1]) * 0.5, (kk[2] + rr[2]) * 0.5};
+    const double ck = s_qeval(q, kk), cr = s_qeval(q, rr), cm = s_qeval(q, mid);
+    cost = ck;
+    best[0] = kk[0]; best[1] = kk[1]; best[2] = kk[2];
+    if (cr < cost) { cost = cr; best[0] = rr[0]; best[1] = rr[1]; best[2] = rr[2]; }
+    if (cm < cost) { cost = cm; best[0] = mid[0]; best[1] = mid[1]; best[2] = mid[2]; }
+  }
+  if (cost < 0.0) cost = 0.0;
+  if (!(cost <= max_err2)) return;
+  e->valid = true;
+  e->cost = cost;
+  e->p[0] = best[0]; e->p[1] = best[1]; e->p[2] = best[2];
+}
+
 // ------------------------------------------------------------------ kernels
 __global__ void __launch_bounds__(256)
     k_simp_init_verts(const uint64_t* __restrict__ vkeys, uint64_t U, double rx, double ry, double rz,
@@ -224,6 +269,38 @@ __global__ void __launch_bounds__(256) k_simp_boundary(Simp s) {
   }
 }
 
+// Initial cost of every canonical half-edge (u < v; label-local order is the global one): the float cost in
+// ecost and the memo of the half-edge in the face's state byte (2 cached, 3 exceeds max_error), which the
+// label kernel's load takes over.  One thread per face, so that the byte has a single writer.  counts[0]
+// += evaluations.
+__global__ void __launch_bounds__(256)
+    k_simp_ecost(Simp s, double max_err2, float* __restrict__ ecost, uint8_t* __restrict__ fstate,
+                 uint32_t* counts) {
+  const uint64_t f = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  uint32_t n = 0;
+  if (f < s.T) {
+    const uint32_t* fv = s.face + 3 * f;
+    uint32_t st = 0;
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+      const uint32_t u = fv[c], v = fv[(c + 1) % 3];
+      if (!(u < v)) continue;
+      SEval ev;
+      s_cost(s.Q, s.pos, max_err2, u, v, u, v, s.vbound[u] != 0, s.vbound[v] != 0, &ev);
+      uint32_t es = 3;
+      if (ev.valid) {
+        ecost[3 * f + c] = __double2float_rn(ev.cost);
+        es = 2;
+      }
+      st |= es << (2 * c);
+      n++;
+    }
+    fstate[f] = (uint8_t)st;
+  }
+  const int tot = __syncthreads_count(n & 1u) + 2 * __syncthreads_count(n >> 1);
+  if (threadIdx.x == 0 && tot) atomicAdd(counts, (uint32_t)tot);
+}
+
 // ------------------------------------------------------------------ per-label rounds
 // One CTA owns one label for ALL of its rounds (labels are independent: keys use
 // label-local half-edge ids and the stop rules are per label).  The topology of the
@@ -235,10 +312,9 @@ __global__ void __launch_bounds__(256) k_simp_boundary(Simp s) {
 // __syncthreads() phases instead of five launches and a host round trip:
 //
 //   P1  key1[v] = MAX, lose[v] = 0                             (vertex parallel)
-//   P2  every canonical half-edge (u < v) of an alive face posts its key to both
-//       endpoints with a shared-memory min reduction; the float cost is memoised until
-//       an endpoint moves (CDIRTY); dropped memos are re-evaluated by per-warp queues on
-//       dense lanes while other warps keep posting                (face parallel)
+//   P2  every canonical half-edge (u < v) of an alive face posts its cached key to both
+//       endpoints with a shared-memory min reduction (the float costs come from k_simp_ecost
+//       and E2d; P2 evaluates none)                                (face parallel)
 //   P3  a vertex LOSEs if a face neighbour holds a smaller key1 (== key2 test of the
 //       round formulation: key2[w] == key1[w] <=> !LOSE[w]); plain byte stores
 //                                                               (face parallel)
@@ -250,21 +326,20 @@ __global__ void __launch_bounds__(256) k_simp_boundary(Simp s) {
 //   E2b one flip test per (winner, side, ring face)              (item parallel)
 //   E2c link condition by ballots / shuffles over the ring lists and the collapse
 //       itself, one HALF warp per winner (whole warps for rings over 16 faces)
+//   E2d the canonical half-edges of each collapse's kept vertex are re-costed (item parallel)
 //
-// Labels that do not fit (more than 16384 faces, or 6U + 9T + 28 KB over the CTA's shared
+// Labels that do not fit (more than 16384 faces, or 6U + 9T + 23 KB over the CTA's shared
 // memory) keep faces and lists in global memory, with keys / flags / states still in
 // shared memory when those fit ("hybrid"), else everything global (SM = false, 64-bit
 // key slots).
-// vertex flags: CDIRTY the vertex moved (cached costs of its edges are stale), RDIRTY its ring
-// changed (parked edges around it may be valid now)
-constexpr uint32_t VF_ALIVE = 1, VF_BOUND = 2, VF_CDIRTY = 4, VF_DONE = 16, VF_END = 32, VF_RDIRTY = 64;
+// vertex flags: RDIRTY the vertex's ring changed (parked edges around it may be valid now)
+constexpr uint32_t VF_ALIVE = 1, VF_BOUND = 2, VF_DONE = 16, VF_END = 32, VF_RDIRTY = 64;
 constexpr int SL_THREADS = 1024;
 // winners validated per selection pass (a round runs as many passes as it needs): every label that fits a
 // class has room for SL_WCAP; a shared-memory label takes more where the class's shared memory leaves room
 // (sl_wcap), since each further pass rescans the vertices (P4) and the alive faces (E1)
 constexpr int SL_WCAP = 128;
-constexpr uint32_t WF_BAD = 1, WF_OK = 2;  // winner flags: failed validation / validated
-constexpr int SL_EQ = 96;      // per-warp queue of faces with half-edges whose cost must be (re)computed
+constexpr uint32_t WF_BAD = 1, WF_OK = 2, WF_DONE = 4;  // winner flags: failed validation / validated / collapsed
 constexpr int SL_LIST_PER = 16;  // list entries per thread held in registers while a list is compacted in place
 
 // Size classes of k_simp_labels: CTA size and CTAs per SM.  A label runs in the smallest class whose
@@ -282,16 +357,15 @@ struct SlWin {
 constexpr size_t SL_WIN_BYTES = sizeof(SlWin) + 2 * S_MAXV * 2;
 
 // dynamic shared-memory layout of a label at `threads` threads with `wcap` winners per pass:
-// winners | cost queues | ring lists | key1 | faces SoA | face list | face state | vertex flags | lose marks
+// winners | ring lists | key1 | faces SoA | face list | face state | vertex flags | lose marks
 // [| original face ids | original vertex ids: a label resumed in a smaller class after migrating]
 struct SlLayout {
-  size_t o_wq, o_ring, o_key, o_f0, o_fl, o_fs, o_vf, o_vl, o_fm, o_vm, need;
+  size_t o_ring, o_key, o_f0, o_fl, o_fs, o_vf, o_vl, o_fm, o_vm, need;
 };
-__host__ __device__ inline SlLayout sl_layout(uint32_t T, uint32_t U, uint32_t threads, bool resumed = false,
+__host__ __device__ inline SlLayout sl_layout(uint32_t T, uint32_t U, bool resumed = false,
                                               uint32_t wcap = SL_WCAP) {
   SlLayout y;
-  y.o_wq = (size_t)wcap * sizeof(SlWin);
-  y.o_ring = y.o_wq + (size_t)(threads / 32) * SL_EQ * 4;
+  y.o_ring = (size_t)wcap * sizeof(SlWin);
   y.o_key = y.o_ring + (size_t)wcap * 2 * S_MAXV * 2;  // shared-memory class: 16-bit face ids in the rings
   y.o_f0 = y.o_key + 4 * (size_t)U;                    // 32-bit keys
   y.o_fl = y.o_f0 + 6 * (size_t)T;
@@ -307,13 +381,13 @@ __host__ __device__ inline SlLayout sl_layout(uint32_t T, uint32_t U, uint32_t t
 __host__ __device__ inline bool sl_fits_smem(uint32_t T, uint32_t U, uint32_t threads, size_t smem_bytes,
                                              bool resumed = false) {
   const uint32_t cap = (uint32_t)SL_LIST_PER * threads;
-  return 3ull * T <= 65536ull && T <= cap && U <= cap && sl_layout(T, U, threads, resumed).need <= smem_bytes;
+  return 3ull * T <= 65536ull && T <= cap && U <= cap && sl_layout(T, U, resumed).need <= smem_bytes;
 }
 // winners per pass of a label that sl_fits_smem accepts: SL_WCAP plus what the rest of the budget holds, at
 // most one per thread (E2a gives each winner a thread) and at most `limit` (IGN_SIMP_WCAP)
 __host__ __device__ inline uint32_t sl_wcap(uint32_t T, uint32_t U, uint32_t threads, size_t smem_bytes,
                                             bool resumed, uint32_t limit) {
-  const size_t w = SL_WCAP + (smem_bytes - sl_layout(T, U, threads, resumed).need) / SL_WIN_BYTES;
+  const size_t w = SL_WCAP + (smem_bytes - sl_layout(T, U, resumed).need) / SL_WIN_BYTES;
   const size_t m = threads < limit ? threads : limit;
   return (uint32_t)(w < m ? w : m);
 }
@@ -343,6 +417,9 @@ struct SlArgs {
   uint32_t* counters;  // [1] max rounds  [2] labels run in shared memory  [3] in global memory
                        // [4 + class] next work item  [8 + class] labels run in the class
                        // [16 + class] labels migrated into the class  [20 + class] next migrated label to resume
+                       // [24] multi-pass label-rounds  [25] winners with a ring over S_MAXV faces
+                       // [26] initial cost evaluations (k_simp_ecost)  [27] re-costs after collapses (E2d)
+                       // [28] canonical half-edges without a cost met by the key pass (always 0)
   double max_err2;
   int max_rounds;
   uint32_t smem_bytes;  // dynamic shared memory of the launch
@@ -371,13 +448,15 @@ constexpr int SL_HIST = 1664, SL_HP = 16, SL_HW = 64, SL_HR = S_MAXV + 2, SL_HCL
 // header of a migrated label: dense label, trace record, next round, slow rounds, alive faces, alive vertices
 constexpr int SL_MREC = 8;
 constexpr int SL_LREC = 7;  // words of a label's IGN_SIMP_TRACE record (SlArgs::lrec)
+constexpr int SL_NPH = 11;  // IGN_SIMP_TRACE phase timers (trace words 1600.., 64 bits each)
 
 struct SlShared {
   uint32_t work, alive, progress, ncol, nwin, stop, slow, counter, nbig, npass, bigring;
   uint32_t rec, valive;  // trace record of the label; alive vertices (one dies per collapse)
   unsigned long long visits, wins;  // IGN_SIMP_TRACE
   long long t_label;
-  unsigned long long ph[10];  // phase timers (IGN_SIMP_TRACE)
+  uint32_t nrecost;  // half-edges re-costed after collapses (E2d)
+  unsigned long long ph[SL_NPH];  // phase timers (IGN_SIMP_TRACE)
   long long t_prev;
 };
 
@@ -398,7 +477,6 @@ struct SlLab {
   key_t* key1;
   bool fmt16;
   uint32_t wcap;   // winners per selection pass (their records are at the start of the dynamic shared memory)
-  uint32_t* wq;    // [warps][SL_EQ] per-warp cost queues of the key pass (shared memory)
   idx_t* ring;     // [wcap][2][S_MAXV] face ids of the winners' rings (shared memory)
   idx_t *flist, *flist2, *vlist, *vlist2;  // alive lists (flist2 / vlist2: global-memory class only)
 };
@@ -475,49 +553,38 @@ __device__ __forceinline__ uint32_t sl_key_edge(const SlLab<SM>& L, typename SlL
   return s_unmix((uint32_t)((unsigned long long)key & 0xFFFFFFFFull)) ^ salt;
 }
 
-// s_cost on label-local ids (same arithmetic, same order)
+// s_cost on label-local ids
 template <bool SM, bool R>
 __device__ __forceinline__ void sl_cost(const SlArgs& A, const SlLab<SM>& L, uint32_t u, uint32_t v, SEval* e) {
-  e->valid = false;
-  const bool bu = L.vflag[u] & VF_BOUND, bv = L.vflag[v] & VF_BOUND;
-  if (bu && bv) return;
-  const uint64_t gu = sl_vg<SM, R>(L, u), gv = sl_vg<SM, R>(L, v);
-  const double* Qu = A.Q + 10 * gu;
-  const double* Qv = A.Q + 10 * gv;
-  double q[10];
+  s_cost(A.Q, A.pos, A.max_err2, u, v, sl_vg<SM, R>(L, u), sl_vg<SM, R>(L, v), (L.vflag[u] & VF_BOUND) != 0,
+         (L.vflag[v] & VF_BOUND) != 0, e);
+}
+
+// Re-cost the canonical half-edges of face f that hold the kept vertex k of a collapse (k -> o1 when k < o1,
+// o2 -> k when o2 < k): cached float cost and memo (2 cached, 3 exceeds max_error).  Returns the face's new
+// state byte; the caller stores it (a face is in exactly one ring list: a single writer).
+template <bool SM, bool R>
+__device__ __forceinline__ uint32_t sl_recost(const SlArgs& A, const SlLab<SM>& L, uint32_t f, uint32_t st,
+                                              uint32_t k, uint32_t* nev) {
+  const uint32_t a[3] = {sl_fget<SM>(L, f, 0), sl_fget<SM>(L, f, 1), sl_fget<SM>(L, f, 2)};
+  const uint32_t ck = a[0] == k ? 0u : (a[1] == k ? 1u : 2u);
+  float* ec = A.ecost + 3 * (uint64_t)(L.tbase + sl_fo<SM, R>(L, f));
 #pragma unroll
-  for (int i = 0; i < 10; i++) q[i] = Qu[i] + Qv[i];
-  const double* pu = A.pos + 3 * gu;
-  const double* pv = A.pos + 3 * gv;
-  double best[3], cost;
-  if (bu) {
-    e->keep = u;
-    e->remove = v;
-    best[0] = pu[0]; best[1] = pu[1]; best[2] = pu[2];
-    cost = s_qeval(q, best);
-  } else if (bv) {
-    e->keep = v;
-    e->remove = u;
-    best[0] = pv[0]; best[1] = pv[1]; best[2] = pv[2];
-    cost = s_qeval(q, best);
-  } else {
-    e->keep = u < v ? u : v;
-    e->remove = u < v ? v : u;
-    const double* pk = u < v ? pu : pv;
-    const double* pr = u < v ? pv : pu;
-    const double kk[3] = {pk[0], pk[1], pk[2]}, rr[3] = {pr[0], pr[1], pr[2]};
-    const double mid[3] = {(kk[0] + rr[0]) * 0.5, (kk[1] + rr[1]) * 0.5, (kk[2] + rr[2]) * 0.5};
-    const double ck = s_qeval(q, kk), cr = s_qeval(q, rr), cm = s_qeval(q, mid);
-    cost = ck;
-    best[0] = kk[0]; best[1] = kk[1]; best[2] = kk[2];
-    if (cr < cost) { cost = cr; best[0] = rr[0]; best[1] = rr[1]; best[2] = rr[2]; }
-    if (cm < cost) { cost = cm; best[0] = mid[0]; best[1] = mid[1]; best[2] = mid[2]; }
+  for (int t = 0; t < 2; t++) {
+    const uint32_t c = t == 0 ? ck : (ck + 2) % 3;  // the corners of k -> o1 and o2 -> k
+    const uint32_t u = a[c], v = a[(c + 1) % 3];
+    if (!(u < v)) continue;
+    SEval ev;
+    sl_cost<SM, R>(A, L, u, v, &ev);
+    uint32_t es = 3;
+    if (ev.valid) {
+      ec[c] = __double2float_rn(ev.cost);
+      es = 2;
+    }
+    st = (st & ~(3u << (2 * c))) | (es << (2 * c));
+    (*nev)++;
   }
-  if (cost < 0.0) cost = 0.0;
-  if (!(cost <= A.max_err2)) return;
-  e->valid = true;
-  e->cost = cost;
-  e->p[0] = best[0]; e->p[1] = best[1]; e->p[2] = best[2];
+  return st;
 }
 
 // does face (a0,a1,a2) flip when vertex w moves to `best`?  (the validation's flip test)
@@ -755,7 +822,7 @@ __device__ __forceinline__ void sl_collapse_pass(const SlArgs& A, const SlLab<SM
       if (gl < 10) Qk[gl] = qk + qr;
       if (gl >= 10 && gl < 13) A.pos[3 * gk + (gl - 10)] = win[slot].best[gl - 10];
       if (gl == 0) {
-        sl_vor<SM>(L.vflag, k, VF_CDIRTY | VF_RDIRTY);  // k moved: cached costs of its edges are stale
+        win[slot].flags |= WF_DONE;  // k moved: E2d re-costs its edges
         sl_vclear<SM>(L.vflag, k, VF_END);
         sl_vclear<SM>(L.vflag, rm, 0xFFu);
         atomicSub(&sh.alive, dead);
@@ -774,8 +841,9 @@ __device__ void sl_migrate(const SlArgs& A, const SlLab<true>& L, SlShared& sh, 
                            int r) {
   const uint32_t FULL = 0xFFFFFFFFu;
   const uint32_t tid = threadIdx.x, NT = blockDim.x, lane = tid & 31u, warp = tid >> 5, NW = NT >> 5;
-  // block-wide exclusive scan of the alive vertices over contiguous chunks (the cost queues are free
-  // between rounds and hold the warp totals)
+  // block-wide exclusive scan of the alive vertices over contiguous chunks (the winner records and ring
+  // lists are free between rounds and hold the warp totals: 184 bytes or more, 4 per warp)
+  uint32_t* const wsum = (uint32_t*)sl_win();
   const uint32_t per = (L.U + NT - 1) / NT, v0 = min(tid * per, L.U), v1 = min(v0 + per, L.U);
   uint32_t cnt = 0;
   for (uint32_t v = v0; v < v1; v++) cnt += L.vflag[v] & VF_ALIVE;
@@ -785,20 +853,20 @@ __device__ void sl_migrate(const SlArgs& A, const SlLab<true>& L, SlShared& sh, 
     const uint32_t o = __shfl_up_sync(FULL, inc, d);
     if ((int)lane >= d) inc += o;
   }
-  if (lane == 31) L.wq[warp] = inc;
+  if (lane == 31) wsum[warp] = inc;
   __syncthreads();
   if (warp == 0) {
-    const uint32_t t = lane < NW ? L.wq[lane] : 0u;
+    const uint32_t t = lane < NW ? wsum[lane] : 0u;
     uint32_t x = t;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
       const uint32_t o = __shfl_up_sync(FULL, x, d);
       if ((int)lane >= d) x += o;
     }
-    if (lane < NW) L.wq[lane] = x - t;
+    if (lane < NW) wsum[lane] = x - t;
   }
   __syncthreads();
-  uint32_t j = L.wq[warp] + inc - cnt;
+  uint32_t j = wsum[warp] + inc - cnt;
   for (uint32_t v = v0; v < v1; v++) {
     const uint32_t fl = L.vflag[v];
     if (!(fl & VF_ALIVE)) continue;
@@ -827,8 +895,9 @@ __device__ void sl_migrate(const SlArgs& A, const SlLab<true>& L, SlShared& sh, 
 // All rounds of one label (R: a label resumed from the header `hdr` after it migrated from a larger class)
 template <bool SM, bool R>
 __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const uint32_t* hdr) {
+  if (threadIdx.x == 0) sh.nrecost = 0;
   if (A.trace != nullptr && threadIdx.x == 0) {
-    for (int q = 0; q < 10; q++) sh.ph[q] = 0;
+    for (int q = 0; q < SL_NPH; q++) sh.ph[q] = 0;
     sh.t_prev = clock64();
     sh.t_label = sh.t_prev;
     sh.visits = 0;
@@ -871,7 +940,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
         sl_fset<SM>(L, f, 1, g[1] - L.vbase);
         sl_fset<SM>(L, f, 2, g[2] - L.vbase);
       }
-      L.fstate[f] = 0x80;
+      L.fstate[f] = (uint8_t)(0x80u | A.fstate[L.tbase + f]);  // alive, memos of k_simp_ecost
       flist[f] = (idx_t)f;
     }
     for (uint32_t v = tid; v < U; v += NT) {
@@ -914,11 +983,9 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
     __syncthreads();
     SL_MARK(0);
     // ---- P2: keys of the canonical half-edges.  A warp takes 32 alive faces per iteration and
-    // posts the cached keys; faces with half-edges whose memoised state was dropped collect in
-    // a per-warp queue that is evaluated (double precision cost) on dense lanes.
+    // posts the cached keys.  No cost is evaluated here: k_simp_ecost costs every half-edge before
+    // the first round and E2d re-costs the edges of every vertex that moved right after its collapse.
     {
-      uint32_t* wq = L.wq + warp * SL_EQ;
-      uint32_t qn = 0;  // faces in the warp's queue (warp uniform)
       // software pipeline: the face id and the three cached costs of the NEXT iteration are
       // requested (global loads, L2 latency) before the current face is processed
       const float* ecb = A.ecost + 3 * (uint64_t)L.tbase;
@@ -945,59 +1012,23 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
           a[0] = sl_fget<SM>(L, f, 0); a[1] = sl_fget<SM>(L, f, 1); a[2] = sl_fget<SM>(L, f, 2);
           fl[0] = L.vflag[a[0]]; fl[1] = L.vflag[a[1]]; fl[2] = L.vflag[a[2]];
         }
-        uint32_t pend = 0, nst = st;
         if (act) {
+          uint32_t nst = st;
 #pragma unroll
           for (int c = 0; c < 3; c++) {
             const uint32_t u = a[c], v = a[(c + 1) % 3];
             const uint32_t fe = fl[c] | fl[(c + 1) % 3];
             if (!(u < v)) continue;  // one key per edge
-            // memo: 0 unknown, 1 parked (won a round, failed validation), 2 cost cached in
-            // ecost, 3 known to exceed max_error.  2 / 3 are dropped when an endpoint moved
-            // (CDIRTY), 1 when an endpoint's ring changed (RDIRTY).
+            // memo: 1 parked (won a round, failed validation), 2 cost cached in ecost, 3 known to
+            // exceed max_error.  A parked edge is un-parked when an endpoint's ring changed (RDIRTY):
+            // its cost was cached when it won, and an endpoint that moved since would have re-costed it.
             uint32_t es = (st >> (2 * c)) & 3u;
-            if (es >= 2 && (fe & VF_CDIRTY)) es = 0;
-            else if (es == 1 && (fe & VF_RDIRTY)) es = 0;
-            if (es == 0) {
-              pend |= 1u << c;
-            } else if (es == 2) {
-              sl_post(L.key1, u, v, sl_key<SM>(L, ec[c], 3u * fo + (uint32_t)c, salt));
-            }
+            if (es == 1 && (fe & VF_RDIRTY)) es = 2;
+            if (es == 2) sl_post(L.key1, u, v, sl_key<SM>(L, ec[c], 3u * fo + (uint32_t)c, salt));
+            else if (es == 0) atomicAdd(&A.counters[28], 1u);  // a half-edge without a cost: a bug
             nst = (nst & ~(3u << (2 * c))) | (es << (2 * c));
           }
-        }
-        if (act && nst != st) L.fstate[f] = (uint8_t)nst;  // pending corners hold memo 0 until they are evaluated
-        // faces with pending corners accumulate in the warp's queue over the iterations; the
-        // queue is evaluated when the next iteration might not fit (>= 3 dense passes) and at the end
-        const uint32_t has = pend ? 1u : 0u;
-        const uint32_t bal = __ballot_sync(FULL, has);
-        if (has) wq[qn + __popc(bal & ((1u << lane) - 1u))] = (f << 3) | pend;
-        qn += __popc(bal);
-        const bool last = base + NT >= nF;
-        if (qn > (uint32_t)SL_EQ - 32 || (last && qn)) {
-          __syncwarp();
-          for (uint32_t j = lane; j < qn; j += 32) {
-            const uint32_t e = wq[j], ef = e >> 3, ep = e & 7u, efo = sl_fo<SM, R>(L, ef);
-            uint32_t est = L.fstate[ef];
-#pragma unroll
-            for (int c = 0; c < 3; c++) {
-              if (!((ep >> c) & 1u)) continue;
-              const uint32_t u = sl_fget<SM>(L, ef, c), v = sl_fget<SM>(L, ef, (c + 1) % 3);
-              SEval ev;
-              sl_cost<SM, R>(A, L, u, v, &ev);
-              uint32_t es = 3;  // exceeds max_error
-              if (ev.valid) {
-                const float cf = __double2float_rn(ev.cost);
-                A.ecost[3 * (uint64_t)(L.tbase + efo) + c] = cf;
-                es = 2;
-                sl_post(L.key1, u, v, sl_key<SM>(L, cf, 3u * efo + (uint32_t)c, salt));
-              }
-              est = (est & ~(3u << (2 * c))) | (es << (2 * c));
-            }
-            L.fstate[ef] = (uint8_t)est;  // the queue holds a face once: single writer
-          }
-          __syncwarp();
-          qn = 0;
+          if (nst != st) L.fstate[f] = (uint8_t)nst;
         }
       }
     }
@@ -1006,7 +1037,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
     // ---- P3: dirty flags consumed; LOSE = a face neighbour holds a smaller key
     for (uint32_t i = tid; i < nV; i += NT) {
       const uint32_t v = SM ? i : (uint32_t)vlist[i];
-      if (L.vflag[v] & (VF_CDIRTY | VF_RDIRTY)) sl_vclear<SM>(L.vflag, v, VF_CDIRTY | VF_RDIRTY);
+      if (L.vflag[v] & VF_RDIRTY) sl_vclear<SM>(L.vflag, v, VF_RDIRTY);
     }
     // two faces per thread and iteration, the loads of both issued before anything depends on them
     for (uint32_t i = tid; i < nF; i += 2 * NT) {
@@ -1164,6 +1195,27 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
       }
       __syncthreads();
       SL_MARK(8);
+      // E2d: the kept vertex k of every collapse has its final quadric and position, and so do its
+      // neighbours (winners are two apart, in this pass and in the later passes of the round), so the
+      // costs of k's edges are final until the next round: re-cost them now, one item per (winner, side,
+      // ring entry) as in E2b.  Every alive face of the two ring lists holds k, and each is in one list.
+      {
+        uint32_t nev = 0;
+        for (uint32_t j0 = 0; j0 < (uint32_t)S_MAXV; j0 += 16) {
+          if (j0 != 0 && !sh.bigring) break;
+          for (uint32_t item = tid; item < nb * 32; item += NT) {
+            const uint32_t i = item >> 5, side = (item >> 4) & 1u, j = j0 + (item & 15u);
+            if (!(win[i].flags & WF_DONE) || j >= win[i].cnt[side]) continue;
+            const uint32_t f = L.ring[(2 * i + side) * S_MAXV + j];
+            const uint32_t st = L.fstate[f];
+            if (!(st & 0x80u)) continue;  // died with the edge
+            L.fstate[f] = (uint8_t)sl_recost<SM, R>(A, L, f, st, win[i].keep, &nev);
+          }
+        }
+        if (nev) atomicAdd(&sh.nrecost, nev);
+      }
+      __syncthreads();  // (the next pass resets sh.bigring and the winner records)
+      SL_MARK(10);
       if (total <= L.wcap) break;
     }
     if (tid == 0) {
@@ -1232,7 +1284,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
   }
   if (tid == 0 && A.trace != nullptr) {
     // a migrated label's record sums the cycles, visits and winners of all its segments
-    for (int q = 0; q < 10; q++) atomicAdd((unsigned long long*)(A.trace + 1600) + q, sh.ph[q]);
+    for (int q = 0; q < SL_NPH; q++) atomicAdd((unsigned long long*)(A.trace + 1600) + q, sh.ph[q]);
     uint32_t* rec = A.lrec + SL_LREC * (size_t)sh.rec;
     const unsigned long long vis = rec[3] + sh.visits;
     const uint32_t kc = (uint32_t)((clock64() - sh.t_label) >> 10);
@@ -1245,6 +1297,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
     if (!R) rec[5] = (SM ? 1u : ((const void*)L.key1 == (const void*)(A.key1 + L.vbase) ? 3u : 2u)) | (A.cls << 2);
   }
   if (tid == 0) {
+    if (sh.nrecost) atomicAdd(&A.counters[27], sh.nrecost);
     if (!migrated) atomicMax(&A.counters[1], (uint32_t)r);
     if (!R) {  // a label counts in the class it started in
       atomicAdd(&A.counters[SM ? 2 : 3], 1u);
@@ -1276,11 +1329,10 @@ __global__ void __launch_bounds__(SL_THREADS, 1) k_simp_labels(SlArgs A) {
     const bool fmt16 = 3ull * T <= 65536ull;
     if (sl_fits_smem(T, U, blockDim.x, A.smem_bytes)) {
       const uint32_t wcap = sl_wcap(T, U, blockDim.x, A.smem_bytes, false, A.wcap_max);
-      const SlLayout y = sl_layout(T, U, blockDim.x, false, wcap);
+      const SlLayout y = sl_layout(T, U, false, wcap);
       SlLab<true> L;
       L.T = T; L.U = U; L.tbase = tbase; L.vbase = vbase; L.target = target;
       L.wcap = wcap;
-      L.wq = (uint32_t*)(sl_smem + y.o_wq);
       L.ring = (uint16_t*)(sl_smem + y.o_ring);
       L.key1 = (uint32_t*)(sl_smem + y.o_key);
       L.fmt16 = true;
@@ -1298,15 +1350,14 @@ __global__ void __launch_bounds__(SL_THREADS, 1) k_simp_labels(SlArgs A) {
       L.fmap = L.vmap = nullptr;
       sl_run<true, false>(A, L, sh, nullptr);
     } else {
-      const SlLayout y = sl_layout(T, U, blockDim.x);
+      const SlLayout y = sl_layout(T, U);
       const size_t o_keyg = y.o_ring + (size_t)SL_WCAP * 2 * S_MAXV * 4;  // 32-bit face ids in the rings
       SlLab<false> L;
       L.T = T; L.U = U; L.tbase = tbase; L.vbase = vbase; L.target = target;
       L.label = l;
       L.fmap = L.vmap = nullptr;
       L.wcap = SL_WCAP < A.wcap_max ? SL_WCAP : A.wcap_max;
-      L.wq = (uint32_t*)(sl_smem + y.o_wq);  // the winners, the cost queues and the ring lists always fit
-      L.ring = (uint32_t*)(sl_smem + y.o_ring);
+      L.ring = (uint32_t*)(sl_smem + y.o_ring);  // the winners and the ring lists always fit
       L.fc0 = L.fc1 = L.fc2 = nullptr;
       L.flist = A.flist + tbase; L.flist2 = A.flist2 + tbase;
       L.vlist = A.vlist + vbase; L.vlist2 = A.vlist2 + vbase;
@@ -1351,12 +1402,11 @@ __global__ void __launch_bounds__(SL_THREADS / 2, 2) k_simp_resume(SlArgs A) {
     const uint32_t l = hdr[0];
     const uint32_t T = hdr[4], U = hdr[5];
     const uint32_t wcap = sl_wcap(T, U, blockDim.x, A.smem_bytes, true, A.wcap_max);
-    const SlLayout y = sl_layout(T, U, blockDim.x, true, wcap);
+    const SlLayout y = sl_layout(T, U, true, wcap);
     SlLab<true> L;
     L.T = T; L.U = U; L.tbase = A.tri_off[l]; L.vbase = A.vert_off[l]; L.target = A.target[l];
     L.label = l;
     L.wcap = wcap;
-    L.wq = (uint32_t*)(sl_smem + y.o_wq);
     L.ring = (uint16_t*)(sl_smem + y.o_ring);
     L.key1 = (uint32_t*)(sl_smem + y.o_key);
     L.fmt16 = true;
@@ -1448,6 +1498,7 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   m->simp_labels_smem = m->simp_labels_gmem = 0;
   for (int c = 0; c < SL_NCLASS; c++) m->simp_labels_class[c] = m->simp_migrations[c] = 0;
   m->simp_passes[0] = m->simp_passes[1] = 0;
+  m->simp_costs[0] = m->simp_costs[1] = m->simp_costs[2] = 0;
   const uint64_t U = m->U, T = m->T, K = m->K;
   if (T == 0 || U == 0) {
     m->simplified = true;
@@ -1559,6 +1610,8 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
              flags + 12);
   IGN_LAUNCH(ctx, k_simp_quadrics, blocks_for(U, 128), 128, 0, s);
   IGN_LAUNCH(ctx, k_simp_boundary, blocks_for(3 * T, 256), 256, 0, s);
+  const double max_err2 = (double)max_error * (double)max_error;
+  IGN_LAUNCH(ctx, k_simp_ecost, blocks_for(T, 256), 256, 0, s, max_err2, ecost, fstate, flags + 26);
 
   // ---- all rounds of every label: one launch per size class, one CTA per label.  The kernel is
   // latency and barrier bound, so labels that fit half (a quarter) of an SM's shared memory run two
@@ -1571,7 +1624,7 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   A.flist = gl_f[0]; A.flist2 = gl_f[1]; A.vlist = gl_v[0]; A.vlist2 = gl_v[1];
   A.tri_off = d_tri_off; A.vert_off = d_vert_off; A.target = d_target;
   A.counters = flags;
-  A.max_err2 = (double)max_error * (double)max_error;
+  A.max_err2 = max_err2;
   A.max_rounds = 400;
   // IGN_SIMP_GMEM=1 (test knob): run every label on the global-memory arrays, the path of
   // labels that do not fit shared memory (only the winners' ring lists stay in smem)
@@ -1695,13 +1748,15 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   if (A.trace) {
     std::vector<uint32_t> tr(1600);
     IGN_CUDA(cudaMemcpy(tr.data(), A.trace, 1600 * 4, cudaMemcpyDeviceToHost));
-    unsigned long long phs[10];
-    IGN_CUDA(cudaMemcpy(phs, A.trace + 1600, 80, cudaMemcpyDeviceToHost));
-    static const char* names[10] = {"P1", "P2 keys", "P3 lose", "P4 select", "setup", "E1 rings", "E2a cost", "E2b flips", "E2c link+collapse", "stop+compact"};
+    unsigned long long phs[SL_NPH];
+    IGN_CUDA(cudaMemcpy(phs, A.trace + 1600, sizeof(phs), cudaMemcpyDeviceToHost));
+    static const char* names[SL_NPH] = {"P1", "P2 keys", "P3 lose", "P4 select", "setup", "E1 rings", "E2a cost", "E2b flips", "E2c link+collapse", "stop+compact", "E2d recost"};
     unsigned long long tot = 0;
-    for (int q = 0; q < 10; q++) tot += phs[q];
-    for (int q = 0; q < 10; q++)
+    for (int q = 0; q < SL_NPH; q++) tot += phs[q];
+    for (int q = 0; q < SL_NPH; q++)
       fprintf(stderr, "phase %-18s %6.2f %%  %10.3f Mcycles\n", names[q], 100.0 * phs[q] / (tot ? tot : 1), phs[q] / 1e6);
+    fprintf(stderr, "cost evaluations: %u initial (k_simp_ecost), %u after collapses (E2d), %u half-edges without a cost in P2\n",
+            hflags[26], hflags[27], hflags[28]);
     {
       // per-label records: where do the cycles go -- per round (fixed latency) or per face visit?
       std::vector<uint32_t> rec(SL_LREC * (size_t)K);
@@ -1769,6 +1824,7 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   for (int c = 0; c < SL_NCLASS; c++) m->simp_migrations[c] = hflags[16 + c];
   m->simp_passes[0] = hflags[24];
   m->simp_passes[1] = hflags[25];
+  for (int i = 0; i < 3; i++) m->simp_costs[i] = hflags[26 + i];
   const uint32_t U2 = last[0] + last[1], T2 = last[2] + last[3];
   IGN_LAUNCH(ctx, k_simp_new_offsets, blocks_for(K + 2, 256), 256, 0, d_vert_off, vscan, (uint32_t)(K + 2), U, U2,
                    d_new_vert_off);
@@ -1813,5 +1869,12 @@ extern "C" int ign_mesh_simplify_passes(ign_mesher* m, uint32_t counts[2]) {
   IGN_REQUIRE(m->simplified, IGN_ERR_INVALID, "mesher is not simplified");
   counts[0] = m->simp_passes[0];
   counts[1] = m->simp_passes[1];
+  return IGN_OK;
+}
+
+extern "C" int ign_mesh_simplify_costs(ign_mesher* m, uint32_t counts[3]) {
+  IGN_REQUIRE(m && counts, IGN_ERR_INVALID, "null argument");
+  IGN_REQUIRE(m->simplified, IGN_ERR_INVALID, "mesher is not simplified");
+  for (int i = 0; i < 3; i++) counts[i] = m->simp_costs[i];
   return IGN_OK;
 }

@@ -399,6 +399,10 @@ IGN_API int ign_mesh_simplify_migrations(ign_mesher* m, uint32_t resumed[3]);
  * validation pass (more winners than the label's per-pass capacity), [1] winners rejected because an
  * endpoint had more than 32 alive incident faces */
 IGN_API int ign_mesh_simplify_passes(ign_mesher* m, uint32_t counts[2]);
+/* edge-cost counters of the simplification that ran: [0] half-edges costed before the first round,
+ * [1] half-edges re-costed after the collapse that moved an endpoint, [2] half-edges the key pass met
+ * without a cached cost (0 unless the simplifier is broken; such an edge posts no key) */
+IGN_API int ign_mesh_simplify_costs(ign_mesher* m, uint32_t counts[3]);
 /* bulk export of every label's mesh (simplified if ign_mesh_simplify ran) in ign_mesh_ids order:
  * vertices f32 [U,3], faces u32 [T,3] (label-local indices), offsets [n_ids+1] */
 IGN_API int ign_mesh_export(ign_mesher* m, const float resolution[3], int voxel_centered,
