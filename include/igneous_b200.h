@@ -359,6 +359,65 @@ IGN_API int ign_edt(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, ui
 IGN_API int ign_edt_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
                         const float anisotropy[3], int black_border, int squared, float* out);
 
+/* ------------------------------------------------ geodesic distances and parents
+ * dijkstra3d.euclidean_distance_field / distance_field / parental_field, as kimimaro's TEASAR calls them
+ *   once per label on a cutout (SkeletonTask, igneous/tasks/skeleton.py:54, :312): here for every label
+ *   of an (sx, sy, sz) volume of u8 / u16 / u32 / u64 labels in the same launches.  The rule of DESIGN.md
+ *   §5e (dijkstra3d parity unpinned): voxels p, q are joined when they are neighbours under `connectivity`
+ *   (6, 18 or 26) and labels[p] == labels[q] != 0.  dist[source] = 0, every step is one float32 addition
+ *   d[q] = fl32(d[p] + w(p -> q)), and dist[q] is the least such value over all paths from any source of
+ *   q's label; +inf on label 0 and where no source reaches.  The result does not depend on the order of
+ *   evaluation and equals a heap Dijkstra with the same additions, bit for bit.
+ *   weights == NULL: w = fl32(sqrt(sum_i (anisotropy[i] * delta_i)^2)), computed once on the host in double
+ *     (anisotropy[i] > 0 and finite).  weights != NULL: w(p -> q) = weights[q], a float32 array of the
+ *     volume's shape, the cost of entering q; every entry must be finite and >= 0 (checked on the device
+ *     in the first pass: IGN_ERR_INVALID), and anisotropy is not read.
+ *   sources: n_sources linear indices x + sx * (y + sy * z) (a DEVICE array for _dev).  A source outside
+ *     the volume or on label 0 -> IGN_ERR_INVALID.  Several sources may share a label.
+ *   parents_out (may be NULL): uint32 of the volume's shape, the linear index + 1 of the chosen predecessor;
+ *     0 for a source, an unreached voxel and label 0.  It is written in one pass over the converged
+ *     distances: the first neighbour p, in (dz, dy, dx) raster order with dx fastest, with
+ *     fl32(dist[p] + w(p -> q)) == dist[q] and (dist[p], p) < (dist[q], q) lexicographically.  The second
+ *     condition keeps the parent graph acyclic where float32 addition stalls (dist[p] + w == dist[p]).  A
+ *     reached voxel that is not a source and has no such neighbour (a plateau entered from a higher index)
+ *     fails the call with IGN_ERR_INVALID (the message names one such voxel); a cycle is never written, and
+ *     parents_out is then unspecified.  The refusal is of the whole call, every label of it.
+ *     With parents_out the volume must have fewer than 2^32 - 1 voxels (IGN_ERR_OVERFLOW).
+ *   Each side below 2^30; 64-bit indexing for the distances.  A label-correcting solver over bricks of
+ *   32 x 8 x 8 voxels: not stream-ordered, the ctx stream is synchronised once per eight rounds to read
+ *   the length of the device-side list of bricks still to relax, and once more for the parents.
+ *   ign_geodesic_round_cap: the number of rounds after which a solve of that shape gives up with
+ *   IGN_ERR_INVALID (one more than the voxel count, a bound no input reaches).
+ *   ign_geodesic_last_stats: diagnostic only (tools/microbench_geodesic.py); thread-local counters of this
+ *   thread's last solve, not part of any result: [0] rounds that relaxed a brick, [1] bricks relaxed over
+ *   all rounds, [2] host synchronisations.
+ */
+IGN_API int ign_geodesic(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
+                         int connectivity, const float anisotropy[3], const float* weights,
+                         const uint64_t* sources, uint64_t n_sources, float* dist_out, uint32_t* parents_out);
+IGN_API int ign_geodesic_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
+                             int connectivity, const float anisotropy[3], const float* weights,
+                             const uint64_t* sources, uint64_t n_sources, float* dist_out,
+                             uint32_t* parents_out);
+IGN_API int ign_geodesic_round_cap(uint64_t sx, uint64_t sy, uint64_t sz, uint64_t* cap);
+IGN_API int ign_geodesic_last_stats(uint64_t stats[3]);
+/* Per label l = 1..max_label of n voxels: index_out[l] = the voxel of greatest finite field value, ties
+ *   to the lowest linear index, and value_out[l] = that value (2^64 - 1 and -inf for a label without a
+ *   finite value; entry 0 likewise).  Both are DEVICE arrays of max_label + 1 entries.  Label 0 and labels
+ *   above max_label are ignored; max_label of 2^32 or more -> IGN_ERR_UNSUPPORTED (renumber first).
+ *   TEASAR's root (argmax of the first distance field) and the per-label maxima of its fields. */
+IGN_API int ign_label_argmax_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t n, const float* field,
+                                 uint64_t max_label, uint64_t* index_out, float* value_out);
+/* TEASAR's penalty field (kimimaro's formula as recalled, parity unpinned; DESIGN.md §5e), float32,
+ *   every operation rounded on its own:
+ *     out[p] = scale * (1 - dbf[p] / (1.01f * dbf_max[l]))^exponent + daf[p] / daf_max[l],   l = labels[p]
+ *   the power by exponent - 1 successive multiplications (exponent a whole number from 1 to 64), the
+ *   second term 0 when daf_max[l] is 0; out[p] = 0 where l is 0 or above max_label or daf[p] is +inf.
+ *   dbf_max, daf_max: DEVICE arrays of max_label + 1 entries, as ign_label_argmax_dev writes them. */
+IGN_API int ign_teasar_pdrf_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t n, const float* dbf,
+                                const float* daf, const float* dbf_max, const float* daf_max,
+                                uint64_t max_label, float scale, int exponent, float* out);
+
 /* --------------------------------------------------------------------- mesh
  * zmesh.Mesher(resolution).mesh(data, preserve_order=False)  igneous/tasks/mesh/mesh.py:151,245
  * Mesher.ids()                                                igneous/tasks/mesh/mesh.py:374
