@@ -80,37 +80,8 @@ def fields(labels, anisotropy=(1, 1, 1), pdrf_scale=100000, pdrf_exponent=4, dbf
       out["mapping"][0] = 0
     if K == 0:
       return out
-    U32 = _shim.IGN_U32
-    d_dbf, d_daf, d_pdrf, d_dist, d_par = (alloc(n * 4) for _ in range(5))
-    index, roots, dbf_max, daf_max = alloc((K + 1) * 8), alloc((K + 1) * 8), alloc((K + 1) * 4), alloc((K + 1) * 4)
-    if dbf is None:
-      _shim.check(lib.ign_edt_dev(h, ptr(lab), U32, *vol.shape, a, 1, 0, ptr(d_dbf)))
-    else:
-      dbf = np.asfortranarray(dbf, dtype=np.float32)
-      if dbf.shape != vol.shape:
-        raise ValueError("teasar.fields: dbf of shape %r for labels of shape %r" % (dbf.shape, vol.shape))
-      ctx.h2d(d_dbf, dbf)
-
-    def argmax(field, values):
-      _shim.check(lib.ign_label_argmax_dev(h, ptr(lab), U32, n, ptr(field), K, ptr(index), ptr(values)))
-
-    def geodesic(sources, weights, dist, parents):
-      # entry 0 of an argmax index belongs to label 0: the K sources start one entry in
-      _shim.check(lib.ign_geodesic_dev(h, ptr(lab), U32, *vol.shape, CONNECTIVITY, a, weights, sources.offset(8), K,
-                                       ptr(dist), parents))
-
-    # the first voxel of every label: the argmax of an all-zero field goes to the lowest index
-    ctx.memset(d_daf, 0, n * 4)
-    argmax(d_daf, daf_max)
-    geodesic(index, None, d_pdrf, None)  # distance from the first voxel, parked in the pdrf buffer
-    argmax(d_pdrf, daf_max)
-    ctx.d2d(roots, index, (K + 1) * 8)
-    geodesic(roots, None, d_daf, None)
-    argmax(d_dbf, dbf_max)
-    argmax(d_daf, daf_max)
-    _shim.check(lib.ign_teasar_pdrf_dev(h, ptr(lab), U32, n, ptr(d_dbf), ptr(d_daf), ptr(dbf_max), ptr(daf_max), K,
-                                        float(pdrf_scale), int(pdrf_exponent), ptr(d_pdrf)))
-    geodesic(roots, ptr(d_pdrf), d_dist, ptr(d_par))
+    d = device_fields(ctx, lab, K, vol.shape, a, pdrf_scale, pdrf_exponent, alloc, dbf=dbf)
+    d_dbf, d_daf, d_pdrf, d_par, roots = d["dbf"], d["daf"], d["pdrf"], d["parents"], d["roots"]
     root_index = np.empty(K + 1, np.uint64)
     ctx.d2h(root_index, roots)
     for name, buf in (("dbf", d_dbf), ("daf", d_daf), ("pdrf", d_pdrf), ("parents", d_par)):
@@ -121,3 +92,50 @@ def fields(labels, anisotropy=(1, 1, 1), pdrf_scale=100000, pdrf_exponent=4, dbf
   finally:
     for b in bufs:
       b.free()
+
+
+def device_fields(ctx, lab, K, shape, a, pdrf_scale, pdrf_exponent, alloc, dbf=None, before=None, parents=True):
+  """The chain of fields() on device buffers: `lab` a device u32 volume of `shape` (F order) with labels
+  1..K, `a` the ctypes anisotropy, `alloc(nbytes)` a device allocator whose buffers the caller frees.
+  dbf: a host array to upload instead of the edt.  before: (device u64 buffer, count) of target voxels;
+  the last one on each label replaces its root.  parents=False leaves the parents out (the distance
+  under the penalty field is still computed).  Returns device buffers {dbf, daf, pdrf, dist, parents
+  (or None), roots, dbf_max}; roots and dbf_max have K + 1 entries, entry 0 unused."""
+  lib, h, ptr = ctx.lib, ctx.handle, _shim.ptr
+  n = int(np.prod(shape))
+  U32 = _shim.IGN_U32
+  d_dbf, d_daf, d_pdrf, d_dist = (alloc(n * 4) for _ in range(4))
+  d_par = alloc(n * 4) if parents else None
+  index, roots, dbf_max, daf_max = alloc((K + 1) * 8), alloc((K + 1) * 8), alloc((K + 1) * 4), alloc((K + 1) * 4)
+  if dbf is None:
+    _shim.check(lib.ign_edt_dev(h, ptr(lab), U32, *shape, a, 1, 0, ptr(d_dbf)))
+  else:
+    dbf = np.asfortranarray(dbf, dtype=np.float32)
+    if dbf.shape != tuple(shape):
+      raise ValueError("teasar.fields: dbf of shape %r for labels of shape %r" % (dbf.shape, tuple(shape)))
+    ctx.h2d(d_dbf, dbf)
+
+  def argmax(field, values):
+    _shim.check(lib.ign_label_argmax_dev(h, ptr(lab), U32, n, ptr(field), K, ptr(index), ptr(values)))
+
+  def geodesic(sources, weights, dist, parents):
+    # entry 0 of an argmax index belongs to label 0: the K sources start one entry in
+    _shim.check(lib.ign_geodesic_dev(h, ptr(lab), U32, *shape, CONNECTIVITY, a, weights, sources.offset(8), K,
+                                     ptr(dist), parents))
+
+  # the first voxel of every label: the argmax of an all-zero field goes to the lowest index
+  ctx.memset(d_daf, 0, n * 4)
+  argmax(d_daf, daf_max)
+  geodesic(index, None, d_pdrf, None)  # distance from the first voxel, parked in the pdrf buffer
+  argmax(d_pdrf, daf_max)
+  ctx.d2d(roots, index, (K + 1) * 8)
+  if before is not None and before[1]:
+    _shim.check(lib.ign_teasar_last_target_dev(h, ptr(lab), n, K, ptr(before[0]), before[1], ptr(roots)))
+  geodesic(roots, None, d_daf, None)
+  argmax(d_dbf, dbf_max)
+  argmax(d_daf, daf_max)
+  _shim.check(lib.ign_teasar_pdrf_dev(h, ptr(lab), U32, n, ptr(d_dbf), ptr(d_daf), ptr(dbf_max), ptr(daf_max), K,
+                                      float(pdrf_scale), int(pdrf_exponent), ptr(d_pdrf)))
+  geodesic(roots, ptr(d_pdrf), d_dist, ptr(d_par) if parents else None)
+  return {"dbf": d_dbf, "daf": d_daf, "pdrf": d_pdrf, "dist": d_dist, "parents": d_par, "roots": roots,
+          "dbf_max": dbf_max}

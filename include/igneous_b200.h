@@ -417,6 +417,45 @@ IGN_API int ign_label_argmax_dev(ign_ctx* ctx, const void* labels, int dtype, ui
 IGN_API int ign_teasar_pdrf_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t n, const float* dbf,
                                 const float* daf, const float* dbf_max, const float* daf_max,
                                 uint64_t max_label, float scale, int exponent, float* out);
+/* TEASAR skeletons (kimimaro.skeletonize as recalled, parity unpinned; DESIGN.md §5f).  Every array is a
+ * DEVICE array; volumes are (sx, sy, sz) F-order with fewer than 2^32 - 1 voxels.
+ * ign_teasar_objects_dev: labels u32 1..max_label (renumbered) -> objects_out u32 1..*n_objects, the parts of
+ *   each label joined under `connectivity` (6 / 18 / 26), numbered by first voxel in linear order; parts of
+ *   fewer than dust_threshold voxels are 0.  One geodesic solve per part of the most-split label.
+ * ign_teasar_border_targets_dev: kimimaro's fix_borders targets (as recalled): for each face in the order
+ *   x = 0, x = sx - 1, y = 0, y = sy - 1, z = 0, z = sz - 1, the 8-connected parts of each object in the
+ *   face plane, ordered by first voxel in the plane's F order, and per part the voxel of greatest 2-D edt
+ *   of the object plane (the plane's two anisotropies, black border), ties to the lowest plane index.
+ *   targets_out: *count linear indices of the volume (at most capacity; the face areas summed suffice).
+ * ign_teasar_last_target_dev: for each object with a target on it, roots[o] (n_objects + 1 entries) = its
+ *   last target in the order given.  Targets on 0 are ignored; one outside the volume -> IGN_ERR_INVALID.
+ * ign_teasar_paths_dev: the path loop for every object 1..n_objects at once.  dbf, daf, pdrf: the fields
+ *   of ign_teasar_pdrf_dev on the objects; roots[o] the root of object o (n_objects + 1 entries).
+ *   fix_branching: dist = the least cost from the roots where entering p costs pdrf[p]; it is lowered in
+ *   place as paths join the skeleton, and parents is NULL.  Otherwise parents = the parent field under that
+ *   cost (ign_geodesic_dev) and dist is NULL.  before / after: target voxels in the order given; the last
+ *   before-target of an object must be its root and is not traced.  scale, cnst finite and >= 0;
+ *   max_paths bounds the paths of the DAF loop of each object.  Out: *count skeleton voxels, skel_out
+ *   their linear indices ascending, next_out the next voxel towards the root (the voxel itself at a root),
+ *   radius_out dbf there; each of n entries at most.  A path voxel without a next voxel -> IGN_ERR_INVALID
+ *   naming it.  The host synchronises once per round (plus the solver's own synchronisations).
+ * ign_teasar_last_stats: diagnostic only; this thread's last paths call: [0] rounds, [1] paths, [2] box
+ *   voxels visited by the invalidation, [3] host synchronisations. */
+IGN_API int ign_teasar_objects_dev(ign_ctx* ctx, const uint32_t* labels, uint64_t sx, uint64_t sy, uint64_t sz,
+                                   uint64_t max_label, int connectivity, uint64_t dust_threshold,
+                                   uint32_t* objects_out, uint64_t* n_objects);
+IGN_API int ign_teasar_border_targets_dev(ign_ctx* ctx, const uint32_t* objects, uint64_t sx, uint64_t sy,
+                                          uint64_t sz, uint64_t n_objects, const float anisotropy[3],
+                                          uint64_t* targets_out, uint64_t capacity, uint64_t* count);
+IGN_API int ign_teasar_last_target_dev(ign_ctx* ctx, const uint32_t* objects, uint64_t n, uint64_t n_objects,
+                                       const uint64_t* targets, uint64_t n_targets, uint64_t* roots);
+IGN_API int ign_teasar_paths_dev(ign_ctx* ctx, const uint32_t* objects, uint64_t sx, uint64_t sy, uint64_t sz,
+                                 uint64_t n_objects, const float anisotropy[3], const float* dbf, const float* daf,
+                                 const float* pdrf, float* dist, const uint32_t* parents, const uint64_t* roots,
+                                 const uint64_t* before, uint64_t n_before, const uint64_t* after,
+                                 uint64_t n_after, float scale, float cnst, uint64_t max_paths,
+                                 uint32_t* skel_out, uint32_t* next_out, float* radius_out, uint64_t* count);
+IGN_API int ign_teasar_last_stats(uint64_t stats[4]);
 
 /* --------------------------------------------------------------------- mesh
  * zmesh.Mesher(resolution).mesh(data, preserve_order=False)  igneous/tasks/mesh/mesh.py:151,245
