@@ -25,6 +25,7 @@ struct ign_mesher {
   uint32_t simp_migrations[3];                  // labels resumed in each class after they shrank
   uint32_t simp_passes[2];                      // multi-pass label-rounds, winners with a ring over 32 faces
   uint32_t simp_costs[3];                       // initial costs, re-costs after collapses, costless keys
+  uint32_t simp_groups[3];                      // winners validated by lane groups of 8, 16 and 32
   std::vector<uint64_t> ids;       // original label of dense id i+1
   std::vector<uint32_t> tri_off;   // [K+2]
   std::vector<uint32_t> vert_off;  // [K+2]

@@ -314,7 +314,7 @@ __global__ void __launch_bounds__(256)
 //   P1  key1[v] = MAX, lose[v] = 0                             (vertex parallel)
 //   P2  every canonical half-edge (u < v) of an alive face posts its cached key to both
 //       endpoints with a shared-memory min reduction (the float costs come from k_simp_ecost
-//       and E2d; P2 evaluates none)                                (face parallel)
+//       and E2; P2 evaluates none)                                 (face parallel)
 //   P3  a vertex LOSEs if a face neighbour holds a smaller key1 (== key2 test of the
 //       round formulation: key2[w] == key1[w] <=> !LOSE[w]); plain byte stores
 //                                                               (face parallel)
@@ -323,10 +323,10 @@ __global__ void __launch_bounds__(256)
 //   E1  the faces that touch a winner's endpoints append themselves to the winner's
 //       two ring lists; the first warps compute the winners' placement and cost (E2a)
 //       at the same time                                         (face parallel)
-//   E2b one flip test per (winner, side, ring face)              (item parallel)
-//   E2c link condition by ballots / shuffles over the ring lists and the collapse
-//       itself, one HALF warp per winner (whole warps for rings over 16 faces)
-//   E2d the canonical half-edges of each collapse's kept vertex are re-costed (item parallel)
+//   E2  one group of 8 lanes per winner (16 / 32 for rings over 8 / 16 faces), a lane per ring
+//       face of each endpoint: flip tests, link condition by ballots / shuffles, the collapse
+//       itself and the re-costs of the kept vertex's canonical half-edges, with no barrier
+//       between them                                             (winner parallel)
 //
 // Labels that do not fit (more than 16384 faces, or 6U + 9T + 23 KB over the CTA's shared
 // memory) keep faces and lists in global memory, with keys / flags / states still in
@@ -339,7 +339,7 @@ constexpr int SL_THREADS = 1024;
 // class has room for SL_WCAP; a shared-memory label takes more where the class's shared memory leaves room
 // (sl_wcap), since each further pass rescans the vertices (P4) and the alive faces (E1)
 constexpr int SL_WCAP = 128;
-constexpr uint32_t WF_BAD = 1, WF_OK = 2, WF_DONE = 4;  // winner flags: failed validation / validated / collapsed
+constexpr uint32_t WF_BAD = 1;  // winner flag: E2a found no valid placement (both endpoints locked, or over max_error)
 constexpr int SL_LIST_PER = 16;  // list entries per thread held in registers while a list is compacted in place
 
 // Size classes of k_simp_labels: CTA size and CTAs per SM.  A label runs in the smallest class whose
@@ -351,7 +351,8 @@ constexpr int SL_CLASS_THREADS[SL_NCLASS] = {1024, 512, 256};
 // a winner of a selection pass: its edge, ring lengths, flags and placement (dynamic shared memory)
 struct SlWin {
   double best[3];
-  uint32_t u, v, h, cnt[2], keep, flags, pad;
+  uint32_t u, v, h, cnt[2], keep, flags;
+  uint32_t order;  // E2 takes the winners in the order win[0].order, win[1].order, ... (8-lane groups first)
 };
 // shared memory a shared-memory label needs per winner of a pass: the record and two 16-bit ring lists
 constexpr size_t SL_WIN_BYTES = sizeof(SlWin) + 2 * S_MAXV * 2;
@@ -418,8 +419,9 @@ struct SlArgs {
                        // [4 + class] next work item  [8 + class] labels run in the class
                        // [16 + class] labels migrated into the class  [20 + class] next migrated label to resume
                        // [24] multi-pass label-rounds  [25] winners with a ring over S_MAXV faces
-                       // [26] initial cost evaluations (k_simp_ecost)  [27] re-costs after collapses (E2d)
+                       // [26] initial cost evaluations (k_simp_ecost)  [27] re-costs after collapses (E2)
                        // [28] canonical half-edges without a cost met by the key pass (always 0)
+                       // [29..31] winners taken by E2 groups of 8, 16 and 32 lanes
   double max_err2;
   int max_rounds;
   uint32_t smem_bytes;  // dynamic shared memory of the launch
@@ -439,6 +441,7 @@ struct SlArgs {
   uint32_t* trace;      // IGN_SIMP_TRACE=1: [round][4] = winners, collapses, alive faces, list length of the largest label
                         // [SL_HIST +] per size class: selection passes, winners, ring lengths per round (SL_H*)
   uint32_t wcap_max;    // most winners per pass (IGN_SIMP_WCAP; default: no limit beyond the budget)
+  uint32_t group_min;   // narrowest lane group of E2: 8, 16 or 32 (IGN_SIMP_GROUP; default 8)
 };
 
 // IGN_SIMP_TRACE histograms, per size class the segment runs in: passes per round (1..SL_HP, last bin more),
@@ -448,14 +451,17 @@ constexpr int SL_HIST = 1664, SL_HP = 16, SL_HW = 64, SL_HR = S_MAXV + 2, SL_HCL
 // header of a migrated label: dense label, trace record, next round, slow rounds, alive faces, alive vertices
 constexpr int SL_MREC = 8;
 constexpr int SL_LREC = 7;  // words of a label's IGN_SIMP_TRACE record (SlArgs::lrec)
-constexpr int SL_NPH = 11;  // IGN_SIMP_TRACE phase timers (trace words 1600.., 64 bits each)
+constexpr int SL_NPH = 9;  // IGN_SIMP_TRACE phase timers (trace words 1600.., 64 bits each)
 
 struct SlShared {
-  uint32_t work, alive, progress, ncol, nwin, stop, slow, counter, nbig, npass, bigring;
+  uint32_t work, alive, progress, ncol, nwin, stop, slow, counter, npass;
+  uint32_t ring8, ring16;  // E1 saw a ring of more than 8 / 16 faces in this pass
+  uint32_t nnarrow, nwide;  // winners of the pass that 8-lane groups take, and the others
   uint32_t rec, valive;  // trace record of the label; alive vertices (one dies per collapse)
   unsigned long long visits, wins;  // IGN_SIMP_TRACE
   long long t_label;
-  uint32_t nrecost;  // half-edges re-costed after collapses (E2d)
+  uint32_t nrecost;    // half-edges re-costed after collapses (E2)
+  uint32_t ngroup[3];  // winners taken by groups of 8, 16 and 32 lanes (E2)
   unsigned long long ph[SL_NPH];  // phase timers (IGN_SIMP_TRACE)
   long long t_prev;
 };
@@ -560,31 +566,22 @@ __device__ __forceinline__ void sl_cost(const SlArgs& A, const SlLab<SM>& L, uin
          (L.vflag[v] & VF_BOUND) != 0, e);
 }
 
-// Re-cost the canonical half-edges of face f that hold the kept vertex k of a collapse (k -> o1 when k < o1,
-// o2 -> k when o2 < k): cached float cost and memo (2 cached, 3 exceeds max_error).  Returns the face's new
-// state byte; the caller stores it (a face is in exactly one ring list: a single writer).
+// The two half-edges of face f that hold the kept vertex k of a collapse: t = 0 is k -> o1, t = 1 is o2 -> k.
+// sl_kcorner gives k's corner, sl_kcorner(..) + 2 * t (mod 3) the corner that starts half-edge t.
+template <bool SM>
+__device__ __forceinline__ uint32_t sl_kcorner(const SlLab<SM>& L, uint32_t f, uint32_t k) {
+  return sl_fget<SM>(L, f, 0) == k ? 0u : (sl_fget<SM>(L, f, 1) == k ? 1u : 2u);
+}
+// Re-cost the half-edge that starts at corner c of face f: cached float cost, and the memo to store (2 cached,
+// 3 exceeds max_error)
 template <bool SM, bool R>
-__device__ __forceinline__ uint32_t sl_recost(const SlArgs& A, const SlLab<SM>& L, uint32_t f, uint32_t st,
-                                              uint32_t k, uint32_t* nev) {
-  const uint32_t a[3] = {sl_fget<SM>(L, f, 0), sl_fget<SM>(L, f, 1), sl_fget<SM>(L, f, 2)};
-  const uint32_t ck = a[0] == k ? 0u : (a[1] == k ? 1u : 2u);
-  float* ec = A.ecost + 3 * (uint64_t)(L.tbase + sl_fo<SM, R>(L, f));
-#pragma unroll
-  for (int t = 0; t < 2; t++) {
-    const uint32_t c = t == 0 ? ck : (ck + 2) % 3;  // the corners of k -> o1 and o2 -> k
-    const uint32_t u = a[c], v = a[(c + 1) % 3];
-    if (!(u < v)) continue;
-    SEval ev;
-    sl_cost<SM, R>(A, L, u, v, &ev);
-    uint32_t es = 3;
-    if (ev.valid) {
-      ec[c] = __double2float_rn(ev.cost);
-      es = 2;
-    }
-    st = (st & ~(3u << (2 * c))) | (es << (2 * c));
-    (*nev)++;
-  }
-  return st;
+__device__ __forceinline__ uint32_t sl_recost(const SlArgs& A, const SlLab<SM>& L, uint32_t f, uint32_t c) {
+  const uint32_t u = sl_fget<SM>(L, f, (int)c), v = sl_fget<SM>(L, f, (int)((c + 1) % 3));
+  SEval ev;
+  sl_cost<SM, R>(A, L, u, v, &ev);
+  if (!ev.valid) return 3;
+  A.ecost[3 * (uint64_t)(L.tbase + sl_fo<SM, R>(L, f)) + c] = __double2float_rn(ev.cost);
+  return 2;
 }
 
 // does face (a0,a1,a2) flip when vertex w moves to `best`?  (the validation's flip test)
@@ -712,39 +709,63 @@ extern __shared__ __align__(16) unsigned char sl_smem[];
 // the winner records of the pass (SlLayout: first in the dynamic shared memory)
 __device__ __forceinline__ SlWin* sl_win() { return (SlWin*)sl_smem; }
 
-// One pass of E2c with groups of W lanes (16: two winners per warp side by side, only winners whose
-// rings fit 16 lanes; 32: the winners left over).  Both halves of a warp run the same instructions;
-// everything that differs between them is predicated and loop counts are made warp uniform.
+// group width that E2 gives a winner whose rings hold nfu and nfv faces: 8, 16 or 32 lanes, at least
+// `wmin` (IGN_SIMP_GROUP).  Rings over S_MAXV faces take 32 lanes and are parked there.
+__device__ __forceinline__ uint32_t sl_width(uint32_t nfu, uint32_t nfv, uint32_t wmin) {
+  const uint32_t n = nfu > nfv ? nfu : nfv;
+  const uint32_t w = n <= 8u ? 8u : (n <= 16u ? 16u : 32u);
+  return w > wmin ? w : wmin;
+}
+
+// One sweep of E2 with groups of W lanes (32 / W winners per warp side by side), each group taking the
+// winners whose width (sl_width) is W.  A group owns its winner from the flip tests to the re-costs, with
+// no barrier in between: that is safe because winners are two apart (§5 of DESIGN.md), so no other
+// group writes a face, a state byte, a quadric or a position that this group reads or writes.  Lane gl
+// holds ring entry gl of each side.  The groups of a warp run the same instructions; everything that
+// differs between them is predicated and loop counts are made warp uniform.  *nev counts the re-costed
+// half-edges.
 template <bool SM, bool R, int W>
-__device__ __forceinline__ void sl_collapse_pass(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, uint32_t nb) {
+__device__ __forceinline__ void sl_group_pass(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, uint32_t first,
+                                              uint32_t last, uint32_t* nev) {
+  static_assert(W == 8 || W == 16 || W == 32, "group width");
   const uint32_t FULL = 0xFFFFFFFFu;
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5, NW = blockDim.x >> 5;
   constexpr uint32_t G = 32 / W;                       // groups per warp
   const uint32_t gl = lane & (W - 1), goff = lane & ~(uint32_t)(W - 1);
-  const uint32_t wmask = W == 32 ? FULL : 0xFFFFu;
+  const uint32_t wmask = W == 32 ? FULL : (1u << W) - 1u;
   const uint32_t gmask = wmask << goff;
   const uint32_t gidx = lane / W;
   SlWin* const win = sl_win();
-  for (uint32_t base = warp * G; base < nb; base += NW * G) {  // warp uniform
-    const uint32_t slot = base + gidx;
-    bool act = slot < nb;
-    uint32_t nfu = 0, nfv = 0;
-    if (act) { nfu = win[slot].cnt[0]; nfv = win[slot].cnt[1]; }
-    const bool big = nfu > 16u || nfv > 16u;
-    if (W == 16) {
-      if (act && big && gl == 0) atomicAdd(&sh.nbig, 1u);
-      act = act && !big;
-    } else {
-      act = act && big;
-      if (act && gl == 0 && (nfu > (uint32_t)S_MAXV || nfv > (uint32_t)S_MAXV)) atomicAdd(&A.counters[25], 1u);
+  for (uint32_t base = first + warp * G; base < last; base += NW * G) {  // warp uniform
+    bool act = base + gidx < last;
+    uint32_t slot = 0, nfu = 0, nfv = 0;
+    if (act) {
+      slot = win[base + gidx].order;
+      nfu = win[slot].cnt[0]; nfv = win[slot].cnt[1];
     }
+    act = act && sl_width(nfu, nfv, A.group_min) == (uint32_t)W;
+    const uint32_t b_act = __ballot_sync(FULL, act && gl == 0);
+    if (!b_act) continue;  // no winner of this width in the warp's slots
+    if (lane == 0) atomicAdd(&sh.ngroup[W == 8 ? 0 : (W == 16 ? 1 : 2)], (uint32_t)__popc(b_act));
+    if (W == 32 && act && gl == 0 && (nfu > (uint32_t)S_MAXV || nfv > (uint32_t)S_MAXV)) atomicAdd(&A.counters[25], 1u);
     uint32_t fu = 0, fv = 0, u = 0, v = 0, hl = 0, k = 0;
     bool ok = false;
     if (act) {
-      if (gl < nfu && gl < (uint32_t)S_MAXV) fu = L.ring[(2 * slot) * S_MAXV + gl];
-      if (gl < nfv && gl < (uint32_t)S_MAXV) fv = L.ring[(2 * slot + 1) * S_MAXV + gl];
+      if (gl < nfu) fu = L.ring[(2 * slot) * S_MAXV + gl];
+      if (gl < nfv) fv = L.ring[(2 * slot + 1) * S_MAXV + gl];
       u = win[slot].u; v = win[slot].v; hl = win[slot].h; k = win[slot].keep;
       ok = !(win[slot].flags & WF_BAD) && nfu <= (uint32_t)S_MAXV && nfv <= (uint32_t)S_MAXV;
+    }
+    uint32_t au[3] = {0, 0, 0}, av[3] = {0, 0, 0};
+    if (ok && gl < nfu) { au[0] = sl_fget<SM>(L, fu, 0); au[1] = sl_fget<SM>(L, fu, 1); au[2] = sl_fget<SM>(L, fu, 2); }
+    if (ok && gl < nfv) { av[0] = sl_fget<SM>(L, fv, 0); av[1] = sl_fget<SM>(L, fv, 1); av[2] = sl_fget<SM>(L, fv, 2); }
+    // flip tests of the faces that survive the collapse (those holding the other endpoint die with the
+    // edge), one side after the other; one flipping face rejects the winner
+    {
+      bool flip = false;
+      if (ok && gl < nfu && au[0] != v && au[1] != v && au[2] != v) flip = sl_flips<SM, R>(A, L, au, u, win[slot].best);
+      if (ok && gl < nfv && av[0] != u && av[1] != u && av[2] != u) flip |= sl_flips<SM, R>(A, L, av, v, win[slot].best);
+      if (__ballot_sync(FULL, flip) & gmask) ok = false;
     }
     const uint32_t rm = (k == u) ? v : u;
     // the quadrics of the two endpoints are needed only if the collapse happens, but the L2 round
@@ -752,24 +773,21 @@ __device__ __forceinline__ void sl_collapse_pass(const SlArgs& A, const SlLab<SM
     const uint64_t gk = sl_vg<SM, R>(L, k), gr = sl_vg<SM, R>(L, rm);
     double* Qk = A.Q + 10 * gk;
     const double* Qr = A.Q + 10 * gr;
-    double qk = 0.0, qr = 0.0;
+    // lane gl sums component gl of the quadrics and lanes 10-12 write the position; with 8 lanes, lanes
+    // 0-1 also sum components 8-9 and lanes 2-4 write the position
+    double qk = 0.0, qr = 0.0, qk2 = 0.0, qr2 = 0.0;
     if (ok && gl < 10) { qk = Qk[gl]; qr = Qr[gl]; }
+    if (W == 8 && ok && gl < 2) { qk2 = Qk[gl + 8]; qr2 = Qr[gl + 8]; }
     const bool hu = ok && gl < nfu, hv = ok && gl < nfv;
-    uint32_t au[3] = {0, 0, 0}, av[3] = {0, 0, 0};
     uint32_t x1 = 0xF0000000u + lane, x2 = 0xF1000000u + lane, y1 = 0xF2000000u + lane, y2 = 0xF3000000u + lane;
-    if (hu) {
-      au[0] = sl_fget<SM>(L, fu, 0); au[1] = sl_fget<SM>(L, fu, 1); au[2] = sl_fget<SM>(L, fu, 2);
-      sl_others(au, u, &x1, &x2);
-    }
-    if (hv) {
-      av[0] = sl_fget<SM>(L, fv, 0); av[1] = sl_fget<SM>(L, fv, 1); av[2] = sl_fget<SM>(L, fv, 2);
-      sl_others(av, v, &y1, &y2);
-    }
+    if (hu) sl_others(au, u, &x1, &x2);
+    if (hv) sl_others(av, v, &y1, &y2);
     // (every lane of the warp takes part in the collectives below; n = 0 for groups without a winner)
     const uint32_t nu = ok ? nfu : 0u, nv = ok ? nfv : 0u;
     uint32_t nmax = nu > nv ? nu : nv;
-    if (W == 16) {
-      const uint32_t o = __shfl_xor_sync(FULL, nmax, 16);
+#pragma unroll
+    for (uint32_t d = W; d < 32u; d <<= 1) {
+      const uint32_t o = __shfl_xor_sync(FULL, nmax, d);
       nmax = o > nmax ? o : nmax;
     }
     // distinct neighbours of u (first occurrences f1 among x1, f2 among x2 not in x1), same for v
@@ -821,8 +839,11 @@ __device__ __forceinline__ void sl_collapse_pass(const SlArgs& A, const SlLab<SM
       if (hv && y1 != u && y2 != u) { sl_vor<SM>(L.vflag, y1, VF_RDIRTY); sl_vor<SM>(L.vflag, y2, VF_RDIRTY); }
       if (gl < 10) Qk[gl] = qk + qr;
       if (gl >= 10 && gl < 13) A.pos[3 * gk + (gl - 10)] = win[slot].best[gl - 10];
+      if (W == 8) {
+        if (gl < 2) Qk[gl + 8] = qk2 + qr2;
+        else if (gl < 5) A.pos[3 * gk + (gl - 2)] = win[slot].best[gl - 2];
+      }
       if (gl == 0) {
-        win[slot].flags |= WF_DONE;  // k moved: E2d re-costs its edges
         sl_vclear<SM>(L.vflag, k, VF_END);
         sl_vclear<SM>(L.vflag, rm, 0xFFu);
         atomicSub(&sh.alive, dead);
@@ -830,6 +851,77 @@ __device__ __forceinline__ void sl_collapse_pass(const SlArgs& A, const SlLab<SM
         atomicOr(&sh.progress, 1u);
       }
     }
+    // k has its final quadric and position, and so do its neighbours (winners are two apart, in this pass
+    // and in the later passes of the round), so the costs of k's edges are final until the next round:
+    // re-cost them now.  Every alive face of the two ring lists holds k, and each is in one list (so its
+    // state byte has one writer: the lane that holds it).  The canonical half-edges of k (bit 2 side + t of
+    // m, sl_kcorner) are dealt out to the group's lanes, item i to lane i mod W, so that a lane evaluates
+    // about one cost instead of up to four one after the other; the memos go back to the lanes that hold
+    // the faces.
+    __syncwarp();  // Q[k], pos[k] and the rewritten faces are visible to the group
+    uint32_t m = 0, ck = 0, st0 = 0, st1 = 0;
+    if (go && gl < nfu) {
+      st0 = L.fstate[fu];
+      if (st0 & 0x80u) {
+        const uint32_t c = sl_kcorner<SM>(L, fu, k);
+        ck = c;
+        m |= (k < sl_fget<SM>(L, fu, (int)((c + 1) % 3)) ? 1u : 0u) | (sl_fget<SM>(L, fu, (int)((c + 2) % 3)) < k ? 2u : 0u);
+      }
+    }
+    if (go && gl < nfv) {
+      st1 = L.fstate[fv];
+      if (st1 & 0x80u) {
+        const uint32_t c = sl_kcorner<SM>(L, fv, k);
+        ck |= c << 2;
+        m |= (k < sl_fget<SM>(L, fv, (int)((c + 1) % 3)) ? 4u : 0u) | (sl_fget<SM>(L, fv, (int)((c + 2) % 3)) < k ? 8u : 0u);
+      }
+    }
+    const uint32_t cnt = __popc(m);
+    uint32_t inc = cnt;
+#pragma unroll
+    for (uint32_t d = 1; d < W; d <<= 1) {
+      const uint32_t o = __shfl_up_sync(FULL, inc, d, W);
+      if (gl >= d) inc += o;
+    }
+    const uint32_t P = inc - cnt, N = __shfl_sync(FULL, inc, W - 1, W);  // first item of the lane, items of the group
+    uint32_t rounds = (N + W - 1) / W;
+#pragma unroll
+    for (uint32_t d = W; d < 32u; d <<= 1) {
+      const uint32_t o = __shfl_xor_sync(FULL, rounds, d);
+      rounds = o > rounds ? o : rounds;
+    }
+    uint32_t res = 0;  // memo of this lane's item of round r in bits 2r..2r+1
+    for (uint32_t r = 0; r < rounds; r++) {  // warp uniform
+      const uint32_t idx = r * W + gl;
+      uint32_t own = 0;  // the lane that holds item idx: the last one whose first item is at most idx
+      for (uint32_t j = 1; j < W; j++)
+        if (__shfl_sync(FULL, P, j, W) <= idx) own = j;
+      const uint32_t mo = __shfl_sync(FULL, m, own, W), po = __shfl_sync(FULL, P, own, W);
+      const uint32_t fuo = __shfl_sync(FULL, fu, own, W), fvo = __shfl_sync(FULL, fv, own, W);
+      const uint32_t cko = __shfl_sync(FULL, ck, own, W);
+      if (idx < N) {
+        uint32_t b = mo;
+        for (uint32_t q = idx - po; q; q--) b &= b - 1;  // the (idx - po)-th item of the owner
+        const uint32_t bit = (uint32_t)__ffs(b) - 1, side = bit >> 1;
+        const uint32_t c = (((cko >> (2 * side)) & 3u) + 2u * (bit & 1u)) % 3u;
+        res |= sl_recost<SM, R>(A, L, side ? fvo : fuo, c) << (2 * r);
+        (*nev)++;
+      }
+    }
+    uint32_t q = P;
+#pragma unroll
+    for (uint32_t bit = 0; bit < 4; bit++) {  // the memos of this lane's items
+      const uint32_t val = __shfl_sync(FULL, res, q % W, W);
+      if ((m >> bit) & 1u) {
+        const uint32_t side = bit >> 1, es = (val >> (2 * (q / W))) & 3u;
+        const uint32_t c = (((ck >> (2 * side)) & 3u) + 2u * (bit & 1u)) % 3u;
+        if (side) st1 = (st1 & ~(3u << (2 * c))) | (es << (2 * c));
+        else st0 = (st0 & ~(3u << (2 * c))) | (es << (2 * c));
+        q++;
+      }
+    }
+    if (m & 3u) L.fstate[fu] = (uint8_t)st0;
+    if (m & 12u) L.fstate[fv] = (uint8_t)st1;
   }
 }
 
@@ -895,7 +987,7 @@ __device__ void sl_migrate(const SlArgs& A, const SlLab<true>& L, SlShared& sh, 
 // All rounds of one label (R: a label resumed from the header `hdr` after it migrated from a larger class)
 template <bool SM, bool R>
 __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const uint32_t* hdr) {
-  if (threadIdx.x == 0) sh.nrecost = 0;
+  if (threadIdx.x == 0) sh.nrecost = sh.ngroup[0] = sh.ngroup[1] = sh.ngroup[2] = 0;
   if (A.trace != nullptr && threadIdx.x == 0) {
     for (int q = 0; q < SL_NPH; q++) sh.ph[q] = 0;
     sh.t_prev = clock64();
@@ -984,7 +1076,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
     SL_MARK(0);
     // ---- P2: keys of the canonical half-edges.  A warp takes 32 alive faces per iteration and
     // posts the cached keys.  No cost is evaluated here: k_simp_ecost costs every half-edge before
-    // the first round and E2d re-costs the edges of every vertex that moved right after its collapse.
+    // the first round and E2 re-costs the edges of every vertex that moved right after its collapse.
     {
       // software pipeline: the face id and the three cached costs of the NEXT iteration are
       // requested (global loads, L2 latency) before the current face is processed
@@ -1071,7 +1163,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
     // ---- P4 + E: the round's winners (marked DONE on both endpoints), L.wcap per pass
     SlWin* const win = sl_win();
     for (;;) {
-      if (tid == 0) { sh.nwin = 0; sh.nbig = 0; sh.bigring = 0; sh.npass++; }
+      if (tid == 0) { sh.nwin = 0; sh.ring8 = 0; sh.ring16 = 0; sh.nnarrow = 0; sh.nwide = 0; sh.npass++; }
       __syncthreads();
       for (uint32_t i = tid; i < nV; i += NT) {
         const uint32_t a = SM ? i : (uint32_t)vlist[i];
@@ -1148,7 +1240,8 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
               const uint32_t sl = (uint32_t)L.key1[x[c]];
               const uint32_t p = atomicAdd(&win[sl >> 1].cnt[sl & 1u], 1u);
               if (p < (uint32_t)S_MAXV) L.ring[sl * S_MAXV + p] = (idx_t)(c < 3 ? fa : fb);
-              if (p == 16u) sh.bigring = 1;  // (every writer stores 1)
+              if (p == 8u) sh.ring8 = 1;  // (every writer stores 1)
+              if (p == 16u) sh.ring16 = 1;
             }
           }
         }
@@ -1162,60 +1255,41 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
           atomicAdd(&A.trace[SL_HIST + SL_HCLS * A.cls + SL_HP + SL_HW + (n <= (uint32_t)S_MAXV ? n : S_MAXV + 1)], 1u);
         }
       }
-      // E2b: one flip test per (winner, side, ring entry).  Rings hold 5-6 faces typically and at most
-      // 16 almost always, so a half warp takes one winner side (entries 0..15); entries 16..31 take a
-      // second sweep, only in passes where some ring has more than 16 faces.
-      for (uint32_t j0 = 0; j0 < (uint32_t)S_MAXV; j0 += 16) {
-        if (j0 != 0 && !sh.bigring) break;
-        for (uint32_t item = tid; item < nb * 32; item += NT) {
-          const uint32_t i = item >> 5, side = (item >> 4) & 1u, j = j0 + (item & 15u);
-          if (win[i].flags & WF_BAD) continue;
-          if (win[i].cnt[0] > (uint32_t)S_MAXV || win[i].cnt[1] > (uint32_t)S_MAXV) continue;  // fails in E2c
-          if (j >= win[i].cnt[side]) continue;
-          const uint32_t w = side ? win[i].v : win[i].u, other = side ? win[i].u : win[i].v;
-          const uint32_t f = L.ring[(2 * i + side) * S_MAXV + j];
-          const uint32_t a[3] = {sl_fget<SM>(L, f, 0), sl_fget<SM>(L, f, 1), sl_fget<SM>(L, f, 2)};
-          if (a[0] == other || a[1] == other || a[2] == other) continue;  // dies with the edge
-          const double best[3] = {win[i].best[0], win[i].best[1], win[i].best[2]};
-          if (sl_flips<SM, R>(A, L, a, w, best)) atomicOr(&win[i].flags, WF_BAD);
+      // E2: flip tests, link condition by ballots / shuffles over the ring lists, the collapse and the
+      // re-costs of the kept vertex's edges, one group of lanes per winner from start to end (a lane holds
+      // one ring face of each endpoint).  Rings hold 5-6 faces typically, so most winners take 8 lanes,
+      // four per warp; the duration of the phase is the number of winners a warp handles one after the
+      // other, each a chain of dependent loads.  Wider rings take 16 or 32 lanes in further sweeps, only
+      // in passes where E1 saw one.  The winners are first ordered by width (8-lane winners to the front,
+      // the others to the back), so that each sweep hands out only its own winners; no barrier between
+      // the sweeps: groups never touch each other's data.
+      for (uint32_t i0 = warp * 32; i0 < nb; i0 += NT) {  // warp uniform
+        const uint32_t i = i0 + lane;
+        const bool have = i < nb;
+        const bool narrow = have && sl_width(win[i].cnt[0], win[i].cnt[1], A.group_min) == 8u;
+        const uint32_t bn = __ballot_sync(FULL, narrow), bw = __ballot_sync(FULL, have && !narrow);
+        uint32_t pn = 0, pw = 0;
+        if (lane == 0) {
+          if (bn) pn = atomicAdd(&sh.nnarrow, (uint32_t)__popc(bn));
+          if (bw) pw = atomicAdd(&sh.nwide, (uint32_t)__popc(bw));
         }
+        pn = __shfl_sync(FULL, pn, 0);
+        pw = __shfl_sync(FULL, pw, 0);
+        const uint32_t below = (1u << lane) - 1u;
+        if (narrow) win[pn + __popc(bn & below)].order = i;
+        else if (have) win[nb - 1 - (pw + __popc(bw & below))].order = i;
       }
       __syncthreads();
-      SL_MARK(7);
-      // E2c: link condition by ballots / shuffles over the ring lists (a lane holds one ring face of
-      // each endpoint), then the collapse itself.  Winners whose rings have at most 16 faces (almost
-      // all) are handled by HALF warps, two winners per warp at a time: the pass is a chain of
-      // dependent shared-memory accesses per winner, so its duration is the number of winners a warp
-      // handles one after the other.  The few winners with larger rings take a second pass with
-      // whole warps.
-      sl_collapse_pass<SM, R, 16>(A, L, sh, nb);
-      __syncthreads();
-      if (sh.nbig) {
-        sl_collapse_pass<SM, R, 32>(A, L, sh, nb);
-      }
-      __syncthreads();
-      SL_MARK(8);
-      // E2d: the kept vertex k of every collapse has its final quadric and position, and so do its
-      // neighbours (winners are two apart, in this pass and in the later passes of the round), so the
-      // costs of k's edges are final until the next round: re-cost them now, one item per (winner, side,
-      // ring entry) as in E2b.  Every alive face of the two ring lists holds k, and each is in one list.
       {
         uint32_t nev = 0;
-        for (uint32_t j0 = 0; j0 < (uint32_t)S_MAXV; j0 += 16) {
-          if (j0 != 0 && !sh.bigring) break;
-          for (uint32_t item = tid; item < nb * 32; item += NT) {
-            const uint32_t i = item >> 5, side = (item >> 4) & 1u, j = j0 + (item & 15u);
-            if (!(win[i].flags & WF_DONE) || j >= win[i].cnt[side]) continue;
-            const uint32_t f = L.ring[(2 * i + side) * S_MAXV + j];
-            const uint32_t st = L.fstate[f];
-            if (!(st & 0x80u)) continue;  // died with the edge
-            L.fstate[f] = (uint8_t)sl_recost<SM, R>(A, L, f, st, win[i].keep, &nev);
-          }
-        }
+        const uint32_t wmin = A.group_min, n8 = sh.nnarrow;
+        if (n8) sl_group_pass<SM, R, 8>(A, L, sh, 0, n8, &nev);
+        if (wmin == 16u || (wmin == 8u && sh.ring8)) sl_group_pass<SM, R, 16>(A, L, sh, n8, nb, &nev);
+        if (wmin == 32u || sh.ring16) sl_group_pass<SM, R, 32>(A, L, sh, n8, nb, &nev);
         if (nev) atomicAdd(&sh.nrecost, nev);
       }
-      __syncthreads();  // (the next pass resets sh.bigring and the winner records)
-      SL_MARK(10);
+      __syncthreads();  // (the next pass resets the ring flags and the winner records)
+      SL_MARK(7);
       if (total <= L.wcap) break;
     }
     if (tid == 0) {
@@ -1245,7 +1319,7 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
       sh.stop = stop;
     }
     __syncthreads();
-    SL_MARK(9);
+    SL_MARK(8);
     if (sh.stop) {
       r++;
       break;
@@ -1298,6 +1372,8 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
   }
   if (tid == 0) {
     if (sh.nrecost) atomicAdd(&A.counters[27], sh.nrecost);
+    for (int w = 0; w < 3; w++)
+      if (sh.ngroup[w]) atomicAdd(&A.counters[29 + w], sh.ngroup[w]);
     if (!migrated) atomicMax(&A.counters[1], (uint32_t)r);
     if (!R) {  // a label counts in the class it started in
       atomicAdd(&A.counters[SM ? 2 : 3], 1u);
@@ -1499,6 +1575,7 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   for (int c = 0; c < SL_NCLASS; c++) m->simp_labels_class[c] = m->simp_migrations[c] = 0;
   m->simp_passes[0] = m->simp_passes[1] = 0;
   m->simp_costs[0] = m->simp_costs[1] = m->simp_costs[2] = 0;
+  m->simp_groups[0] = m->simp_groups[1] = m->simp_groups[2] = 0;
   const uint64_t U = m->U, T = m->T, K = m->K;
   if (T == 0 || U == 0) {
     m->simplified = true;
@@ -1641,6 +1718,11 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   // IGN_SIMP_WCAP=n (test knob): at most n winners per selection pass, so that rounds take several passes
   const char* wcap_env = getenv("IGN_SIMP_WCAP");
   A.wcap_max = wcap_env && atoi(wcap_env) > 0 ? (uint32_t)atoi(wcap_env) : 0xFFFFFFFFu;
+  // IGN_SIMP_GROUP=16|32 (test knob): the narrowest lane group E2 gives a winner, so that the wider sweeps
+  // take the winners with small rings too
+  const char* group_env = getenv("IGN_SIMP_GROUP");
+  const int group = group_env ? atoi(group_env) : 0;
+  A.group_min = group == 16 || group == 32 ? (uint32_t)group : 8u;
   {
     const int slot = prof_begin(ctx, IGN_PROF_SIMP);
     // default: one CTA per label (SMs are handed back to the block scheduler after every label, so
@@ -1750,13 +1832,14 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
     IGN_CUDA(cudaMemcpy(tr.data(), A.trace, 1600 * 4, cudaMemcpyDeviceToHost));
     unsigned long long phs[SL_NPH];
     IGN_CUDA(cudaMemcpy(phs, A.trace + 1600, sizeof(phs), cudaMemcpyDeviceToHost));
-    static const char* names[SL_NPH] = {"P1", "P2 keys", "P3 lose", "P4 select", "setup", "E1 rings", "E2a cost", "E2b flips", "E2c link+collapse", "stop+compact", "E2d recost"};
+    static const char* names[SL_NPH] = {"P1", "P2 keys", "P3 lose", "P4 select", "setup", "E1 rings", "E2a cost", "E2 validate+collapse+recost", "stop+compact"};
     unsigned long long tot = 0;
     for (int q = 0; q < SL_NPH; q++) tot += phs[q];
     for (int q = 0; q < SL_NPH; q++)
-      fprintf(stderr, "phase %-18s %6.2f %%  %10.3f Mcycles\n", names[q], 100.0 * phs[q] / (tot ? tot : 1), phs[q] / 1e6);
-    fprintf(stderr, "cost evaluations: %u initial (k_simp_ecost), %u after collapses (E2d), %u half-edges without a cost in P2\n",
+      fprintf(stderr, "phase %-27s %6.2f %%  %10.3f Mcycles\n", names[q], 100.0 * phs[q] / (tot ? tot : 1), phs[q] / 1e6);
+    fprintf(stderr, "cost evaluations: %u initial (k_simp_ecost), %u after collapses (E2), %u half-edges without a cost in P2\n",
             hflags[26], hflags[27], hflags[28]);
+    fprintf(stderr, "winners by E2 group width: %u of 8 lanes, %u of 16, %u of 32\n", hflags[29], hflags[30], hflags[31]);
     {
       // per-label records: where do the cycles go -- per round (fixed latency) or per face visit?
       std::vector<uint32_t> rec(SL_LREC * (size_t)K);
@@ -1825,6 +1908,7 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   m->simp_passes[0] = hflags[24];
   m->simp_passes[1] = hflags[25];
   for (int i = 0; i < 3; i++) m->simp_costs[i] = hflags[26 + i];
+  for (int i = 0; i < 3; i++) m->simp_groups[i] = hflags[29 + i];
   const uint32_t U2 = last[0] + last[1], T2 = last[2] + last[3];
   IGN_LAUNCH(ctx, k_simp_new_offsets, blocks_for(K + 2, 256), 256, 0, d_vert_off, vscan, (uint32_t)(K + 2), U, U2,
                    d_new_vert_off);
@@ -1876,5 +1960,12 @@ extern "C" int ign_mesh_simplify_costs(ign_mesher* m, uint32_t counts[3]) {
   IGN_REQUIRE(m && counts, IGN_ERR_INVALID, "null argument");
   IGN_REQUIRE(m->simplified, IGN_ERR_INVALID, "mesher is not simplified");
   for (int i = 0; i < 3; i++) counts[i] = m->simp_costs[i];
+  return IGN_OK;
+}
+
+extern "C" int ign_mesh_simplify_groups(ign_mesher* m, uint32_t counts[3]) {
+  IGN_REQUIRE(m && counts, IGN_ERR_INVALID, "null argument");
+  IGN_REQUIRE(m->simplified, IGN_ERR_INVALID, "mesher is not simplified");
+  for (int i = 0; i < 3; i++) counts[i] = m->simp_groups[i];
   return IGN_OK;
 }

@@ -501,6 +501,10 @@ IGN_API int ign_mesh_simplify_passes(ign_mesher* m, uint32_t counts[2]);
  * [1] half-edges re-costed after the collapse that moved an endpoint, [2] half-edges the key pass met
  * without a cached cost (0 unless the simplifier is broken; such an edge posts no key) */
 IGN_API int ign_mesh_simplify_costs(ign_mesher* m, uint32_t counts[3]);
+/* winners of the simplification that ran, by the width of the lane group that validated, collapsed and
+ * re-costed them: [0] 8 lanes (rings of at most 8 faces), [1] 16 lanes, [2] 32 lanes (rings over 16 faces,
+ * and those over 32 that are rejected); IGN_SIMP_GROUP=16 or 32 sets the narrowest width */
+IGN_API int ign_mesh_simplify_groups(ign_mesher* m, uint32_t counts[3]);
 /* bulk export of every label's mesh (simplified if ign_mesh_simplify ran) in ign_mesh_ids order:
  * vertices f32 [U,3], faces u32 [T,3] (label-local indices), offsets [n_ids+1] */
 IGN_API int ign_mesh_export(ign_mesher* m, const float resolution[3], int voxel_centered,
