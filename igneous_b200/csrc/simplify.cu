@@ -122,20 +122,11 @@ struct SEval {
   double p[3];
 };
 
-// collapse cost of the edge (u, v) (min over {u, v, midpoint} of p^T (Qu+Qv) p, boundary endpoints stay
-// put): u / v are vertex ids of any one numbering (they pick the kept vertex), gu / gv their rows of Q and
-// pos.  Invalid when both endpoints are on the boundary or the cost exceeds max_err2.
-__device__ __forceinline__ void s_cost(const double* Q, const double* pos, double max_err2, uint32_t u, uint32_t v,
-                                       uint64_t gu, uint64_t gv, bool bu, bool bv, SEval* e) {
+// s_cost from the summed quadric q = Qu + Qv and the endpoint positions pu, pv (memory or registers)
+__device__ __forceinline__ void s_cost_q(const double* q, const double* pu, const double* pv, double max_err2,
+                                         uint32_t u, uint32_t v, bool bu, bool bv, SEval* e) {
   e->valid = false;
   if (bu && bv) return;
-  const double* Qu = Q + 10 * gu;
-  const double* Qv = Q + 10 * gv;
-  double q[10];
-#pragma unroll
-  for (int i = 0; i < 10; i++) q[i] = Qu[i] + Qv[i];
-  const double* pu = pos + 3 * gu;
-  const double* pv = pos + 3 * gv;
   double best[3], cost;
   if (bu) {
     e->keep = u;
@@ -150,9 +141,10 @@ __device__ __forceinline__ void s_cost(const double* Q, const double* pos, doubl
   } else {
     e->keep = u < v ? u : v;
     e->remove = u < v ? v : u;
-    const double* pk = u < v ? pu : pv;
-    const double* pr = u < v ? pv : pu;
-    const double kk[3] = {pk[0], pk[1], pk[2]}, rr[3] = {pr[0], pr[1], pr[2]};
+    // (selected per component: a pointer select would put register arrays in local memory)
+    const bool uk = u < v;
+    const double kk[3] = {uk ? pu[0] : pv[0], uk ? pu[1] : pv[1], uk ? pu[2] : pv[2]};
+    const double rr[3] = {uk ? pv[0] : pu[0], uk ? pv[1] : pu[1], uk ? pv[2] : pu[2]};
     const double mid[3] = {(kk[0] + rr[0]) * 0.5, (kk[1] + rr[1]) * 0.5, (kk[2] + rr[2]) * 0.5};
     const double ck = s_qeval(q, kk), cr = s_qeval(q, rr), cm = s_qeval(q, mid);
     cost = ck;
@@ -165,6 +157,21 @@ __device__ __forceinline__ void s_cost(const double* Q, const double* pos, doubl
   e->valid = true;
   e->cost = cost;
   e->p[0] = best[0]; e->p[1] = best[1]; e->p[2] = best[2];
+}
+
+// collapse cost of the edge (u, v) (min over {u, v, midpoint} of p^T (Qu+Qv) p, boundary endpoints stay
+// put): u / v are vertex ids of any one numbering (they pick the kept vertex), gu / gv their rows of Q and
+// pos.  Invalid when both endpoints are on the boundary or the cost exceeds max_err2.
+__device__ __forceinline__ void s_cost(const double* Q, const double* pos, double max_err2, uint32_t u, uint32_t v,
+                                       uint64_t gu, uint64_t gv, bool bu, bool bv, SEval* e) {
+  e->valid = false;
+  if (bu && bv) return;
+  const double* Qu = Q + 10 * gu;
+  const double* Qv = Q + 10 * gv;
+  double q[10];
+#pragma unroll
+  for (int i = 0; i < 10; i++) q[i] = Qu[i] + Qv[i];
+  s_cost_q(q, pos + 3 * gu, pos + 3 * gv, max_err2, u, v, bu, bv, e);
 }
 
 // ------------------------------------------------------------------ kernels
@@ -452,6 +459,9 @@ constexpr int SL_HIST = 1664, SL_HP = 16, SL_HW = 64, SL_HR = S_MAXV + 2, SL_HCL
 constexpr int SL_MREC = 8;
 constexpr int SL_LREC = 7;  // words of a label's IGN_SIMP_TRACE record (SlArgs::lrec)
 constexpr int SL_NPH = 9;  // IGN_SIMP_TRACE phase timers (trace words 1600.., 64 bits each)
+// IGN_SIMP_TRACE E2 flip tests (trace words SL_TFLIP..): winners rejected by flips on the u side only, on the
+// v side only, on both sides
+constexpr int SL_TFLIP = 1620;
 
 struct SlShared {
   uint32_t work, alive, progress, ncol, nwin, stop, slow, counter, npass;
@@ -572,13 +582,35 @@ template <bool SM>
 __device__ __forceinline__ uint32_t sl_kcorner(const SlLab<SM>& L, uint32_t f, uint32_t k) {
   return sl_fget<SM>(L, f, 0) == k ? 0u : (sl_fget<SM>(L, f, 1) == k ? 1u : 2u);
 }
-// Re-cost the half-edge that starts at corner c of face f: cached float cost, and the memo to store (2 cached,
-// 3 exceeds max_error)
-template <bool SM, bool R>
-__device__ __forceinline__ uint32_t sl_recost(const SlArgs& A, const SlLab<SM>& L, uint32_t f, uint32_t c) {
-  const uint32_t u = sl_fget<SM>(L, f, (int)c), v = sl_fget<SM>(L, f, (int)((c + 1) % 3));
+// Re-cost the half-edge that starts at corner c of face f (if `has`), one of whose endpoints is the vertex k
+// that a collapse of the lane's group has just moved: cached float cost, and the memo to store (2 cached,
+// 3 exceeds max_error).  k's new quadric comes by shuffles from the group lanes that summed it (component i
+// in lane i; with 8 lanes, components 8-9 in qs2 of lanes 0-1) and its new position is the winner's
+// placement pk, so only the other endpoint's rows of Q and pos are loaded.  Every lane of the warp calls it.
+template <bool SM, bool R, int W>
+__device__ __forceinline__ uint32_t sl_recost_k(const SlArgs& A, const SlLab<SM>& L, bool has, uint32_t f,
+                                                uint32_t c, uint32_t k, double qs, double qs2, const double* pk) {
+  uint32_t u = k, v = k;
+  if (has) { u = sl_fget<SM>(L, f, (int)c); v = sl_fget<SM>(L, f, (int)((c + 1) % 3)); }
+  const bool ku = (u == k);
+  const uint64_t go = sl_vg<SM, R>(L, ku ? v : u);
+  double q[10], po[3] = {0.0, 0.0, 0.0};
+#pragma unroll
+  for (int i = 0; i < 10; i++) q[i] = has ? A.Q[10 * go + i] : 0.0;
+  if (has) { po[0] = A.pos[3 * go]; po[1] = A.pos[3 * go + 1]; po[2] = A.pos[3 * go + 2]; }
+#pragma unroll
+  for (int i = 0; i < 10; i++)  // Q[k] + Q[o]: IEEE addition is commutative, so the sum has s_cost's bits
+    q[i] += __shfl_sync(0xFFFFFFFFu, (W == 8 && i >= 8) ? qs2 : qs, (W == 8 && i >= 8) ? i - 8 : i, W);
+  if (!has) return 0;
+  double pu[3], pv[3];
+#pragma unroll
+  for (int i = 0; i < 3; i++) {
+    const double b = pk[i];
+    pu[i] = ku ? b : po[i];
+    pv[i] = ku ? po[i] : b;
+  }
   SEval ev;
-  sl_cost<SM, R>(A, L, u, v, &ev);
+  s_cost_q(q, pu, pv, A.max_err2, u, v, (L.vflag[u] & VF_BOUND) != 0, (L.vflag[v] & VF_BOUND) != 0, &ev);
   if (!ev.valid) return 3;
   A.ecost[3 * (uint64_t)(L.tbase + sl_fo<SM, R>(L, f)) + c] = __double2float_rn(ev.cost);
   return 2;
@@ -722,11 +754,12 @@ __device__ __forceinline__ uint32_t sl_width(uint32_t nfu, uint32_t nfv, uint32_
 // no barrier in between: that is safe because winners are two apart (§5 of DESIGN.md), so no other
 // group writes a face, a state byte, a quadric or a position that this group reads or writes.  Lane gl
 // holds ring entry gl of each side.  The groups of a warp run the same instructions; everything that
-// differs between them is predicated and loop counts are made warp uniform.  *nev counts the re-costed
-// half-edges.
+// differs between them is predicated and loop counts are made warp uniform.  Warp w0 takes the first G
+// winners and the warps after it (cyclically) the next ones, so that a sweep starts on the warps that the
+// previous sweep's last round left idle.  *nev counts the re-costed half-edges.
 template <bool SM, bool R, int W>
 __device__ __forceinline__ void sl_group_pass(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, uint32_t first,
-                                              uint32_t last, uint32_t* nev) {
+                                              uint32_t last, uint32_t w0, uint32_t* nev) {
   static_assert(W == 8 || W == 16 || W == 32, "group width");
   const uint32_t FULL = 0xFFFFFFFFu;
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5, NW = blockDim.x >> 5;
@@ -736,7 +769,7 @@ __device__ __forceinline__ void sl_group_pass(const SlArgs& A, const SlLab<SM>& 
   const uint32_t gmask = wmask << goff;
   const uint32_t gidx = lane / W;
   SlWin* const win = sl_win();
-  for (uint32_t base = first + warp * G; base < last; base += NW * G) {  // warp uniform
+  for (uint32_t base = first + ((warp + NW - w0) % NW) * G; base < last; base += NW * G) {  // warp uniform
     bool act = base + gidx < last;
     uint32_t slot = 0, nfu = 0, nfv = 0;
     if (act) {
@@ -748,12 +781,12 @@ __device__ __forceinline__ void sl_group_pass(const SlArgs& A, const SlLab<SM>& 
     if (!b_act) continue;  // no winner of this width in the warp's slots
     if (lane == 0) atomicAdd(&sh.ngroup[W == 8 ? 0 : (W == 16 ? 1 : 2)], (uint32_t)__popc(b_act));
     if (W == 32 && act && gl == 0 && (nfu > (uint32_t)S_MAXV || nfv > (uint32_t)S_MAXV)) atomicAdd(&A.counters[25], 1u);
-    uint32_t fu = 0, fv = 0, u = 0, v = 0, hl = 0, k = 0;
+    uint32_t fu = 0, fv = 0, u = 0, v = 0, k = 0;
     bool ok = false;
     if (act) {
       if (gl < nfu) fu = L.ring[(2 * slot) * S_MAXV + gl];
       if (gl < nfv) fv = L.ring[(2 * slot + 1) * S_MAXV + gl];
-      u = win[slot].u; v = win[slot].v; hl = win[slot].h; k = win[slot].keep;
+      u = win[slot].u; v = win[slot].v; k = win[slot].keep;
       ok = !(win[slot].flags & WF_BAD) && nfu <= (uint32_t)S_MAXV && nfv <= (uint32_t)S_MAXV;
     }
     uint32_t au[3] = {0, 0, 0}, av[3] = {0, 0, 0};
@@ -761,11 +794,13 @@ __device__ __forceinline__ void sl_group_pass(const SlArgs& A, const SlLab<SM>& 
     if (ok && gl < nfv) { av[0] = sl_fget<SM>(L, fv, 0); av[1] = sl_fget<SM>(L, fv, 1); av[2] = sl_fget<SM>(L, fv, 2); }
     // flip tests of the faces that survive the collapse (those holding the other endpoint die with the
     // edge), one side after the other; one flipping face rejects the winner
-    {
-      bool flip = false;
-      if (ok && gl < nfu && au[0] != v && au[1] != v && au[2] != v) flip = sl_flips<SM, R>(A, L, au, u, win[slot].best);
-      if (ok && gl < nfv && av[0] != u && av[1] != u && av[2] != u) flip |= sl_flips<SM, R>(A, L, av, v, win[slot].best);
-      if (__ballot_sync(FULL, flip) & gmask) ok = false;
+    uint32_t flip = 0;  // bit 0: the lane's u-side face flips, bit 1: its v-side face
+    if (ok && gl < nfu && au[0] != v && au[1] != v && au[2] != v && sl_flips<SM, R>(A, L, au, u, win[slot].best)) flip = 1u;
+    if (ok && gl < nfv && av[0] != u && av[1] != u && av[2] != u && sl_flips<SM, R>(A, L, av, v, win[slot].best)) flip |= 2u;
+    if (__ballot_sync(FULL, flip != 0) & gmask) ok = false;
+    if (A.trace != nullptr) {
+      const uint32_t b_u = __ballot_sync(FULL, flip & 1u) & gmask, b_v = __ballot_sync(FULL, flip & 2u) & gmask;
+      if (act && gl == 0 && (b_u || b_v)) atomicAdd(&A.trace[SL_TFLIP + (b_u && b_v ? 2 : (b_u ? 0 : 1))], 1u);
     }
     const uint32_t rm = (k == u) ? v : u;
     // the quadrics of the two endpoints are needed only if the collapse happens, but the L2 round
@@ -782,6 +817,9 @@ __device__ __forceinline__ void sl_group_pass(const SlArgs& A, const SlLab<SM>& 
     uint32_t x1 = 0xF0000000u + lane, x2 = 0xF1000000u + lane, y1 = 0xF2000000u + lane, y2 = 0xF3000000u + lane;
     if (hu) sl_others(au, u, &x1, &x2);
     if (hv) sl_others(av, v, &y1, &y2);
+    const bool rm_is_u = (rm == u);
+    // rm's corner of the lane's face of rm (the collapse writes k there)
+    const uint32_t crm = rm_is_u ? (au[0] == u ? 0u : (au[1] == u ? 1u : 2u)) : (av[0] == v ? 0u : (av[1] == v ? 1u : 2u));
     // (every lane of the warp takes part in the collectives below; n = 0 for groups without a winner)
     const uint32_t nu = ok ? nfu : 0u, nv = ok ? nfv : 0u;
     uint32_t nmax = nu > nv ? nu : nv;
@@ -815,32 +853,31 @@ __device__ __forceinline__ void sl_group_pass(const SlArgs& A, const SlLab<SM>& 
     const uint32_t common = __popc(b_c1 & gmask) + __popc(b_c2 & gmask), shared = __popc(b_sh & gmask);
     const bool go = ok && nnu <= (uint32_t)S_MAXV && nnv <= (uint32_t)S_MAXV && shared == 2 && common == 2;
     if (act && !go && gl == 0) {  // park the edge until one of its endpoints' rings changes
-      const uint32_t f = hl / 3, c = hl - 3 * f;
+      const uint32_t hl = win[slot].h, f = hl / 3, c = hl - 3 * f;
       const uint32_t st = L.fstate[f];  // (winners of one pass never share a face: byte accesses are disjoint)
       L.fstate[f] = (uint8_t)((st & ~(3u << (2 * c))) | (1u << (2 * c)));
       sl_vclear<SM>(L.vflag, u, VF_END);
       sl_vclear<SM>(L.vflag, v, VF_END);
       atomicOr(&sh.progress, 1u);
     }
-    const bool rm_is_u = (rm == u);
     const bool hr = go && (rm_is_u ? hu : hv);
     const uint32_t rf = rm_is_u ? fu : fv;
-    const uint32_t r0 = rm_is_u ? au[0] : av[0], r1 = rm_is_u ? au[1] : av[1], r2 = rm_is_u ? au[2] : av[2];
     // faces of rm: those that also hold k die, the others get k in rm's corner
-    const bool dies = hr && (r0 == k || r1 == k || r2 == k);
+    const bool dies = hr && (rm_is_u ? (x1 == k || x2 == k) : (y1 == k || y2 == k));
     if (hr) {
       if (dies) L.fstate[rf] = (uint8_t)(L.fstate[rf] & 0x7Fu);
-      else sl_fset<SM>(L, rf, r0 == rm ? 0 : (r1 == rm ? 1 : 2), k);
+      else sl_fset<SM>(L, rf, (int)crm, k);
     }
     const uint32_t dead = __popc(__ballot_sync(FULL, dies) & gmask);
+    const double qs = qk + qr, qs2 = qk2 + qr2;  // k's new quadric: component gl (8-lane groups: gl + 8 in qs2)
     if (go) {
       // the new ring of k: parked edges around it may be valid now
       if (hu && x1 != v && x2 != v) { sl_vor<SM>(L.vflag, x1, VF_RDIRTY); sl_vor<SM>(L.vflag, x2, VF_RDIRTY); }
       if (hv && y1 != u && y2 != u) { sl_vor<SM>(L.vflag, y1, VF_RDIRTY); sl_vor<SM>(L.vflag, y2, VF_RDIRTY); }
-      if (gl < 10) Qk[gl] = qk + qr;
+      if (gl < 10) Qk[gl] = qs;
       if (gl >= 10 && gl < 13) A.pos[3 * gk + (gl - 10)] = win[slot].best[gl - 10];
       if (W == 8) {
-        if (gl < 2) Qk[gl + 8] = qk2 + qr2;
+        if (gl < 2) Qk[gl + 8] = qs2;
         else if (gl < 5) A.pos[3 * gk + (gl - 2)] = win[slot].best[gl - 2];
       }
       if (gl == 0) {
@@ -857,8 +894,8 @@ __device__ __forceinline__ void sl_group_pass(const SlArgs& A, const SlLab<SM>& 
     // state byte has one writer: the lane that holds it).  The canonical half-edges of k (bit 2 side + t of
     // m, sl_kcorner) are dealt out to the group's lanes, item i to lane i mod W, so that a lane evaluates
     // about one cost instead of up to four one after the other; the memos go back to the lanes that hold
-    // the faces.
-    __syncwarp();  // Q[k], pos[k] and the rewritten faces are visible to the group
+    // the faces.  k's quadric and position come from the group's registers (sl_recost_k).
+    __syncwarp();  // the rewritten faces and state bytes are visible to the group
     uint32_t m = 0, ck = 0, st0 = 0, st1 = 0;
     if (go && gl < nfu) {
       st0 = L.fstate[fu];
@@ -899,14 +936,17 @@ __device__ __forceinline__ void sl_group_pass(const SlArgs& A, const SlLab<SM>& 
       const uint32_t mo = __shfl_sync(FULL, m, own, W), po = __shfl_sync(FULL, P, own, W);
       const uint32_t fuo = __shfl_sync(FULL, fu, own, W), fvo = __shfl_sync(FULL, fv, own, W);
       const uint32_t cko = __shfl_sync(FULL, ck, own, W);
-      if (idx < N) {
+      const bool has = idx < N;
+      uint32_t f = 0, c = 0;
+      if (has) {
         uint32_t b = mo;
         for (uint32_t q = idx - po; q; q--) b &= b - 1;  // the (idx - po)-th item of the owner
         const uint32_t bit = (uint32_t)__ffs(b) - 1, side = bit >> 1;
-        const uint32_t c = (((cko >> (2 * side)) & 3u) + 2u * (bit & 1u)) % 3u;
-        res |= sl_recost<SM, R>(A, L, side ? fvo : fuo, c) << (2 * r);
+        c = (((cko >> (2 * side)) & 3u) + 2u * (bit & 1u)) % 3u;
+        f = side ? fvo : fuo;
         (*nev)++;
       }
+      res |= sl_recost_k<SM, R, W>(A, L, has, f, c, k, qs, qs2, win[slot].best) << (2 * r);
     }
     uint32_t q = P;
 #pragma unroll
@@ -1283,9 +1323,18 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
       {
         uint32_t nev = 0;
         const uint32_t wmin = A.group_min, n8 = sh.nnarrow;
-        if (n8) sl_group_pass<SM, R, 8>(A, L, sh, 0, n8, &nev);
-        if (wmin == 16u || (wmin == 8u && sh.ring8)) sl_group_pass<SM, R, 16>(A, L, sh, n8, nb, &nev);
-        if (wmin == 32u || sh.ring16) sl_group_pass<SM, R, 32>(A, L, sh, n8, nb, &nev);
+        // each sweep continues the deal of winners to warps where the previous one stopped: the wide
+        // winners go to the warps that the 8-lane sweep's last round left without a winner
+        uint32_t w0 = 0;
+        if (n8) {
+          sl_group_pass<SM, R, 8>(A, L, sh, 0, n8, w0, &nev);
+          w0 = (w0 + (n8 + 3u) / 4u) % NW;
+        }
+        if (wmin == 16u || (wmin == 8u && sh.ring8)) {
+          sl_group_pass<SM, R, 16>(A, L, sh, n8, nb, w0, &nev);
+          w0 = (w0 + (nb - n8 + 1u) / 2u) % NW;
+        }
+        if (wmin == 32u || sh.ring16) sl_group_pass<SM, R, 32>(A, L, sh, n8, nb, w0, &nev);
         if (nev) atomicAdd(&sh.nrecost, nev);
       }
       __syncthreads();  // (the next pass resets the ring flags and the winner records)
@@ -1828,8 +1877,8 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
     return IGN_ERR_UNSUPPORTED;
   }
   if (A.trace) {
-    std::vector<uint32_t> tr(1600);
-    IGN_CUDA(cudaMemcpy(tr.data(), A.trace, 1600 * 4, cudaMemcpyDeviceToHost));
+    std::vector<uint32_t> tr(SL_HIST);
+    IGN_CUDA(cudaMemcpy(tr.data(), A.trace, SL_HIST * 4, cudaMemcpyDeviceToHost));
     unsigned long long phs[SL_NPH];
     IGN_CUDA(cudaMemcpy(phs, A.trace + 1600, sizeof(phs), cudaMemcpyDeviceToHost));
     static const char* names[SL_NPH] = {"P1", "P2 keys", "P3 lose", "P4 select", "setup", "E1 rings", "E2a cost", "E2 validate+collapse+recost", "stop+compact"};
@@ -1840,6 +1889,8 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
     fprintf(stderr, "cost evaluations: %u initial (k_simp_ecost), %u after collapses (E2), %u half-edges without a cost in P2\n",
             hflags[26], hflags[27], hflags[28]);
     fprintf(stderr, "winners by E2 group width: %u of 8 lanes, %u of 16, %u of 32\n", hflags[29], hflags[30], hflags[31]);
+    fprintf(stderr, "winners rejected by E2 flip tests: %u on the u side only, %u on the v side only, %u on both\n",
+            tr[SL_TFLIP], tr[SL_TFLIP + 1], tr[SL_TFLIP + 2]);
     {
       // per-label records: where do the cycles go -- per round (fixed latency) or per face visit?
       std::vector<uint32_t> rec(SL_LREC * (size_t)K);
