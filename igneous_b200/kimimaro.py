@@ -8,8 +8,10 @@ each label; each gets the fields of `teasar.fields`, then every object traces it
 round: the target is the valid voxel farthest from the root, the path runs to the skeleton built so far,
 and every path voxel invalidates a box of half-extents floor((scale * DBF + const) / anisotropy) around it.
 Objects, fields, the loop and the compaction of the skeleton run in libigneous_b200
-(igneous_b200/csrc/geodesic.cu); the host splits the compacted skeleton by label.  There is no CPU
-fallback.
+(igneous_b200/csrc/geodesic.cu), and so does the split of the compacted skeleton into one neuroglancer
+precomputed skeleton per label (igneous_b200/csrc/skeleton.cu, DESIGN.md §5g): the host copies the packed
+blobs back once and every Skeleton's arrays are views into them.  export_skeletons is the same call with a
+vertex offset, the blobs and the bounding boxes, for SkeletonTask.  There is no CPU fallback.
 """
 import ctypes
 import time
@@ -19,7 +21,7 @@ import numpy as np
 from . import _shim
 from .teasar import device_fields
 
-__all__ = ["skeletonize", "Skeleton", "DEFAULT_TEASAR_PARAMS"]
+__all__ = ["skeletonize", "export_skeletons", "Skeleton", "DEFAULT_TEASAR_PARAMS"]
 
 # seconds per phase of the last call, each ending where the host already waits for the device (diagnostic)
 last_phase_seconds = {}
@@ -63,10 +65,26 @@ def skeletonize(all_labels, teasar_params=DEFAULT_TEASAR_PARAMS, object_ids=None
                 dust_threshold=1000, progress=False, fix_branching=True, in_place=False, fix_borders=True,
                 parallel=1, parallel_chunk_size=100, extra_targets_before=[], extra_targets_after=[],
                 fill_holes=False, fix_avocados=False, voxel_graph=None, ctx=None):
-  """{label: Skeleton} of every label of a 3-D array with an object of at least dust_threshold voxels.
-  `progress`, `parallel`, `parallel_chunk_size` and `in_place` are accepted and ignored.  fill_holes,
-  fix_avocados, voxel_graph and soma mode (an object whose largest DBF exceeds soma_detection_threshold)
-  raise NotImplementedError.  last_phase_seconds holds the host-clock time of each phase of the last call."""
+  """{label: Skeleton} of every label of a 3-D array with an object of at least dust_threshold voxels,
+  in ascending label order.  `progress`, `parallel`, `parallel_chunk_size` and `in_place` are accepted and
+  ignored.  fill_holes, fix_avocados, voxel_graph and soma mode (an object whose largest DBF exceeds
+  soma_detection_threshold) raise NotImplementedError.  last_phase_seconds holds the host-clock time of
+  each phase of the last call.  A Skeleton's arrays are writable views into one buffer of the call."""
+  return export_skeletons(all_labels, teasar_params=teasar_params, object_ids=object_ids, anisotropy=anisotropy,
+                          dust_threshold=dust_threshold, fix_branching=fix_branching, fix_borders=fix_borders,
+                          extra_targets_before=extra_targets_before, extra_targets_after=extra_targets_after,
+                          fill_holes=fill_holes, fix_avocados=fix_avocados, voxel_graph=voxel_graph, ctx=ctx)[0]
+
+
+def export_skeletons(all_labels, offset=(0.0, 0.0, 0.0), vertex_types=True, teasar_params=DEFAULT_TEASAR_PARAMS,
+                     object_ids=None, anisotropy=(1, 1, 1), dust_threshold=1000, fix_branching=True,
+                     fix_borders=True, extra_targets_before=[], extra_targets_after=[], fill_holes=False,
+                     fix_avocados=False, voxel_graph=None, ctx=None):
+  """skeletonize with every vertex moved by `offset` (float64, added as numpy adds it to float32 vertices:
+  fl32((double)v + offset)), encoded on the device.  Returns three dicts keyed alike, in ascending label
+  order: {label: Skeleton}, {label: uint8 array of its neuroglancer precomputed skeleton (vertices, edges,
+  radius, and vertex_types when `vertex_types`)}, {label: float32 (6,) min xyz, max xyz of its vertices}.
+  Every array is a view into one host buffer."""
   if fill_holes or fix_avocados or voxel_graph is not None:
     raise NotImplementedError("igneous_b200 kimimaro.skeletonize: fill_holes, fix_avocados and voxel_graph are "
                               "not supported")
@@ -91,8 +109,11 @@ def skeletonize(all_labels, teasar_params=DEFAULT_TEASAR_PARAMS, object_ids=None
   n = vol.size
   before = _targets(extra_targets_before, arr, "extra_targets_before")
   after = _targets(extra_targets_after, arr, "extra_targets_after")
+  shift = tuple(float(v) for v in offset)
+  if len(shift) != 3 or not all(np.isfinite(shift)):
+    raise ValueError("kimimaro.export_skeletons: offset %r must be three finite values" % (offset,))
   if n == 0:
-    return {}
+    return {}, {}, {}
   ctx = ctx or _shim.default_context()
   lib, h, ptr = ctx.lib, ctx.handle, _shim.ptr
   ca = (ctypes.c_float * 3)(*a)
@@ -119,14 +140,15 @@ def skeletonize(all_labels, teasar_params=DEFAULT_TEASAR_PARAMS, object_ids=None
     _shim.check(lib.ign_renumber_dev(h, ptr(raw), _shim.dtype_code(vol.dtype), n, ptr(lab), None, 0,
                                      ctypes.byref(k)))
     K = int(k.value)
-    if K and object_ids is not None:
+    orig = np.empty(K, np.uint64)
+    if K:
       # the original label of each renumbered one: renumber again into a table of K entries
       uniq = alloc(K * 8)
       _shim.check(lib.ign_renumber_dev(h, ptr(raw), _shim.dtype_code(vol.dtype), n, ptr(lab), ptr(uniq), K,
                                        ctypes.byref(k)))
-      orig = np.empty(K, np.uint64)
       ctx.d2h(orig, uniq)
       ctx.sync()
+    if K and object_ids is not None:
       wanted = np.asarray(list(object_ids)).astype(arr.dtype).view(_UNSIGNED[arr.dtype.itemsize]).astype(np.uint64)
       drop = np.ascontiguousarray(np.nonzero(~np.isin(orig, wanted))[0] + 1, dtype=np.uint64)
       if drop.size:
@@ -139,7 +161,7 @@ def skeletonize(all_labels, teasar_params=DEFAULT_TEASAR_PARAMS, object_ids=None
     M = int(m.value)
     phase("upload_objects")
     if M == 0:
-      return {}
+      return {}, {}, {}
     if fix_borders:
       # kimimaro's order: the caller's before-targets, then the border targets
       cap = 2 * (vol.shape[1] * vol.shape[2] + vol.shape[0] * vol.shape[2] + vol.shape[0] * vol.shape[1])
@@ -178,45 +200,64 @@ def skeletonize(all_labels, teasar_params=DEFAULT_TEASAR_PARAMS, object_ids=None
       ptr(d["dist"]) if fix_branching else None, None if fix_branching else ptr(d["parents"]), ptr(d["roots"]),
       ptr(d_before), before.size, ptr(d_after), after.size, scale, const, max_paths, ptr(skel), ptr(nxt), ptr(rad),
       ctypes.byref(count)))
-    c = int(count.value)
-    index, following, radii = np.empty(c, np.uint32), np.empty(c, np.uint32), np.empty(c, np.float32)
-    if c:
-      ctx.d2h(index, skel, c * 4)
-      ctx.d2h(following, nxt, c * 4)
-      ctx.d2h(radii, rad, c * 4)
-      ctx.sync()
+    ctx.sync()
     phase("loop")
+    buf, table, boxes = _export(ctx, lab, vol.shape, K, skel, nxt, rad, int(count.value), ca, shift, vertex_types,
+                                alloc)
   finally:
     for b in bufs:
       b.free()
-  out = _assemble(arr, index, following, radii, a)
+  out = _views(buf, table, boxes, orig, arr.dtype, vertex_types)
   phase("assembly")
   return out
 
 
-def _assemble(arr, index, following, radii, anisotropy):
-  """split the compacted skeleton (ascending F-order indices, next voxel, radius) by label"""
-  labels = arr.reshape(-1, order="F")[index]
-  order = np.argsort(labels, kind="stable")  # within a label the indices stay ascending
-  rank = np.empty(order.size, np.int64)
-  rank[order] = np.arange(order.size)
-  starts = np.concatenate([[0], np.flatnonzero(np.diff(labels[order])) + 1, [order.size]])
-  group = np.repeat(np.arange(starts.size - 1), np.diff(starts))  # label group of each sorted position
-  # edges (v, next(v)) as positions within the label, smaller first, sorted per label
-  tree = following != index
-  e0, e1 = rank[tree], rank[np.searchsorted(index, following[tree])]
-  g = group[e0]
-  lo, hi = np.minimum(e0, e1) - starts[g], np.maximum(e0, e1) - starts[g]
-  eo = np.lexsort((hi, lo, g))
-  edges = np.stack([lo[eo], hi[eo]], axis=1).astype(np.uint32)
-  ecut = np.searchsorted(g[eo], np.arange(starts.size))
-  coords = np.stack(np.unravel_index(index[order].astype(np.int64), arr.shape, order="F"), axis=1)
-  vertices = coords.astype(np.float32) * np.asarray(anisotropy, dtype=np.float32)
-  rad = radii[order].astype(np.float32)
-  out = {}
-  for j in range(starts.size - 1):
-    a, b = starts[j], starts[j + 1]
-    label = int(labels[order[a]])
-    out[label] = Skeleton(vertices[a:b], np.ascontiguousarray(edges[ecut[j]:ecut[j + 1]]), rad[a:b],
-                          np.zeros(b - a, np.uint8), label)
-  return out
+def _export(ctx, lab, shape, K, skel, nxt, rad, count, ca, offset, vertex_types, alloc):
+  """ign_skeleton_export_dev on the loop's output -> (packed blobs, table rows, boxes), copied back once"""
+  lib, h, ptr = ctx.lib, ctx.handle, _shim.ptr
+  cap = ctypes.c_uint64(0)
+  _shim.check(lib.ign_skeleton_export_capacity(count, K, ctypes.byref(cap)))
+  rows = min(K, count)
+  d_buf, d_table, d_boxes = alloc(cap.value), alloc(rows * 32), alloc(rows * 24)
+  ns, nb = ctypes.c_uint64(0), ctypes.c_uint64(0)
+  _shim.check(lib.ign_skeleton_export_dev(h, ptr(lab), *shape, K, ptr(skel), ptr(nxt), ptr(rad), count, ca,
+                                          (ctypes.c_double * 3)(*offset), int(bool(vertex_types)), ptr(d_buf),
+                                          cap.value, ptr(d_table), ptr(d_boxes), ctypes.byref(ns), ctypes.byref(nb)))
+  S, B = int(ns.value), int(nb.value)
+  buf = np.empty((B + 7) // 8 * 8, np.uint8)  # whole words, so that typed views of the buffer exist
+  buf[B:] = 0
+  table, boxes = np.empty((S, 4), np.uint64), np.empty((S, 6), np.float32)
+  if S:
+    ctx.d2h(buf, d_buf, B)
+    ctx.d2h(table, d_table)
+    ctx.d2h(boxes, d_boxes)
+    ctx.sync()
+  return buf, table, boxes
+
+
+def _views(buf, table, boxes, orig, dtype, vertex_types):
+  """split the packed blobs into {label: Skeleton}, {label: blob}, {label: box}, in ascending label order of
+  the caller's dtype; every array is a view into buf (or, without vertex_types, into one zero array)"""
+  unsigned = _UNSIGNED[np.dtype(dtype).itemsize]
+  values = orig[table[:, 0].astype(np.int64) - 1].astype(unsigned).view(dtype)
+  order = np.argsort(values, kind="stable")
+  keys = (values.astype(np.uint8) if values.dtype == np.bool_ else values)[order].tolist()
+  f32, u32 = buf.view(np.float32), buf.view(np.uint32)
+  zeros = None if vertex_types else np.zeros(int(table[:, 2].sum()), np.uint8)
+  skeletons, blobs, bx = {}, {}, {}
+  z = 0
+  for label, (off, nv, ne), box in zip(keys, table[order, 1:].tolist(), boxes[order]):
+    w = off // 4 + 2  # the vertices, in words
+    e = w + 3 * nv
+    r = e + 2 * ne
+    end = 4 * (r + nv)
+    if vertex_types:
+      vt = buf[end:end + nv]
+      end += nv
+    else:
+      vt = zeros[z:z + nv]
+      z += nv
+    skeletons[label] = Skeleton(f32[w:e].reshape(nv, 3), u32[e:r].reshape(ne, 2), f32[r:r + nv], vt, label)
+    blobs[label] = buf[off:end]
+    bx[label] = box
+  return skeletons, blobs, bx

@@ -296,6 +296,67 @@ class _MeshMeta:
   spatial_index = _SpatialIndex()
 
 
+# cloudvolume's default skeleton info, as recalled (unpinned): identity transform, radius then vertex_types
+DEFAULT_SKELETON_INFO = {
+  "@type": "neuroglancer_skeletons",
+  "transform": [1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0],
+  "vertex_attributes": [{"id": "radius", "data_type": "float32", "num_components": 1},
+                        {"id": "vertex_types", "data_type": "uint8", "num_components": 1}],
+  "sharding": None,
+  "spatial_index": None,
+}
+
+
+class _SkeletonMeta:
+  """cv.skeleton.meta: the skeleton directory's info ({info['skeletons']}/info, cloudvolume's default
+  when the file is absent) and commit_info()."""
+
+  def __init__(self, cv, subdir):
+    self._cv, self.subdir = cv, subdir
+    self.info = cv.cf.get_json(subdir + "/info") or copy.deepcopy(DEFAULT_SKELETON_INFO)
+
+  def commit_info(self):
+    self._cv.cf.put_json(self.subdir + "/info", self.info)
+
+
+class _SkeletonSource:
+  """cv.skeleton: meta, path, spatial_index (cv.mesh's) and get(segid) of unsharded precomputed skeletons."""
+
+  def __init__(self, cv):
+    subdir = cv.info.get("skeletons", "skeletons")  # cloudvolume's default directory, as recalled
+    self._cv = cv
+    self.meta = _SkeletonMeta(cv, subdir)
+    self.path = cv.cf.join(cv.cloudpath, subdir)
+    self.spatial_index = cv.mesh.spatial_index
+
+  def get(self, segid):
+    """The skeleton {dir}/{segid} decoded per meta.info['vertex_attributes'] (a list of ids -> a list)."""
+    if isinstance(segid, (list, tuple)):
+      return [self.get(s) for s in segid]
+    from .kimimaro import Skeleton
+    data = self._cv.cf.get("%s/%d" % (self.meta.subdir, int(segid)))
+    if data is None:
+      raise FileNotFoundError("no skeleton %d in %s" % (int(segid), self.path))
+    buf = np.frombuffer(data, dtype=np.uint8)
+    nv, ne = (int(v) for v in buf[:8].view(np.uint32))
+    at = 8
+    vertices = buf[at:at + 12 * nv].view(np.float32).reshape(nv, 3).copy()
+    at += 12 * nv
+    edges = buf[at:at + 8 * ne].view(np.uint32).reshape(ne, 2).copy()
+    at += 8 * ne
+    attrs = {}
+    for attr in self.meta.info.get("vertex_attributes") or []:
+      dt, k = np.dtype(attr["data_type"]), int(attr.get("num_components", 1))
+      size = nv * k * dt.itemsize
+      a = buf[at:at + size].view(dt).copy()
+      attrs[attr["id"]] = a if k == 1 else a.reshape(nv, k)
+      at += size
+    if at != buf.size:
+      raise ValueError("skeleton %d: %d bytes, the info's attributes describe %d" % (int(segid), buf.size, at))
+    radii = attrs.get("radius", np.zeros(nv, np.float32))
+    return Skeleton(vertices, edges, radii, attrs.get("vertex_types", np.zeros(nv, np.uint8)), int(segid))
+
+
 class _Meta:
   """cv.meta: per-mip accessors (cloudvolume's PrecomputedMetadata subset)."""
 
@@ -403,7 +464,7 @@ class CloudVolume:
     self.cf = CloudFiles(cloudpath)
     self.provenance = _Provenance()
     self.mesh = _MeshMeta()
-    self.skeleton = self.mesh  # cv.skeleton.spatial_index.precision is cv.mesh's
+    self._skeleton = None
     if info is not None:
       self.info = copy.deepcopy(info)
     else:
@@ -422,6 +483,13 @@ class CloudVolume:
   @property
   def image(self):
     return _ImageSource(self)
+
+  @property
+  def skeleton(self):
+    """the skeleton source, read on first use (its info file and directory follow info['skeletons'])"""
+    if self._skeleton is None:
+      self._skeleton = _SkeletonSource(self)
+    return self._skeleton
 
   @classmethod
   def create_new_info(cls, num_channels, layer_type, data_type, encoding, resolution, voxel_offset,

@@ -1,5 +1,98 @@
-"""create_spatial_index_skeleton_tasks (igneous/task_creation/skeleton.py:795-867)."""
-from .common import spatial_index_tasks
+"""create_skeletonizing_tasks (igneous/task_creation/skeleton.py:68-388) and
+create_spatial_index_skeleton_tasks (:795-867)."""
+from time import strftime
+
+import numpy as np
+
+from .._compat import CloudVolume, CloudFiles, Vec
+from ..tasks import SkeletonTask
+from ..tasks.skeleton import refuse
+from .common import FinelyDividedTaskIterator, operator_contact, spatial_index_tasks
+
+
+def create_skeletonizing_tasks(cloudpath, mip, shape=Vec(512, 512, 512), teasar_params={"scale": 10, "const": 10},
+                               info=None, object_ids=None, mask_ids=None, fix_branching=True, fix_borders=True,
+                               fix_avocados=False, fill_holes=0, dust_threshold=1000, progress=False, parallel=1,
+                               fill_missing=False, sharded=False, frag_path=None, spatial_index=True, synapses=None,
+                               num_synapses=None, dust_global=False, fix_autapses=False, cross_sectional_area=False,
+                               cross_sectional_area_smoothing_window=5, timestamp=None, root_ids_cloudpath=None,
+                               cross_sectional_area_repair_sec_per_label=0):
+  """Tasks with one voxel of overlap on the high side in a regular grid, to be densely skeletonized
+  (SkeletonTask); the fragments are merged by the reference's merge stage.  Records the layer's skeleton
+  directory (skeletons_mip_{mip} unless it has one), the skeleton info's @type, spatial_index, mip and
+  float32-only vertex_attributes, the frag_path info, and the provenance on completion.
+  The options SkeletonTask refuses (sharded, dust_global, synapses, cross_sectional_area, fix_autapses /
+  timestamp / root_ids_cloudpath, fix_avocados, fill_holes > 0) raise NotImplementedError here, before any
+  write.  The reference narrows the grid to the mesh bounds of up to four object_ids (bounds_from_mesh);
+  that needs mesh reads the storage layer here does not have, so the grid always covers the full bounds."""
+  assert 0 <= fill_holes <= 103, "fill_holes must be between 0 to 103 inclusive."
+  refuse("create_skeletonizing_tasks", sharded, dust_global, synapses, cross_sectional_area, fix_autapses,
+         timestamp, root_ids_cloudpath, fix_avocados, fill_holes)
+  shape = Vec(*shape)
+  vol = CloudVolume(cloudpath, mip=mip, info=info)
+  if "skeletons" not in vol.info:
+    vol.info["skeletons"] = "skeletons_mip_{}".format(mip)
+    vol.commit_info()
+
+  skel_info = vol.skeleton.meta.info
+  if spatial_index:
+    if "spatial_index" not in skel_info or not skel_info["spatial_index"]:
+      skel_info["spatial_index"] = {}
+    skel_info["@type"] = "neuroglancer_skeletons"
+    skel_info["spatial_index"]["resolution"] = tuple(vol.resolution.tolist())
+    skel_info["spatial_index"]["chunk_size"] = tuple((shape * vol.resolution).tolist())
+  skel_info["mip"] = int(mip)
+  skel_info["vertex_attributes"] = [attr for attr in skel_info["vertex_attributes"]
+                                    if attr["data_type"] == "float32"]
+  skel_info["vertex_attributes"] = [attr for attr in skel_info["vertex_attributes"]
+                                    if attr["id"] != "cross_sectional_area"]
+  vol.skeleton.meta.commit_info()
+
+  if frag_path:
+    cf = CloudFiles(frag_path)
+    frag_info = cf.get_json("info")
+    if not frag_info:
+      cf.put_json("info", vol.skeleton.meta.info)
+    elif "scales" in frag_info:
+      cf.put_json(cf.join(vol.info["skeletons"], "info"), vol.skeleton.meta.info)
+
+  will_postprocess = bool(np.any(vol.bounds.size3() > shape))
+  bounds = vol.bounds.clone()
+
+  class SkeletonTaskIterator(FinelyDividedTaskIterator):
+    def task(self, shape, offset):
+      return SkeletonTask(
+        cloudpath=cloudpath, shape=(shape + 1).clone(), offset=offset.clone(), mip=mip,
+        teasar_params=teasar_params, will_postprocess=will_postprocess, info=info, object_ids=object_ids,
+        mask_ids=mask_ids, fix_branching=fix_branching, fix_borders=fix_borders, fix_avocados=fix_avocados,
+        dust_threshold=dust_threshold, progress=progress, parallel=parallel, fill_missing=bool(fill_missing),
+        sharded=bool(sharded), frag_path=frag_path, spatial_index=bool(spatial_index),
+        spatial_grid_shape=shape.clone(), synapses=None, dust_global=dust_global, fix_autapses=bool(fix_autapses),
+        timestamp=timestamp, cross_sectional_area=bool(cross_sectional_area),
+        cross_sectional_area_smoothing_window=int(cross_sectional_area_smoothing_window),
+        root_ids_cloudpath=root_ids_cloudpath, fill_holes=fill_holes,
+        cross_sectional_area_repair_sec_per_label=int(cross_sectional_area_repair_sec_per_label))
+
+    def on_finish(self):
+      vol.provenance.processing.append({
+        "method": {
+          "task": "SkeletonTask", "cloudpath": cloudpath, "mip": mip, "shape": shape.tolist(),
+          "dust_threshold": dust_threshold, "teasar_params": teasar_params, "object_ids": object_ids,
+          "mask_ids": mask_ids, "will_postprocess": will_postprocess, "fix_branching": fix_branching,
+          "fix_borders": fix_borders, "fix_avocados": fix_avocados, "progress": progress, "parallel": parallel,
+          "fill_missing": bool(fill_missing), "sharded": bool(sharded), "spatial_index": bool(spatial_index),
+          "synapses": bool(synapses), "dust_global": bool(dust_global), "fix_autapses": bool(fix_autapses),
+          "timestamp": timestamp, "cross_sectional_area": bool(cross_sectional_area),
+          "cross_sectional_area_smoothing_window": int(cross_sectional_area_smoothing_window),
+          "cross_sectional_area_repair_sec_per_label": int(cross_sectional_area_repair_sec_per_label),
+          "root_ids_cloudpath": root_ids_cloudpath, "fill_holes": int(fill_holes),
+        },
+        "by": operator_contact(),
+        "date": strftime("%Y-%m-%d %H:%M %Z"),
+      })
+      vol.commit_provenance()
+
+  return SkeletonTaskIterator(bounds, shape)
 
 
 def create_spatial_index_skeleton_tasks(cloudpath, shape=(448, 448, 448), mip=0, fill_missing=False, compress="gzip",

@@ -456,6 +456,34 @@ IGN_API int ign_teasar_paths_dev(ign_ctx* ctx, const uint32_t* objects, uint64_t
                                  uint64_t n_after, float scale, float cnst, uint64_t max_paths,
                                  uint32_t* skel_out, uint32_t* next_out, float* radius_out, uint64_t* count);
 IGN_API int ign_teasar_last_stats(uint64_t stats[4]);
+/* Per-label export of a chunk's skeleton (SkeletonTask's vertex shift, spatial index and upload,
+ * igneous/tasks/skeleton.py:229-236, :772-807, and kimimaro.skeletonize's split by label; DESIGN.md §5g).
+ * Every array is a DEVICE array.
+ * ign_skeleton_export_dev: labels u32 1..max_label (renumbered) of an (sx, sy, sz) F-order volume; skel, next,
+ *   radius: the count entries of ign_teasar_paths_dev (skel ascending).  Out, for every label with a skeleton
+ *   voxel, in ascending label order, *n_skeletons of them (at most min(max_label, count)):
+ *     blobs_out  one neuroglancer precomputed skeleton per label, each starting on an 8-byte boundary (the
+ *                padding between blobs is zeros and belongs to none): uint32 nv, uint32 ne,
+ *                float32 vertices[nv][3], uint32 edges[ne][2], float32 radius[nv], and with vertex_types != 0
+ *                uint8 vertex_types[nv], all 0.  *nbytes = the end of the last blob.
+ *     table_out  uint64 [][4] rows (label, byte offset, nv, ne).
+ *     boxes_out  float32 [][6] rows (min x, min y, min z, max x, max y, max z) of the label's vertices.
+ *   A label's vertices are its skeleton voxels in ascending linear index; vertex i of voxel (x, y, z) is
+ *   fl32((double)fl32(fl32(x) * anisotropy[0]) + offset[0]), and likewise for y and z.  Every voxel v with
+ *   next(v) != v gives one edge (min, max) of the two local vertex indices; a label's edges are sorted by
+ *   (min, max).  capacity (bytes) must be at least count * 25 + min(max_label, count) * 16
+ *   (ign_skeleton_export_capacity), IGN_ERR_INVALID otherwise, before any launch.  A skeleton voxel outside
+ *   the volume, not above the one before it or on label 0 or above max_label, and a next voxel that is not
+ *   a skeleton voxel or lies on another label -> IGN_ERR_INVALID naming the lowest such voxel by linear
+ *   index; no cross-label edge is ever written.  The skeleton voxels are checked before any pass that
+ *   relies on them, the next voxels before any output is written.  The host synchronises three times.
+ * ign_skeleton_export_capacity: that bound for count skeleton voxels (IGN_ERR_OVERFLOW from 2^31). */
+IGN_API int ign_skeleton_export_dev(ign_ctx* ctx, const uint32_t* labels, uint64_t sx, uint64_t sy, uint64_t sz,
+                                    uint64_t max_label, const uint32_t* skel, const uint32_t* next,
+                                    const float* radius, uint64_t count, const float anisotropy[3],
+                                    const double offset[3], int vertex_types, uint8_t* blobs_out, uint64_t capacity,
+                                    uint64_t* table_out, float* boxes_out, uint64_t* n_skeletons, uint64_t* nbytes);
+IGN_API int ign_skeleton_export_capacity(uint64_t count, uint64_t max_label, uint64_t* bytes);
 
 /* --------------------------------------------------------------------- mesh
  * zmesh.Mesher(resolution).mesh(data, preserve_order=False)  igneous/tasks/mesh/mesh.py:151,245
