@@ -33,7 +33,8 @@ def _stale(target, deps):
 
 # simplify.cu must match the CPU oracle bit for bit, and contrast.cu the float32 rules of
 # DESIGN.md §5b (each product rounded on its own), geodesic.cu the penalty field of §5e: no FMA contraction
-PER_FILE_FLAGS = {"simplify.cu": ["-fmad=false"], "contrast.cu": ["-fmad=false"], "geodesic.cu": ["-fmad=false"]}
+PER_FILE_FLAGS = {"simplify.cu": ["-fmad=false"], "contrast.cu": ["-fmad=false"], "geodesic.cu": ["-fmad=false"],
+                  "skelmerge.cu": ["-fmad=false"]}
 
 
 def _compile(src, obj, log):

@@ -11,7 +11,8 @@ Objects, fields, the loop and the compaction of the skeleton run in libigneous_b
 (igneous_b200/csrc/geodesic.cu), and so does the split of the compacted skeleton into one neuroglancer
 precomputed skeleton per label (igneous_b200/csrc/skeleton.cu, DESIGN.md §5g): the host copies the packed
 blobs back once and every Skeleton's arrays are views into them.  export_skeletons is the same call with a
-vertex offset, the blobs and the bounding boxes, for SkeletonTask.  There is no CPU fallback.
+vertex offset, the blobs and the bounding boxes, for SkeletonTask.  postprocess and merge_fragments run
+the merge stage (igneous_b200/csrc/skelmerge.cu, DESIGN.md §5h).  There is no CPU fallback.
 """
 import ctypes
 import time
@@ -21,7 +22,7 @@ import numpy as np
 from . import _shim
 from .teasar import device_fields
 
-__all__ = ["skeletonize", "export_skeletons", "Skeleton", "DEFAULT_TEASAR_PARAMS"]
+__all__ = ["skeletonize", "export_skeletons", "postprocess", "merge_fragments", "Skeleton", "DEFAULT_TEASAR_PARAMS"]
 
 # seconds per phase of the last call, each ending where the host already waits for the device (diagnostic)
 last_phase_seconds = {}
@@ -261,3 +262,131 @@ def _views(buf, table, boxes, orig, dtype, vertex_types):
     blobs[label] = buf[off:end]
     bx[label] = box
   return skeletons, blobs, bx
+
+
+def crop_box(bbox, crop, resolution):
+  """The crop box of a fragment whose physical box is `bbox` (a Bbox, from its file name): shrunk by
+  crop * resolution on every side, float64 (min xyz, max xyz); None when crop <= 0 or the shrunk box has
+  volume <= 0, and then the fragment is kept whole (DESIGN.md §5h)."""
+  if crop <= 0:
+    return None
+  r = np.asarray(resolution, np.float64)[:3] * crop
+  lo, hi = np.asarray(bbox.minpt, np.float64) + r, np.asarray(bbox.maxpt, np.float64) - r
+  if np.prod(hi - lo) <= 0:
+    return None
+  return np.concatenate([lo, hi])
+
+
+def pack_fragments(fragments, crop=0, resolution=(1, 1, 1)):
+  """(segids, packed arrays) of {segid: [(bbox, Skeleton), ...]} in the layout of ign_skeleton_merge_dev: the
+  labels in the dict's order, each label's fragments in the order given.  bbox None keeps a fragment whole."""
+  segids = list(fragments)
+  whole = np.array([-np.inf] * 3 + [np.inf] * 3)
+  label_frag, frag_vert, frag_edge, boxes = [0], [0], [0], []
+  verts, radii, types, edges = [], [], [], []
+  for segid in segids:
+    for bbox, s in fragments[segid]:
+      v = np.asarray(s.vertices, np.float32).reshape(-1, 3)
+      e = np.asarray(s.edges).reshape(-1, 2)
+      if e.size and (e.min() < 0 or e.max() > 0xFFFFFFFF):
+        raise ValueError("skeleton merge: label %d has an edge index outside uint32" % segid)
+      box = None if bbox is None else crop_box(bbox, crop, resolution)
+      boxes.append(whole if box is None else box)
+      verts.append(v)
+      radii.append(np.asarray(s.radii, np.float32).reshape(-1) if s.radii is not None else np.zeros(len(v), np.float32))
+      types.append(np.asarray(s.vertex_types, np.uint8).reshape(-1) if s.vertex_types is not None
+                   else np.zeros(len(v), np.uint8))
+      if radii[-1].size != len(v) or types[-1].size != len(v):
+        raise ValueError("skeleton merge: label %d has a fragment whose radii or vertex_types do not match its "
+                         "%d vertices" % (segid, len(v)))
+      edges.append(e.astype(np.uint32))
+      frag_vert.append(frag_vert[-1] + len(v))
+      frag_edge.append(frag_edge[-1] + len(e))
+    label_frag.append(len(boxes))
+  cat = lambda parts, shape, dt: np.ascontiguousarray(np.concatenate(parts).reshape(shape) if parts
+                                                      else np.zeros((0,) + shape[1:], dt), dtype=dt)
+  return segids, {
+    "label_frag": np.array(label_frag, np.uint64), "frag_vert": np.array(frag_vert, np.uint64),
+    "frag_edge": np.array(frag_edge, np.uint64), "frag_box": cat(boxes, (-1, 6), np.float64),
+    "vertices": cat(verts, (-1, 3), np.float32), "radius": cat(radii, (-1,), np.float32),
+    "vertex_types": cat(types, (-1,), np.uint8), "edges": cat(edges, (-1, 2), np.uint32),
+  }
+
+
+def merge_packed(packed, dust_threshold=4000, tick_threshold=6000, max_cable_length=None, vertex_types=True,
+                 ctx=None):
+  """ign_skeleton_merge_dev on packed arrays: (bytes buffer, uint64 table (L, 4) of (label row, byte offset,
+  nv, ne)), uploaded once and copied back once"""
+  L = packed["label_frag"].size - 1
+  V, E, F = packed["radius"].size, packed["edges"].shape[0], packed["frag_box"].shape[0]
+  mc = float("inf") if max_cable_length is None else float(max_cable_length)
+  if L == 0:
+    return np.zeros(0, np.uint8), np.zeros((0, 4), np.uint64)
+  ctx = ctx or _shim.default_context()
+  lib, h, ptr = ctx.lib, ctx.handle, _shim.ptr
+  cap = ctypes.c_uint64(0)
+  _shim.check(lib.ign_skeleton_merge_capacity(L, V, E, ctypes.byref(cap)))
+  names = ("label_frag", "frag_vert", "frag_edge", "frag_box", "vertices", "radius", "vertex_types", "edges")
+  bufs = []
+  try:
+    d = {}
+    for k in names:
+      bufs.append(ctx.alloc(max(packed[k].nbytes, 8)))
+      d[k] = bufs[-1]
+      if packed[k].nbytes:
+        ctx.h2d(d[k], packed[k])
+    bufs.append(ctx.alloc(max(int(cap.value), 8)))
+    d_buf = bufs[-1]
+    bufs.append(ctx.alloc(L * 32))
+    d_table = bufs[-1]
+    nb = ctypes.c_uint64(0)
+    _shim.check(lib.ign_skeleton_merge_dev(
+      h, L, ptr(d["label_frag"]), F, ptr(d["frag_vert"]), ptr(d["frag_edge"]), ptr(d["frag_box"]),
+      ptr(d["vertices"]), ptr(d["radius"]), ptr(d["vertex_types"]), V, ptr(d["edges"]), E, float(dust_threshold),
+      float(tick_threshold), mc, int(bool(vertex_types)), ptr(d_buf), cap.value, ptr(d_table), ctypes.byref(nb)))
+    B = int(nb.value)
+    buf = np.zeros((B + 7) // 8 * 8, np.uint8)  # whole words, so that typed views of the buffer exist
+    table = np.empty((L, 4), np.uint64)
+    ctx.d2h(buf, d_buf, B)
+    ctx.d2h(table, d_table)
+    ctx.sync()
+  finally:
+    for b in bufs:
+      b.free()
+  return buf, table
+
+
+def _split(buf, table, segids, vertex_types):
+  """{segid: (Skeleton, blob)}: every array a view into buf"""
+  f32, u32 = buf.view(np.float32), buf.view(np.uint32)
+  out = {}
+  for segid, (off, nv, ne) in zip(segids, table[:, 1:].tolist()):
+    w = off // 4 + 2
+    e, r = w + 3 * nv, w + 3 * nv + 2 * ne
+    end = 4 * (r + nv)
+    vt = buf[end:end + nv] if vertex_types else np.zeros(nv, np.uint8)
+    if vertex_types:
+      end += nv
+    out[segid] = (Skeleton(f32[w:e].reshape(nv, 3), u32[e:r].reshape(ne, 2), f32[r:r + nv], vt, segid),
+                  buf[off:end])
+  return out
+
+
+def merge_fragments(fragments, crop=0, resolution=(1, 1, 1), dust_threshold=4000, tick_threshold=6000,
+                    max_cable_length=None, vertex_types=True, ctx=None):
+  """UnshardedSkeletonMergeTask's fuse and postprocess for many labels in one device call (DESIGN.md §5h).
+  fragments: {segid: [(bbox, Skeleton), ...]}, each label's fragments in ascending file name order; bbox is
+  the fragment's physical Bbox (None: never cropped).  Returns {segid: (Skeleton, blob)} in the same order,
+  the blob its neuroglancer precomputed skeleton (radius, then vertex_types when `vertex_types`); every array
+  is a view into one host buffer."""
+  segids, packed = pack_fragments(fragments, crop, resolution)
+  buf, table = merge_packed(packed, dust_threshold, tick_threshold, max_cable_length, vertex_types, ctx)
+  return _split(buf, table, segids, vertex_types)
+
+
+def postprocess(skeleton, dust_threshold=1500, tick_threshold=3000, ctx=None):
+  """Drop-in for kimimaro.postprocess: consolidate, remove dust, break loops, connect nearby pieces and trim
+  ticks (DESIGN.md §5h), on the device through the batched entry point.  Returns a new Skeleton."""
+  segid = skeleton.id
+  return merge_fragments({segid: [(None, skeleton)]}, dust_threshold=dust_threshold, tick_threshold=tick_threshold,
+                         ctx=ctx)[segid][0]

@@ -16,6 +16,7 @@ import math
 import gzip
 import json
 import os
+import re
 
 import numpy as np
 
@@ -94,9 +95,12 @@ class Bbox:
 
   @classmethod
   def from_filename(cls, name):
-    parts = os.path.basename(name).split(".")[0].split("_")
-    lo, hi = zip(*[[int(v) for v in p.split("-")] for p in parts[-3:]])
-    return cls(lo, hi)
+    """the box in a file name such as 0-64_0-64_0-32.spatial or 5:0-64_0-64_0-32 (a skeleton fragment)"""
+    m = re.search(r"(-?\d+)-(-?\d+)_(-?\d+)-(-?\d+)_(-?\d+)-(-?\d+)", os.path.basename(name))
+    if m is None:
+      raise ValueError("no bounding box in the file name %r" % name)
+    v = [int(x) for x in m.groups()]
+    return cls(v[0::2], v[1::2])
 
   @classmethod
   def clamp(cls, box, bounds):
@@ -314,6 +318,11 @@ class _SkeletonMeta:
   def __init__(self, cv, subdir):
     self._cv, self.subdir = cv, subdir
     self.info = cv.cf.get_json(subdir + "/info") or copy.deepcopy(DEFAULT_SKELETON_INFO)
+
+  @property
+  def mip(self):
+    """the mip the skeletons were made at (the info's `mip`; 0 when absent)"""
+    return int(self.info.get("mip") or 0)
 
   def commit_info(self):
     self._cv.cf.put_json(self.subdir + "/info", self.info)

@@ -4,4 +4,5 @@ from .image import (create_downsampling_tasks, create_image_shard_downsample_tas
                     create_contrast_normalization_tasks, create_luminance_levels_tasks, create_clahe_tasks,
                     create_quantized_affinity_info, create_quantize_tasks, create_voxel_counting_tasks)
 from .mesh import create_meshing_tasks, create_spatial_index_mesh_tasks
-from .skeleton import create_skeletonizing_tasks, create_spatial_index_skeleton_tasks
+from .skeleton import (create_skeletonizing_tasks, create_spatial_index_skeleton_tasks,
+                       create_unsharded_skeleton_merge_tasks)

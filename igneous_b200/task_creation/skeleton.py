@@ -1,11 +1,11 @@
-"""create_skeletonizing_tasks (igneous/task_creation/skeleton.py:68-388) and
-create_spatial_index_skeleton_tasks (:795-867)."""
+"""create_skeletonizing_tasks (igneous/task_creation/skeleton.py:68-388),
+create_unsharded_skeleton_merge_tasks (:535-591) and create_spatial_index_skeleton_tasks (:795-867)."""
 from time import strftime
 
 import numpy as np
 
 from .._compat import CloudVolume, CloudFiles, Vec
-from ..tasks import SkeletonTask
+from ..tasks import SkeletonTask, UnshardedSkeletonMergeTask
 from ..tasks.skeleton import refuse
 from .common import FinelyDividedTaskIterator, operator_contact, spatial_index_tasks
 
@@ -18,7 +18,7 @@ def create_skeletonizing_tasks(cloudpath, mip, shape=Vec(512, 512, 512), teasar_
                                cross_sectional_area_smoothing_window=5, timestamp=None, root_ids_cloudpath=None,
                                cross_sectional_area_repair_sec_per_label=0):
   """Tasks with one voxel of overlap on the high side in a regular grid, to be densely skeletonized
-  (SkeletonTask); the fragments are merged by the reference's merge stage.  Records the layer's skeleton
+  (SkeletonTask); the fragments are merged by create_unsharded_skeleton_merge_tasks.  Records the layer's skeleton
   directory (skeletons_mip_{mip} unless it has one), the skeleton info's @type, spatial_index, mip and
   float32-only vertex_attributes, the frag_path info, and the provenance on completion.
   The options SkeletonTask refuses (sharded, dust_global, synapses, cross_sectional_area, fix_autapses /
@@ -93,6 +93,38 @@ def create_skeletonizing_tasks(cloudpath, mip, shape=Vec(512, 512, 512), teasar_
       vol.commit_provenance()
 
   return SkeletonTaskIterator(bounds, shape)
+
+
+def create_unsharded_skeleton_merge_tasks(layer_path, crop=0, magnitude=3, dust_threshold=4000, max_cable_length=None,
+                                          tick_threshold=6000, delete_fragments=False):
+  """UnshardedSkeletonMergeTasks over every label of the layer's skeleton fragments, split by file name
+  prefix: "1:" ... "{10^(m-1) - 1}:" for the labels below 10^(m-1), then 10^(m-1) ... 10^m - 1, each of
+  which also matches the longer labels that start with it.  The provenance is appended after iteration."""
+  assert int(magnitude) == magnitude
+  start, end = 10 ** (magnitude - 1), 10 ** magnitude
+
+  class UnshardedSkeletonMergeTaskIterator:
+    def __len__(self):
+      return 10 ** magnitude
+
+    def __iter__(self):
+      for prefix in [str(p) + ":" for p in range(1, start)] + list(range(start, end)):
+        yield UnshardedSkeletonMergeTask(cloudpath=layer_path, prefix=prefix, crop=crop,
+                                         dust_threshold=dust_threshold, max_cable_length=max_cable_length,
+                                         tick_threshold=tick_threshold, delete_fragments=delete_fragments)
+      vol = CloudVolume(layer_path)
+      vol.provenance.processing.append({
+        "method": {
+          "task": "UnshardedSkeletonMergeTask", "cloudpath": layer_path, "crop": crop,
+          "dust_threshold": dust_threshold, "tick_threshold": tick_threshold, "delete_fragments": delete_fragments,
+          "max_cable_length": max_cable_length,
+        },
+        "by": operator_contact(),
+        "date": strftime("%Y-%m-%d %H:%M %Z"),
+      })
+      vol.commit_provenance()
+
+  return UnshardedSkeletonMergeTaskIterator()
 
 
 def create_spatial_index_skeleton_tasks(cloudpath, shape=(448, 448, 448), mip=0, fill_missing=False, compress="gzip",

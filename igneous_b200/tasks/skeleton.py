@@ -6,9 +6,14 @@ kimimaro.skeletonize is replaced by igneous_b200.kimimaro.export_skeletons, whic
 to dataset coordinates, encodes each skeleton in the precomputed format and boxes it on the device
 (DESIGN.md §5g); fastremap by igneous_b200.fastremap.  The download is not renumbered on the host: the
 device renumbers, and the export keys skeletons by original label.
+
+UnshardedSkeletonMergeTask mirrors igneous/tasks/skeleton.py:810-916; its fuse and kimimaro.postprocess run on
+the device (igneous_b200.kimimaro.merge_fragments, DESIGN.md §5h).
 """
 import pickle
+import re
 import time
+from collections import defaultdict
 
 import numpy as np
 
@@ -143,3 +148,54 @@ class SkeletonTask(RegisteredTask):
     precision = vol.skeleton.spatial_index.precision
     CloudFiles(path).put_json("%s.spatial" % bbox.to_filename(precision), spatial_index, compress="gzip",
                               cache_control=False)
+
+
+SEGIDRE = re.compile(r"(\d+):")
+
+
+class UnshardedSkeletonMergeTask(RegisteredTask):
+  """Stage 2 of skeletonization (igneous/tasks/skeleton.py:810-916): fuse every fragment of the labels whose
+  file names start with `prefix`, postprocess them and write one precomputed skeleton per label.  The fuse and
+  kimimaro.postprocess run for the whole prefix in one device call (kimimaro.merge_fragments, DESIGN.md §5h).
+  A prefix like "1" also matches labels 10, 100, ...; "1:" matches label 1 alone."""
+
+  def __init__(self, cloudpath, prefix, crop=0, dust_threshold=4000, max_cable_length=None, tick_threshold=6000,
+               delete_fragments=False):
+    super().__init__(cloudpath, prefix, crop, dust_threshold, max_cable_length, tick_threshold, delete_fragments)
+    self.cloudpath, self.prefix, self.crop = cloudpath, prefix, crop
+    self.dust_threshold, self.tick_threshold = dust_threshold, tick_threshold
+    self.max_cable_length = float(max_cable_length) if max_cable_length is not None else None
+    self.delete_fragments = bool(delete_fragments)
+
+  def execute(self):
+    last_phase_seconds.clear()
+    t0 = time.perf_counter()
+    vol = CloudVolume(self.cloudpath)
+    vol.mip = vol.skeleton.meta.mip
+    cf = CloudFiles(vol.skeleton.path)
+    # names without "{segid}:" are the info, the .spatial files and finished skeletons
+    filenames = [name for name in cf.list(prefix=str(self.prefix)) if SEGIDRE.search(name)]
+    contents = cf.get(filenames, return_dict=True)
+    t1 = time.perf_counter()
+    fragments = defaultdict(list)
+    for name in filenames:
+      try:
+        skel = pickle.loads(contents[name])
+      except Exception as e:
+        raise ValueError("UnshardedSkeletonMergeTask: cannot unpickle the fragment %s: %s" % (name, e)) from e
+      if not isinstance(skel, kimimaro.Skeleton):
+        raise ValueError("UnshardedSkeletonMergeTask: the fragment %s holds a %s, not an igneous_b200 Skeleton"
+                         % (name, type(skel).__name__))
+      fragments[int(SEGIDRE.search(name).group(1))].append((Bbox.from_filename(name), skel))
+    t2 = time.perf_counter()
+    vertex_types = any(a["id"] == "vertex_types" for a in vol.skeleton.meta.info.get("vertex_attributes") or [])
+    merged = kimimaro.merge_fragments(fragments, crop=self.crop, resolution=vol.resolution,
+                                      dust_threshold=self.dust_threshold, tick_threshold=self.tick_threshold,
+                                      max_cable_length=self.max_cable_length, vertex_types=vertex_types)
+    t3 = time.perf_counter()
+    cf.puts(((str(segid), blob.tobytes()) for segid, (_, blob) in merged.items()), compress="gzip",
+            content_type="application/octet-stream", cache_control=False)
+    if self.delete_fragments:
+      cf.delete(filenames)
+    last_phase_seconds.update(list=t1 - t0, unpickle=t2 - t1, merge=t3 - t2, writes=time.perf_counter() - t3)
+    return merged

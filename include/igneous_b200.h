@@ -485,6 +485,32 @@ IGN_API int ign_skeleton_export_dev(ign_ctx* ctx, const uint32_t* labels, uint64
                                     uint64_t* table_out, float* boxes_out, uint64_t* n_skeletons, uint64_t* nbytes);
 IGN_API int ign_skeleton_export_capacity(uint64_t count, uint64_t max_label, uint64_t* bytes);
 
+/* ------------------------------------------------------------- skeleton merge
+ * UnshardedSkeletonMergeTask's fuse and kimimaro.postprocess (igneous/tasks/skeleton.py:810-916) for a batch
+ * of labels in one call; the rule is DESIGN.md §5h.  Every array is a DEVICE array.
+ * ign_skeleton_merge_dev: n_labels labels; label l owns fragments [label_frag[l], label_frag[l + 1]), fragment f
+ *   owns vertices [frag_vert[f], frag_vert[f + 1]) and edges [frag_edge[f], frag_edge[f + 1]) (label_frag,
+ *   frag_vert and frag_edge ascend from 0 to n_frags, n_vertices and n_edges).  vertices float32 [][3],
+ *   radius float32 [], vertex_types_in uint8 [] per vertex; edges uint32 [][2], indices local to their
+ *   fragment; frag_box float64 [][6] (min xyz, max xyz) per fragment: a vertex outside it is cropped
+ *   (-inf / +inf keeps all).  Each label is fused; unless its cable length exceeds max_cable_length (+inf:
+ *   never) it is postprocessed with dust_threshold and tick_threshold (0 skips a step).  Out, one row per
+ *   label in label order: blobs_out as ign_skeleton_export_dev's (radius, then vertex_types when
+ *   vertex_types != 0, 8-byte aligned, an empty result is nv = ne = 0), table_out uint64 [][4] (label row,
+ *   byte offset, nv, ne), *nbytes = the end of the last blob.  capacity (bytes) must be at least
+ *   16 * n_labels + 25 * n_vertices + 8 * n_edges (ign_skeleton_merge_capacity).  Ranges that do not ascend,
+ *   a non-finite vertex or an edge index outside its fragment -> IGN_ERR_INVALID before any output is
+ *   written.  The host synchronises five times.
+ * ign_skeleton_merge_capacity: that bound (IGN_ERR_OVERFLOW from 2^30 vertices or edges). */
+IGN_API int ign_skeleton_merge_dev(ign_ctx* ctx, uint64_t n_labels, const uint64_t* label_frag, uint64_t n_frags,
+                                   const uint64_t* frag_vert, const uint64_t* frag_edge, const double* frag_box,
+                                   const float* vertices, const float* radius, const uint8_t* vertex_types_in,
+                                   uint64_t n_vertices, const uint32_t* edges, uint64_t n_edges,
+                                   double dust_threshold, double tick_threshold, double max_cable_length,
+                                   int vertex_types, uint8_t* blobs_out, uint64_t capacity, uint64_t* table_out,
+                                   uint64_t* nbytes);
+IGN_API int ign_skeleton_merge_capacity(uint64_t n_labels, uint64_t n_vertices, uint64_t n_edges, uint64_t* bytes);
+
 /* --------------------------------------------------------------------- mesh
  * zmesh.Mesher(resolution).mesh(data, preserve_order=False)  igneous/tasks/mesh/mesh.py:151,245
  * Mesher.ids()                                                igneous/tasks/mesh/mesh.py:374
