@@ -92,6 +92,23 @@ __device__ __forceinline__ unsigned long long s_key(double cost, uint32_t h, uin
   return ((unsigned long long)__float_as_uint(c) << 32) | s_mix(h ^ salt);
 }
 
+// Key and cost format of a label of T faces (oracle: simp_key): 32-bit keys when its 3T half-edge ids fit 16
+// bits, else 64-bit keys.
+__host__ __device__ __forceinline__ bool s_fmt16(uint64_t T) { return 3 * T <= 65536ull; }
+// the 16 cost bits of a 32-bit key (8 exponent + 8 mantissa bits of the non-negative float cost)
+__device__ __forceinline__ uint32_t s_kfield(float cost) { return (__float_as_uint(cost) >> 15) & 0xFFFFu; }
+// Cached costs (ecost: 12 bytes per face of the task, a label's slice [12 tbase, 12 (tbase + T))).  A label
+// with 64-bit keys keeps the float cost of half-edge 3i + c at float 3 (tbase + i) + c.  A label with 32-bit
+// keys needs only their 16 cost bits: the fields of face i's corners 0..2 (bits 16c.., 16 bits of padding) are
+// one 8-byte word, word i from the slice's first 8-byte boundary (it ends in the slice: 8T + 4 <= 12T).
+__device__ __forceinline__ unsigned long long* s_cwords(float* ecost, uint32_t tbase) {
+  return (unsigned long long*)(ecost + 3 * (uint64_t)tbase + (tbase & 1u));
+}
+// the field of corner c in word i (the index arithmetic of s_cwords, in 2-byte units)
+__device__ __forceinline__ uint16_t* s_cfield(float* ecost, uint32_t tbase, uint32_t i, uint32_t c) {
+  return (uint16_t*)ecost + 2 * (3 * (uint64_t)tbase + (tbase & 1u) + 2 * i) + c;
+}
+
 __device__ __forceinline__ double s_qeval(const double* q, const double* p) {
   const double x = p[0], y = p[1], z = p[2];
   return q[0] * x * x + 2.0 * q[1] * x * y + 2.0 * q[2] * x * z + 2.0 * q[3] * x + q[4] * y * y +
@@ -276,10 +293,10 @@ __global__ void __launch_bounds__(256) k_simp_boundary(Simp s) {
   }
 }
 
-// Initial cost of every canonical half-edge (u < v; label-local order is the global one): the float cost in
-// ecost and the memo of the half-edge in the face's state byte (2 cached, 3 exceeds max_error), which the
-// label kernel's load takes over.  One thread per face, so that the byte has a single writer.  counts[0]
-// += evaluations.
+// Initial cost of every canonical half-edge (u < v; label-local order is the global one): the cost in ecost,
+// in the label's format (s_cwords), and the memo of the half-edge in the face's state byte (2 cached, 3 exceeds
+// max_error), which the label kernel's load takes over.  One thread per face, so that the byte has a single
+// writer.  counts[0] += evaluations.
 __global__ void __launch_bounds__(256)
     k_simp_ecost(Simp s, double max_err2, float* __restrict__ ecost, uint8_t* __restrict__ fstate,
                  uint32_t* counts) {
@@ -287,7 +304,10 @@ __global__ void __launch_bounds__(256)
   uint32_t n = 0;
   if (f < s.T) {
     const uint32_t* fv = s.face + 3 * f;
+    const uint32_t l = s.flabel[f], tbase = s.tri_off[l];
+    const bool fmt16 = s_fmt16(s.tri_off[l + 1] - tbase);
     uint32_t st = 0;
+    unsigned long long word = 0;
 #pragma unroll
     for (int c = 0; c < 3; c++) {
       const uint32_t u = fv[c], v = fv[(c + 1) % 3];
@@ -296,12 +316,15 @@ __global__ void __launch_bounds__(256)
       s_cost(s.Q, s.pos, max_err2, u, v, u, v, s.vbound[u] != 0, s.vbound[v] != 0, &ev);
       uint32_t es = 3;
       if (ev.valid) {
-        ecost[3 * f + c] = __double2float_rn(ev.cost);
+        const float cf = __double2float_rn(ev.cost);
+        if (fmt16) word |= (unsigned long long)s_kfield(cf) << (16 * c);
+        else ecost[3 * f + c] = cf;
         es = 2;
       }
       st |= es << (2 * c);
       n++;
     }
+    if (fmt16) s_cwords(ecost, tbase)[f - tbase] = word;
     fstate[f] = (uint8_t)st;
   }
   const int tot = __syncthreads_count(n & 1u) + 2 * __syncthreads_count(n >> 1);
@@ -315,12 +338,12 @@ __global__ void __launch_bounds__(256)
 // + a 2-bit memo per half-edge), a flag byte and a "lose" byte per vertex, the 32-bit round
 // keys and the ring lists of the round's winners -- lives in SHARED MEMORY for the whole
 // run; only the double-precision data that a round touches sparsely (positions, quadrics,
-// cached float costs) stays in global memory (L2).  A round is a handful of
+// cached costs) stays in global memory (L2).  A round is a handful of
 // __syncthreads() phases instead of five launches and a host round trip:
 //
 //   P1  key1[v] = MAX, lose[v] = 0                             (vertex parallel)
 //   P2  every canonical half-edge (u < v) of an alive face posts its cached key to both
-//       endpoints with a shared-memory min reduction (the float costs come from k_simp_ecost
+//       endpoints with a shared-memory min reduction (the cached costs come from k_simp_ecost
 //       and E2; P2 evaluates none)                                 (face parallel)
 //   P3  a vertex LOSEs if a face neighbour holds a smaller key1 (== key2 test of the
 //       round formulation: key2[w] == key1[w] <=> !LOSE[w]); plain byte stores
@@ -389,7 +412,7 @@ __host__ __device__ inline SlLayout sl_layout(uint32_t T, uint32_t U, bool resum
 __host__ __device__ inline bool sl_fits_smem(uint32_t T, uint32_t U, uint32_t threads, size_t smem_bytes,
                                              bool resumed = false) {
   const uint32_t cap = (uint32_t)SL_LIST_PER * threads;
-  return 3ull * T <= 65536ull && T <= cap && U <= cap && sl_layout(T, U, resumed).need <= smem_bytes;
+  return s_fmt16(T) && T <= cap && U <= cap && sl_layout(T, U, resumed).need <= smem_bytes;
 }
 // winners per pass of a label that sl_fits_smem accepts: SL_WCAP plus what the rest of the budget holds, at
 // most one per thread (E2a gives each winner a thread) and at most `limit` (IGN_SIMP_WCAP)
@@ -407,7 +430,7 @@ struct SlArgs {
   uint8_t* falive;        // T   (out)
   uint8_t* valive;        // U   (out)
   const uint8_t* vbound;  // U
-  float* ecost;           // 3T  memoised float cost per half-edge
+  float* ecost;           // 3T  memoised cost per half-edge, in the label's key format (s_cwords)
   // global-memory class only (labels that do not fit shared memory)
   unsigned long long* key1;  // U
   uint8_t* fstate;           // T
@@ -458,10 +481,14 @@ constexpr int SL_HIST = 1664, SL_HP = 16, SL_HW = 64, SL_HR = S_MAXV + 2, SL_HCL
 // header of a migrated label: dense label, trace record, next round, slow rounds, alive faces, alive vertices
 constexpr int SL_MREC = 8;
 constexpr int SL_LREC = 7;  // words of a label's IGN_SIMP_TRACE record (SlArgs::lrec)
+#ifdef IGN_SIMP_P2_PROBE
+constexpr int SL_NPH = 12;  // IGN_SIMP_TRACE phase timers (trace words 1600.., 64 bits each), and the P2 probes
+#else
 constexpr int SL_NPH = 9;  // IGN_SIMP_TRACE phase timers (trace words 1600.., 64 bits each)
+#endif
 // IGN_SIMP_TRACE E2 flip tests (trace words SL_TFLIP..): winners rejected by flips on the u side only, on the
 // v side only, on both sides
-constexpr int SL_TFLIP = 1620;
+constexpr int SL_TFLIP = 1624;
 
 struct SlShared {
   uint32_t work, alive, progress, ncol, nwin, stop, slow, counter, npass;
@@ -556,12 +583,15 @@ __device__ __forceinline__ void sl_post(uint32_t* key1, uint32_t u, uint32_t v, 
   if (key < *(volatile uint32_t*)&key1[v])
     asm volatile("red.shared.min.u32 [%0], %1;" ::"r"((uint32_t)__cvta_generic_to_shared(key1 + v)), "r"(key) : "memory");
 }
+// 32-bit key from the cost field s_kfield(cost) (as cached for labels with 32-bit keys, s_cwords)
+__device__ __forceinline__ uint32_t sl_key(uint32_t field, uint32_t hl, uint32_t salt) {
+  return (field << 16) | s_mix16((hl ^ salt) & 0xFFFFu);
+}
 template <bool SM>
 __device__ __forceinline__ typename SlLab<SM>::key_t sl_key(const SlLab<SM>& L, float cost, uint32_t hl, uint32_t salt) {
   typedef typename SlLab<SM>::key_t key_t;
-  const uint32_t bits = __float_as_uint(cost);
-  if (SM || L.fmt16) return (key_t)((((bits >> 15) & 0xFFFFu) << 16) | s_mix16((hl ^ salt) & 0xFFFFu));
-  return (key_t)(((unsigned long long)bits << 32) | s_mix(hl ^ salt));
+  if (SM || L.fmt16) return (key_t)sl_key(s_kfield(cost), hl, salt);
+  return (key_t)(((unsigned long long)__float_as_uint(cost) << 32) | s_mix(hl ^ salt));
 }
 template <bool SM>
 __device__ __forceinline__ uint32_t sl_key_edge(const SlLab<SM>& L, typename SlLab<SM>::key_t key, uint32_t salt) {
@@ -612,7 +642,10 @@ __device__ __forceinline__ uint32_t sl_recost_k(const SlArgs& A, const SlLab<SM>
   SEval ev;
   s_cost_q(q, pu, pv, A.max_err2, u, v, (L.vflag[u] & VF_BOUND) != 0, (L.vflag[v] & VF_BOUND) != 0, &ev);
   if (!ev.valid) return 3;
-  A.ecost[3 * (uint64_t)(L.tbase + sl_fo<SM, R>(L, f)) + c] = __double2float_rn(ev.cost);
+  const float cf = __double2float_rn(ev.cost);
+  const uint32_t fo = sl_fo<SM, R>(L, f);
+  if (SM || L.fmt16) *s_cfield(A.ecost, L.tbase, fo, c) = (uint16_t)s_kfield(cf);
+  else A.ecost[3 * (uint64_t)(L.tbase + fo) + c] = cf;
   return 2;
 }
 
@@ -1024,6 +1057,93 @@ __device__ void sl_migrate(const SlArgs& A, const SlLab<true>& L, SlShared& sh, 
   }
 }
 
+// P2: every canonical half-edge (u < v) of an alive face posts its cached key to both endpoints.  A warp takes
+// 32 alive faces per iteration.  The cached costs are the only global loads: PK (32-bit keys) one packed word
+// per face (s_cwords), requested two iterations ahead; else three floats, one iteration ahead.  A resumed label
+// addresses them by the original face id.  PROBE (IGN_SIMP_P2_PROBE builds only): 1 loads and keys without
+// posts or state writes, 2 posts with every cost taken as 0 and no loads.
+template <bool SM, bool R, bool PK, int PROBE = 0>
+__device__ __forceinline__ void sl_keys(const SlArgs& A, const SlLab<SM>& L, const typename SlLab<SM>::idx_t* flist,
+                                        uint32_t nF, uint32_t salt) {
+  typedef typename SlLab<SM>::key_t key_t;
+  constexpr int D = PK ? 2 : 1;
+  constexpr bool LOAD = PROBE != 2;
+  const uint32_t tid = threadIdx.x, NT = blockDim.x, lane = tid & 31u, warp = tid >> 5;
+  const unsigned long long* cw = s_cwords(A.ecost, L.tbase);
+  const float* ecb = A.ecost + 3 * (uint64_t)L.tbase;
+  // stage s: face id, original face id and cached costs of the lane's face s iterations after the current one
+  uint32_t f_n[D], fo_n[D];
+  unsigned long long w_n[D];
+  float ec_n[D][3];
+#pragma unroll
+  for (int s = 0; s < D; s++) {
+    const uint32_t i = warp * 32 + lane + s * NT;
+    f_n[s] = fo_n[s] = 0;
+    w_n[s] = 0;
+    ec_n[s][0] = ec_n[s][1] = ec_n[s][2] = 0.f;
+    if (i < nF) {
+      f_n[s] = flist[i];
+      fo_n[s] = sl_fo<SM, R>(L, f_n[s]);
+      if (LOAD && PK) w_n[s] = cw[fo_n[s]];
+      if (LOAD && !PK) { ec_n[s][0] = ecb[3 * (uint64_t)fo_n[s]]; ec_n[s][1] = ecb[3 * (uint64_t)fo_n[s] + 1]; ec_n[s][2] = ecb[3 * (uint64_t)fo_n[s] + 2]; }
+    }
+  }
+  unsigned long long sink = 0;  // PROBE 1: keeps the loads and keys that are not posted
+  for (uint32_t base = warp * 32; base < nF; base += NT) {
+    const uint32_t i = base + lane;
+    const uint32_t f = f_n[0], fo = fo_n[0];
+    const unsigned long long w = w_n[0];
+    const float ec[3] = {ec_n[0][0], ec_n[0][1], ec_n[0][2]};
+#pragma unroll
+    for (int s = 0; s + 1 < D; s++) {
+      f_n[s] = f_n[s + 1]; fo_n[s] = fo_n[s + 1]; w_n[s] = w_n[s + 1];
+      ec_n[s][0] = ec_n[s + 1][0]; ec_n[s][1] = ec_n[s + 1][1]; ec_n[s][2] = ec_n[s + 1][2];
+    }
+    if (i + D * NT < nF) {
+      f_n[D - 1] = flist[i + D * NT];
+      fo_n[D - 1] = sl_fo<SM, R>(L, f_n[D - 1]);
+      if (LOAD && PK) w_n[D - 1] = cw[fo_n[D - 1]];
+      if (LOAD && !PK) {
+        const float* e = ecb + 3 * (uint64_t)fo_n[D - 1];
+        ec_n[D - 1][0] = e[0]; ec_n[D - 1][1] = e[1]; ec_n[D - 1][2] = e[2];
+      }
+    }
+    uint32_t st = 0, a[3] = {0, 0, 0}, fl[3] = {0, 0, 0};
+    if (i < nF) st = L.fstate[f];
+    bool act = (st & 0x80u) != 0;
+    if (act) {
+      a[0] = sl_fget<SM>(L, f, 0); a[1] = sl_fget<SM>(L, f, 1); a[2] = sl_fget<SM>(L, f, 2);
+      fl[0] = L.vflag[a[0]]; fl[1] = L.vflag[a[1]]; fl[2] = L.vflag[a[2]];
+    }
+    if (act) {
+      uint32_t nst = st;
+#pragma unroll
+      for (int c = 0; c < 3; c++) {
+        const uint32_t u = a[c], v = a[(c + 1) % 3];
+        const uint32_t fe = fl[c] | fl[(c + 1) % 3];
+        if (!(u < v)) continue;  // one key per edge
+        // memo: 1 parked (won a round, failed validation), 2 cost cached in ecost, 3 known to
+        // exceed max_error.  A parked edge is un-parked when an endpoint's ring changed (RDIRTY):
+        // its cost was cached when it won, and an endpoint that moved since would have re-costed it.
+        uint32_t es = (st >> (2 * c)) & 3u;
+        if (es == 1 && (fe & VF_RDIRTY)) es = 2;
+        if (es == 2) {
+          const uint32_t hl = 3u * fo + (uint32_t)c;
+          const key_t key = PK ? (key_t)sl_key((uint32_t)(w >> (16 * c)) & 0xFFFFu, hl, salt)
+                               : sl_key<SM>(L, ec[c], hl, salt);
+          if (PROBE == 1) sink += key;
+          else sl_post(L.key1, u, v, key);
+        } else if (es == 0 && PROBE == 0) {
+          atomicAdd(&A.counters[28], 1u);  // a half-edge without a cost: a bug
+        }
+        nst = (nst & ~(3u << (2 * c))) | (es << (2 * c));
+      }
+      if (PROBE == 0 && nst != st) L.fstate[f] = (uint8_t)nst;
+    }
+  }
+  if (PROBE == 1 && sink == 0x9E3779B97F4A7C15ull) A.trace[SL_TFLIP + 3] = 1;
+}
+
 // All rounds of one label (R: a label resumed from the header `hdr` after it migrated from a larger class)
 template <bool SM, bool R>
 __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const uint32_t* hdr) {
@@ -1114,56 +1234,29 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
     }
     __syncthreads();
     SL_MARK(0);
-    // ---- P2: keys of the canonical half-edges.  A warp takes 32 alive faces per iteration and
-    // posts the cached keys.  No cost is evaluated here: k_simp_ecost costs every half-edge before
-    // the first round and E2 re-costs the edges of every vertex that moved right after its collapse.
-    {
-      // software pipeline: the face id and the three cached costs of the NEXT iteration are
-      // requested (global loads, L2 latency) before the current face is processed
-      const float* ecb = A.ecost + 3 * (uint64_t)L.tbase;
-      uint32_t f_n = 0, fo_n = 0;
-      float ec_n[3] = {0.f, 0.f, 0.f};
-      if (warp * 32 + lane < nF) {
-        f_n = flist[warp * 32 + lane];
-        fo_n = sl_fo<SM, R>(L, f_n);
-        ec_n[0] = ecb[3 * (uint64_t)fo_n]; ec_n[1] = ecb[3 * (uint64_t)fo_n + 1]; ec_n[2] = ecb[3 * (uint64_t)fo_n + 2];
-      }
-      for (uint32_t base = warp * 32; base < nF; base += NT) {
-        const uint32_t i = base + lane;
-        const uint32_t f = f_n, fo = fo_n;
-        const float ec[3] = {ec_n[0], ec_n[1], ec_n[2]};
-        if (i + NT < nF) {
-          f_n = flist[i + NT];
-          fo_n = sl_fo<SM, R>(L, f_n);
-          ec_n[0] = ecb[3 * (uint64_t)fo_n]; ec_n[1] = ecb[3 * (uint64_t)fo_n + 1]; ec_n[2] = ecb[3 * (uint64_t)fo_n + 2];
-        }
-        uint32_t st = 0, a[3] = {0, 0, 0}, fl[3] = {0, 0, 0};
-        if (i < nF) st = L.fstate[f];
-        bool act = (st & 0x80u) != 0;
-        if (act) {
-          a[0] = sl_fget<SM>(L, f, 0); a[1] = sl_fget<SM>(L, f, 1); a[2] = sl_fget<SM>(L, f, 2);
-          fl[0] = L.vflag[a[0]]; fl[1] = L.vflag[a[1]]; fl[2] = L.vflag[a[2]];
-        }
-        if (act) {
-          uint32_t nst = st;
-#pragma unroll
-          for (int c = 0; c < 3; c++) {
-            const uint32_t u = a[c], v = a[(c + 1) % 3];
-            const uint32_t fe = fl[c] | fl[(c + 1) % 3];
-            if (!(u < v)) continue;  // one key per edge
-            // memo: 1 parked (won a round, failed validation), 2 cost cached in ecost, 3 known to
-            // exceed max_error.  A parked edge is un-parked when an endpoint's ring changed (RDIRTY):
-            // its cost was cached when it won, and an endpoint that moved since would have re-costed it.
-            uint32_t es = (st >> (2 * c)) & 3u;
-            if (es == 1 && (fe & VF_RDIRTY)) es = 2;
-            if (es == 2) sl_post(L.key1, u, v, sl_key<SM>(L, ec[c], 3u * fo + (uint32_t)c, salt));
-            else if (es == 0) atomicAdd(&A.counters[28], 1u);  // a half-edge without a cost: a bug
-            nst = (nst & ~(3u << (2 * c))) | (es << (2 * c));
-          }
-          if (nst != st) L.fstate[f] = (uint8_t)nst;
-        }
-      }
-    }
+#ifdef IGN_SIMP_P2_PROBE
+    // P2 taken apart (with IGN_SIMP_TRACE=1): its loads and keys without the posts, in the float layout
+    // (three loads per face) and in the label's own, then its posts with every cost taken as 0 and no
+    // loads; then P1's key reset again
+    sl_keys<SM, R, false, 1>(A, L, flist, nF, salt);
+    __syncthreads();
+    SL_MARK(9);
+    if (SM || L.fmt16) sl_keys<SM, R, true, 1>(A, L, flist, nF, salt);
+    else sl_keys<SM, R, false, 1>(A, L, flist, nF, salt);
+    __syncthreads();
+    SL_MARK(10);
+    sl_keys<SM, R, false, 2>(A, L, flist, nF, salt);
+    __syncthreads();
+    SL_MARK(11);
+    for (uint32_t i = tid; i < nV; i += NT) L.key1[SM ? i : (uint32_t)vlist[i]] = (key_t)S_KEYMAX;
+    __syncthreads();
+    SL_MARK(0);
+#endif
+    // ---- P2: keys of the canonical half-edges.  No cost is evaluated here: k_simp_ecost costs every
+    // half-edge before the first round and E2 re-costs the edges of every vertex that moved right after
+    // its collapse.
+    if (SM || L.fmt16) sl_keys<SM, R, true>(A, L, flist, nF, salt);
+    else sl_keys<SM, R, false>(A, L, flist, nF, salt);
     __syncthreads();
     SL_MARK(1);
     // ---- P3: dirty flags consumed; LOSE = a face neighbour holds a smaller key
@@ -1451,7 +1544,7 @@ __global__ void __launch_bounds__(SL_THREADS, 1) k_simp_labels(SlArgs A) {
     const uint32_t vbase = A.vert_off[l], U = A.vert_off[l + 1] - vbase;
     const uint32_t target = A.target[l];
     if (T == 0 || T <= target) continue;  // init left every face / vertex alive
-    const bool fmt16 = 3ull * T <= 65536ull;
+    const bool fmt16 = s_fmt16(T);
     if (sl_fits_smem(T, U, blockDim.x, A.smem_bytes)) {
       const uint32_t wcap = sl_wcap(T, U, blockDim.x, A.smem_bytes, false, A.wcap_max);
       const SlLayout y = sl_layout(T, U, false, wcap);
@@ -1881,7 +1974,11 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
     IGN_CUDA(cudaMemcpy(tr.data(), A.trace, SL_HIST * 4, cudaMemcpyDeviceToHost));
     unsigned long long phs[SL_NPH];
     IGN_CUDA(cudaMemcpy(phs, A.trace + 1600, sizeof(phs), cudaMemcpyDeviceToHost));
-    static const char* names[SL_NPH] = {"P1", "P2 keys", "P3 lose", "P4 select", "setup", "E1 rings", "E2a cost", "E2 validate+collapse+recost", "stop+compact"};
+    static const char* names[SL_NPH] = {"P1", "P2 keys", "P3 lose", "P4 select", "setup", "E1 rings", "E2a cost", "E2 validate+collapse+recost", "stop+compact"
+#ifdef IGN_SIMP_P2_PROBE
+        , "P2 probe: float loads", "P2 probe: own loads", "P2 probe: posts of 0"
+#endif
+    };
     unsigned long long tot = 0;
     for (int q = 0; q < SL_NPH; q++) tot += phs[q];
     for (int q = 0; q < SL_NPH; q++)
