@@ -32,9 +32,10 @@ def _stale(target, deps):
 
 
 # simplify.cu must match the CPU oracle bit for bit, and contrast.cu the float32 rules of
-# DESIGN.md §5b (each product rounded on its own), geodesic.cu the penalty field of §5e: no FMA contraction
+# DESIGN.md §5b (each product rounded on its own), geodesic.cu the penalty field of §5e, xsection.cu the
+# membership test of §5i: no FMA contraction
 PER_FILE_FLAGS = {"simplify.cu": ["-fmad=false"], "contrast.cu": ["-fmad=false"], "geodesic.cu": ["-fmad=false"],
-                  "skelmerge.cu": ["-fmad=false"]}
+                  "skelmerge.cu": ["-fmad=false"], "xsection.cu": ["-fmad=false"]}
 # IGN_SIMP_P2_PROBE=1 (a measurement build; rebuild with --force when switching): IGN_SIMP_TRACE=1 also times the
 # simplifier's key pass taken apart into its loads and its posts (DESIGN.md §8)
 if os.environ.get("IGN_SIMP_P2_PROBE") == "1":

@@ -12,7 +12,9 @@ Objects, fields, the loop and the compaction of the skeleton run in libigneous_b
 precomputed skeleton per label (igneous_b200/csrc/skeleton.cu, DESIGN.md §5g): the host copies the packed
 blobs back once and every Skeleton's arrays are views into them.  export_skeletons is the same call with a
 vertex offset, the blobs and the bounding boxes, for SkeletonTask.  postprocess and merge_fragments run
-the merge stage (igneous_b200/csrc/skelmerge.cu, DESIGN.md §5h).  There is no CPU fallback.
+the merge stage (igneous_b200/csrc/skelmerge.cu, DESIGN.md §5h).  cross_sectional_area measures the section of
+each label across its skeleton at every vertex (igneous_b200/csrc/xsection.cu, DESIGN.md §5i).  There is no
+CPU fallback.
 """
 import ctypes
 import time
@@ -22,10 +24,14 @@ import numpy as np
 from . import _shim
 from .teasar import device_fields
 
-__all__ = ["skeletonize", "export_skeletons", "postprocess", "merge_fragments", "Skeleton", "DEFAULT_TEASAR_PARAMS"]
+__all__ = ["skeletonize", "export_skeletons", "postprocess", "merge_fragments", "cross_sectional_area", "Skeleton",
+           "DEFAULT_TEASAR_PARAMS"]
 
 # seconds per phase of the last call, each ending where the host already waits for the device (diagnostic)
 last_phase_seconds = {}
+# cross_sectional_area's last call: voxels of every section, vertices whose section outgrew the one-warp path,
+# voxels that path visited in them, and CTAs the large path ran with (diagnostic)
+last_stats = [0, 0, 0, 0]
 
 _UNSIGNED = {1: np.uint8, 2: np.uint16, 4: np.uint32, 8: np.uint64}
 
@@ -38,7 +44,11 @@ DEFAULT_TEASAR_PARAMS = {
 
 class Skeleton:
   """One label's skeleton: vertices (N, 3) float32 in physical units, edges (E, 2) uint32, radii (N,)
-  float32, vertex_types (N,) uint8 and the label as id."""
+  float32, vertex_types (N,) uint8 and the label as id.  cross_sectional_area (N,) float32 and
+  cross_sectional_area_contacts (N,) uint8 are None until cross_sectional_area sets them."""
+
+  cross_sectional_area = None
+  cross_sectional_area_contacts = None
 
   def __init__(self, vertices, edges, radii, vertex_types, id):
     self.vertices, self.edges, self.radii, self.vertex_types, self.id = vertices, edges, radii, vertex_types, id
@@ -390,3 +400,141 @@ def postprocess(skeleton, dust_threshold=1500, tick_threshold=3000, ctx=None):
   segid = skeleton.id
   return merge_fragments({segid: [(None, skeleton)]}, dust_threshold=dust_threshold, tick_threshold=tick_threshold,
                          ctx=ctx)[segid][0]
+
+
+def cross_sectional_area(all_labels, skeletons, anisotropy=(1, 1, 1), smoothing_window=1, progress=False,
+                         in_place=False, fill_holes=False, repair_contacts=False, ctx=None):
+  """Drop-in for kimimaro.cross_sectional_area (DESIGN.md §5i): at every vertex of every skeleton, the area
+  (float32, physical units squared) of the section of its label through the vertex's voxel across the skeleton's
+  smoothed direction there, and the faces of the array that section touches (uint8: bit 0 x = 0, 1 x = sx - 1,
+  2 y = 0, 3 y = sy - 1, 4 z = 0, 5 z = sz - 1), as cross_sectional_area and cross_sectional_area_contacts.
+  skeletons: {label: Skeleton}, a list of Skeletons or one Skeleton (the label is its id); the result has the
+  same shape, the caller's objects when in_place, else new Skeletons with copies of the arrays in their own
+  dtypes.  A label the array's dtype cannot hold raises ValueError.  `progress` is
+  accepted and ignored; fill_holes and repair_contacts raise NotImplementedError.  last_phase_seconds holds
+  the host-clock time of each phase of the last call."""
+  if fill_holes or repair_contacts:
+    raise NotImplementedError("igneous_b200 kimimaro.cross_sectional_area: fill_holes and repair_contacts are not "
+                              "supported")
+  arr = np.asarray(all_labels)
+  if arr.ndim != 3:
+    raise ValueError("kimimaro.cross_sectional_area: expected a 3-D label array, got shape %r" % (arr.shape,))
+  if not (arr.dtype == np.bool_ or arr.dtype.kind in "iu"):
+    raise NotImplementedError("igneous_b200 kimimaro.cross_sectional_area: label dtype %s is not supported"
+                              % arr.dtype)
+  a = tuple(float(v) for v in anisotropy)
+  if len(a) != 3 or not all(np.isfinite(v) and v > 0 for v in a):
+    raise ValueError("kimimaro.cross_sectional_area: anisotropy %r must be three positive finite values"
+                     % (anisotropy,))
+  w = smoothing_window
+  if isinstance(w, (bool, np.bool_)) or not isinstance(w, (int, np.integer)) or w < 1:
+    raise ValueError("kimimaro.cross_sectional_area: smoothing_window %r must be an integer >= 1" % (w,))
+  last_phase_seconds.clear()
+  last_stats[:] = [0, 0, 0, 0]
+  t0 = time.perf_counter()
+
+  def phase(name):
+    nonlocal t0
+    t = time.perf_counter()
+    last_phase_seconds[name] = t - t0
+    t0 = t
+
+  if isinstance(skeletons, Skeleton):
+    items = [(skeletons.id, skeletons)]
+  elif isinstance(skeletons, dict):
+    items = list(skeletons.items())
+  else:
+    items = [(s.id, s) for s in skeletons]
+  verts = [np.asarray(s.vertices).reshape(-1, 3) for _, s in items]
+  edges = [np.asarray(s.edges).reshape(-1, 2) for _, s in items]
+  counts = np.array([len(v) for v in verts], np.int64)
+  bounds = np.concatenate([[0], np.cumsum(counts)])
+  V = int(bounds[-1])
+  vall = np.concatenate(verts).astype(np.float64) if V else np.zeros((0, 3))
+  c = np.rint(vall / np.array(a, np.float64))
+  shape = np.array(arr.shape, np.int64)
+  bad = np.nonzero(~np.all(np.isfinite(c) & (c >= 0) & (c < shape), axis=1))[0]
+  if bad.size:
+    k = int(np.searchsorted(bounds, bad[0], side="right")) - 1
+    raise ValueError("kimimaro.cross_sectional_area: vertex %d %r of label %r lies outside the array of shape %r"
+                     % (int(bad[0] - bounds[k]), tuple(float(x) for x in vall[bad[0]]), items[k][0], arr.shape))
+  ecounts = np.array([len(e) for e in edges], np.int64)
+  eall = np.concatenate(edges).astype(np.int64) if ecounts.sum() else np.zeros((0, 2), np.int64)
+  local_max = np.repeat(counts, ecounts)
+  wrong = np.nonzero((eall.min(axis=1) < 0) | (eall.max(axis=1) >= local_max))[0] if eall.size else []
+  if len(wrong):
+    k = int(np.searchsorted(np.cumsum(ecounts), wrong[0], side="right"))
+    raise ValueError("kimimaro.cross_sectional_area: label %r has an edge index outside its %d vertices"
+                     % (items[k][0], counts[k]))
+  vox = np.ascontiguousarray(c, dtype=np.int64)
+  edg = np.ascontiguousarray(eall + np.repeat(bounds[:-1], ecounts)[:, None], dtype=np.uint32)
+  unsigned = _UNSIGNED[arr.dtype.itemsize]
+  # a label outside the array's dtype would wrap onto another label: refuse it
+  lo, hi = (0, 1) if arr.dtype == np.bool_ else (int(np.iinfo(arr.dtype).min), int(np.iinfo(arr.dtype).max))
+  keys = []
+  for label, _ in items:
+    if not isinstance(label, (bool, int, np.bool_, np.integer)) or not lo <= int(label) <= hi:
+      raise ValueError("kimimaro.cross_sectional_area: label %r is not an integer the array's dtype %s holds"
+                       % (label, arr.dtype))
+    keys.append(int(label))
+  values = np.array(keys, np.int64 if lo < 0 else np.uint64).astype(arr.dtype).view(unsigned).astype(np.uint64)
+  lab = np.ascontiguousarray(np.repeat(values, counts))
+  if not in_place:
+    def copied(parts):
+      """copies of the caller's arrays in their own dtypes: views into one buffer when they share a dtype"""
+      arrays = [None if p is None else np.asarray(p) for p in parts]
+      kinds = {(p.dtype, p.shape[1:]) for p in arrays if p is not None and p.ndim}
+      if not arrays or len(kinds) != 1 or any(p is None or not p.ndim for p in arrays):
+        return [None if p is None else np.array(p, copy=True) for p in arrays]
+      ends = np.cumsum([len(p) for p in arrays])
+      flat = np.concatenate(arrays)
+      return [flat[e - len(p):e] for p, e in zip(arrays, ends)]
+    cv, ce, cr, ct = (copied([getattr(s, f) for _, s in items]) for f in ("vertices", "edges", "radii", "vertex_types"))
+    items = [(label, Skeleton(v, e, r, t, s.id)) for (label, s), v, e, r, t in zip(items, cv, ce, cr, ct)]
+  area, contacts = np.zeros(V, np.float32), np.zeros(V, np.uint8)
+  if V:
+    ctx = ctx or _shim.default_context()
+    lib, h, ptr = ctx.lib, ctx.handle, _shim.ptr
+    vol = np.asfortranarray(arr.view(unsigned))
+    ca = (ctypes.c_double * 3)(*a)
+    bufs = []
+    try:
+      bufs.append(ctx.alloc(vol.nbytes))
+      d_vol = bufs[-1]
+      ctx.h2d(d_vol, vol)
+      ctx.sync()
+      phase("upload")
+      normals = np.empty((V, 3), np.float64)
+      _shim.check(lib.ign_cross_section_normals(V, ptr(vox), edg.shape[0], ptr(edg), ca, int(w), ptr(normals)))
+      phase("normals")
+      lin = np.ascontiguousarray(vox[:, 0] + shape[0] * (vox[:, 1] + shape[1] * vox[:, 2]), dtype=np.uint64)
+      d = []
+      for host in (lin, lab, normals):
+        bufs.append(ctx.alloc(host.nbytes))
+        d.append(bufs[-1])
+        ctx.h2d(d[-1], host)
+      bufs.append(ctx.alloc(V * 4))
+      d_area = bufs[-1]
+      bufs.append(ctx.alloc(V))
+      d_contacts = bufs[-1]
+      stats = (ctypes.c_uint64 * 4)()
+      _shim.check(lib.ign_cross_section_dev(h, ptr(d_vol), _shim.dtype_code(vol.dtype), *vol.shape, ptr(d[0]),
+                                            ptr(d[1]), ptr(d[2]), V, ca, ptr(d_area), ptr(d_contacts), stats))
+      phase("sections")
+      ctx.d2h(area, d_area)
+      ctx.d2h(contacts, d_contacts)
+      ctx.sync()
+      last_stats[:] = [int(x) for x in stats]
+    finally:
+      for b in bufs:
+        b.free()
+  for (label, s), b, e in zip(items, bounds[:-1], bounds[1:]):
+    s.cross_sectional_area = area[b:e]  # views into one array per call
+    s.cross_sectional_area_contacts = contacts[b:e]
+  if V:
+    phase("copy_back")
+  if isinstance(skeletons, Skeleton):
+    return items[0][1]
+  if isinstance(skeletons, dict):
+    return dict(items)
+  return [s for _, s in items]

@@ -511,6 +511,34 @@ IGN_API int ign_skeleton_merge_dev(ign_ctx* ctx, uint64_t n_labels, const uint64
                                    uint64_t* nbytes);
 IGN_API int ign_skeleton_merge_capacity(uint64_t n_labels, uint64_t n_vertices, uint64_t n_edges, uint64_t* bytes);
 
+/* ------------------------------------------------------- cross-sectional area
+ * kimimaro.cross_sectional_area (igneous/tasks/skeleton.py:219-226, :400-475); the rule is DESIGN.md §5i.
+ * ign_cross_section_normals: HOST arrays.  n_vertices vertices (below 2^32, else IGN_ERR_UNSUPPORTED) of any
+ *   number of skeletons, voxels int64 [][3] the voxel of each; n_edges edges uint32 [][2] into the same list
+ *   (an index >= n_vertices -> IGN_ERR_INVALID; self edges are ignored).  Per component of the edge graph: the
+ *   root is the vertex farthest in hops from its lowest vertex, every vertex lies on the path from the shallowest
+ *   leaf of its subtree to the root, and normals_out float64 [][3] is the sum of the voxel steps
+ *   c_u - c_parent(u) over `window` (>= 1) path positions centred on it (numpy 'symmetric' padding at the ends),
+ *   times anisotropy; its own step when that sum is zero; 0 for a vertex on no edge.  Host code only.
+ * ign_cross_section_dev: DEVICE arrays, except anisotropy and stats.  labels (dtype u8/u16/u32/u64) of an
+ *   (sx, sy, sz) F-order volume of fewer than 2^32 voxels (IGN_ERR_UNSUPPORTED otherwise); n_points points:
+ *   voxel uint64 its linear index, label uint64 its skeleton's label, normal float64 [][3].  Out per point:
+ *   area_out float32 the area of the section of the label through the voxel's centre across the normal (0 for
+ *   a zero normal or a voxel of another label), contacts_out uint8 the faces of the volume it touches: bit 0
+ *   x = 0, 1 x = sx - 1, 2 y = 0, 3 y = sy - 1, 4 z = 0, 5 z = sz - 1.  A voxel outside the volume or a
+ *   non-finite normal -> IGN_ERR_INVALID naming the lowest such point.  stats: [0] voxels of every section,
+ *   [1] points whose section outgrew the one-warp path, [2] voxels that path visited in them, [3] CTAs
+ *   the large path ran with (each takes large points until none is left; at most one per SM, and fewer when
+ *   their bitmaps and queues, 13 bytes per column of the largest projection each, would pass 512 MB).  The host
+ *   synchronises once, twice when a section outgrows the one-warp path. */
+IGN_API int ign_cross_section_normals(uint64_t n_vertices, const int64_t* voxels, uint64_t n_edges,
+                                      const uint32_t* edges, const double anisotropy[3], uint64_t window,
+                                      double* normals_out);
+IGN_API int ign_cross_section_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
+                                  const uint64_t* voxel, const uint64_t* label, const double* normal,
+                                  uint64_t n_points, const double anisotropy[3], float* area_out,
+                                  uint8_t* contacts_out, uint64_t stats[4]);
+
 /* --------------------------------------------------------------------- mesh
  * zmesh.Mesher(resolution).mesh(data, preserve_order=False)  igneous/tasks/mesh/mesh.py:151,245
  * Mesher.ids()                                                igneous/tasks/mesh/mesh.py:374
