@@ -36,10 +36,6 @@ def _stale(target, deps):
 # membership test of §5i: no FMA contraction
 PER_FILE_FLAGS = {"simplify.cu": ["-fmad=false"], "contrast.cu": ["-fmad=false"], "geodesic.cu": ["-fmad=false"],
                   "skelmerge.cu": ["-fmad=false"], "xsection.cu": ["-fmad=false"]}
-# IGN_SIMP_P2_PROBE=1 (a measurement build; rebuild with --force when switching): IGN_SIMP_TRACE=1 also times the
-# simplifier's key pass taken apart into its loads and its posts (DESIGN.md §8)
-if os.environ.get("IGN_SIMP_P2_PROBE") == "1":
-  PER_FILE_FLAGS["simplify.cu"] = PER_FILE_FLAGS["simplify.cu"] + ["-DIGN_SIMP_P2_PROBE"]
 
 
 def _compile(src, obj, log):

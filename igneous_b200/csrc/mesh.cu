@@ -303,7 +303,6 @@ int ign_mesh_begin_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx,
   m->d_pos_f = nullptr;
   m->simp_factor = 0;
   m->simp_max_error = 0;
-  m->simp_rounds = 0;
   // a failed build frees the half-built mesher
   struct Guard {
     ign_mesher* m;

@@ -19,13 +19,7 @@ struct ign_mesher {
   float res[3];
   int simp_factor;
   float simp_max_error;
-  int simp_rounds;
-  uint32_t simp_labels_smem, simp_labels_gmem;  // labels simplified in shared / global memory
-  uint32_t simp_labels_class[3];                // labels simplified in 1024-, 512- and 256-thread CTAs
-  uint32_t simp_migrations[3];                  // labels resumed in each class after they shrank
-  uint32_t simp_passes[2];                      // multi-pass label-rounds, winners with a ring over 32 faces
-  uint32_t simp_costs[3];                       // initial costs, re-costs after collapses, costless keys
-  uint32_t simp_groups[3];                      // winners validated by lane groups of 8, 16 and 32
+  uint32_t simp_counters[17];  // ign_mesh_simplify_counters
   std::vector<uint64_t> ids;       // original label of dense id i+1
   std::vector<uint32_t> tri_off;   // [K+2]
   std::vector<uint32_t> vert_off;  // [K+2]

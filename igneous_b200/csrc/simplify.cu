@@ -35,6 +35,7 @@
 #include <cub/device/device_scan.cuh>
 
 #include <stdlib.h>
+#include <string.h>
 
 #include <algorithm>
 #include <type_traits>
@@ -481,11 +482,7 @@ constexpr int SL_HIST = 1664, SL_HP = 16, SL_HW = 64, SL_HR = S_MAXV + 2, SL_HCL
 // header of a migrated label: dense label, trace record, next round, slow rounds, alive faces, alive vertices
 constexpr int SL_MREC = 8;
 constexpr int SL_LREC = 7;  // words of a label's IGN_SIMP_TRACE record (SlArgs::lrec)
-#ifdef IGN_SIMP_P2_PROBE
-constexpr int SL_NPH = 12;  // IGN_SIMP_TRACE phase timers (trace words 1600.., 64 bits each), and the P2 probes
-#else
 constexpr int SL_NPH = 9;  // IGN_SIMP_TRACE phase timers (trace words 1600.., 64 bits each)
-#endif
 // IGN_SIMP_TRACE E2 flip tests (trace words SL_TFLIP..): winners rejected by flips on the u side only, on the
 // v side only, on both sides
 constexpr int SL_TFLIP = 1624;
@@ -1060,14 +1057,12 @@ __device__ void sl_migrate(const SlArgs& A, const SlLab<true>& L, SlShared& sh, 
 // P2: every canonical half-edge (u < v) of an alive face posts its cached key to both endpoints.  A warp takes
 // 32 alive faces per iteration.  The cached costs are the only global loads: PK (32-bit keys) one packed word
 // per face (s_cwords), requested two iterations ahead; else three floats, one iteration ahead.  A resumed label
-// addresses them by the original face id.  PROBE (IGN_SIMP_P2_PROBE builds only): 1 loads and keys without
-// posts or state writes, 2 posts with every cost taken as 0 and no loads.
-template <bool SM, bool R, bool PK, int PROBE = 0>
+// addresses them by the original face id.
+template <bool SM, bool R, bool PK>
 __device__ __forceinline__ void sl_keys(const SlArgs& A, const SlLab<SM>& L, const typename SlLab<SM>::idx_t* flist,
                                         uint32_t nF, uint32_t salt) {
   typedef typename SlLab<SM>::key_t key_t;
   constexpr int D = PK ? 2 : 1;
-  constexpr bool LOAD = PROBE != 2;
   const uint32_t tid = threadIdx.x, NT = blockDim.x, lane = tid & 31u, warp = tid >> 5;
   const unsigned long long* cw = s_cwords(A.ecost, L.tbase);
   const float* ecb = A.ecost + 3 * (uint64_t)L.tbase;
@@ -1084,11 +1079,10 @@ __device__ __forceinline__ void sl_keys(const SlArgs& A, const SlLab<SM>& L, con
     if (i < nF) {
       f_n[s] = flist[i];
       fo_n[s] = sl_fo<SM, R>(L, f_n[s]);
-      if (LOAD && PK) w_n[s] = cw[fo_n[s]];
-      if (LOAD && !PK) { ec_n[s][0] = ecb[3 * (uint64_t)fo_n[s]]; ec_n[s][1] = ecb[3 * (uint64_t)fo_n[s] + 1]; ec_n[s][2] = ecb[3 * (uint64_t)fo_n[s] + 2]; }
+      if (PK) w_n[s] = cw[fo_n[s]];
+      else { ec_n[s][0] = ecb[3 * (uint64_t)fo_n[s]]; ec_n[s][1] = ecb[3 * (uint64_t)fo_n[s] + 1]; ec_n[s][2] = ecb[3 * (uint64_t)fo_n[s] + 2]; }
     }
   }
-  unsigned long long sink = 0;  // PROBE 1: keeps the loads and keys that are not posted
   for (uint32_t base = warp * 32; base < nF; base += NT) {
     const uint32_t i = base + lane;
     const uint32_t f = f_n[0], fo = fo_n[0];
@@ -1102,8 +1096,8 @@ __device__ __forceinline__ void sl_keys(const SlArgs& A, const SlLab<SM>& L, con
     if (i + D * NT < nF) {
       f_n[D - 1] = flist[i + D * NT];
       fo_n[D - 1] = sl_fo<SM, R>(L, f_n[D - 1]);
-      if (LOAD && PK) w_n[D - 1] = cw[fo_n[D - 1]];
-      if (LOAD && !PK) {
+      if (PK) w_n[D - 1] = cw[fo_n[D - 1]];
+      else {
         const float* e = ecb + 3 * (uint64_t)fo_n[D - 1];
         ec_n[D - 1][0] = e[0]; ec_n[D - 1][1] = e[1]; ec_n[D - 1][2] = e[2];
       }
@@ -1131,17 +1125,15 @@ __device__ __forceinline__ void sl_keys(const SlArgs& A, const SlLab<SM>& L, con
           const uint32_t hl = 3u * fo + (uint32_t)c;
           const key_t key = PK ? (key_t)sl_key((uint32_t)(w >> (16 * c)) & 0xFFFFu, hl, salt)
                                : sl_key<SM>(L, ec[c], hl, salt);
-          if (PROBE == 1) sink += key;
-          else sl_post(L.key1, u, v, key);
-        } else if (es == 0 && PROBE == 0) {
+          sl_post(L.key1, u, v, key);
+        } else if (es == 0) {
           atomicAdd(&A.counters[28], 1u);  // a half-edge without a cost: a bug
         }
         nst = (nst & ~(3u << (2 * c))) | (es << (2 * c));
       }
-      if (PROBE == 0 && nst != st) L.fstate[f] = (uint8_t)nst;
+      if (nst != st) L.fstate[f] = (uint8_t)nst;
     }
   }
-  if (PROBE == 1 && sink == 0x9E3779B97F4A7C15ull) A.trace[SL_TFLIP + 3] = 1;
 }
 
 // All rounds of one label (R: a label resumed from the header `hdr` after it migrated from a larger class)
@@ -1234,24 +1226,6 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
     }
     __syncthreads();
     SL_MARK(0);
-#ifdef IGN_SIMP_P2_PROBE
-    // P2 taken apart (with IGN_SIMP_TRACE=1): its loads and keys without the posts, in the float layout
-    // (three loads per face) and in the label's own, then its posts with every cost taken as 0 and no
-    // loads; then P1's key reset again
-    sl_keys<SM, R, false, 1>(A, L, flist, nF, salt);
-    __syncthreads();
-    SL_MARK(9);
-    if (SM || L.fmt16) sl_keys<SM, R, true, 1>(A, L, flist, nF, salt);
-    else sl_keys<SM, R, false, 1>(A, L, flist, nF, salt);
-    __syncthreads();
-    SL_MARK(10);
-    sl_keys<SM, R, false, 2>(A, L, flist, nF, salt);
-    __syncthreads();
-    SL_MARK(11);
-    for (uint32_t i = tid; i < nV; i += NT) L.key1[SM ? i : (uint32_t)vlist[i]] = (key_t)S_KEYMAX;
-    __syncthreads();
-    SL_MARK(0);
-#endif
     // ---- P2: keys of the canonical half-edges.  No cost is evaluated here: k_simp_ecost costs every
     // half-edge before the first round and E2 re-costs the edges of every vertex that moved right after
     // its collapse.
@@ -1524,6 +1498,31 @@ __device__ void sl_run(const SlArgs& A, const SlLab<SM>& L, SlShared& sh, const 
   }
 }
 
+// A shared-memory label of T faces and U vertices laid out as y, with wcap winners per pass; a resumed
+// label also has the maps of its compacted faces and vertices.  The caller sets tbase, vbase, target, label.
+__device__ __forceinline__ SlLab<true> sl_lab_smem(uint32_t T, uint32_t U, uint32_t wcap, const SlLayout& y,
+                                                   bool resumed) {
+  SlLab<true> L;
+  L.T = T; L.U = U;
+  L.wcap = wcap;
+  L.ring = (uint16_t*)(sl_smem + y.o_ring);
+  L.key1 = (uint32_t*)(sl_smem + y.o_key);
+  L.fmt16 = true;
+  L.fc0 = (uint16_t*)(sl_smem + y.o_f0);
+  L.fc1 = L.fc0 + T;
+  L.fc2 = L.fc1 + T;
+  L.flist = (uint16_t*)(sl_smem + y.o_fl);
+  L.vlist = nullptr;
+  L.flist2 = L.vlist2 = nullptr;
+  L.gface = nullptr;
+  L.fstate = sl_smem + y.o_fs;
+  L.vflag = sl_smem + y.o_vf;
+  L.vlose = sl_smem + y.o_vl;
+  L.fmap = resumed ? (uint16_t*)(sl_smem + y.o_fm) : nullptr;
+  L.vmap = resumed ? (uint16_t*)(sl_smem + y.o_vm) : nullptr;
+  return L;
+}
+
 // One label per CTA (the launch has one CTA per label of its size class; a CTA takes the next label of
 // the size-sorted order from a counter, so big labels start first whatever order the hardware dispatches
 // CTAs in).  The block size is the class's (1024, 512 or 256 threads); 64 registers per thread let two
@@ -1547,25 +1546,8 @@ __global__ void __launch_bounds__(SL_THREADS, 1) k_simp_labels(SlArgs A) {
     const bool fmt16 = s_fmt16(T);
     if (sl_fits_smem(T, U, blockDim.x, A.smem_bytes)) {
       const uint32_t wcap = sl_wcap(T, U, blockDim.x, A.smem_bytes, false, A.wcap_max);
-      const SlLayout y = sl_layout(T, U, false, wcap);
-      SlLab<true> L;
-      L.T = T; L.U = U; L.tbase = tbase; L.vbase = vbase; L.target = target;
-      L.wcap = wcap;
-      L.ring = (uint16_t*)(sl_smem + y.o_ring);
-      L.key1 = (uint32_t*)(sl_smem + y.o_key);
-      L.fmt16 = true;
-      L.fc0 = (uint16_t*)(sl_smem + y.o_f0);
-      L.fc1 = L.fc0 + T;
-      L.fc2 = L.fc1 + T;
-      L.flist = (uint16_t*)(sl_smem + y.o_fl);
-      L.vlist = nullptr;
-      L.flist2 = L.vlist2 = nullptr;
-      L.gface = nullptr;
-      L.fstate = sl_smem + y.o_fs;
-      L.vflag = sl_smem + y.o_vf;
-      L.vlose = sl_smem + y.o_vl;
-      L.label = l;
-      L.fmap = L.vmap = nullptr;
+      SlLab<true> L = sl_lab_smem(T, U, wcap, sl_layout(T, U, false, wcap), false);
+      L.tbase = tbase; L.vbase = vbase; L.target = target; L.label = l;
       sl_run<true, false>(A, L, sh, nullptr);
     } else {
       const SlLayout y = sl_layout(T, U);
@@ -1620,26 +1602,8 @@ __global__ void __launch_bounds__(SL_THREADS / 2, 2) k_simp_resume(SlArgs A) {
     const uint32_t l = hdr[0];
     const uint32_t T = hdr[4], U = hdr[5];
     const uint32_t wcap = sl_wcap(T, U, blockDim.x, A.smem_bytes, true, A.wcap_max);
-    const SlLayout y = sl_layout(T, U, true, wcap);
-    SlLab<true> L;
-    L.T = T; L.U = U; L.tbase = A.tri_off[l]; L.vbase = A.vert_off[l]; L.target = A.target[l];
-    L.label = l;
-    L.wcap = wcap;
-    L.ring = (uint16_t*)(sl_smem + y.o_ring);
-    L.key1 = (uint32_t*)(sl_smem + y.o_key);
-    L.fmt16 = true;
-    L.fc0 = (uint16_t*)(sl_smem + y.o_f0);
-    L.fc1 = L.fc0 + T;
-    L.fc2 = L.fc1 + T;
-    L.flist = (uint16_t*)(sl_smem + y.o_fl);
-    L.vlist = nullptr;
-    L.flist2 = L.vlist2 = nullptr;
-    L.gface = nullptr;
-    L.fstate = sl_smem + y.o_fs;
-    L.vflag = sl_smem + y.o_vf;
-    L.vlose = sl_smem + y.o_vl;
-    L.fmap = (uint16_t*)(sl_smem + y.o_fm);
-    L.vmap = (uint16_t*)(sl_smem + y.o_vm);
+    SlLab<true> L = sl_lab_smem(T, U, wcap, sl_layout(T, U, true, wcap), true);
+    L.tbase = A.tri_off[l]; L.vbase = A.vert_off[l]; L.target = A.target[l]; L.label = l;
     sl_run<true, true>(A, L, sh, hdr);
   } while (A.persist);
 }
@@ -1712,12 +1676,7 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   m->res[2] = resolution[2];
   m->simp_factor = reduction_factor;
   m->simp_max_error = max_error;
-  m->simp_rounds = 0;
-  m->simp_labels_smem = m->simp_labels_gmem = 0;
-  for (int c = 0; c < SL_NCLASS; c++) m->simp_labels_class[c] = m->simp_migrations[c] = 0;
-  m->simp_passes[0] = m->simp_passes[1] = 0;
-  m->simp_costs[0] = m->simp_costs[1] = m->simp_costs[2] = 0;
-  m->simp_groups[0] = m->simp_groups[1] = m->simp_groups[2] = 0;
+  memset(m->simp_counters, 0, sizeof(m->simp_counters));
   const uint64_t U = m->U, T = m->T, K = m->K;
   if (T == 0 || U == 0) {
     m->simplified = true;
@@ -1974,11 +1933,7 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
     IGN_CUDA(cudaMemcpy(tr.data(), A.trace, SL_HIST * 4, cudaMemcpyDeviceToHost));
     unsigned long long phs[SL_NPH];
     IGN_CUDA(cudaMemcpy(phs, A.trace + 1600, sizeof(phs), cudaMemcpyDeviceToHost));
-    static const char* names[SL_NPH] = {"P1", "P2 keys", "P3 lose", "P4 select", "setup", "E1 rings", "E2a cost", "E2 validate+collapse+recost", "stop+compact"
-#ifdef IGN_SIMP_P2_PROBE
-        , "P2 probe: float loads", "P2 probe: own loads", "P2 probe: posts of 0"
-#endif
-    };
+    static const char* names[SL_NPH] = {"P1", "P2 keys", "P3 lose", "P4 select", "setup", "E1 rings", "E2a cost", "E2 validate+collapse+recost", "stop+compact"};
     unsigned long long tot = 0;
     for (int q = 0; q < SL_NPH; q++) tot += phs[q];
     for (int q = 0; q < SL_NPH; q++)
@@ -2048,15 +2003,9 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
     for (int r = 0; r < 400 && getenv("IGN_SIMP_TRACE_ROUNDS") && (tr[4 * r + 2] || tr[4 * r + 3]); r++)
       fprintf(stderr, "gpu round %d progress %u collapses %u alive %u list %u\n", r, tr[4 * r], tr[4 * r + 1], tr[4 * r + 2], tr[4 * r + 3]);
   }
-  m->simp_rounds = (int)hflags[1];
-  m->simp_labels_smem = hflags[2];
-  m->simp_labels_gmem = hflags[3];
-  for (int c = 0; c < SL_NCLASS; c++) m->simp_labels_class[c] = hflags[8 + c];
-  for (int c = 0; c < SL_NCLASS; c++) m->simp_migrations[c] = hflags[16 + c];
-  m->simp_passes[0] = hflags[24];
-  m->simp_passes[1] = hflags[25];
-  for (int i = 0; i < 3; i++) m->simp_costs[i] = hflags[26 + i];
-  for (int i = 0; i < 3; i++) m->simp_groups[i] = hflags[29 + i];
+  // the SlArgs::counters words that ign_mesh_simplify_counters returns, in its order
+  static const int word[17] = {1, 2, 3, 8, 9, 10, 16, 17, 18, 24, 25, 26, 27, 28, 29, 30, 31};
+  for (int i = 0; i < 17; i++) m->simp_counters[i] = hflags[word[i]];
   const uint32_t U2 = last[0] + last[1], T2 = last[2] + last[3];
   IGN_LAUNCH(ctx, k_simp_new_offsets, blocks_for(K + 2, 256), 256, 0, d_vert_off, vscan, (uint32_t)(K + 2), U, U2,
                    d_new_vert_off);
@@ -2079,41 +2028,9 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   return IGN_OK;
 }
 
-extern "C" int ign_mesh_simplify_stats(ign_mesher* m, uint32_t stats[6]) {
-  IGN_REQUIRE(m && stats, IGN_ERR_INVALID, "null argument");
+extern "C" int ign_mesh_simplify_counters(ign_mesher* m, uint32_t counters[17]) {
+  IGN_REQUIRE(m && counters, IGN_ERR_INVALID, "null argument");
   IGN_REQUIRE(m->simplified, IGN_ERR_INVALID, "mesher is not simplified");
-  stats[0] = (uint32_t)m->simp_rounds;
-  stats[1] = m->simp_labels_smem;
-  stats[2] = m->simp_labels_gmem;
-  for (int c = 0; c < SL_NCLASS; c++) stats[3 + c] = m->simp_labels_class[c];
-  return IGN_OK;
-}
-
-extern "C" int ign_mesh_simplify_migrations(ign_mesher* m, uint32_t resumed[3]) {
-  IGN_REQUIRE(m && resumed, IGN_ERR_INVALID, "null argument");
-  IGN_REQUIRE(m->simplified, IGN_ERR_INVALID, "mesher is not simplified");
-  for (int c = 0; c < SL_NCLASS; c++) resumed[c] = m->simp_migrations[c];
-  return IGN_OK;
-}
-
-extern "C" int ign_mesh_simplify_passes(ign_mesher* m, uint32_t counts[2]) {
-  IGN_REQUIRE(m && counts, IGN_ERR_INVALID, "null argument");
-  IGN_REQUIRE(m->simplified, IGN_ERR_INVALID, "mesher is not simplified");
-  counts[0] = m->simp_passes[0];
-  counts[1] = m->simp_passes[1];
-  return IGN_OK;
-}
-
-extern "C" int ign_mesh_simplify_costs(ign_mesher* m, uint32_t counts[3]) {
-  IGN_REQUIRE(m && counts, IGN_ERR_INVALID, "null argument");
-  IGN_REQUIRE(m->simplified, IGN_ERR_INVALID, "mesher is not simplified");
-  for (int i = 0; i < 3; i++) counts[i] = m->simp_costs[i];
-  return IGN_OK;
-}
-
-extern "C" int ign_mesh_simplify_groups(ign_mesher* m, uint32_t counts[3]) {
-  IGN_REQUIRE(m && counts, IGN_ERR_INVALID, "null argument");
-  IGN_REQUIRE(m->simplified, IGN_ERR_INVALID, "mesher is not simplified");
-  for (int i = 0; i < 3; i++) counts[i] = m->simp_groups[i];
+  memcpy(counters, m->simp_counters, sizeof(m->simp_counters));
   return IGN_OK;
 }

@@ -567,26 +567,22 @@ IGN_API int ign_mesh_get(ign_mesher* m, uint64_t id, const float resolution[3], 
  * calls it on first use; ign_mesh_export then returns the simplified meshes. */
 IGN_API int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int reduction_factor,
                               float max_error);
-/* counters of the simplification that ran: [0] most rounds of any label, [1] labels simplified
- * in shared memory, [2] in global memory, [3..5] labels simplified in the 1024-, 512- and 256-thread
- * size classes (a label runs in the smallest CTA whose shared-memory budget holds it) */
-IGN_API int ign_mesh_simplify_stats(ign_mesher* m, uint32_t stats[6]);
-/* labels of the simplification that ran which continued in the 1024-, 512- and 256-thread size class
- * after migrating from the next larger one, once their alive faces and vertices fit it ([0] is always 0;
- * a label that migrates twice counts in both smaller classes) */
-IGN_API int ign_mesh_simplify_migrations(ign_mesher* m, uint32_t resumed[3]);
-/* selection counters of the simplification that ran: [0] label-rounds whose winners took more than one
- * validation pass (more winners than the label's per-pass capacity), [1] winners rejected because an
- * endpoint had more than 32 alive incident faces */
-IGN_API int ign_mesh_simplify_passes(ign_mesher* m, uint32_t counts[2]);
-/* edge-cost counters of the simplification that ran: [0] half-edges costed before the first round,
- * [1] half-edges re-costed after the collapse that moved an endpoint, [2] half-edges the key pass met
- * without a cached cost (0 unless the simplifier is broken; such an edge posts no key) */
-IGN_API int ign_mesh_simplify_costs(ign_mesher* m, uint32_t counts[3]);
-/* winners of the simplification that ran, by the width of the lane group that validated, collapsed and
- * re-costed them: [0] 8 lanes (rings of at most 8 faces), [1] 16 lanes, [2] 32 lanes (rings over 16 faces,
- * and those over 32 that are rejected); IGN_SIMP_GROUP=16 or 32 sets the narrowest width */
-IGN_API int ign_mesh_simplify_groups(ign_mesher* m, uint32_t counts[3]);
+/* counters of the simplification that ran:
+ * [0] most rounds of any label, [1] labels simplified in shared memory, [2] in global memory,
+ * [3..5] labels simplified in the 1024-, 512- and 256-thread size classes (a label runs in the smallest
+ *   CTA whose shared-memory budget holds it);
+ * [6..8] labels which continued in the 1024-, 512- and 256-thread size class after migrating from the
+ *   next larger one, once their alive faces and vertices fit it ([6] is always 0; a label that migrates
+ *   twice counts in both smaller classes);
+ * [9] label-rounds whose winners took more than one validation pass (more winners than the label's
+ *   per-pass capacity), [10] winners rejected because an endpoint had more than 32 alive incident faces;
+ * [11] half-edges costed before the first round, [12] half-edges re-costed after the collapse that moved
+ *   an endpoint, [13] half-edges the key pass met without a cached cost (0 unless the simplifier is
+ *   broken; such an edge posts no key);
+ * [14..16] winners by the width of the lane group that validated, collapsed and re-costed them: 8 lanes
+ *   (rings of at most 8 faces), 16 lanes, 32 lanes (rings over 16 faces, and those over 32 that are
+ *   rejected); IGN_SIMP_GROUP=16 or 32 sets the narrowest width */
+IGN_API int ign_mesh_simplify_counters(ign_mesher* m, uint32_t counters[17]);
 /* bulk export of every label's mesh (simplified if ign_mesh_simplify ran) in ign_mesh_ids order:
  * vertices f32 [U,3], faces u32 [T,3] (label-local indices), offsets [n_ids+1] */
 IGN_API int ign_mesh_export(ign_mesher* m, const float resolution[3], int voxel_centered,
