@@ -13,11 +13,7 @@
 //                 index list, the key (lo rank << 32) | hi rank; a next voxel off the skeleton or on
 //                 another label fails the call before any output is written
 //   (sort)        the edge keys: runs are contiguous in rank, so this is the order (label, lo, hi)
-//   k_sx_sizes    per run: nv, ne (two binary searches in the sorted keys), the blob size padded to 8
-//   (scan)        exclusive sum of the padded sizes -> byte offsets
-//   k_sx_table    the table rows and the blob headers
-//   k_sx_verts    the vertices and radii
-//   k_sx_write_edges  the edges
+//   (encode)      skelblob_encode (skelblob.cuh): a row per run, the sorted positions as final vertices
 //   k_sx_boxes    one warp per run: min / max of its vertices
 //
 // Every voxel's vertex is computed by sx_vertex, so the boxes are the min / max of the written values.
@@ -27,6 +23,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "skelblob.cuh"
 
 namespace ign {
 
@@ -127,88 +124,23 @@ __global__ void __launch_bounds__(256) k_sx_edges(const uint32_t* __restrict__ l
   if ((threadIdx.x & 31) == 0 && m) atomicAdd(&ctl->ne, (unsigned long long)__popc(m));
 }
 
-__device__ __forceinline__ uint64_t sx_lower(const uint64_t* __restrict__ a, uint64_t n, uint64_t x) {
-  uint64_t lo = 0, hi = n;
-  while (lo < hi) {
-    const uint64_t mid = (lo + hi) >> 1;
-    if (a[mid] < x) lo = mid + 1; else hi = mid;
+// the rows of skelblob_encode: one per run; final vertex j is sorted position j
+struct SxSource {
+  const uint32_t *start, *labels, *run, *val_s, *skel;
+  const float* radius;
+  uint64_t runs, count, sx, sy;
+  float a0, a1, a2;
+  double o0, o1, o2;
+  __device__ uint64_t vstart(uint64_t g) const { return g < runs ? start[g] : count; }
+  __device__ uint64_t label(uint64_t g) const { return labels[g]; }
+  __device__ uint32_t row(uint64_t j) const { return run[j] - 1; }
+  __device__ void vertex(uint64_t j, float c[3], float& r, uint8_t& t) const {
+    const uint32_t i = val_s[j];
+    sx_vertex(skel[i], sx, sy, a0, a1, a2, o0, o1, o2, c);
+    r = radius[i];
+    t = 0;
   }
-  return lo;
-}
-
-__device__ __forceinline__ uint64_t sx_blob_bytes(uint64_t nv, uint64_t ne, int vt) {
-  return 8 + 16 * nv + 8 * ne + (vt ? nv : 0);
-}
-
-__global__ void __launch_bounds__(256) k_sx_sizes(const uint32_t* __restrict__ start, uint64_t runs, uint64_t count,
-                                                  const uint64_t* __restrict__ ekey_s, const SxCtl* __restrict__ ctl,
-                                                  int vt, uint32_t* __restrict__ ebegin,
-                                                  uint64_t* __restrict__ size) {
-  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= runs) return;
-  const uint64_t ne_all = ctl->ne;
-  const uint64_t a = start[g], b = g + 1 < runs ? start[g + 1] : count;
-  const uint64_t e0 = sx_lower(ekey_s, ne_all, a << 32), e1 = sx_lower(ekey_s, ne_all, b << 32);
-  ebegin[g] = (uint32_t)e0;
-  size[g] = (sx_blob_bytes(b - a, e1 - e0, vt) + 7) & ~7ull;
-}
-
-__global__ void __launch_bounds__(256) k_sx_table(const uint32_t* __restrict__ start, const uint32_t* __restrict__ label,
-                                                  const uint32_t* __restrict__ ebegin, const uint64_t* __restrict__ off,
-                                                  uint64_t runs, uint64_t count, int vt, uint64_t* __restrict__ table,
-                                                  uint8_t* __restrict__ blobs, SxCtl* ctl) {
-  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= runs) return;
-  const uint64_t ne_all = ctl->ne;
-  const uint64_t nv = (g + 1 < runs ? start[g + 1] : count) - start[g];
-  const uint64_t ne = (g + 1 < runs ? ebegin[g + 1] : ne_all) - ebegin[g];
-  table[4 * g + 0] = label[g];
-  table[4 * g + 1] = off[g];
-  table[4 * g + 2] = nv;
-  table[4 * g + 3] = ne;
-  uint32_t* h = (uint32_t*)(blobs + off[g]);
-  h[0] = (uint32_t)nv;
-  h[1] = (uint32_t)ne;
-  const uint64_t end = off[g] + sx_blob_bytes(nv, ne, vt);
-  for (uint64_t b = end; b & 7; ++b) blobs[b] = 0;  // the padding up to the next blob
-  if (g + 1 == runs) ctl->bytes = end;
-}
-
-__global__ void __launch_bounds__(256) k_sx_verts(const uint32_t* __restrict__ skel, const float* __restrict__ radius,
-                                                  const uint32_t* __restrict__ val_s, const uint32_t* __restrict__ run,
-                                                  const uint32_t* __restrict__ start,
-                                                  const uint64_t* __restrict__ table, uint64_t count, uint64_t sx,
-                                                  uint64_t sy, float a0, float a1, float a2, double o0, double o1,
-                                                  double o2, int vt, uint8_t* __restrict__ blobs) {
-  const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= count) return;
-  const uint32_t g = run[p] - 1, i = val_s[p];
-  const uint64_t j = p - start[g], off = table[4 * g + 1], nv = table[4 * g + 2], ne = table[4 * g + 3];
-  float c[3];
-  sx_vertex(skel[i], sx, sy, a0, a1, a2, o0, o1, o2, c);
-  float* vert = (float*)(blobs + off + 8) + 3 * j;
-  vert[0] = c[0];
-  vert[1] = c[1];
-  vert[2] = c[2];
-  ((float*)(blobs + off + 8 + 12 * nv + 8 * ne))[j] = radius[i];
-  if (vt) blobs[off + 8 + 16 * nv + 8 * ne + j] = 0;
-}
-
-__global__ void __launch_bounds__(256) k_sx_write_edges(const uint64_t* __restrict__ ekey_s, const SxCtl* __restrict__ ctl,
-                                                        const uint32_t* __restrict__ run,
-                                                        const uint32_t* __restrict__ start,
-                                                        const uint32_t* __restrict__ ebegin,
-                                                        const uint64_t* __restrict__ table, uint8_t* __restrict__ blobs) {
-  const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= ctl->ne) return;
-  const uint64_t k = ekey_s[e];
-  const uint32_t lo = (uint32_t)(k >> 32), hi = (uint32_t)k;
-  const uint32_t g = run[lo] - 1, a = start[g];
-  const uint64_t off = table[4 * g + 1], nv = table[4 * g + 2];
-  uint32_t* edge = (uint32_t*)(blobs + off + 8 + 12 * nv) + 2 * (e - ebegin[g]);
-  edge[0] = lo - a;
-  edge[1] = hi - a;
-}
+};
 
 __global__ void __launch_bounds__(256) k_sx_boxes(const uint32_t* __restrict__ skel, const uint32_t* __restrict__ val_s,
                                                   const uint32_t* __restrict__ start, uint64_t runs, uint64_t count,
@@ -312,8 +244,8 @@ int ign_skeleton_export_dev(ign_ctx* ctx, const uint32_t* labels, uint64_t sx, u
   const uint64_t rows = std::max<uint64_t>(std::min(max_label, count), 1);
   ScratchFrame f(ctx);
   SxCtl* ctl;
-  uint32_t *key, *val, *key_s, *val_s, *head, *run, *rank, *start, *label, *ebegin;
-  uint64_t *ekey, *ekey_s, *size, *off;
+  uint32_t *key, *val, *key_s, *val_s, *head, *run, *rank, *start, *label;
+  uint64_t *ekey, *ekey_s;
   IGN_TRY(f.take(&ctl, 1));
   IGN_TRY(f.take(&key, count));
   IGN_TRY(f.take(&val, count));
@@ -326,9 +258,6 @@ int ign_skeleton_export_dev(ign_ctx* ctx, const uint32_t* labels, uint64_t sx, u
   IGN_TRY(f.take(&ekey_s, count));
   IGN_TRY(f.take(&start, rows));
   IGN_TRY(f.take(&label, rows));
-  IGN_TRY(f.take(&ebegin, rows));
-  IGN_TRY(f.take(&size, rows));
-  IGN_TRY(f.take(&off, rows));
   const int items = (int)count;
   const int label_bits = std::max(1, bit_width(max_label));
   const int edge_bits = 32 + bit_width(count);
@@ -338,8 +267,6 @@ int ign_skeleton_export_dev(ign_ctx* ctx, const uint32_t* labels, uint64_t sx, u
   IGN_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, t, ekey, ekey_s, items, 0, edge_bits, ctx->stream));
   tb = std::max(tb, t);
   IGN_CUDA(cub::DeviceScan::InclusiveSum(nullptr, t, head, run, items, ctx->stream));
-  tb = std::max(tb, t);
-  IGN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, t, size, off, (int)rows, ctx->stream));
   tb = std::max(tb, t);
   void* tmp;
   IGN_TRY(f.take(&tmp, tb));
@@ -367,18 +294,11 @@ int ign_skeleton_export_dev(ign_ctx* ctx, const uint32_t* labels, uint64_t sx, u
   IGN_TRY(sx_fail_host(h));
   const uint64_t runs = runs32;
   IGN_CUDA(cub::DeviceRadixSort::SortKeys(tmp, tb, ekey, ekey_s, items, 0, edge_bits, ctx->stream));
-  const unsigned rgrid = blocks_for(runs, 256);
-  IGN_LAUNCH(ctx, k_sx_sizes, rgrid, 256, 0, start, runs, count, ekey_s, ctl, vertex_types, ebegin, size);
-  IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, size, off, (int)runs, ctx->stream));
-  IGN_LAUNCH(ctx, k_sx_table, rgrid, 256, 0, start, label, ebegin, off, runs, count, vertex_types, table_out,
-             blobs_out, ctl);
   const float a0 = anisotropy[0], a1 = anisotropy[1], a2 = anisotropy[2];
   const double o0 = offset[0], o1 = offset[1], o2 = offset[2];
-  IGN_LAUNCH(ctx, k_sx_verts, grid, 256, 0, skel, radius, val_s, run, start, table_out, count, sx, sy, a0, a1, a2,
-             o0, o1, o2, vertex_types, blobs_out);
-  if (h.ne)
-    IGN_LAUNCH(ctx, k_sx_write_edges, blocks_for(h.ne, 256), 256, 0, ekey_s, ctl, run, start, ebegin, table_out,
-               blobs_out);
+  const SxSource src{start, label, run, val_s, skel, radius, runs, count, sx, sy, a0, a1, a2, o0, o1, o2};
+  IGN_TRY(skelblob_encode(ctx, f, src, runs, count, ekey_s, h.ne, &ctl->ne, vertex_types, table_out, blobs_out,
+                          &ctl->bytes));
   IGN_LAUNCH(ctx, k_sx_boxes, blocks_for(runs * 32, 256), 256, 0, skel, val_s, start, runs, count, sx, sy, a0, a1, a2,
              o0, o1, o2, boxes_out);
   IGN_TRY(small_d2h(ctx, &h, ctl, sizeof(SxCtl)));

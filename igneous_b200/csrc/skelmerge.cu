@@ -17,14 +17,16 @@
 // Per label, one CTA (k_mg_post): cable length against max_cable_length, dust, loops (thread 0: cycles are
 // rare), connect pieces (Borůvka rounds, every thread searching candidates), ticks (block-wide argmin per
 // removal).  Edges live in a per-label slice of 2 * ne + nv + 1 entries of global vertex indices.
-// Final consolidate and encode: the vertices left with an edge, the live edges sorted as 64-bit keys, blob
-// sizes, an exclusive scan, and one write pass for vertices, radii, types and edges.
+// Final consolidate and encode: the vertices left with an edge numbered by a scan (fnew) and listed in that
+// order (k_mg_src), the live edges sorted as 64-bit keys of the new numbers, then skelblob_encode
+// (skelblob.cuh) with a row per label.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 
 #include "common.cuh"
+#include "skelblob.cuh"
 
 namespace ign {
 
@@ -708,92 +710,30 @@ __global__ void __launch_bounds__(256) k_mg_fkeys(const MgEdge* __restrict__ pe,
   if ((threadIdx.x & 31) == 0 && m) atomicAdd(&ctl->ne, (unsigned long long)__popc(m));
 }
 
-__device__ __forceinline__ uint64_t mg_blob_bytes(uint64_t nv, uint64_t ne, int vt) {
-  return 8 + 16 * nv + 8 * ne + (vt ? nv : 0);
-}
-
-__device__ __forceinline__ uint64_t mg_lower64(const uint64_t* __restrict__ a, uint64_t n, uint64_t x) {
-  uint64_t lo = 0, hi = n;
-  while (lo < hi) {
-    const uint64_t mid = (lo + hi) >> 1;
-    if (a[mid] < x) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
-
-// per label: final vertex range [fv[l], fv[l + 1]), edge range [fe[l], fe[l + 1]), padded blob size
-__global__ void __launch_bounds__(256) k_mg_sizes(const uint32_t* __restrict__ vs, const uint32_t* __restrict__ fnew,
-                                                  uint64_t L, const uint64_t* __restrict__ key, const MgCtl* ctl,
-                                                  int vt, uint32_t* __restrict__ fv, uint32_t* __restrict__ fe,
-                                                  uint64_t* __restrict__ size) {
-  const uint64_t l = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (l > L) return;
-  const uint32_t v = fnew[vs[l]];
-  fv[l] = v;
-  fe[l] = (uint32_t)mg_lower64(key, ctl->ne, (uint64_t)v << 32);
-  if (l < L) {
-    const uint32_t v1 = fnew[vs[l + 1]];
-    const uint64_t e1 = mg_lower64(key, ctl->ne, (uint64_t)v1 << 32);
-    size[l] = (mg_blob_bytes(v1 - v, e1 - fe[l], vt) + 7) & ~7ull;
-  }
-}
-
-__global__ void __launch_bounds__(256) k_mg_table(const uint32_t* __restrict__ fv, const uint32_t* __restrict__ fe,
-                                                  const uint64_t* __restrict__ off, uint64_t L, int vt,
-                                                  uint64_t* __restrict__ table, uint8_t* __restrict__ blobs,
-                                                  MgCtl* ctl) {
-  const uint64_t l = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (l >= L) return;
-  const uint64_t nv = fv[l + 1] - fv[l], ne = fe[l + 1] - fe[l];
-  table[4 * l + 0] = l;
-  table[4 * l + 1] = off[l];
-  table[4 * l + 2] = nv;
-  table[4 * l + 3] = ne;
-  uint32_t* h = (uint32_t*)(blobs + off[l]);
-  h[0] = (uint32_t)nv;
-  h[1] = (uint32_t)ne;
-  const uint64_t end = off[l] + mg_blob_bytes(nv, ne, vt);
-  for (uint64_t b = end; b & 7; ++b) blobs[b] = 0;
-  if (l + 1 == L) ctl->bytes = end;
-}
-
-__global__ void __launch_bounds__(256) k_mg_write_v(const uint32_t* __restrict__ keep, const uint32_t* __restrict__ fnew,
-                                                    uint32_t nv, const uint32_t* __restrict__ clab,
-                                                    const float* __restrict__ cv, const float* __restrict__ cr,
-                                                    const uint8_t* __restrict__ ct, const uint32_t* __restrict__ fv,
-                                                    const uint32_t* __restrict__ fe, const uint64_t* __restrict__ off,
-                                                    int vt, uint8_t* __restrict__ blobs) {
+// the final vertices in order: src[fnew[i]] = i
+__global__ void __launch_bounds__(256) k_mg_src(const uint32_t* __restrict__ keep, const uint32_t* __restrict__ fnew,
+                                                uint32_t nv, uint32_t* __restrict__ src) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= nv || !keep[i]) return;
-  const uint32_t l = clab[i], j = fnew[i] - fv[l];
-  const uint64_t o = off[l], n = fv[l + 1] - fv[l], ne = fe[l + 1] - fe[l];
-  float* vert = (float*)(blobs + o + 8) + 3 * j;
-  vert[0] = cv[3 * i];
-  vert[1] = cv[3 * i + 1];
-  vert[2] = cv[3 * i + 2];
-  ((float*)(blobs + o + 8 + 12 * n + 8 * ne))[j] = cr[i];
-  if (vt) blobs[o + 8 + 16 * n + 8 * ne + j] = ct[i];
+  if (i < nv && keep[i]) src[fnew[i]] = i;
 }
 
-__global__ void __launch_bounds__(256) k_mg_write_e(const uint64_t* __restrict__ key, const MgCtl* ctl,
-                                                    const uint32_t* __restrict__ flab, const uint32_t* __restrict__ fv,
-                                                    const uint32_t* __restrict__ fe, const uint64_t* __restrict__ off,
-                                                    uint8_t* __restrict__ blobs) {
-  const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= ctl->ne) return;
-  const uint32_t lo = (uint32_t)(key[e] >> 32), hi = (uint32_t)key[e], l = flab[lo];
-  const uint64_t n = fv[l + 1] - fv[l];
-  uint32_t* edge = (uint32_t*)(blobs + off[l] + 8 + 12 * n) + 2 * (e - fe[l]);
-  edge[0] = lo - fv[l];
-  edge[1] = hi - fv[l];
-}
-
-__global__ void __launch_bounds__(256) k_mg_flab(const uint32_t* __restrict__ keep, const uint32_t* __restrict__ fnew,
-                                                 const uint32_t* __restrict__ clab, uint32_t nv,
-                                                 uint32_t* __restrict__ flab) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < nv && keep[i]) flab[fnew[i]] = clab[i];
-}
+// the rows of skelblob_encode: one per label; final vertex j is compacted vertex src[j]
+struct MgSource {
+  const uint32_t *vs, *fnew, *src, *clab;
+  const float *cv, *cr;
+  const uint8_t* ct;
+  __device__ uint64_t vstart(uint64_t l) const { return fnew[vs[l]]; }
+  __device__ uint64_t label(uint64_t l) const { return l; }
+  __device__ uint32_t row(uint64_t j) const { return clab[src[j]]; }
+  __device__ void vertex(uint64_t j, float c[3], float& r, uint8_t& t) const {
+    const uint32_t i = src[j];
+    c[0] = cv[3 * i];
+    c[1] = cv[3 * i + 1];
+    c[2] = cv[3 * i + 2];
+    r = cr[i];
+    t = ct[i];
+  }
+};
 
 uint64_t merge_bound(uint64_t L, uint64_t V, uint64_t E) { return 16 * L + 25 * V + 8 * E; }
 
@@ -893,10 +833,10 @@ int ign_skeleton_merge_dev(ign_ctx* ctx, uint64_t n_labels, const uint64_t* labe
   const uint64_t P_cap = 2 * E + V + L;
   float *cv, *cr;
   uint8_t *ct, *alive;
-  uint32_t *clab, *vs, *es, *deg, *uf, *aux, *aux2, *off, *adj, *eid, *tend, *keep, *fnew, *flab, *fv, *fe;
+  uint32_t *clab, *vs, *es, *deg, *uf, *aux, *aux2, *off, *adj, *eid, *tend, *keep, *fnew, *src;
   MgEdge *ce, *pe;
   double* dv;
-  uint64_t *fkey, *fkey_s, *size, *boff;
+  uint64_t *fkey, *fkey_s;
   IGN_TRY(f.take(&cv, 3 * Vs));
   IGN_TRY(f.take(&cr, Vs));
   IGN_TRY(f.take(&ct, Vs));
@@ -917,13 +857,9 @@ int ign_skeleton_merge_dev(ign_ctx* ctx, uint64_t n_labels, const uint64_t* labe
   IGN_TRY(f.take(&tend, Vs));
   IGN_TRY(f.take(&keep, Vs + 1));
   IGN_TRY(f.take(&fnew, Vs + 1));
-  IGN_TRY(f.take(&flab, Vs));
-  IGN_TRY(f.take(&fv, L + 1));
-  IGN_TRY(f.take(&fe, L + 1));
+  IGN_TRY(f.take(&src, Vs));
   IGN_TRY(f.take(&fkey, P_cap));
   IGN_TRY(f.take(&fkey_s, P_cap));
-  IGN_TRY(f.take(&size, L));
-  IGN_TRY(f.take(&boff, L));
   size_t tb = 0, t;
   const int vitems = (int)Vs, eitems = (int)Es;
   IGN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t, tk, tk2, perm, perm2, vitems, 0, 32, ctx->stream));
@@ -937,8 +873,6 @@ int ign_skeleton_merge_dev(ign_ctx* ctx, uint64_t n_labels, const uint64_t* labe
   IGN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, t, used, vnew, vitems + 1, ctx->stream));
   tb = std::max(tb, t);
   IGN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, t, ehead, enew, eitems + 1, ctx->stream));
-  tb = std::max(tb, t);
-  IGN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, t, size, boff, (int)L, ctx->stream));
   tb = std::max(tb, t);
   void* tmp;
   IGN_TRY(f.take(&tmp, tb));
@@ -993,16 +927,10 @@ int ign_skeleton_merge_dev(ign_ctx* ctx, uint64_t n_labels, const uint64_t* labe
   IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, keep, fnew, (int)nv1 + 1, ctx->stream));
   IGN_LAUNCH(ctx, k_mg_fkeys, blocks_for(slots, 256), 256, 0, pe, alive, slots, fnew, fkey, ctl);
   IGN_CUDA(cub::DeviceRadixSort::SortKeys(tmp, tb, fkey, fkey_s, (int)slots, 0, 64, ctx->stream));
-  if (nv1) IGN_LAUNCH(ctx, k_mg_flab, blocks_for(nv1, 256), 256, 0, keep, fnew, clab, nv1, flab);
-  IGN_LAUNCH(ctx, k_mg_sizes, blocks_for(L + 1, 256), 256, 0, vs, fnew, L, fkey_s, ctl, vertex_types, fv, fe, size);
-  IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, size, boff, (int)L, ctx->stream));
-  IGN_LAUNCH(ctx, k_mg_table, blocks_for(L, 256), 256, 0, fv, fe, boff, L, vertex_types, table_out, blobs_out,
-             ctl);
-  if (nv1)
-    IGN_LAUNCH(ctx, k_mg_write_v, blocks_for(nv1, 256), 256, 0, keep, fnew, nv1, clab, cv, cr, ct, fv, fe, boff,
-               vertex_types, blobs_out);
-  IGN_LAUNCH(ctx, k_mg_write_e, blocks_for(std::max<uint64_t>(slots, 1), 256), 256, 0, fkey_s, ctl, flab, fv, fe,
-             boff, blobs_out);
+  if (nv1) IGN_LAUNCH(ctx, k_mg_src, blocks_for(nv1, 256), 256, 0, keep, fnew, nv1, src);
+  const MgSource source{vs, fnew, src, clab, cv, cr, ct};
+  IGN_TRY(skelblob_encode(ctx, f, source, L, nv1, fkey_s, slots, &ctl->ne, vertex_types, table_out, blobs_out,
+                          &ctl->bytes));
   IGN_TRY(small_d2h(ctx, &h, ctl, sizeof(MgCtl)));
   IGN_TRY(small_sync(ctx));
   *nbytes = h.bytes;

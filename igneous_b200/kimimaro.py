@@ -60,6 +60,51 @@ class Skeleton:
     return "Skeleton(id=%r, vertices=%d, edges=%d)" % (self.id, self.vertices.shape[0], self.edges.shape[0])
 
 
+# the vertex attributes of the blobs the device writes: radius, then vertex_types when asked
+ATTRIBUTES = [{"id": "radius", "data_type": "float32", "num_components": 1},
+              {"id": "vertex_types", "data_type": "uint8", "num_components": 1}]
+
+
+def split_blobs(buf, rows, ids, attributes):
+  """([Skeleton], [blob]), one of each per row, of the neuroglancer precomputed skeletons in buf (a uint8
+  array).  rows: (byte offset, nv, ne) of each blob; ids: each Skeleton's id; attributes: the info's
+  vertex_attributes ({id, data_type, num_components}) in the order they follow the edges.  A blob is
+  uint32 nv, ne, float32 vertices[nv][3], uint32 edges[ne][2], then each attribute's values for every vertex
+  (DESIGN.md §5g).  A Skeleton's radii and vertex_types are the attributes of those ids, zeros when absent.
+  Every array is a view into buf; the zeros are views into one array per missing attribute.  ValueError when
+  a blob runs past the end of buf."""
+  rows = np.asarray(rows, np.int64).reshape(-1, 3)
+  off, nv, ne = rows[:, 0], rows[:, 1], rows[:, 2]
+
+  def cut(dt, start, count):  # per row, count values of dt from byte start
+    s = np.dtype(dt).itemsize
+    if (start % s).any():  # after an attribute of a smaller type
+      return [buf[a:a + s * n].view(dt) for a, n in zip(start.tolist(), count.tolist())]
+    typed = buf[:buf.size // s * s].view(dt)
+    return [typed[a:a + n] for a, n in zip((start // s).tolist(), count.tolist())]
+
+  def shaped(col, c):
+    return col if c == 1 else [v.reshape(-1, c) for v in col]
+
+  attrs = [(a["id"], np.dtype(a["data_type"]), int(a.get("num_components", 1))) for a in attributes]
+  starts = [off + 8, off + 8 + 12 * nv, off + 8 + 12 * nv + 8 * ne]  # vertices, edges, each attribute
+  for _, dt, c in attrs:
+    starts.append(starts[-1] + c * dt.itemsize * nv)
+  end = starts.pop()
+  if (end > buf.size).any():
+    g = int(np.argmax(end > buf.size))
+    raise ValueError("skeleton %r: its blob ends at byte %d, past the %d bytes of its buffer" % (ids[g], end[g],
+                                                                                               buf.size))
+  values = {k: shaped(cut(dt, at, c * nv), c) for (k, dt, c), at in zip(attrs, starts[2:])}
+  for k, dt in (("radius", np.float32), ("vertex_types", np.uint8)):
+    if k not in values:
+      zeros = np.zeros(int(nv.sum()), dt)
+      values[k] = [zeros[a:a + n] for a, n in zip((np.cumsum(nv) - nv).tolist(), nv.tolist())]
+  vertices, edges = shaped(cut(np.float32, starts[0], 3 * nv), 3), shaped(cut(np.uint32, starts[1], 2 * ne), 2)
+  skeletons = list(map(Skeleton, vertices, edges, values["radius"], values["vertex_types"], ids))
+  return skeletons, [buf[a:b] for a, b in zip(off.tolist(), end.tolist())]
+
+
 def _targets(points, arr, what):
   """linear F-order indices of voxels (x, y, z) of the caller's array; ValueError on background"""
   pts = np.asarray(points, dtype=np.int64).reshape(-1, 3) if len(points) else np.zeros((0, 3), np.int64)
@@ -253,25 +298,8 @@ def _views(buf, table, boxes, orig, dtype, vertex_types):
   values = orig[table[:, 0].astype(np.int64) - 1].astype(unsigned).view(dtype)
   order = np.argsort(values, kind="stable")
   keys = (values.astype(np.uint8) if values.dtype == np.bool_ else values)[order].tolist()
-  f32, u32 = buf.view(np.float32), buf.view(np.uint32)
-  zeros = None if vertex_types else np.zeros(int(table[:, 2].sum()), np.uint8)
-  skeletons, blobs, bx = {}, {}, {}
-  z = 0
-  for label, (off, nv, ne), box in zip(keys, table[order, 1:].tolist(), boxes[order]):
-    w = off // 4 + 2  # the vertices, in words
-    e = w + 3 * nv
-    r = e + 2 * ne
-    end = 4 * (r + nv)
-    if vertex_types:
-      vt = buf[end:end + nv]
-      end += nv
-    else:
-      vt = zeros[z:z + nv]
-      z += nv
-    skeletons[label] = Skeleton(f32[w:e].reshape(nv, 3), u32[e:r].reshape(ne, 2), f32[r:r + nv], vt, label)
-    blobs[label] = buf[off:end]
-    bx[label] = box
-  return skeletons, blobs, bx
+  skeletons, blobs = split_blobs(buf, table[order, 1:], keys, ATTRIBUTES[:2 if vertex_types else 1])
+  return dict(zip(keys, skeletons)), dict(zip(keys, blobs)), dict(zip(keys, boxes[order]))
 
 
 def crop_box(bbox, crop, resolution):
@@ -366,22 +394,6 @@ def merge_packed(packed, dust_threshold=4000, tick_threshold=6000, max_cable_len
   return buf, table
 
 
-def _split(buf, table, segids, vertex_types):
-  """{segid: (Skeleton, blob)}: every array a view into buf"""
-  f32, u32 = buf.view(np.float32), buf.view(np.uint32)
-  out = {}
-  for segid, (off, nv, ne) in zip(segids, table[:, 1:].tolist()):
-    w = off // 4 + 2
-    e, r = w + 3 * nv, w + 3 * nv + 2 * ne
-    end = 4 * (r + nv)
-    vt = buf[end:end + nv] if vertex_types else np.zeros(nv, np.uint8)
-    if vertex_types:
-      end += nv
-    out[segid] = (Skeleton(f32[w:e].reshape(nv, 3), u32[e:r].reshape(ne, 2), f32[r:r + nv], vt, segid),
-                  buf[off:end])
-  return out
-
-
 def merge_fragments(fragments, crop=0, resolution=(1, 1, 1), dust_threshold=4000, tick_threshold=6000,
                     max_cable_length=None, vertex_types=True, ctx=None):
   """UnshardedSkeletonMergeTask's fuse and postprocess for many labels in one device call (DESIGN.md §5h).
@@ -391,7 +403,8 @@ def merge_fragments(fragments, crop=0, resolution=(1, 1, 1), dust_threshold=4000
   is a view into one host buffer."""
   segids, packed = pack_fragments(fragments, crop, resolution)
   buf, table = merge_packed(packed, dust_threshold, tick_threshold, max_cable_length, vertex_types, ctx)
-  return _split(buf, table, segids, vertex_types)
+  skeletons, blobs = split_blobs(buf, table[:, 1:], segids, ATTRIBUTES[:2 if vertex_types else 1])
+  return dict(zip(segids, zip(skeletons, blobs)))
 
 
 def postprocess(skeleton, dust_threshold=1500, tick_threshold=3000, ctx=None):

@@ -342,28 +342,17 @@ class _SkeletonSource:
     """The skeleton {dir}/{segid} decoded per meta.info['vertex_attributes'] (a list of ids -> a list)."""
     if isinstance(segid, (list, tuple)):
       return [self.get(s) for s in segid]
-    from .kimimaro import Skeleton
+    from .kimimaro import split_blobs
     data = self._cv.cf.get("%s/%d" % (self.meta.subdir, int(segid)))
     if data is None:
       raise FileNotFoundError("no skeleton %d in %s" % (int(segid), self.path))
-    buf = np.frombuffer(data, dtype=np.uint8)
+    buf = np.frombuffer(bytearray(data), dtype=np.uint8)  # writable: the Skeleton's arrays are views into it
     nv, ne = (int(v) for v in buf[:8].view(np.uint32))
-    at = 8
-    vertices = buf[at:at + 12 * nv].view(np.float32).reshape(nv, 3).copy()
-    at += 12 * nv
-    edges = buf[at:at + 8 * ne].view(np.uint32).reshape(ne, 2).copy()
-    at += 8 * ne
-    attrs = {}
-    for attr in self.meta.info.get("vertex_attributes") or []:
-      dt, k = np.dtype(attr["data_type"]), int(attr.get("num_components", 1))
-      size = nv * k * dt.itemsize
-      a = buf[at:at + size].view(dt).copy()
-      attrs[attr["id"]] = a if k == 1 else a.reshape(nv, k)
-      at += size
-    if at != buf.size:
-      raise ValueError("skeleton %d: %d bytes, the info's attributes describe %d" % (int(segid), buf.size, at))
-    radii = attrs.get("radius", np.zeros(nv, np.float32))
-    return Skeleton(vertices, edges, radii, attrs.get("vertex_types", np.zeros(nv, np.uint8)), int(segid))
+    skeletons, blobs = split_blobs(buf, [(0, nv, ne)], [int(segid)], self.meta.info.get("vertex_attributes") or [])
+    if blobs[0].size != buf.size:
+      raise ValueError("skeleton %d: %d bytes, the info's attributes describe %d" % (int(segid), buf.size,
+                                                                                      blobs[0].size))
+    return skeletons[0]
 
 
 class _Meta:
