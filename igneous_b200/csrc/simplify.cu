@@ -861,7 +861,8 @@ __device__ __forceinline__ void sl_group_pass(const SlArgs& A, const SlLab<SM>& 
     // distinct neighbours of u (first occurrences f1 among x1, f2 among x2 not in x1), same for v
     const uint32_t mu1 = __match_any_sync(FULL, x1) & gmask, mu2 = __match_any_sync(FULL, x2) & gmask;
     const uint32_t mv1 = __match_any_sync(FULL, y1) & gmask, mv2 = __match_any_sync(FULL, y2) & gmask;
-    bool inu = false, inv = false, c1 = false, c2 = false;
+    // coinc: the lane's face {u, x1, x2} and a face {v, x1, x2} would both become {k, x1, x2}
+    bool inu = false, inv = false, c1 = false, c2 = false, coinc = false;
     for (uint32_t j = 0; j < nmax; j++) {
       const uint32_t sx1 = __shfl_sync(FULL, x1, j, W), sy1 = __shfl_sync(FULL, y1, j, W), sy2 = __shfl_sync(FULL, y2, j, W);
       if (j < nu) inu |= (sx1 == x2);
@@ -869,6 +870,7 @@ __device__ __forceinline__ void sl_group_pass(const SlArgs& A, const SlLab<SM>& 
         inv |= (sy1 == y2);
         c1 |= (x1 == sy1) | (x1 == sy2);
         c2 |= (x2 == sy1) | (x2 == sy2);
+        coinc |= ((x1 == sy1) & (x2 == sy2)) | ((x1 == sy2) & (x2 == sy1));
       }
     }
     const bool f1 = hu && ((int)lane == __ffs(mu1) - 1);
@@ -881,7 +883,9 @@ __device__ __forceinline__ void sl_group_pass(const SlArgs& A, const SlLab<SM>& 
     const uint32_t b_sh = __ballot_sync(FULL, hu && (x1 == v || x2 == v));
     const uint32_t nnu = __popc(b_f1 & gmask) + __popc(b_f2 & gmask), nnv = __popc(b_g1 & gmask) + __popc(b_g2 & gmask);
     const uint32_t common = __popc(b_c1 & gmask) + __popc(b_c2 & gmask), shared = __popc(b_sh & gmask);
-    const bool go = ok && nnu <= (uint32_t)S_MAXV && nnv <= (uint32_t)S_MAXV && shared == 2 && common == 2;
+    // link condition for an interior edge, except on a tetrahedron (two faces on the wings would coincide)
+    const uint32_t b_co = __ballot_sync(FULL, hu && coinc) & gmask;
+    const bool go = ok && nnu <= (uint32_t)S_MAXV && nnv <= (uint32_t)S_MAXV && shared == 2 && common == 2 && !b_co;
     if (act && !go && gl == 0) {  // park the edge until one of its endpoints' rings changes
       const uint32_t hl = win[slot].h, f = hl / 3, c = hl - 3 * f;
       const uint32_t st = L.fstate[f];  // (winners of one pass never share a face: byte accesses are disjoint)

@@ -750,6 +750,19 @@ static void simp_evaluate(const simp_t* s, uint32_t u, uint32_t v, double max_er
   for (int i = 0; i < nfu; i++)
     for (int j = 0; j < nfv; j++) shared += (fu[i] == fv[j]);
   if (shared != 2 || common != 2) return; /* link condition for an interior edge */
+  /* ... except on a tetrahedron: a surviving face {u, a, b} next to a face {v, a, b} (a, b the
+     wings) would become a second face on {k, a, b}, a zero-volume pair of opposite windings */
+  for (int i = 0; i < nfu; i++) {
+    const uint32_t* fx = s->face + 3 * (uint64_t)fu[i];
+    if (fx[0] == v || fx[1] == v || fx[2] == v) continue; /* dies */
+    for (int j = 0; j < nfv; j++) {
+      const uint32_t* fy = s->face + 3 * (uint64_t)fv[j];
+      int same = 0; /* both of a, b in fy: fy is {v, a, b} */
+      for (int k = 0; k < 3; k++)
+        if (fx[k] != u) same += (fy[0] == fx[k]) | (fy[1] == fx[k]) | (fy[2] == fx[k]);
+      if (same == 2) return;
+    }
+  }
   for (int pass = 0; pass < 2; pass++) {
     const uint32_t* fl = pass ? fv : fu;
     const int n = pass ? nfv : nfu;
@@ -829,11 +842,12 @@ uint32_t orc_simp_unmix16(uint32_t x) { return simp_unmix16(x); }
  * target[K+1]: stop when a label's alive faces <= target.  tri_off[K+1]: first face of
  * each label (priorities use label-local half-edge ids so that the result does not depend
  * on the order labels are stored in).  valive/falive are outputs.
- * Returns the number of rounds executed in *rounds.
+ * Returns the number of rounds executed in *rounds.  rep[U] (optional, NULL to skip): the surviving
+ * vertex each input vertex was collapsed into (itself when it survives).
  */
 int orc_simplify(uint64_t U, uint64_t T, double* pos, uint32_t* face, const uint32_t* flabel,
                  uint32_t K, const uint32_t* target, const uint32_t* tri_off, double max_err2, int max_rounds,
-                 uint8_t* valive, uint8_t* falive, int* rounds) {
+                 uint8_t* valive, uint8_t* falive, int* rounds, uint32_t* rep) {
   simp_t s;
   s.U = U; s.T = T; s.pos = pos; s.face = face; s.flabel = flabel; s.falive = falive; s.valive = valive;
   s.Q = (double*)calloc(10 * (U ? U : 1), sizeof(double));
@@ -851,6 +865,7 @@ int orc_simplify(uint64_t U, uint64_t T, double* pos, uint32_t* face, const uint
   if (!s.Q || !s.vbound || !s.next || !s.head || !s.tail || !s.key1 || !s.key2 || !alive_faces || !label_active)
     return ORC_ENOMEM;
   for (uint64_t v = 0; v < U; v++) { s.head[v] = s.tail[v] = SIMP_NONE; valive[v] = 1; }
+  if (rep) for (uint64_t v = 0; v < U; v++) rep[v] = (uint32_t)v;
   /* incident lists in ascending node order */
   for (uint64_t h = 0; h < 3 * T; h++) {
     const uint32_t v = face[h];
@@ -961,6 +976,7 @@ int orc_simplify(uint64_t U, uint64_t T, double* pos, uint32_t* face, const uint
       s.next[s.tail[k]] = s.head[rm];
       s.tail[k] = s.tail[rm];
       valive[rm] = 0;
+      if (rep) rep[rm] = k;
       ncol[lab]++;
       vdirty[k] = 1;
       for (uint32_t hh = s.head[k]; hh != SIMP_NONE; hh = s.next[hh]) {
@@ -979,6 +995,7 @@ int orc_simplify(uint64_t U, uint64_t T, double* pos, uint32_t* face, const uint
   }
   free(stopped); free(slow); free(nsel); free(ncol);
   *rounds = r;
+  if (rep) for (uint64_t v = 0; v < U; v++) while (!valive[rep[v]]) rep[v] = rep[rep[v]];
   free(s.Q); free(s.vbound); free(s.next); free(s.head); free(s.tail); free(s.key1); free(s.key2);
   free(alive_faces); free(label_active); free(estate); free(vdirty); free(fmt16);
   return ORC_OK;

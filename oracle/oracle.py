@@ -355,11 +355,12 @@ class WeldedMeshes:
 
 
 def simplify_welded(W, resolution=(1, 1, 1), reduction_factor=100, max_error=40.0,
-                    voxel_centered=True, max_rounds=400):
+                    voxel_centered=True, max_rounds=400, with_rep=False):
   """Mesher.get(id, reduction_factor, max_error, voxel_centered) for every label of a
   WeldedMeshes (igneous/tasks/mesh/mesh.py:376-381): round-based quadric edge
   collapse (see orc_simplify; parity with zmesh unpinned).  Returns
-  ({label: (vertices f32, faces u32)}, rounds)."""
+  ({label: (vertices f32, faces u32)}, rounds), and with with_rep=True also
+  {label: rep}, rep[i] the output vertex that input vertex i of W.get(label) ended in."""
   U, T = len(W.ulabel), len(W.faces)
   res = np.asarray(resolution, dtype=np.float64)
   pos = np.ascontiguousarray(W.uxyz.astype(np.float64) * 0.5 * res)
@@ -372,13 +373,15 @@ def simplify_welded(W, resolution=(1, 1, 1), reduction_factor=100, max_error=40.
   valive = np.zeros(max(U, 1), dtype=np.uint8)
   falive = np.zeros(max(T, 1), dtype=np.uint8)
   rounds = ctypes.c_int(0)
+  rep = np.zeros(max(U, 1), dtype=np.uint32) if with_rep else None
   tri_off = np.zeros(K + 1, dtype=np.uint32)
   tri_off[1:] = W.f0.astype(np.uint32)
   rc = lib().orc_simplify(ctypes.c_uint64(U), ctypes.c_uint64(T), _ptr(pos), _ptr(faces), _ptr(dense),
                           ctypes.c_uint32(K), _ptr(target), _ptr(tri_off), ctypes.c_double(float(max_error) ** 2),
-                          ctypes.c_int(max_rounds), _ptr(valive), _ptr(falive), ctypes.byref(rounds))
+                          ctypes.c_int(max_rounds), _ptr(valive), _ptr(falive), ctypes.byref(rounds),
+                          _ptr(rep) if with_rep else None)
   assert rc == 0
-  out = {}
+  out, reps = {}, {}
   shift = (np.float32(0.5) * np.asarray(resolution, dtype=np.float32)) if voxel_centered else np.zeros(3, np.float32)
   newid = np.cumsum(valive[:U].astype(np.int64)) - 1
   for j, lab in enumerate(W.labels):
@@ -390,7 +393,9 @@ def simplify_welded(W, resolution=(1, 1, 1), reduction_factor=100, max_error=40.
     f = faces[f0:f1][fa].astype(np.int64)
     f = (newid[f] - base).astype(np.uint32)
     out[int(lab)] = (verts.astype(np.float32), f)
-  return out, int(rounds.value)
+    if with_rep:
+      reps[int(lab)] = (newid[rep[v0:v1].astype(np.int64)] - base).astype(np.uint32)
+  return (out, int(rounds.value), reps) if with_rep else (out, int(rounds.value))
 
 
 def pack_vertex(v):
