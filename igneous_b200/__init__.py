@@ -12,7 +12,7 @@ __version__ = "0.1.0"
 # The import surface of igneous/__init__.py:1-4 (`from igneous import DownsampleTask, MeshTask,
 # Mesher, LocalTaskQueue, CloudVolume ...`, used by test/test_tasks.py:18-23), resolved lazily so
 # that importing the package stays free of side effects (no native library, no storage layer).
-_TASK_NAMES = ("DownsampleTask", "TransferTask", "ImageShardDownsampleTask", "CCLFacesTask", "CCLEquivalancesTask", "RelabelCCLTask",
+_TASK_NAMES = ("DownsampleTask", "TransferTask", "ImageShardTransferTask", "ImageShardDownsampleTask", "CCLFacesTask", "CCLEquivalancesTask", "RelabelCCLTask",
                "create_relabeling", "clean_intermediate_files", "MeshTask", "downsample_and_upload",
                "downsample_method_to_fn", "threshold_image", "blackout_non_face_rails", "DisjointSet",
                "QuantizeTask", "CLAHETask", "ContrastNormalizationTask", "LuminanceLevelsTask",

@@ -21,7 +21,8 @@ import numpy as np
 
 from . import _shim
 
-__all__ = ["cseg_encode", "cseg_decode", "jpeg_encode", "jpeg_decode", "jpeg_encode_batch", "jpeg_decode_batch"]
+__all__ = ["cseg_encode", "cseg_decode", "jpeg_encode", "jpeg_decode", "jpeg_encode_batch", "jpeg_decode_batch",
+           "cseg_encode_batch_dev", "cseg_decode_batch_dev", "jpeg_encode_batch_dev", "jpeg_decode_batch_dev"]
 
 
 def _chunk(labels):
@@ -170,3 +171,98 @@ def jpeg_decode_batch(datas, shapes, ctx=None):
 def jpeg_decode(data, shape, ctx=None):
   """jpeg file bytes -> uint8 chunk of `shape` ([x,y,z] or [x,y,z,1], Fortran order)."""
   return jpeg_decode_batch([data], [shape], ctx)[0]
+
+
+# ------------------------------------------------------------------ device batches
+# The storage layer's read and write paths: chunks packed back to back in device memory (chunk i an
+# F-order [sx, sy, sz, sc] array, shapes an n x 3 uint32 host array), one call per batch.
+
+def cseg_capacity_words(shapes, sc, dtype, block_size):
+  """words that the compressed_segmentation files of these chunks can need at most: per channel the
+  offset word, two header words per block and (label words + one index word) per block voxel"""
+  bx, by, bz = (int(v) for v in block_size)
+  per = np.dtype(dtype).itemsize // 4 + 1
+  total = 0
+  for sx, sy, sz in np.asarray(shapes, dtype=np.int64).reshape(-1, 3):
+    g = (-(-int(sx) // bx)) * (-(-int(sy) // by)) * (-(-int(sz) // bz))
+    total += int(sc) * (1 + 2 * g + per * g * bx * by * bz)
+  return total
+
+
+def cseg_encode_batch_dev(chunks, dtype, shapes, sc, block_size=(8, 8, 8), ctx=None):
+  """device chunks -> list of compressed_segmentation files (bytes): one batched encode, one D2H"""
+  ctx = ctx or _shim.default_context()
+  dtype = np.dtype(dtype)
+  shapes = np.ascontiguousarray(np.asarray(shapes, dtype=np.uint32).reshape(-1, 3))
+  n = shapes.shape[0]
+  if n == 0:
+    return []
+  cap = cseg_capacity_words(shapes, sc, dtype, block_size)
+  out = ctx.alloc(cap * 4)
+  d_off = ctx.alloc((n + 1) * 8)
+  nw = c.c_uint64(0)
+  bx, by, bz = (int(v) for v in block_size)
+  _shim.check(ctx.lib.ign_cseg_encode_batch_dev(ctx.handle, _shim.ptr(chunks), _shim.dtype_code(dtype), n,
+                                                _shim.ptr(shapes), int(sc), bx, by, bz, _shim.ptr(out), cap,
+                                                _shim.ptr(d_off), c.byref(nw)))
+  words = np.empty(max(int(nw.value), 1), dtype=np.uint32)
+  offs = np.empty(n + 1, dtype=np.uint64)
+  ctx.d2h(words, out, int(nw.value) * 4)
+  ctx.d2h(offs, d_off)
+  ctx.sync()
+  return [words[int(offs[i]):int(offs[i + 1])].tobytes() for i in range(n)]
+
+
+def cseg_decode_batch_dev(streams, byte_offsets, dtype, shapes, sc, block_size, out, ctx=None):
+  """compressed_segmentation files packed in device memory (stream i at byte_offsets[i] ..
+  byte_offsets[i+1], host) -> the packed chunks in `out` (device)"""
+  ctx = ctx or _shim.default_context()
+  byte_offsets = np.asarray(byte_offsets, dtype=np.int64)
+  if np.any(byte_offsets % 4):
+    bad = int(np.nonzero(byte_offsets % 4)[0][0])
+    raise ValueError("compressed_segmentation stream %d does not start or end on a 4-byte word" % max(bad - 1, 0))
+  shapes = np.ascontiguousarray(np.asarray(shapes, dtype=np.uint32).reshape(-1, 3))
+  woff = np.ascontiguousarray(byte_offsets // 4, dtype=np.uint64)
+  bx, by, bz = (int(v) for v in block_size)
+  _shim.check(ctx.lib.ign_cseg_decode_batch_dev(ctx.handle, _shim.ptr(streams), _shim.ptr(woff), shapes.shape[0],
+                                                _shim.dtype_code(dtype), _shim.ptr(shapes), int(sc), bx, by, bz,
+                                                _shim.ptr(out)))
+
+
+def jpeg_encode_batch_dev(chunks, shapes, quality=85, ctx=None):
+  """uint8 device chunks (one channel) -> list of jpeg files: one batched encode, one D2H"""
+  ctx = ctx or _shim.default_context()
+  quality = int(quality)
+  if not 1 <= quality <= 100:
+    raise ValueError("jpeg quality must be in 1..100, got %d" % quality)
+  shapes = np.ascontiguousarray(np.array([_jpeg_shape(s) for s in np.asarray(shapes).reshape(-1, 3)],
+                                         dtype=np.uint32).reshape(-1, 3))
+  n = shapes.shape[0]
+  if n == 0:
+    return []
+  px = int(shapes.astype(np.int64).prod(axis=1).sum())
+  offsets = np.zeros(n + 1, dtype=np.uint64)
+  need = c.c_uint64(0)
+  args = [ctx.handle, _shim.ptr(chunks), n, _shim.ptr(shapes), quality, _restart(None)]
+  cap = max(4096, px // 2 + 1024 * n)  # as jpeg_encode_batch: a first guess, the call reports the size
+  out = ctx.alloc(cap)
+  _shim.check(ctx.lib.ign_jpeg_encode_dev(*args, _shim.ptr(out), cap, _shim.ptr(offsets), c.byref(need)))
+  if need.value > cap:
+    cap = int(need.value)
+    out = ctx.alloc(cap)
+    _shim.check(ctx.lib.ign_jpeg_encode_dev(*args, _shim.ptr(out), cap, _shim.ptr(offsets), c.byref(need)))
+  host = np.empty(max(int(need.value), 1), dtype=np.uint8)
+  ctx.d2h(host, out, int(need.value))
+  ctx.sync()
+  return [host[int(offsets[i]):int(offsets[i + 1])].tobytes() for i in range(n)]
+
+
+def jpeg_decode_batch_dev(streams, byte_offsets, shapes, out, ctx=None):
+  """jpeg files packed in device memory (stream i at byte_offsets[i] .. byte_offsets[i+1], host) ->
+  the packed uint8 chunks in `out` (device)"""
+  ctx = ctx or _shim.default_context()
+  shapes = np.ascontiguousarray(np.array([_jpeg_shape(s) for s in np.asarray(shapes).reshape(-1, 3)],
+                                         dtype=np.uint32).reshape(-1, 3))
+  offs = np.ascontiguousarray(np.asarray(byte_offsets, dtype=np.uint64))
+  _shim.check(ctx.lib.ign_jpeg_decode_dev(ctx.handle, _shim.ptr(streams), _shim.ptr(offs), shapes.shape[0],
+                                          _shim.ptr(shapes), _shim.ptr(out)))

@@ -25,6 +25,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
+#include <algorithm>
 #include <vector>
 
 #include "common.cuh"
@@ -271,31 +272,41 @@ __global__ void __launch_bounds__(256)
   tab_off[b] = 2 * nblock + scan[o] + (obits * bvox + 31) / 32;
 }
 
+// value of voxel (x, y, z) in block b of one channel stream of nwords words; false: malformed stream
+template <typename T>
+__device__ __forceinline__ bool cs_decode_voxel(const uint32_t* __restrict__ in, uint64_t nwords, const CsegDims& d,
+                                                uint32_t x, uint32_t y, uint32_t z, uint64_t b, uint64_t* out) {
+  constexpr int WORDS = sizeof(T) / 4;
+  if (2 * b + 1 >= nwords) return false;
+  const uint32_t h0 = in[2 * b], h1 = in[2 * b + 1];
+  const uint32_t bits = h0 >> 24;
+  const uint64_t toff = h0 & 0xFFFFFFu, voff = h1;
+  if (!(bits == 0 || bits == 1 || bits == 2 || bits == 4 || bits == 8 || bits == 16 || bits == 32)) return false;
+  uint64_t idx = 0;
+  if (bits) {
+    const uint64_t bitpos = (uint64_t)(((z % d.bz) * d.by + (y % d.by)) * d.bx + (x % d.bx)) * bits;
+    const uint64_t w = voff + bitpos / 32;
+    if (w >= nwords) return false;
+    idx = (in[w] >> (bitpos % 32)) & (bits == 32 ? 0xFFFFFFFFu : ((1u << bits) - 1u));
+  }
+  const uint64_t tw = toff + idx * WORDS;
+  if (tw + WORDS > nwords) return false;
+  uint64_t v = in[tw];
+  if (WORDS == 2) v |= (uint64_t)in[tw + 1] << 32;
+  *out = v;
+  return true;
+}
+
 template <typename T>
 __global__ void __launch_bounds__(256)
     k_cseg_decode(const uint32_t* __restrict__ in, uint64_t nwords, CsegDims d, T* __restrict__ out, uint32_t* err) {
-  constexpr int WORDS = sizeof(T) / 4;
   const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   const uint64_t n = (uint64_t)d.sx * d.sy * d.sz;
   if (i >= n) return;
   const uint32_t x = (uint32_t)(i % d.sx), y = (uint32_t)((i / d.sx) % d.sy), z = (uint32_t)(i / ((uint64_t)d.sx * d.sy));
   const uint64_t b = (x / d.bx) + (uint64_t)d.gx * ((y / d.by) + (uint64_t)d.gy * (z / d.bz));
-  if (2 * b + 1 >= nwords) { *err = 1; return; }
-  const uint32_t h0 = in[2 * b], h1 = in[2 * b + 1];
-  const uint32_t bits = h0 >> 24;
-  const uint64_t toff = h0 & 0xFFFFFFu, voff = h1;
-  if (!(bits == 0 || bits == 1 || bits == 2 || bits == 4 || bits == 8 || bits == 16 || bits == 32)) { *err = 1; return; }
-  uint64_t idx = 0;
-  if (bits) {
-    const uint64_t bitpos = (uint64_t)(((z % d.bz) * d.by + (y % d.by)) * d.bx + (x % d.bx)) * bits;
-    const uint64_t w = voff + bitpos / 32;
-    if (w >= nwords) { *err = 1; return; }
-    idx = (in[w] >> (bitpos % 32)) & (bits == 32 ? 0xFFFFFFFFu : ((1u << bits) - 1u));
-  }
-  const uint64_t tw = toff + idx * WORDS;
-  if (tw + WORDS > nwords) { *err = 1; return; }
-  uint64_t v = in[tw];
-  if (WORDS == 2) v |= (uint64_t)in[tw + 1] << 32;
+  uint64_t v;
+  if (!cs_decode_voxel<T>(in, nwords, d, x, y, z, b, &v)) { *err = 1; return; }
   out[i] = (T)v;
 }
 
@@ -421,6 +432,364 @@ static int cseg_encode_channel(ign_ctx* ctx, const T* in, const CsegDims& d, uin
 #undef CS_LAUNCH_PL
 }
 
+
+// ------------------------------------------------------------------ batches
+// N chunks x sc channels are S = N*sc segments, one channel stream each, and all their blocks one
+// global block range (segment-major, raster order inside a segment).  The passes of the one-chunk
+// encoder above run once over that range: a table's owner is still the first block OF ITS SEGMENT
+// with an identical table (the segment joins the hash, and verify / resolve compare it), so every
+// chunk's stream is the one cseg_encode_channel writes for it.  One exclusive scan over all blocks
+// places every segment: segment s = (chunk i, channel c) starts at word
+//   scan[b0_s] + 2*b0_s + sc*(i + 1)
+// of the concatenated chunk files (chunk i's sc-word channel table precedes its channels).
+struct CsegSeg {
+  CsegDims d;
+  uint64_t in_off;    // element offset of the channel in the packed chunks
+  uint64_t b0;        // first global block
+  uint64_t chunk;     // i
+  uint32_t chan;      // c
+};
+
+__device__ __forceinline__ uint64_t cb_find(const CsegSeg* __restrict__ segs, uint64_t nseg, uint64_t g) {
+  uint64_t lo = 0, hi = nseg;  // last segment whose b0 <= g
+  while (hi - lo > 1) {
+    const uint64_t mid = (lo + hi) / 2;
+    if (segs[mid].b0 <= g) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// k_cb_scan and k_cb_resolve hold their segment's dims in registers, where the one-chunk kernels read
+// them from the parameter bank; under __launch_bounds__(128) ptxas spilled a few of them (16 / 40
+// bytes).  An explicit register cap lets it keep everything in registers.  Both launch 128 threads.
+template <typename T, bool WRITE, int CS_PER_LANE>
+__global__ void __maxnreg__(128)
+    k_cb_scan(const T* __restrict__ in, const CsegSeg* __restrict__ segs, uint64_t nseg, uint64_t nblock, uint64_t sc,
+              uint32_t* __restrict__ info_n, uint32_t* __restrict__ bseg, unsigned long long* __restrict__ hash,
+              unsigned long long hash_mask, unsigned long long* __restrict__ lo, unsigned long long* __restrict__ hi,
+              const unsigned long long* __restrict__ scan, const uint32_t* __restrict__ owner, uint32_t* __restrict__ out) {
+  constexpr int WORDS = sizeof(T) / 4;
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint64_t g = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5;
+  if (g >= nblock) return;
+  const uint64_t s = cb_find(segs, nseg, g);
+  const CsegDims d = segs[s].d;
+  const uint64_t b0 = segs[s].b0, chunk = segs[s].chunk;
+  const uint64_t b = g - b0;
+  const T* src = in + segs[s].in_off;
+  uint64_t val[CS_PER_LANE];
+  uint32_t idx[CS_PER_LANE] = {};
+  const uint32_t have = cs_load<T, CS_PER_LANE>(src, d, b, lane, val);
+  uint32_t todo = have;
+  uint32_t n = 0;
+  // the segment joins the hash from the start, so that it need not stay live through the extraction
+  uint64_t h = WRITE ? 0 : mix64(0x9E3779B97F4A7C15ull ^ (s * 0xD6E8FEB86659FD93ull)), first = 0, m = 0;
+  if (!WRITE && lane == 0) bseg[g] = (uint32_t)s;
+  uint32_t* seg_out = nullptr;
+  uint32_t toff = 0, eoff = 0;
+  bool own = false;
+  const uint32_t nb = d.gx * d.gy * d.gz;
+  if (WRITE) {
+    const uint64_t base0 = scan[b0];
+    seg_out = out + base0 + 2 * b0 + sc * (chunk + 1);
+    const uint32_t o = owner[g];
+    own = o == (uint32_t)g;
+    eoff = (uint32_t)(2 * nb + scan[g] - base0);
+    toff = (uint32_t)(2 * nb + scan[o] - base0 + (cs_bits(info_n[o]) * d.bvox + 31) / 32);
+  }
+  while (__any_sync(CS_FULL, todo != 0)) {
+    m = cs_warp_min<CS_PER_LANE>(val, todo);
+#pragma unroll
+    for (int k = 0; k < CS_PER_LANE; k++)
+      if (((todo >> k) & 1u) && val[k] == m) {
+        idx[k] = n;
+        todo &= ~(1u << k);
+      }
+    if (WRITE) {
+      if (own && lane == 0) {
+        seg_out[toff + n * WORDS] = (uint32_t)m;
+        if (WORDS == 2) seg_out[toff + n * WORDS + 1] = (uint32_t)(m >> 32);
+      }
+    } else {
+      if (n == 0) first = m;
+      h = mix64(h ^ m);
+    }
+    n++;
+  }
+  const uint32_t bits = cs_bits(n);
+  if (!WRITE) {
+    if (lane == 0) {
+      info_n[g] = n;
+      hash[g] = mix64(h + n) & hash_mask;
+      lo[g] = first;
+      hi[g] = m;
+    }
+    return;
+  }
+  if (bits) {
+    const uint32_t per = 32 / bits;
+    const uint32_t nwords = (bits * d.bvox + 31) / 32;
+#pragma unroll
+    for (int k = 0; k < CS_PER_LANE; k++) {
+      const uint32_t p = lane + 32 * k;
+      if (32 * k >= d.bvox) break;
+      const uint32_t v = ((have >> k) & 1u) ? idx[k] : 0u;
+      uint32_t word = v << ((p % per) * bits);
+      for (uint32_t sh = 1; sh < per; sh <<= 1) word |= __shfl_xor_sync(CS_FULL, word, sh);
+      if (p < d.bvox && (p % per) == 0 && p / per < nwords) seg_out[eoff + p / per] = word;
+    }
+  }
+  if (lane == 0) {
+    seg_out[2 * b] = toff | (bits << 24);
+    seg_out[2 * b + 1] = eoff;
+  }
+}
+
+// owner of every block whose hash run head is in another segment or holds another table -> *collided
+template <typename T, int CS_PER_LANE>
+__global__ void __launch_bounds__(128)
+    k_cb_verify(const T* __restrict__ in, const CsegSeg* __restrict__ segs, uint32_t nblock,
+                const uint32_t* __restrict__ bseg, const uint32_t* __restrict__ n, const unsigned long long* __restrict__ lo,
+                const unsigned long long* __restrict__ hi, const uint32_t* __restrict__ owner, uint32_t* __restrict__ collided) {
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t g = (uint32_t)((blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5);
+  if (g >= nblock) return;
+  const uint32_t o = owner[g];
+  if (o == g) return;
+  bool same = bseg[o] == bseg[g] && n[o] == n[g] && lo[o] == lo[g] && hi[o] == hi[g];
+  if (same && n[g] > 2) {
+    const uint32_t sg = bseg[g];
+    const CsegDims d = segs[sg].d;
+    const uint32_t b0 = (uint32_t)segs[sg].b0;
+    same = cs_same_table<T, CS_PER_LANE>(in + segs[sg].in_off, d, o - b0, g - b0, n[g], lane);
+  }
+  if (!same && lane == 0) *collided = 1;
+}
+
+template <typename T, int CS_PER_LANE>
+__global__ void __maxnreg__(255)
+    k_cb_resolve(const T* __restrict__ in, const CsegSeg* __restrict__ segs, uint32_t nblock,
+                 const uint32_t* __restrict__ bseg, const uint32_t* __restrict__ n, const unsigned long long* __restrict__ lo,
+                 const unsigned long long* __restrict__ hi, const uint32_t* __restrict__ sblock,
+                 const uint32_t* __restrict__ headpos, uint32_t* __restrict__ owner) {
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t i = (uint32_t)((blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5);
+  if (i >= nblock) return;
+  const uint32_t g = sblock[i];
+  const uint32_t sg = bseg[g], ng = n[g];
+  const unsigned long long log = lo[g], hig = hi[g];
+  const CsegDims d = segs[sg].d;
+  const T* src = in + segs[sg].in_off;
+  const uint32_t b0 = (uint32_t)segs[sg].b0;
+  uint32_t own = g;
+  for (uint32_t base = headpos[i]; base < i && own == g; base += 32) {
+    const uint32_t j = base + lane;
+    const uint32_t c = j < i ? sblock[j] : 0u;
+    uint32_t cand = __ballot_sync(CS_FULL, j < i && bseg[c] == sg && n[c] == ng && lo[c] == log && hi[c] == hig);
+    while (cand) {
+      const uint32_t cb = __shfl_sync(CS_FULL, c, __ffs(cand) - 1);
+      if (ng <= 2 || cs_same_table<T, CS_PER_LANE>(src, d, cb - b0, g - b0, ng, lane)) {
+        own = cb;
+        break;
+      }
+      cand &= cand - 1;
+    }
+  }
+  if (lane == 0) owner[g] = own;
+}
+
+template <int WORDS>
+__global__ void __launch_bounds__(256)
+    k_cb_sizes(const CsegSeg* __restrict__ segs, const uint32_t* __restrict__ bseg, const uint32_t* __restrict__ n,
+               const uint32_t* __restrict__ owner, uint32_t nblock, unsigned long long* __restrict__ size) {
+  const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= nblock) return;
+  const uint32_t bvox = segs[bseg[g]].d.bvox;
+  size[g] = (cs_bits(n[g]) * bvox + 31) / 32 + (owner[g] == g ? n[g] * WORDS : 0u);
+}
+
+// one thread per segment: its stream length (-> *too_long past the format's 24-bit offsets), its
+// entry in its chunk's channel table, and (channel 0) the chunk's word offset in the output
+__global__ void __launch_bounds__(256)
+    k_cb_segments(const CsegSeg* __restrict__ segs, uint64_t nseg, uint64_t sc, const unsigned long long* __restrict__ scan,
+                  uint32_t* __restrict__ too_long, uint32_t* __restrict__ out, unsigned long long* __restrict__ chunk_off) {
+  const uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (s >= nseg) return;
+  const CsegSeg& S = segs[s];
+  const uint64_t nb = (uint64_t)S.d.gx * S.d.gy * S.d.gz;
+  const uint64_t start = scan[S.b0] + 2 * S.b0 + sc * (S.chunk + 1);
+  const uint64_t words = 2 * nb + scan[S.b0 + nb] - scan[S.b0];
+  if (words > 0xFFFFFFull + 1024) atomicMax(too_long, 1u);
+  const uint64_t cstart = scan[segs[s - S.chan].b0] + 2 * segs[s - S.chan].b0 + sc * S.chunk;  // chunk i's first word
+  if (out) out[cstart + S.chan] = (uint32_t)(start - cstart);
+  if (S.chan == 0) chunk_off[S.chunk] = cstart;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256)
+    k_cb_decode(const uint32_t* __restrict__ in, const unsigned long long* __restrict__ word_off,
+                const CsegSeg* __restrict__ segs, uint64_t nseg, uint64_t sc, T* __restrict__ out, uint32_t* __restrict__ bad) {
+  for (uint64_t s = blockIdx.y; s < nseg; s += gridDim.y) {
+    const CsegSeg& S = segs[s];
+    const CsegDims d = S.d;
+    const uint64_t i0 = word_off[S.chunk], nw = word_off[S.chunk + 1] - i0;
+    const uint32_t* chunk = in + i0;
+    const uint64_t n = (uint64_t)d.sx * d.sy * d.sz;
+    const uint64_t base = sc <= nw ? chunk[S.chan] : ~0ull;
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+      if (base > nw) { atomicMin(bad, (uint32_t)S.chunk); break; }
+      const uint32_t* ch = chunk + base;
+      const uint64_t nwords = nw - base;
+      const uint32_t x = (uint32_t)(i % d.sx), y = (uint32_t)((i / d.sx) % d.sy), z = (uint32_t)(i / ((uint64_t)d.sx * d.sy));
+      const uint64_t b = (x / d.bx) + (uint64_t)d.gx * ((y / d.by) + (uint64_t)d.gy * (z / d.bz));
+      uint64_t v;
+      if (!cs_decode_voxel<T>(ch, nwords, d, x, y, z, b, &v)) { atomicMin(bad, (uint32_t)S.chunk); break; }
+      out[S.in_off + i] = (T)v;
+    }
+  }
+}
+
+// the segment table of n chunks of shapes[i] (host n x 3) with sc channels; *nblock = blocks in all
+static int cb_segments(const uint32_t* shapes, uint64_t n, uint64_t sc, uint32_t bx, uint32_t by, uint32_t bz,
+                       std::vector<CsegSeg>& segs, uint64_t* nblock) {
+  segs.resize(n * sc);
+  uint64_t b0 = 0, off = 0;
+  for (uint64_t i = 0; i < n; i++) {
+    CsegDims d;
+    const int st = cseg_dims(shapes[3 * i], shapes[3 * i + 1], shapes[3 * i + 2], bx, by, bz, &d);
+    if (st != IGN_OK) {
+      set_error("cseg batch: chunk %llu: bad shape or block size (%u x %u x %u, block %u x %u x %u)",
+                (unsigned long long)i, shapes[3 * i], shapes[3 * i + 1], shapes[3 * i + 2], bx, by, bz);
+      return st;
+    }
+    const uint64_t nb = (uint64_t)d.gx * d.gy * d.gz, vox = (uint64_t)d.sx * d.sy * d.sz;
+    for (uint64_t c = 0; c < sc; c++) {
+      segs[i * sc + c] = CsegSeg{d, off, b0, i, (uint32_t)c};
+      off += vox;
+      b0 += nb;
+    }
+  }
+  *nblock = b0;
+  return IGN_OK;
+}
+
+template <typename T>
+static int cseg_encode_batch(ign_ctx* ctx, const T* in, const std::vector<CsegSeg>& hsegs, uint64_t nblock, uint64_t n,
+                             uint64_t sc, uint32_t bvox, uint32_t* out, uint64_t cap_words, uint64_t* offsets,
+                             uint64_t* n_words) {
+  constexpr int WORDS = sizeof(T) / 4;
+  const uint64_t nseg = hsegs.size();
+  IGN_REQUIRE(nblock < (1ull << 31), IGN_ERR_OVERFLOW, "cseg batch: %llu blocks in one call (at most 2^31 - 1)",
+              (unsigned long long)nblock);
+  const uint32_t nb = (uint32_t)nblock;
+  unsigned long long hash_mask = ~0ull;
+  if (const char* e = getenv("IGN_CSEG_HASH_BITS")) {
+    const int k = atoi(e);
+    hash_mask = k >= 64 ? ~0ull : k <= 0 ? 0ull : (1ull << k) - 1;
+  }
+  size_t sortb = 0, scanb = 0, maxb = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, sortb, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                  (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)nb);
+  cub::DeviceScan::ExclusiveSum(nullptr, scanb, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)nb + 1);
+  cub::DeviceScan::InclusiveScan(nullptr, maxb, (const uint32_t*)nullptr, (uint32_t*)nullptr, cub::Max(), (int)nb);
+  const size_t tmpb = std::max(sortb, std::max(scanb, maxb)) + 256;
+  ScratchFrame f(ctx);
+  CsegSeg* segs;
+  unsigned long long *hash, *shash, *lo, *hi, *scan, *chunk_off;
+  unsigned long long* size;
+  uint32_t *cnt, *bseg, *blk, *sblk, *owner, *headpos, *runhead, *flags;
+  void* tmp;
+  IGN_TRY(f.take(&segs, nseg));
+  IGN_TRY(f.take(&hash, nb));
+  IGN_TRY(f.take(&shash, nb));
+  IGN_TRY(f.take(&lo, nb));
+  IGN_TRY(f.take(&hi, nb));
+  IGN_TRY(f.take(&scan, (size_t)nb + 1));
+  IGN_TRY(f.take(&chunk_off, n + 1));
+  IGN_TRY(f.take(&cnt, (size_t)nb + 1));
+  IGN_TRY(f.take(&bseg, (size_t)nb + 1));
+  IGN_TRY(f.take(&blk, (size_t)nb + 1));
+  IGN_TRY(f.take(&sblk, (size_t)nb + 1));
+  IGN_TRY(f.take(&owner, (size_t)nb + 1));
+  IGN_TRY(f.take(&size, (size_t)nb + 1));
+  IGN_TRY(f.take(&headpos, (size_t)nb + 1));
+  IGN_TRY(f.take(&runhead, (size_t)nb + 1));
+  IGN_TRY(f.take(&flags, 2));  // [collided, too_long]
+  IGN_TRY(f.take(&tmp, tmpb));
+  IGN_CUDA(cudaMemcpyAsync(segs, hsegs.data(), nseg * sizeof(CsegSeg), cudaMemcpyHostToDevice, ctx->stream));
+  IGN_CUDA(cudaMemsetAsync(flags, 0, 8, ctx->stream));
+  const unsigned gw = blocks_for((uint64_t)nb * 32, 128);
+  const bool wide = bvox > 512;
+#define CB_LAUNCH_PL(kernel, ...)                                        \
+  do {                                                                   \
+    if (!wide) IGN_LAUNCH(ctx, (kernel<T, 16>), gw, 128, 0, __VA_ARGS__); \
+    else IGN_LAUNCH(ctx, (kernel<T, 32>), gw, 128, 0, __VA_ARGS__);       \
+  } while (0)
+  if (!wide)
+    IGN_LAUNCH(ctx, (k_cb_scan<T, false, 16>), gw, 128, 0, in, (const CsegSeg*)segs, nseg, nblock, sc, cnt, bseg, hash,
+               hash_mask, lo, hi, (const unsigned long long*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr);
+  else
+    IGN_LAUNCH(ctx, (k_cb_scan<T, false, 32>), gw, 128, 0, in, (const CsegSeg*)segs, nseg, nblock, sc, cnt, bseg, hash,
+               hash_mask, lo, hi, (const unsigned long long*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr);
+  IGN_LAUNCH(ctx, k_iota32, blocks_for(nb, 256), 256, 0, blk, nb);
+  {
+    size_t tb = tmpb;
+    IGN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, hash, shash, blk, sblk, (int)nb, 0, 64, ctx->stream));
+    ctx->launches += 9;
+  }
+  IGN_LAUNCH(ctx, k_cseg_heads, blocks_for(nb, 256), 256, 0, shash, nb, headpos);
+  {
+    size_t tb = tmpb;
+    IGN_CUDA(cub::DeviceScan::InclusiveScan(tmp, tb, headpos, runhead, cub::Max(), (int)nb, ctx->stream));
+    ctx->launches += 2;
+  }
+  IGN_LAUNCH(ctx, k_cseg_owner, blocks_for(nb, 256), 256, 0, runhead, sblk, nb, owner);
+  CB_LAUNCH_PL(k_cb_verify, in, (const CsegSeg*)segs, nb, (const uint32_t*)bseg, (const uint32_t*)cnt,
+               (const unsigned long long*)lo, (const unsigned long long*)hi, (const uint32_t*)owner, flags);
+  uint32_t hflags[2] = {0, 0};
+  IGN_TRY(small_d2h(ctx, hflags, flags, 4));
+  IGN_TRY(small_sync(ctx));
+  if (hflags[0])
+    CB_LAUNCH_PL(k_cb_resolve, in, (const CsegSeg*)segs, nb, (const uint32_t*)bseg, (const uint32_t*)cnt,
+                 (const unsigned long long*)lo, (const unsigned long long*)hi, (const uint32_t*)sblk,
+                 (const uint32_t*)runhead, owner);
+#undef CB_LAUNCH_PL
+  IGN_LAUNCH(ctx, (k_cb_sizes<WORDS>), blocks_for(nb, 256), 256, 0, (const CsegSeg*)segs, (const uint32_t*)bseg,
+             (const uint32_t*)cnt, (const uint32_t*)owner, nb, size);
+  IGN_CUDA(cudaMemsetAsync(size + nb, 0, 8, ctx->stream));
+  {
+    size_t tb = tmpb;
+    IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, size, scan, (int)nb + 1, ctx->stream));
+    ctx->launches += 2;
+  }
+  // the sizes pass: chunk offsets and the 24-bit check, nothing written yet
+  IGN_LAUNCH(ctx, k_cb_segments, blocks_for(nseg, 256), 256, 0, (const CsegSeg*)segs, nseg, sc,
+             (const unsigned long long*)scan, flags + 1, (uint32_t*)nullptr, chunk_off);
+  unsigned long long total_data = 0;
+  IGN_TRY(small_d2h(ctx, &total_data, scan + nb, 8));
+  IGN_TRY(small_d2h(ctx, hflags + 1, flags + 1, 4));
+  IGN_TRY(small_sync(ctx));
+  const uint64_t total = total_data + 2ull * nb + sc * n;
+  *n_words = total;
+  IGN_REQUIRE(hflags[1] == 0, IGN_ERR_OVERFLOW,
+              "cseg batch: a chunk's channel stream exceeds the format's 24-bit table offsets");
+  IGN_REQUIRE(total <= cap_words, IGN_ERR_OVERFLOW, "cseg batch: %llu words needed, the output holds %llu",
+              (unsigned long long)total, (unsigned long long)cap_words);
+  IGN_CUDA(cudaMemcpyAsync(chunk_off + n, &total, 8, cudaMemcpyHostToDevice, ctx->stream));
+  IGN_LAUNCH(ctx, k_cb_segments, blocks_for(nseg, 256), 256, 0, (const CsegSeg*)segs, nseg, sc,
+             (const unsigned long long*)scan, flags + 1, out, chunk_off);
+  if (!wide)
+    IGN_LAUNCH(ctx, (k_cb_scan<T, true, 16>), gw, 128, 0, in, (const CsegSeg*)segs, nseg, nblock, sc, cnt,
+               (uint32_t*)nullptr, (unsigned long long*)nullptr, hash_mask, (unsigned long long*)nullptr,
+               (unsigned long long*)nullptr, (const unsigned long long*)scan, (const uint32_t*)owner, out);
+  else
+    IGN_LAUNCH(ctx, (k_cb_scan<T, true, 32>), gw, 128, 0, in, (const CsegSeg*)segs, nseg, nblock, sc, cnt,
+               (uint32_t*)nullptr, (unsigned long long*)nullptr, hash_mask, (unsigned long long*)nullptr,
+               (unsigned long long*)nullptr, (const unsigned long long*)scan, (const uint32_t*)owner, out);
+  IGN_CUDA(cudaMemcpyAsync(offsets, chunk_off, (n + 1) * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+  return IGN_OK;
+}
+
 }  // namespace ign
 
 using namespace ign;
@@ -480,6 +849,66 @@ int ign_cseg_decode_dev(ign_ctx* ctx, const uint32_t* in, uint64_t n_words, int 
   IGN_CUDA(cudaMemcpyAsync(&herr, err, 4, cudaMemcpyDeviceToHost, ctx->stream));
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   IGN_REQUIRE(herr == 0, IGN_ERR_INVALID, "cseg: malformed stream");
+  return IGN_OK;
+}
+
+int ign_cseg_encode_batch_dev(ign_ctx* ctx, const void* chunks, int dtype, uint64_t n_chunks, const uint32_t* shapes,
+                              uint64_t sc, uint32_t bx, uint32_t by, uint32_t bz, uint32_t* out, uint64_t cap_words,
+                              uint64_t* offsets, uint64_t* n_words) {
+  IGN_TRY(activate(ctx));
+  IGN_REQUIRE(n_words && sc >= 1 && (n_chunks == 0 || (chunks && shapes && out && offsets)), IGN_ERR_INVALID,
+              "cseg batch: null argument");
+  IGN_REQUIRE(dtype == IGN_U32 || dtype == IGN_U64, IGN_ERR_UNSUPPORTED, "compressed_segmentation holds uint32 / uint64 labels");
+  *n_words = 0;
+  if (n_chunks == 0) return IGN_OK;
+  std::vector<CsegSeg> segs;
+  uint64_t nblock = 0;
+  IGN_TRY(cb_segments(shapes, n_chunks, sc, bx, by, bz, segs, &nblock));
+  const uint32_t bvox = bx * by * bz;
+  if (dtype == IGN_U32)
+    return cseg_encode_batch<uint32_t>(ctx, (const uint32_t*)chunks, segs, nblock, n_chunks, sc, bvox, out, cap_words,
+                                       offsets, n_words);
+  return cseg_encode_batch<uint64_t>(ctx, (const uint64_t*)chunks, segs, nblock, n_chunks, sc, bvox, out, cap_words,
+                                     offsets, n_words);
+}
+
+int ign_cseg_decode_batch_dev(ign_ctx* ctx, const uint32_t* streams, const uint64_t* word_offsets, uint64_t n_streams,
+                              int dtype, const uint32_t* shapes, uint64_t sc, uint32_t bx, uint32_t by, uint32_t bz,
+                              void* out) {
+  IGN_TRY(activate(ctx));
+  IGN_REQUIRE(sc >= 1 && (n_streams == 0 || (streams && word_offsets && shapes && out)), IGN_ERR_INVALID,
+              "cseg batch: null argument");
+  IGN_REQUIRE(dtype == IGN_U32 || dtype == IGN_U64, IGN_ERR_UNSUPPORTED, "compressed_segmentation holds uint32 / uint64 labels");
+  if (n_streams == 0) return IGN_OK;
+  for (uint64_t i = 0; i < n_streams; i++)
+    IGN_REQUIRE(word_offsets[i] <= word_offsets[i + 1], IGN_ERR_INVALID, "cseg batch: stream %llu has a negative length",
+                (unsigned long long)i);
+  std::vector<CsegSeg> hsegs;
+  uint64_t nblock = 0, most = 0;
+  IGN_TRY(cb_segments(shapes, n_streams, sc, bx, by, bz, hsegs, &nblock));
+  for (const CsegSeg& S : hsegs) most = std::max(most, (uint64_t)S.d.sx * S.d.sy * S.d.sz);
+  ScratchFrame f(ctx);
+  CsegSeg* segs;
+  unsigned long long* woff;
+  uint32_t* bad;
+  IGN_TRY(f.take(&segs, hsegs.size()));
+  IGN_TRY(f.take(&woff, n_streams + 1));
+  IGN_TRY(f.take(&bad, 1));
+  IGN_CUDA(cudaMemcpyAsync(segs, hsegs.data(), hsegs.size() * sizeof(CsegSeg), cudaMemcpyHostToDevice, ctx->stream));
+  IGN_CUDA(cudaMemcpyAsync(woff, word_offsets, (n_streams + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
+  IGN_CUDA(cudaMemsetAsync(bad, 0xFF, 4, ctx->stream));
+  const uint64_t gx = std::min<uint64_t>(blocks_for(most, 256), 1024);
+  const dim3 grid((unsigned)gx, (unsigned)std::min<uint64_t>(hsegs.size(), 65535));
+  if (dtype == IGN_U32)
+    IGN_LAUNCH(ctx, k_cb_decode<uint32_t>, grid, 256, 0, streams, (const unsigned long long*)woff, (const CsegSeg*)segs,
+               (uint64_t)hsegs.size(), sc, (uint32_t*)out, bad);
+  else
+    IGN_LAUNCH(ctx, k_cb_decode<uint64_t>, grid, 256, 0, streams, (const unsigned long long*)woff, (const CsegSeg*)segs,
+               (uint64_t)hsegs.size(), sc, (uint64_t*)out, bad);
+  uint32_t hbad = 0;
+  IGN_TRY(small_d2h(ctx, &hbad, bad, 4));
+  IGN_TRY(small_sync(ctx));
+  IGN_REQUIRE(hbad == 0xFFFFFFFFu, IGN_ERR_INVALID, "cseg batch: stream %u is malformed", hbad);
   return IGN_OK;
 }
 

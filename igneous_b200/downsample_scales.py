@@ -5,6 +5,7 @@ Mirrors the functions of igneous/downsample_scales.py that sit on the hot path:
   axis_to_factor         :174-182
   compute_scales         :184-212
   create_downsample_scales :214-244 adds the new scales to the info file
+  downsample_shape_from_memory_target :280-358 the task shape of a transfer
 """
 import copy
 import math
@@ -106,3 +107,47 @@ def add_scales(layer_path, mip, num_mips, preserve_chunk_size=True, chunk_size=N
     mip += 1
     vol.mip = mip
   return vol
+
+
+def downsample_shape_from_memory_target(data_width, cx, cy, cz, factor, byte_target, max_mips=float("inf")):
+  """The task shape (whole chunks of cx x cy x cz voxels of `data_width` bytes) that yields the most
+  downsamples while the task's image and its pyramid stay within `byte_target` bytes.
+
+  factor (2,2,1): the pyramid adds a third, so the image may hold V = 3/4 * target / (w * cz) voxels
+    per z-slab one chunk thick.  That budget is shared between x and y so that each axis's extent is
+    its chunk size raised to one common power e: cx^e * cy^e = V.  Each axis then takes chunk * 2^k,
+    k the integer part of log2(c^e / c), at most max_mips; z stays one chunk.
+  factor (2,2,2): the same with V = 7/8 * target / w shared by x, y and z (cx^e * cy^e * cz^e = V).
+    Non-square chunks thus get different doubling counts per axis.
+  factor (1,1,1): no pyramid; a single chunk-thick slab of about byte_target bytes that is as square
+    as whole chunks allow: n = floor(sqrt(target / (w*cx*cy*cz))) chunks in x, floor(n*cx/cy) in y.
+  Example: uint64, 128 x 128 x 64 chunks, 3 GB, (2,2,1) -> 2048 x 2048 x 64 (2.9 GB with its pyramid)."""
+  factor = tuple(int(f) for f in factor)
+  if byte_target <= 0:
+    raise ValueError("Unable to pick a shape for a byte budget <= 0. Got: %r" % (byte_target,))
+  if cx * cy * cz <= 0:
+    raise ValueError("Chunk size must have a positive integer volume. Got: <%r,%r,%r>" % (cx, cy, cz))
+  chunk = (int(cx), int(cy), int(cz))
+  if factor == (1, 1, 1):
+    n = int(math.sqrt(byte_target / (float(data_width) * cx * cy * cz)))
+    out = Vec(n * cx, int(n * cx / cy) * cy, cz)
+  elif factor in ((2, 2, 1), (2, 2, 2)):
+    pooled = 2 if factor == (2, 2, 1) else 3
+    budget = 3.0 / 4.0 * byte_target / data_width / cz if pooled == 2 else 7.0 / 8.0 * byte_target / data_width
+    prod = float(np.prod(chunk[:pooled]))
+    ks = []
+    for c in chunk[:pooled]:
+      if prod == 1:  # the common power is undefined: an even split
+        k = int(math.log2(budget ** (1.0 / pooled)))
+      else:
+        e = math.log(budget) / math.log(prod)
+        k = int(math.log2((c ** e) / c))
+      ks.append(int(min(k, max_mips)))
+    out = Vec(*[c * 2.0 ** k for c, k in zip(chunk[:pooled], ks)] + ([cz] if pooled == 2 else []))
+  else:
+    raise ValueError("Only the factors (1,1,1), (2,2,1) and (2,2,2) are supported. Got: %r" % (factor,))
+  out = out.astype(int)
+  if np.any(np.asarray(out) < np.asarray(chunk)):
+    raise ValueError("Too little memory allocated to create a valid task. Got: %r Predicted Shape: %r "
+                     "Minimum Shape: %r" % (byte_target, list(out), list(chunk)))
+  return out

@@ -185,6 +185,70 @@ class Bbox:
     return "Bbox(%s, %s)" % (list(self.minpt), list(self.maxpt))
 
 
+# ------------------------------------------------------------ device cutouts
+class DeviceCutout:
+  """An F-order [x, y, z, c] array in device memory: what download_dev returns and upload_dev,
+  make_shard_chunks and downsample_and_upload take, so that a cutout's chunks are decoded, re-cut,
+  pooled and re-encoded without passing through host memory."""
+
+  def __init__(self, buf, shape, dtype, ctx):
+    self.buf, self.shape, self.dtype, self.ctx = buf, tuple(int(v) for v in shape), np.dtype(dtype), ctx
+
+  @classmethod
+  def empty(cls, shape, dtype, ctx=None):
+    from . import _shim
+    ctx = ctx or _shim.default_context()
+    nbytes = int(np.prod(shape)) * np.dtype(dtype).itemsize
+    return cls(ctx.alloc(max(nbytes, 8)), shape, dtype, ctx)
+
+  @classmethod
+  def from_host(cls, arr, ctx=None):
+    arr = np.asarray(arr)
+    if arr.ndim == 3:
+      arr = arr[..., np.newaxis]
+    out = cls.empty(arr.shape, arr.dtype, ctx)
+    if arr.size:
+      out.ctx.h2d(out.buf, np.asfortranarray(arr))
+    return out
+
+  @property
+  def ptr(self):
+    from . import _shim
+    return _shim.ptr(self.buf)
+
+  @property
+  def size(self):
+    return int(np.prod(self.shape))
+
+  @property
+  def nbytes(self):
+    return self.size * self.dtype.itemsize
+
+  def to_host(self):
+    out = np.empty(self.shape, dtype=self.dtype, order="F")
+    if out.size:
+      self.ctx.d2h(out, self.buf)
+    self.ctx.sync()
+    return out
+
+
+def _packed_offsets(sizes):
+  """byte offsets of buffers of the given sizes packed back to back, and the total"""
+  offs = np.zeros(len(sizes) + 1, dtype=np.int64)
+  np.cumsum(np.asarray(sizes, dtype=np.int64), out=offs[1:])
+  return offs
+
+
+def _upload_bytes(ctx, datas):
+  """one H2D of byte strings packed back to back -> (device buffer, byte offsets)"""
+  offs = _packed_offsets([len(d) for d in datas])
+  host = np.frombuffer(b"".join(bytes(d) for d in datas), dtype=np.uint8)
+  buf = ctx.alloc(max(int(offs[-1]), 8))
+  if host.size:
+    ctx.h2d(buf, host)
+  return buf, offs
+
+
 # --------------------------------------------------------------------- files
 def _strip(path):
   if path.startswith("file://"):
@@ -403,17 +467,15 @@ class _Meta:
 
 class _ImageSource:
   """cv.image: the two shard builders ImageShardDownsampleTask calls
-  (igneous/tasks/image/image.py:664-669,818,833)."""
+  (igneous/tasks/image/image.py:664-669,818,833) and transfer_to (image.py:483-496)."""
 
   def __init__(self, cv):
     self._cv = cv
 
   def make_shard_chunks(self, img, bbox, mip):
-    """Cut `img` (occupying `bbox` at `mip`) into the scale's chunks -> {chunk id: encoded bytes}."""
+    """Cut `img` (occupying `bbox` at `mip`; a host array or a DeviceCutout) into the scale's chunks
+    -> {chunk id: encoded bytes}, cut and encoded on the device."""
     cv = self._cv
-    img = np.asarray(img)
-    if img.ndim == 3:
-      img = img[..., np.newaxis]
     bbox = Bbox.create(bbox) if not isinstance(bbox, Bbox) else bbox
     spec = cv._sharding(mip)
     if spec is None:
@@ -421,20 +483,38 @@ class _ImageSource:
     cs, off = cv.chunk_size_at(mip), cv.voxel_offset_at(mip)
     if np.any((np.asarray(bbox.minpt) - np.asarray(off)) % np.asarray(cs)):
       raise ValueError("shard cutout %r is not chunk aligned" % (bbox,))
-    out = {}
-    jpeg = {}  # jpeg chunks are encoded in one call
-    for c in cv._chunks(mip, Bbox.clamp(bbox, cv.bounds_at(mip))):
-      src = tuple(slice(int(a - o), int(b - o)) for a, b, o in zip(c.minpt, c.maxpt, bbox.minpt))
-      block = np.asfortranarray(img[src].astype(cv.dtype, copy=False))
-      if tuple(block.shape[:3]) != tuple(int(v) for v in c.size3()):
-        raise ValueError("image %r does not cover chunk %r of %r" % (img.shape, c, bbox))
-      if cv._encoding(mip) == "jpeg":
-        jpeg[cv._chunk_id(mip, c)] = block
+    shape = img.shape if isinstance(img, DeviceCutout) else np.shape(img)
+    boxes = list(cv._chunks(mip, Bbox.clamp(bbox, cv.bounds_at(mip))))
+    for c in boxes:
+      if np.any(np.asarray(c.maxpt) - np.asarray(bbox.minpt) > np.asarray(shape[:3])):
+        raise ValueError("image %r does not cover chunk %r of %r" % (tuple(shape), c, bbox))
+    files, _ = cv._chunk_files(img, [c - bbox.minpt for c in boxes], mip)
+    return {cv._chunk_id(mip, c): f for c, f in zip(boxes, files)}
+
+  def transfer_to(self, dest_path, bbox, mip, compress="gzip"):
+    """Copy the chunk files under `bbox` to the same names in dest_path's layer without decoding them
+    (cloudvolume's image.transfer_to).  The destination scale must have this scale's chunk grid (chunk
+    size and bounds, which fix the names and extents of the files) and encoding; the files are stored
+    with `compress`."""
+    cv = self._cv
+    dest = CloudVolume(dest_path, mip=mip)
+    if dest._sharding(mip) is not None:
+      raise NotImplementedError("transfer_to writes unsharded chunk files; a sharded destination takes whole shards")
+    a, b = cv.scales[mip], dest.scales[mip]
+    if not (np.array_equal(cv.chunk_size_at(mip), dest.chunk_size_at(mip)) and cv.bounds_at(mip) == dest.bounds_at(mip)
+            and all(a.get(k) == b.get(k) for k in ("encoding", "compressed_segmentation_block_size", "jpeg_quality"))
+            and cv.dtype == dest.dtype and cv.num_channels == dest.num_channels):
+      raise ValueError("transfer_to copies files as they are: %s and %s differ in chunk grid or encoding at mip %d"
+                       % (cv.cloudpath, dest_path, mip))
+    bbox = Bbox.clamp(cv._to_bbox(bbox), cv.bounds_at(mip))
+    shard_cache = {}
+    for c in cv._chunks(mip, bbox):
+      data = cv._read_chunk(mip, c, shard_cache)
+      if data is None:
+        if not cv.fill_missing:
+          raise EmptyVolumeException(cv._chunk_name(mip, c))
         continue
-      out[cv._chunk_id(mip, c)] = cv._encode_chunk(block, mip)
-    if jpeg:
-      out.update(zip(jpeg.keys(), cv._jpeg_encode(list(jpeg.values()), mip)))
-    return out
+      dest.cf.put(dest._chunk_name(mip, c), data, compress=None if cv._encoding(mip) == "jpeg" else compress)
 
   def make_shard(self, img, bbox, mip, progress=False):
     """-> (file name, shard bytes).  `img` is an array or a {chunk id: bytes} dict."""
@@ -667,7 +747,7 @@ class CloudVolume:
     return None if blob is None else spec.read_chunk(blob, cid)
 
   # chunk codecs: `raw` is the bytes of the Fortran-order array; `compressed_segmentation` and
-  # `jpeg` go through the device codecs (igneous_b200.codecs), jpeg a whole read or write per call;
+  # `jpeg` go through the device codecs (igneous_b200.codecs), a whole read or write per call;
   # anything else the Precomputed format knows (png, compresso, crackle, ...) is outside this stand-in
   def _encoding(self, mip):
     return self.info["scales"][mip].get("encoding", "raw")
@@ -677,40 +757,119 @@ class CloudVolume:
       raise NotImplementedError("storage stand-in: jpeg scales hold one uint8 channel (got %s x %d)"
                                 % (self.dtype, self.num_channels))
 
-  def _jpeg_encode(self, blocks, mip):
-    self._jpeg_check(mip)
-    from . import codecs
-    return codecs.jpeg_encode_batch(blocks, quality=int(self.info["scales"][mip].get("jpeg_quality", 85)))
-
-  def _jpeg_decode(self, datas, mip, shapes):
-    self._jpeg_check(mip)
-    from . import codecs
-    return codecs.jpeg_decode_batch(datas, shapes)
-
   def _cseg_block(self, mip):
     return tuple(int(v) for v in self.info["scales"][mip].get("compressed_segmentation_block_size", (8, 8, 8)))
 
-  def _encode_chunk(self, block, mip):
-    enc = self._encoding(mip)
-    if enc == "raw":
-      return block.tobytes(order="F")
-    if enc == "compressed_segmentation":
-      from . import codecs
-      return codecs.cseg_encode(block, self._cseg_block(mip))
-    if enc == "jpeg":
-      return self._jpeg_encode([block], mip)[0]
-    raise NotImplementedError("storage stand-in: chunk encoding %r is not supported" % enc)
+  def _device_cutout(self, img):
+    """img (a host array or a DeviceCutout) as a DeviceCutout of this layer's dtype"""
+    if isinstance(img, DeviceCutout):
+      if img.dtype == self.dtype:
+        return img
+      img = img.to_host()
+    img = np.asarray(img)
+    if img.ndim == 3:
+      img = img[..., np.newaxis]
+    return DeviceCutout.from_host(img.astype(self.dtype, copy=False))
 
-  def _decode_chunk(self, data, mip, shape):
+  def _chunk_files(self, img, boxes, mip):
+    """chunk files of `mip` for boxes (relative Bboxes) of a host array or DeviceCutout -> (list of
+    bytes, list of all-background flags).  `raw` files of a host array are its own bytes and need no
+    device; everything else is cut and encoded on the device."""
+    if not isinstance(img, DeviceCutout) and self._encoding(mip) == "raw":
+      return self._raw_boxes(img, boxes)
+    return self._encode_boxes(self._device_cutout(img), boxes, mip)
+
+  def _raw_boxes(self, img, boxes):
+    """`raw` chunk files of boxes of a host array: the boxes' F-order bytes, which need no device"""
+    img = np.asarray(img)
+    if img.ndim == 3:
+      img = img[..., np.newaxis]
+    img = img.astype(self.dtype, copy=False)
+    blocks = [np.asfortranarray(img[b.to_slices()]) for b in boxes]
+    return [b.tobytes(order="F") for b in blocks], [not np.any(b != self.background_color) for b in blocks]
+
+  def _encode_boxes(self, cutout, boxes, mip):
+    """Encode boxes (Bboxes relative to the cutout) of a device cutout as chunk files of `mip`: one
+    cut, one batched encode and one D2H -> (list of bytes, list of all-background flags)."""
+    from . import _shim
+    ctx = cutout.ctx
     enc = self._encoding(mip)
+    if enc not in ("raw", "compressed_segmentation", "jpeg"):
+      raise NotImplementedError("storage stand-in: chunk encoding %r is not supported" % enc)
+    if enc == "jpeg":
+      self._jpeg_check(mip)
+    if not boxes:
+      return [], []
+    nc, es = cutout.shape[3], cutout.dtype.itemsize
+    sizes = [np.asarray(b.size3(), dtype=np.int64) for b in boxes]
+    offs = _packed_offsets([int(np.prod(z)) * nc * es for z in sizes])
+    rows = np.ascontiguousarray(np.array([list(b.minpt) + list(z) + [o] for b, z, o in zip(boxes, sizes, offs[:-1])],
+                                         dtype=np.uint64))
+    packed = ctx.alloc(max(int(offs[-1]), 8))
+    flags_dev = ctx.alloc(4 * len(boxes))
+    want = np.asarray(self.background_color)
+    typed = want.astype(cutout.dtype).reshape(1)
+    # a background the dtype cannot hold (-1 for uint8) matches no voxel: no box is all background
+    representable = bool(typed[0] == want)
+    bg = typed.view(np.dtype("u%d" % es))[0]
+    X, Y, Z = cutout.shape[:3]
+    _shim.check(ctx.lib.ign_chunks_cut_dev(ctx.handle, cutout.ptr, _shim.dtype_code(cutout.dtype), X, Y, Z, nc,
+                                           _shim.ptr(rows), len(boxes), int(bg), _shim.ptr(packed),
+                                           _shim.ptr(flags_dev)))
+    flags = np.empty(len(boxes), dtype=np.uint32)
+    ctx.d2h(flags, flags_dev)
+    shapes = np.ascontiguousarray(np.array(sizes, dtype=np.uint32).reshape(len(boxes), 3))
     if enc == "raw":
-      return np.frombuffer(data, dtype=self.dtype).reshape(shape, order="F")
+      host = np.empty(int(offs[-1]), dtype=np.uint8)
+      ctx.d2h(host, packed)
+      ctx.sync()
+      return [host[offs[i]:offs[i + 1]].tobytes() for i in range(len(boxes))], [representable and bool(f) for f in flags]
     if enc == "compressed_segmentation":
       from . import codecs
-      return codecs.cseg_decode(data, shape, self.dtype, self._cseg_block(mip))
+      files = codecs.cseg_encode_batch_dev(packed, cutout.dtype, shapes, nc, self._cseg_block(mip), ctx)
+      ctx.sync()
+      return files, [representable and bool(f) for f in flags]
+    from . import codecs
+    files = codecs.jpeg_encode_batch_dev(packed, shapes, int(self.info["scales"][mip].get("jpeg_quality", 85)), ctx)
+    ctx.sync()
+    return files, [representable and bool(f) for f in flags]
+
+  def _decode_into(self, cutout, pieces, mip):
+    """Decode chunk files into their places in a device cutout: one H2D of the files, one batched
+    decode, one place.  pieces: (chunk shape [x, y, z], file bytes, source corner in the chunk, box
+    size, destination corner in the cutout)."""
+    from . import _shim
+    ctx = cutout.ctx
+    enc = self._encoding(mip)
+    if enc not in ("raw", "compressed_segmentation", "jpeg"):
+      raise NotImplementedError("storage stand-in: chunk encoding %r is not supported" % enc)
     if enc == "jpeg":
-      return self._jpeg_decode([data], mip, [shape])[0]
-    raise NotImplementedError("storage stand-in: chunk encoding %r is not supported" % enc)
+      self._jpeg_check(mip)
+    if not pieces:
+      return
+    nc, es = cutout.shape[3], cutout.dtype.itemsize
+    shapes = np.ascontiguousarray(np.array([p[0] for p in pieces], dtype=np.uint32).reshape(len(pieces), 3))
+    offs = _packed_offsets([int(np.prod(p[0], dtype=np.int64)) * nc * es for p in pieces])
+    streams, soffs = _upload_bytes(ctx, [p[1] for p in pieces])
+    if enc == "raw":
+      for i, p in enumerate(pieces):
+        if soffs[i + 1] - soffs[i] != offs[i + 1] - offs[i]:
+          raise ValueError("raw chunk %d: %d bytes for a %r x %d chunk of %s" % (i, soffs[i + 1] - soffs[i],
+                                                                               tuple(p[0]), nc, cutout.dtype))
+      packed = streams
+    else:
+      packed = ctx.alloc(max(int(offs[-1]), 8))
+      from . import codecs
+      if enc == "compressed_segmentation":
+        codecs.cseg_decode_batch_dev(streams, soffs, cutout.dtype, shapes, nc, self._cseg_block(mip), packed, ctx)
+      else:
+        codecs.jpeg_decode_batch_dev(streams, soffs, shapes, packed, ctx)
+    rows = np.ascontiguousarray(np.array([list(p[0]) + [o] + list(p[2]) + list(p[3]) + list(p[4])
+                                          for p, o in zip(pieces, offs[:-1])], dtype=np.uint64))
+    X, Y, Z = cutout.shape[:3]
+    _shim.check(ctx.lib.ign_chunks_place_dev(ctx.handle, _shim.ptr(packed), _shim.dtype_code(cutout.dtype), nc,
+                                             _shim.ptr(rows), len(pieces), cutout.ptr, X, Y, Z))
+    ctx.sync()
 
   def _to_bbox(self, key):
     if isinstance(key, Bbox):
@@ -726,8 +885,8 @@ class CloudVolume:
     raise TypeError(key)
 
   def download(self, bbox, mip=None, renumber=False, **kwargs):
-    """Cutout as an F-order [x, y, z, c] array.  renumber=True -> (array of the smallest
-    dtype holding 1..N, {old: new}) with the relabelling done on the GPU
+    """Cutout as an F-order [x, y, z, c] array (download_dev + one D2H).  renumber=True -> (array of
+    the smallest dtype holding 1..N, {old: new}) with the relabelling done on the GPU
     (cloudvolume's download(renumber=True), image.py:745-752)."""
     if renumber:
       from . import fastremap
@@ -735,12 +894,24 @@ class CloudVolume:
       small, mapping = fastremap.renumber(img, preserve_zero=True, in_place=False)
       return small, mapping
     mip = self._mip if mip is None else mip
+    if self._encoding(mip) != "raw":
+      return self.download_dev(bbox, mip=mip).to_host()
+    # `raw` chunks are the cutout's own bytes: assembled on the host, with no device needed
+    bbox, pieces = self._pieces(bbox, mip)
+    out = np.zeros(tuple(int(v) for v in bbox.size3()) + (self.num_channels,), dtype=self.dtype, order="F")
+    for shape, data, src, size, dst in pieces:
+      chunk = np.frombuffer(data, dtype=self.dtype).reshape(tuple(shape) + (self.num_channels,), order="F")
+      out[tuple(slice(d, d + z) for d, z in zip(dst, size))] = chunk[tuple(slice(a, a + z) for a, z in zip(src, size))]
+    return out
+
+  def _pieces(self, bbox, mip):
+    """(bbox, the chunk files under it) for a read: (chunk shape, file bytes, corner in the chunk, box size,
+    corner in the cutout) per chunk that is present; a missing chunk raises unless fill_missing"""
     bbox = self._to_bbox(bbox)
     if self.bounded and not (np.all(bbox.minpt >= self.bounds_at(mip).minpt) and np.all(bbox.maxpt <= self.bounds_at(mip).maxpt)):
       raise OutOfBoundsError("%r is outside %r" % (bbox, self.bounds_at(mip)))
-    out = np.zeros(tuple(int(v) for v in bbox.size3()) + (self.num_channels,), dtype=self.dtype, order="F")
     shard_cache = {}
-    jpeg = []  # (chunk, intersection, bytes): jpeg chunks are decoded in one call
+    pieces = []
     for c in self._chunks(mip, bbox):
       data = self._read_chunk(mip, c, shard_cache)
       inter = Bbox.intersection(c, bbox)
@@ -750,55 +921,57 @@ class CloudVolume:
         if not self.fill_missing:
           raise EmptyVolumeException(self._chunk_name(mip, c))
         continue
-      if self._encoding(mip) == "jpeg":
-        jpeg.append((c, inter, data))
-        continue
-      chunk = self._decode_chunk(data, mip, tuple(int(v) for v in c.size3()) + (self.num_channels,))
-      src = tuple(slice(int(a - o), int(b - o)) for a, b, o in zip(inter.minpt, inter.maxpt, c.minpt))
-      dst = tuple(slice(int(a - o), int(b - o)) for a, b, o in zip(inter.minpt, inter.maxpt, bbox.minpt))
-      out[dst] = chunk[src]
-    if jpeg:
-      shapes = [tuple(int(v) for v in c.size3()) + (self.num_channels,) for c, _, _ in jpeg]
-      for (c, inter, _), chunk in zip(jpeg, self._jpeg_decode([d for _, _, d in jpeg], mip, shapes)):
-        src = tuple(slice(int(a - o), int(b - o)) for a, b, o in zip(inter.minpt, inter.maxpt, c.minpt))
-        dst = tuple(slice(int(a - o), int(b - o)) for a, b, o in zip(inter.minpt, inter.maxpt, bbox.minpt))
-        out[dst] = chunk[src]
+      pieces.append(([int(v) for v in c.size3()], data, [int(v) for v in inter.minpt - c.minpt],
+                     [int(v) for v in inter.size3()], [int(v) for v in inter.minpt - bbox.minpt]))
+    return bbox, pieces
+
+  def download_dev(self, bbox, mip=None, ctx=None):
+    """Cutout as a DeviceCutout: the chunk files are read (unsharded files or shard reads), sent to
+    the device in one copy, decoded in one batched call and placed in one launch.  Voxels outside
+    the volume, and missing chunks under fill_missing, are 0."""
+    from . import _shim
+    mip = self._mip if mip is None else mip
+    bbox, pieces = self._pieces(bbox, mip)
+    ctx = ctx or _shim.default_context()
+    out = DeviceCutout.empty(tuple(int(v) for v in bbox.size3()) + (self.num_channels,), self.dtype, ctx)
+    ctx.memset(out.buf, 0, out.nbytes)
+    self._decode_into(out, pieces, mip)
     return out
 
   def __getitem__(self, key):
     return self.download(key)
 
   def __setitem__(self, key, img):
-    mip = self._mip
-    bbox = self._to_bbox(key)
-    img = np.asarray(img)
-    if img.ndim == 3:
-      img = img[..., np.newaxis]
-    if tuple(img.shape[:3]) != tuple(int(v) for v in bbox.size3()):
-      raise ValueError("image %r does not fit %r" % (img.shape, bbox))
-    img = img.astype(self.dtype, copy=False)
+    self.upload_dev(self._to_bbox(key), img, mip=self._mip)
+
+  def upload_dev(self, bbox, img, mip=None):
+    """Write a chunk-aligned cutout (a DeviceCutout, or a host array that is sent over first): one
+    cut, one batched encode and one D2H, then one file per chunk.  Under delete_black_uploads the
+    chunks that hold only background_color are deleted instead."""
+    mip = self._mip if mip is None else mip
+    bbox = self._to_bbox(bbox)
+    shape = img.shape if isinstance(img, DeviceCutout) else np.shape(img)
+    if tuple(shape[:3]) != tuple(int(v) for v in bbox.size3()):
+      raise ValueError("image %r does not fit %r" % (tuple(shape), bbox))
     if self._sharding(mip) is not None:
       raise NotImplementedError("writes to a sharded scale go through image.make_shard (whole shards only)")
-    jpeg = []  # (name, block): jpeg chunks are encoded in one call
+    boxes = []
     for c in self._chunks(mip, bbox):
       inter = Bbox.intersection(c, bbox)
       if inter.subvoxel():
         continue
       if not (inter == c):
         raise ValueError("writes must be chunk aligned: %r vs chunk %r" % (bbox, c))
-      src = tuple(slice(int(a - o), int(b - o)) for a, b, o in zip(c.minpt, c.maxpt, bbox.minpt))
-      block = np.asfortranarray(img[src])
+      boxes.append(c)
+    files, black = self._chunk_files(img, [c - bbox.minpt for c in boxes], mip)
+    # jpeg files are already entropy coded: stored without gzip, as CloudVolume stores jpeg chunks
+    compress = None if self._encoding(mip) == "jpeg" else self.compress
+    for c, data, bg in zip(boxes, files, black):
       name = self._chunk_name(mip, c)
-      if self.delete_black_uploads and not np.any(block != self.background_color):
+      if self.delete_black_uploads and bg:
         self.cf.delete(name)
         continue
-      if self._encoding(mip) == "jpeg":
-        jpeg.append((name, block))
-        continue
-      self.cf.put(name, self._encode_chunk(block, mip), compress=self.compress)
-    if jpeg:  # already entropy coded: stored without gzip, as CloudVolume stores jpeg chunks
-      for (name, _), data in zip(jpeg, self._jpeg_encode([b for _, b in jpeg], mip)):
-        self.cf.put(name, data)
+      self.cf.put(name, data, compress=compress)
 
 
 # --------------------------------------------------------------------- queue

@@ -1,6 +1,6 @@
-"""create_downsampling_tasks, create_image_shard_downsample_tasks, the contrast / CLAHE /
-quantize creators, the three CCL task creators and create_voxel_counting_tasks
-(igneous/task_creation/image.py:170-345, 639-770, 1247-1618, 1726-1936): same
+"""create_downsampling_tasks, create_image_shard_downsample_tasks, the transfer creators, the
+contrast / CLAHE / quantize creators, the three CCL task creators and create_voxel_counting_tasks
+(igneous/task_creation/image.py:170-345, 507-637, 639-770, 815-1133, 1247-1618, 1726-1936): same
 signatures, same info / provenance side effects, tasks from igneous_b200.tasks."""
 import copy
 import math
@@ -11,7 +11,7 @@ import numpy as np
 
 from .. import downsample_scales, fastremap, sharding, shards
 from .._compat import Bbox, CloudVolume, CloudFiles, InfoUnavailableError, Vec, min2
-from ..tasks import (DownsampleTask, ImageShardDownsampleTask, CCLFacesTask, CCLEquivalancesTask, RelabelCCLTask,
+from ..tasks import (DownsampleTask, TransferTask, ImageShardTransferTask, ImageShardDownsampleTask, CCLFacesTask, CCLEquivalancesTask, RelabelCCLTask,
                      QuantizeTask, CLAHETask, ContrastNormalizationTask, LuminanceLevelsTask, CountVoxelsTask)
 from ..types import DownsampleMethods
 from .common import FinelyDividedTaskIterator, get_bounds, operator_contact
@@ -159,6 +159,259 @@ def create_image_shard_downsample_tasks(cloudpath, mip=0, fill_missing=False, sp
            encoding_level=encoding_level, encoding_effort=encoding_effort, num_mips=int(num_mips))
 
   return ImageShardDownsampleTaskIterator(roi, shape)
+
+
+# ------------------------------------------------------------------------ transfer
+# task_creation/image.py:507-637 and 815-1133.
+
+# encodings the chunk codecs of this implementation cannot write
+_UNSUPPORTED_ENCODINGS = ("png", "jxl", "jpegxl", "compresso", "crackle", "fpzip", "kempressed", "zfpc")
+
+
+def _refuse_transfer(encoding, compress, agglomerate, timestamp, stop_layer):
+  """what the transfer creators refuse, before any info file is written"""
+  if agglomerate or timestamp is not None or stop_layer is not None:
+    raise NotImplementedError("transfer: agglomerate / timestamp / stop_layer need a graphene source")
+  if encoding is not None and str(encoding).lower() in _UNSUPPORTED_ENCODINGS:
+    raise NotImplementedError("transfer: the %r chunk encoding is not implemented (raw, jpeg and "
+                              "compressed_segmentation are)" % encoding)
+  if compress == "br":
+    raise NotImplementedError("transfer: brotli compression is not implemented (gzip is)")
+
+
+def _refuse_layer_encodings(src_vol, dest_path, mip, encoding):
+  """the source scale's encoding, and the destination's when it exists and `encoding` keeps it, must be
+  ones the chunk codecs read and write; checked before any info file is written"""
+  found = [("source", src_vol.scales[mip].get("encoding", "raw"))]
+  if encoding is None:
+    try:
+      dest = CloudVolume(dest_path, mip=mip)
+      if len(dest.scales) > mip:
+        found.append(("destination", dest.scales[mip].get("encoding", "raw")))
+    except InfoUnavailableError:
+      pass
+  for which, enc in found:
+    if str(enc).lower() in _UNSUPPORTED_ENCODINGS:
+      raise NotImplementedError("transfer: the %s's %r chunk encoding is not implemented (raw, jpeg and "
+                                "compressed_segmentation are)" % (which, enc))
+
+
+def clean_xfer_info(info):
+  """Removes fields that could interfere with additional processing."""
+  info.pop("mesh", None)
+  info.pop("meshing", None)
+  info.pop("skeletons", None)
+  return info
+
+
+def create_transfer_cloudvolume(src_vol, dst_cloudpath, dest_voxel_offset, mip, bounds_mip, encoding, encoding_level,
+                                encoding_effort, chunk_size, truncate_scales, clean_info, cutout, bounds):
+  """The destination layer of a transfer: the existing one, or a copy of the source's info (cut to
+  `bounds` when `cutout`), with the voxel offset, encoding, chunk size and scale edits of the request."""
+  intify = lambda lst: [int(x) for x in lst]
+  bounds_resolution = np.asarray(src_vol.meta.resolution(bounds_mip), dtype=np.float64)
+  try:
+    dest_vol = CloudVolume(dst_cloudpath, mip=mip)
+  except InfoUnavailableError:
+    dest_vol = CloudVolume(dst_cloudpath, info=copy.deepcopy(src_vol.info), mip=mip)
+    if cutout:
+      for i in range(mip + 1):
+        f = bounds_resolution / np.asarray(dest_vol.meta.resolution(i), dtype=np.float64)
+        dest_vol.info["scales"][i]["voxel_offset"] = intify(np.asarray(bounds.minpt) * f)
+        dest_vol.info["scales"][i]["size"] = intify(np.asarray(bounds.size3()) * f)
+    dest_vol.commit_info()
+  if len(dest_vol.scales) <= mip:  # cloudvolume's ScaleUnavailableError branch
+    dest_vol.scales.append(copy.deepcopy(src_vol.scales[mip]))
+    dest_vol.commit_info()
+  if bounds is None:
+    bounds = Bbox([0, 0, 0], [1, 1, 1], dtype=int)
+  if dest_voxel_offset is not None:
+    for i in range(mip + 1):
+      f = bounds_resolution / np.asarray(dest_vol.meta.resolution(i), dtype=np.float64)
+      dest_vol.info["scales"][i]["voxel_offset"] = intify((np.asarray(dest_voxel_offset) + np.asarray(bounds.minpt)) * f)
+  set_encoding(dest_vol, mip, encoding, encoding_level, encoding_effort)
+  if truncate_scales:
+    dest_vol.info["scales"] = dest_vol.info["scales"][:mip + 1]
+  dest_vol.info["scales"][mip]["chunk_sizes"] = [[int(v) for v in chunk_size]]
+  if clean_info:
+    dest_vol.info = clean_xfer_info(dest_vol.info)
+  return dest_vol
+
+
+def _select_compression_by_encoding(encoding):
+  if encoding.lower() in ("raw", "compressed_segmentation", "compresso", "crackle"):
+    return "gzip"
+  return False
+
+
+def _downsample_ratio(vol, mip):
+  return Vec(*(np.asarray(vol.meta.resolution(mip), dtype=np.float64)
+               / np.asarray(vol.meta.resolution(0), dtype=np.float64)).astype(int))
+
+
+def create_transfer_tasks(src_layer_path, dest_layer_path, chunk_size=None, shape=None, fill_missing=False,
+                          translate=None, bounds=None, mip=0, preserve_chunk_size=True, encoding=None,
+                          skip_downsamples=False, delete_black_uploads=False, background_color=0, agglomerate=False,
+                          timestamp=None, compress="auto", factor=None, sparse=False, dest_voxel_offset=None,
+                          memory_target=MEMORY_TARGET, max_mips=5, clean_info=False, no_src_update=False,
+                          bounds_mip=0, encoding_level=None, truncate_scales=True, cutout=False, stop_layer=None,
+                          downsample_method=DownsampleMethods.AUTO, encoding_effort=None, use_https_for_source=False):
+  """Transfer a layer to a new one, re-chunked, re-encoded, re-compressed, moved (translate,
+  dest_voxel_offset) or cropped (bounds, cutout), with its downsamples unless skip_downsamples
+  (task_creation/image.py:884-1133).  The task shape comes from memory_target unless `shape` is
+  given.  use_https_for_source is accepted and has no effect (file:// sources)."""
+  _refuse_transfer(encoding, compress, agglomerate, timestamp, stop_layer)
+  src_vol = CloudVolume(src_layer_path, mip=mip)
+  _refuse_layer_encodings(src_vol, dest_layer_path, mip, encoding)
+  no_src_update = no_src_update or use_https_for_source
+  if dest_voxel_offset:
+    dest_voxel_offset = Vec(*dest_voxel_offset, dtype=int)
+  if factor is None:
+    factor = (2, 2, 1)
+  if skip_downsamples:
+    factor = (1, 1, 1)
+  if not chunk_size:
+    chunk_size = src_vol.info["scales"][mip]["chunk_sizes"][0]
+  chunk_size = Vec(*chunk_size)
+  dest_vol = create_transfer_cloudvolume(src_vol, dest_layer_path, dest_voxel_offset, mip, bounds_mip, encoding,
+                                         encoding_level, encoding_effort, chunk_size, truncate_scales, clean_info,
+                                         cutout, bounds)
+  if compress == "auto":
+    compress = _select_compression_by_encoding(dest_vol.scales[mip]["encoding"])
+  if translate is None:
+    translate = dest_vol.meta.voxel_offset(mip) - src_vol.meta.voxel_offset(mip)
+  else:
+    translate = Vec(*translate) // _downsample_ratio(src_vol, mip)
+  if cutout:
+    dest_vol.scales[mip].pop("sharding", None)
+  dest_vol.commit_info()
+  dest_cs = dest_vol.meta.chunk_size(mip)
+  if shape is None:
+    if memory_target is None:
+      raise ValueError("Either shape or memory_target must be specified.")
+    shape = downsample_scales.downsample_shape_from_memory_target(
+      np.dtype(src_vol.dtype).itemsize * src_vol.num_channels, int(dest_cs[0]), int(dest_cs[1]), int(dest_cs[2]),
+      factor, memory_target, max_mips)
+  shape = Vec(*shape)
+  if factor[2] == 1:
+    shape.z = int(dest_cs[2] * max(round(shape.z / dest_cs[2]), 1))
+  if not skip_downsamples:
+    downsample_scales.create_downsample_scales(dest_layer_path, mip=mip, ds_shape=shape, factor=factor,
+                                               preserve_chunk_size=preserve_chunk_size, encoding=encoding)
+  if not cutout:
+    dest_bounds = get_bounds(dest_vol, bounds, mip, bounds_mip=bounds_mip, chunk_size=chunk_size)
+  else:
+    dest_bounds = dest_vol.bbox_to_mip(Bbox.create(bounds), mip=bounds_mip, to_mip=mip)
+    dest_bounds = Bbox.clamp(dest_bounds, dest_vol.meta.bounds(mip))
+
+  class TransferTaskIterator(FinelyDividedTaskIterator):
+    def task(self, shape, offset):
+      return partial(TransferTask, src_path=src_layer_path, dest_path=dest_layer_path, shape=shape.clone(),
+                     offset=offset.clone(), fill_missing=fill_missing, translate=translate, mip=mip,
+                     skip_downsamples=skip_downsamples, delete_black_uploads=bool(delete_black_uploads),
+                     background_color=background_color, agglomerate=agglomerate, timestamp=timestamp,
+                     compress=compress, factor=factor, sparse=sparse, stop_layer=stop_layer,
+                     downsample_method=int(downsample_method), use_https_for_source=use_https_for_source)
+
+    def on_finish(self):
+      job_details = {
+        "method": {
+          "task": "TransferTask", "src": src_layer_path, "dest": dest_layer_path,
+          "shape": list(map(int, shape)), "fill_missing": fill_missing, "translate": list(map(int, translate)),
+          "skip_downsamples": skip_downsamples, "delete_black_uploads": bool(delete_black_uploads),
+          "background_color": background_color,
+          "bounds": [dest_bounds.minpt.tolist(), dest_bounds.maxpt.tolist()],
+          "mip": mip, "agglomerate": bool(agglomerate), "timestamp": timestamp, "compress": compress,
+          "encoding": encoding, "memory_target": memory_target, "factor": (tuple(factor) if factor else None),
+          "sparse": bool(sparse), "encoding_level": encoding_level, "encoding_effort": encoding_effort,
+          "stop_layer": stop_layer, "downsample_method": int(downsample_method),
+          "use_https_for_source": bool(use_https_for_source),
+        },
+        "by": operator_contact(),
+        "date": strftime("%Y-%m-%d %H:%M %Z"),
+      }
+      dvol = CloudVolume(dest_layer_path)
+      dvol.provenance.sources = [src_layer_path]
+      dvol.provenance.processing.append(job_details)
+      dvol.commit_provenance()
+      if not no_src_update:
+        src_vol.provenance.processing.append(job_details)
+        src_vol.commit_provenance()
+
+  return TransferTaskIterator(dest_bounds, shape)
+
+
+def create_image_shard_transfer_tasks(src_layer_path, dst_layer_path, mip=0, chunk_size=None, encoding=None,
+                                      bounds=None, bounds_mip=0, fill_missing=False, translate=(0, 0, 0),
+                                      dest_voxel_offset=None, agglomerate=False, timestamp=None,
+                                      memory_target=MEMORY_TARGET, clean_info=False, encoding_level=None,
+                                      truncate_scales=True, compress="auto", cutout=False,
+                                      minishard_index_encoding="gzip", stop_layer=None, encoding_effort=None,
+                                      use_https_for_source=False):
+  """Copy a layer at `mip` into a sharded scale, one task per shard (task_creation/image.py:507-637).
+  use_https_for_source is accepted and has no effect (file:// sources)."""
+  _refuse_transfer(encoding, compress, agglomerate, timestamp, stop_layer)
+  if compress not in ("auto", True, "gzip", False, None):
+    raise ValueError("%s can only be True or 'gzip' for sharded images." % compress)
+  src_vol = CloudVolume(src_layer_path, mip=mip)
+  _refuse_layer_encodings(src_vol, dst_layer_path, mip, encoding)
+  if dest_voxel_offset:
+    dest_voxel_offset = Vec(*dest_voxel_offset, dtype=int)
+  if not chunk_size:
+    chunk_size = src_vol.info["scales"][mip]["chunk_sizes"][0]
+  chunk_size = Vec(*chunk_size)
+  dest_vol = create_transfer_cloudvolume(src_vol, dst_layer_path, dest_voxel_offset, mip, bounds_mip, encoding,
+                                         encoding_level, encoding_effort, chunk_size, truncate_scales, clean_info,
+                                         cutout, bounds)
+  if compress == "auto":
+    compress = _select_compression_by_encoding(dest_vol.scales[mip]["encoding"])
+  compress = compress in (True, "gzip")
+  if translate is None:
+    translate = dest_vol.meta.voxel_offset(mip) - src_vol.meta.voxel_offset(mip)
+  else:
+    translate = Vec(*translate) // _downsample_ratio(src_vol, mip)
+  scale = dest_vol.scales[mip]
+  spec = sharding.create_sharded_image_info(
+    dataset_size=scale["size"], chunk_size=scale["chunk_sizes"][0], encoding=scale["encoding"], dtype=dest_vol.dtype,
+    uncompressed_shard_bytesize=memory_target, data_encoding=("gzip" if compress else "raw"),
+    minishard_index_encoding=minishard_index_encoding)
+  scale["sharding"] = spec
+  if clean_info:
+    dest_vol.info = clean_xfer_info(dest_vol.info)
+  dest_vol.commit_info()
+  shape = shards.image_shard_shape_from_spec(spec, scale["size"], chunk_size)
+  if not cutout:
+    bounds = get_bounds(dest_vol, bounds, mip, bounds_mip=bounds_mip, chunk_size=chunk_size)
+  else:
+    bounds = dest_vol.bbox_to_mip(Bbox.create(bounds), mip=bounds_mip, to_mip=mip)
+    bounds = Bbox.clamp(bounds, dest_vol.meta.bounds(mip))
+  bounds = bounds.expand_to_chunk_size(shape, offset=bounds.minpt)
+
+  class ImageShardTransferTaskIterator(FinelyDividedTaskIterator):
+    def task(self, shape, offset):
+      return partial(ImageShardTransferTask, src_layer_path, dst_layer_path, shape=shape, offset=offset,
+                     fill_missing=fill_missing, translate=translate, mip=mip, agglomerate=agglomerate,
+                     timestamp=timestamp, stop_layer=stop_layer, use_https_for_source=bool(use_https_for_source))
+
+    def on_finish(self):
+      job_details = {
+        "method": {
+          "task": "ImageShardTransferTask", "src": src_layer_path, "dest": dst_layer_path,
+          "shape": list(map(int, shape)), "fill_missing": fill_missing, "translate": list(map(int, translate)),
+          "bounds": [bounds.minpt.tolist(), bounds.maxpt.tolist()], "mip": mip,
+          "encoding_level": encoding_level, "stop_layer": stop_layer, "encoding_effort": encoding_effort,
+          "timestamp": timestamp, "use_https_for_source": bool(use_https_for_source),
+        },
+        "by": operator_contact(),
+        "date": strftime("%Y-%m-%d %H:%M %Z"),
+      }
+      if not use_https_for_source:
+        dvol = CloudVolume(dst_layer_path)
+        dvol.provenance.sources = [src_layer_path]
+        dvol.provenance.processing.append(job_details)
+        dvol.commit_provenance()
+
+  return ImageShardTransferTaskIterator(bounds, shape)
 
 
 def _ccl_creator(task_fn, task_name, cloudpath, mip, shape, **opts):

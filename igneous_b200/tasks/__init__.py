@@ -1,4 +1,4 @@
-from .image import (DownsampleTask, TransferTask, ImageShardDownsampleTask, downsample_and_upload,
+from .image import (DownsampleTask, TransferTask, ImageShardTransferTask, ImageShardDownsampleTask, downsample_and_upload,
                     downsample_method_to_fn, QuantizeTask, CLAHETask, ContrastNormalizationTask,
                     LuminanceLevelsTask, CountVoxelsTask)
 from .ccl import (CCLFacesTask, CCLEquivalancesTask, RelabelCCLTask, create_relabeling,

@@ -2,7 +2,7 @@
 
 Same names, arguments and side effects as igneous/tasks/image/image.py:
   downsample_method_to_fn :37-55, downsample_and_upload :57-100,
-  TransferTask :434-516, DownsampleTask :518-549.
+  TransferTask :434-516, DownsampleTask :518-549, ImageShardTransferTask :595-670.
   ImageShardDownsampleTask :672-843, CountVoxelsTask :845-880.
   QuantizeTask :145-162, CLAHETask :164-209, ContrastNormalizationTask :211-343,
   LuminanceLevelsTask :345-432 (per-voxel work in igneous_b200.contrast).
@@ -20,7 +20,8 @@ from functools import partial
 import numpy as np
 
 from .. import contrast, downsample_scales, fastremap, sharding, shards, tinybrain
-from .._compat import CloudVolume, CloudFiles, Bbox, Vec, min2, queueable, RegisteredTask
+from .._compat import CloudVolume, CloudFiles, Bbox, EmptyVolumeException, Vec, min2, queueable, RegisteredTask
+from ..storage import DeviceCutout
 from ..types import DownsampleMethods
 
 
@@ -39,8 +40,20 @@ def downsample_method_to_fn(method, sparse, vol):
   return tinybrain.downsample_with_striding
 
 
+def _method_kind(method, vol):
+  """the pooling rule downsample_method_to_fn picks, by name (tinybrain.downsample_dev)"""
+  if method == DownsampleMethods.AUTO:
+    method = {"image": DownsampleMethods.AVERAGE_POOLING,
+              "segmentation": DownsampleMethods.MODE_POOLING}.get(vol.layer_type, DownsampleMethods.STRIDING)
+  return {DownsampleMethods.AVERAGE_POOLING: "average", DownsampleMethods.MODE_POOLING: "mode",
+          DownsampleMethods.MIN_POOLING: "min", DownsampleMethods.MAX_POOLING: "max"}.get(method, "striding")
+
+
 def downsample_and_upload(image, bounds, vol, ds_shape, mip=0, axis="z", skip_first=False,
                           sparse=False, factor=None, max_mips=None, method=DownsampleMethods.AUTO):
+  """Write `image` (a host array or a DeviceCutout) at `bounds` and its pyramid above it.  The image
+  goes to the device once; the mips are pooled, cut and encoded there (tinybrain.downsample_dev,
+  the layer's upload_dev)."""
   ds_shape = min2(vol.meta.volume_size(mip), Vec(*ds_shape[:3]))
   underlying = (mip + 1) if (mip + 1) in vol.available_mips else mip
   chunk = np.asarray(vol.meta.chunk_size(underlying), dtype=np.float32)
@@ -50,18 +63,20 @@ def downsample_and_upload(image, bounds, vol, ds_shape, mip=0, axis="z", skip_fi
   if max_mips is not None:
     factors = factors[:max_mips]
   vol.mip = mip
+  if not isinstance(image, DeviceCutout) and not (skip_first and not factors):
+    image = DeviceCutout.from_host(image)  # pooled in its own dtype, converted to the layer's on upload
   if not skip_first:
-    vol[bounds] = image
+    vol.upload_dev(bounds, image, mip=mip)
   if not factors:
     return
-  fn = downsample_method_to_fn(method, sparse, vol)
-  mips = fn(image, factors[0], num_mips=len(factors))  # <- the kernel call (image.py:91)
+  # <- the kernel call (image.py:91)
+  mips = tinybrain.downsample_dev(image, _method_kind(method, vol), factors[0], len(factors), sparse=bool(sparse))
   box = bounds.clone()
   for f3, mipped in zip(factors, mips):
     vol.mip += 1
     box //= f3
     box.maxpt = box.minpt + Vec(*mipped.shape[:3])
-    vol[box] = mipped
+    vol.upload_dev(box, mipped, mip=vol.mip)
 
 
 @queueable
@@ -76,13 +91,64 @@ def TransferTask(src_path, dest_path, mip, shape, offset, translate=(0, 0, 0), f
                      delete_black_uploads=bool(delete_black_uploads),
                      background_color=background_color, compress=compress)
   dst_box = Bbox.clamp(Bbox(offset, shape + offset), dest.meta.bounds(mip))
-  image = src.download(dst_box - translate)
+  if skip_downsamples and _same_chunks(src, dest, mip) and dest._sharding(mip) is None and not np.any(translate):
+    # the files are copied as they are (image.py:483-496)
+    src.image.transfer_to(dest_path, dst_box, mip, compress=compress)
+    return
+  image = src.download_dev(dst_box - translate)
   if skip_downsamples:
-    dest[dst_box] = image
+    dest.upload_dev(dst_box, image, mip=mip)
     return
   downsample_and_upload(image, dst_box, dest, shape, mip=mip, skip_first=bool(skip_first),
                         sparse=bool(sparse), axis=axis, factor=factor, max_mips=max_mips,
                         method=downsample_method)
+
+
+def _same_chunks(src, dest, mip):
+  """Can dest's chunk files at `mip` be src's files as they are?  The reference asks for the same
+  chunk size and dtype; the stand-in copies files without decoding them, so it also asks for the same
+  encoding (and its parameters), channel count and scale bounds: chunk names and the extent of the
+  edge chunks follow each scale's own bounds, so a cropped destination needs its chunks re-cut."""
+  a, b = src.scales[mip], dest.scales[mip]
+  keys = ("encoding", "compressed_segmentation_block_size", "jpeg_quality")
+  return (np.array_equal(src.meta.chunk_size(mip), dest.meta.chunk_size(mip)) and src.dtype == dest.dtype
+          and src.num_channels == dest.num_channels and all(a.get(k) == b.get(k) for k in keys)
+          and src.meta.bounds(mip) == dest.meta.bounds(mip))
+
+
+@queueable
+def ImageShardTransferTask(src_path, dst_path, shape, offset, mip=0, fill_missing=False, translate=(0, 0, 0),
+                           agglomerate=False, timestamp=None, stop_layer=None, use_https_for_source=False):
+  """One shard of a sharded copy of a layer at `mip`, without downsamples (image.py:595-670).  The
+  box is expanded to whole chunks; when it needs no translation and the two scales have the same
+  chunk grid and encoding, the source's encoded chunks go into the shard as they are, otherwise the cutout is built on the device
+  and its chunks encoded there.  The shard file is written once."""
+  if agglomerate or timestamp is not None or stop_layer is not None:
+    raise NotImplementedError("ImageShardTransferTask: agglomerate / timestamp / stop_layer need a graphene source")
+  shape, offset, translate = Vec(*shape), Vec(*offset), Vec(*translate)
+  mip = int(mip)
+  src = CloudVolume(src_path, fill_missing=bool(fill_missing), mip=mip, bounded=False)
+  dst = CloudVolume(dst_path, fill_missing=bool(fill_missing), mip=mip, compress=None)
+  dst_box = Bbox.clamp(Bbox(offset, offset + shape), dst.meta.bounds(mip))
+  dst_box = dst_box.expand_to_chunk_size(dst.meta.chunk_size(mip), offset=dst.meta.voxel_offset(mip))
+  src_box = dst_box - translate
+  if src_box == dst_box and _same_chunks(src, dst, mip):
+    shard_cache, chunks = {}, {}
+    for c in dst._chunks(mip, Bbox.clamp(dst_box, dst.meta.bounds(mip))):
+      data = src._read_chunk(mip, c, shard_cache)
+      if data is None:
+        if not fill_missing:
+          raise EmptyVolumeException(src._chunk_name(mip, c))
+        continue
+      chunks[dst._chunk_id(mip, c)] = data
+    if not chunks:
+      return
+    filename, shard = dst.image.make_shard(chunks, dst_box, mip)
+  else:
+    img = src.download_dev(src_box, mip=mip)
+    filename, shard = dst.image.make_shard(img, dst_box, mip)
+    del img
+  CloudFiles(dst.meta.join(dst.cloudpath, dst.meta.key(mip))).put(filename, shard, compress=None)
 
 
 @queueable

@@ -117,6 +117,51 @@ def _select(img, factor, num_mips, op, ctx):
   return [o[:, :, 0] for o in res] if img.ndim == 2 else res
 
 
+def downsample_dev(cutout, method, factor, num_mips, sparse=False, rounding=None, ctx=None):
+  """The pyramid of a device cutout ([x,y,z,c] F-order, storage.DeviceCutout) as a list of `num_mips`
+  device cutouts, computed where the cutout is.  method: "mode", "average", "min", "max" or
+  "striding"; the same kernels, rules and refusals as the host functions above."""
+  from .storage import DeviceCutout
+  num_mips = int(num_mips)
+  if num_mips < 1:
+    return []
+  ctx = ctx or _shim.default_context()
+  dt = np.dtype(cutout.dtype)
+  rounding = DEFAULT_ROUNDING if rounding is None else rounding
+  sx, sy, sz, nc = cutout.shape
+  if method == "average" and dt == np.uint64:
+    raise NotImplementedError("igneous_b200 averaging: uint64 images are not supported")
+  if _is_221(factor) and (method == "mode" or (method == "average" and not sparse)):
+    if method == "average":
+      _shim.require_unsigned(dt, "averaging")
+    outs = [DeviceCutout.empty(s + (nc,), dt, ctx) for s in _out_shapes((sx, sy, sz), num_mips)]
+    if cutout.size:
+      fn = ctx.lib.ign_pool_mode_2x2x1_dev if method == "mode" else ctx.lib.ign_pool_avg_2x2x1_dev
+      _shim.check(fn(ctx.handle, cutout.ptr, _shim.dtype_code(dt), sx, sy, sz * nc, num_mips,
+                     int(sparse) if method == "mode" else int(rounding), _shim.void_pp([o.buf.ptr for o in outs])))
+    return outs
+  op = {"min": _OP_MIN, "max": _OP_MAX, "striding": _OP_STRIDE,
+        "mode": _OP_MODE_SPARSE if sparse else _OP_MODE,
+        "average": (_OP_AVG_SPARSE if sparse else _OP_AVG) + int(rounding)}[method]
+  f = tuple(int(v) for v in factor)
+  if len(f) < 3 or any(v not in (1, 2) for v in f[:3]) or any(v != 1 for v in f[3:]):
+    raise NotImplementedError("igneous_b200 pooling: factors must be 1 or 2 per axis, got %r" % (factor,))
+  if op not in (_OP_STRIDE, _OP_MODE):
+    _shim.require_unsigned(dt, "min / max / average / sparse pooling")
+  shapes, shp = [], (sx, sy, sz)
+  for _ in range(num_mips):
+    shp = tuple((s + ff - 1) // ff for s, ff in zip(shp, f[:3]))
+    shapes.append(shp)
+  outs = [DeviceCutout.empty(s + (nc,), dt, ctx) for s in shapes]
+  if cutout.size:
+    for c in range(nc):  # one channel per call, as the host path does
+      ins = cutout.buf.ptr + c * sx * sy * sz * dt.itemsize
+      chans = [o.buf.ptr + c * int(np.prod(s)) * dt.itemsize for o, s in zip(outs, shapes)]
+      _shim.check(ctx.lib.ign_pool_select_dev(ctx.handle, ins, _shim.dtype_code(dt), sx, sy, sz, *f[:3], num_mips,
+                                              op, _shim.void_pp(chans)))
+  return outs
+
+
 def downsample_with_min_pooling(img, factor, num_mips=1, ctx=None):
   return _select(img, factor, num_mips, _OP_MIN, ctx)
 

@@ -611,6 +611,44 @@ IGN_API int ign_cseg_decode_dev(ign_ctx* ctx, const uint32_t* in, uint64_t n_wor
                                 uint64_t sy, uint64_t sz, uint64_t sc, uint32_t bx, uint32_t by,
                                 uint32_t bz, void* out);
 
+/* Batches of chunks (the read and write paths of a layer, one call per cutout).  Chunk i is an F-order
+ * [sx, sy, sz, sc] array, shapes[3*i .. 3*i+2] (host) = {sx, sy, sz}; chunks and decoded outputs are
+ * packed back to back in the order given.
+ * encode: writes the n files back to back into out (device); offsets (device, n + 1 words) delimit file
+ * i as out[offsets[i] : offsets[i+1]] in words; *n_words = words of all files.  One size pass for the
+ * whole batch; when the files need more than cap_words words nothing is written and the call fails
+ * with IGN_ERR_OVERFLOW (*n_words still reports the need).  Every file is byte-identical to what
+ * ign_cseg_encode writes for that chunk alone.
+ * decode: stream i is streams[word_offsets[i] : word_offsets[i+1]] (word_offsets on the host); a
+ * malformed stream fails the call with IGN_ERR_INVALID, and the message names the first such index. */
+IGN_API int ign_cseg_encode_batch_dev(ign_ctx* ctx, const void* chunks, int dtype, uint64_t n_chunks,
+                                      const uint32_t* shapes, uint64_t sc, uint32_t bx, uint32_t by, uint32_t bz,
+                                      uint32_t* out, uint64_t cap_words, uint64_t* offsets, uint64_t* n_words);
+IGN_API int ign_cseg_decode_batch_dev(ign_ctx* ctx, const uint32_t* streams, const uint64_t* word_offsets,
+                                      uint64_t n_streams, int dtype, const uint32_t* shapes, uint64_t sc,
+                                      uint32_t bx, uint32_t by, uint32_t bz, void* out);
+
+/* ------------------------------------------------------------- chunk placement
+ * The storage layer's cutouts stay on the device between decode, pooling and encode.
+ * ign_chunks_place_dev: one launch copies many decoded chunks (packed, device) into one F-order
+ * [X, Y, Z, nc] device cutout.  rows (host) holds n_rows rows of IGN_PLACE_ROW uint64 words:
+ *   {sx, sy, sz, byte offset of the chunk in packed, x0, y0, z0, bx, by, bz, dx, dy, dz}
+ * copying the chunk's sub-box [x0, x0+bx) x [y0, y0+by) x [z0, z0+bz) (every channel) to the cutout
+ * at (dx, dy, dz).  Rows must write disjoint boxes; voxels no row covers keep their values.
+ * ign_chunks_cut_dev: the reverse.  rows (host): n_rows rows of IGN_CUT_ROW words
+ *   {x0, y0, z0, bx, by, bz, byte offset in packed}
+ * box r of the cutout (every channel) is written F-order contiguous at its offset -- a `raw` chunk
+ * file byte for byte; all_bg[r] (device) is non-zero when every value of the box equals `background`
+ * (the value's bit pattern, zero-extended; float32 boxes compare as floats).
+ * dtype: IGN_U8 / U16 / U32 / U64 / F32.  64-bit indexing throughout. */
+#define IGN_PLACE_ROW 13
+#define IGN_CUT_ROW 7
+IGN_API int ign_chunks_place_dev(ign_ctx* ctx, const void* packed, int dtype, uint64_t nc, const uint64_t* rows,
+                                 uint64_t n_rows, void* cutout, uint64_t X, uint64_t Y, uint64_t Z);
+IGN_API int ign_chunks_cut_dev(ign_ctx* ctx, const void* cutout, int dtype, uint64_t X, uint64_t Y, uint64_t Z,
+                               uint64_t nc, const uint64_t* rows, uint64_t n_rows, uint64_t background,
+                               void* packed, uint32_t* all_bg);
+
 /* ------------------------------------------------------------------ jpeg codec
  * The Precomputed `jpeg` chunk encoding of uint8 image layers, which CloudVolume applies on the host
  * around the image tasks (igneous/tasks/image/image.py:95-100 uploads; the CLI's image encoding,
