@@ -16,7 +16,8 @@ _TASK_NAMES = ("DownsampleTask", "TransferTask", "ImageShardTransferTask", "Imag
                "create_relabeling", "clean_intermediate_files", "MeshTask", "downsample_and_upload",
                "downsample_method_to_fn", "threshold_image", "blackout_non_face_rails", "DisjointSet",
                "QuantizeTask", "CLAHETask", "ContrastNormalizationTask", "LuminanceLevelsTask",
-               "SpatialIndexTask", "CountVoxelsTask", "SkeletonTask", "UnshardedSkeletonMergeTask")
+               "SpatialIndexTask", "CountVoxelsTask", "SkeletonTask", "UnshardedSkeletonMergeTask",
+               "BlackoutTask", "TouchTask", "DeleteTask")
 _COMPAT_NAMES = ("CloudVolume", "EmptyVolumeException", "LocalTaskQueue", "RegisteredTask", "queueable")
 __all__ = ["Mesher", "__version__"] + list(_TASK_NAMES) + list(_COMPAT_NAMES)
 

@@ -5,8 +5,11 @@
 // its corner of the F-order [X, Y, Z, nc] cutout.  The write path is the reverse: `cut` copies a
 // list of boxes of the cutout into one packed buffer, each box F-order contiguous -- a `raw` chunk
 // file byte for byte, and what the batch encoders read -- and flags the boxes that hold only the
-// background value.  All indexing is 64-bit: a 2048 x 2048 x 128 uint64 cutout is 4.3 GB.
+// background value.  `fill_box` sets one box of a cutout to one value (BlackoutTask).  All indexing is
+// 64-bit: a 2048 x 2048 x 128 uint64 cutout is 4.3 GB.
 #include <string.h>
+
+#include <algorithm>
 
 #include "common.cuh"
 
@@ -62,12 +65,15 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-// f(T{}) with T the element type of dtype: the label types, and float for IGN_F32 (whose background
-// test then follows float equality, as numpy's does)
-template <typename F>
-static int dispatch_chunk(int dtype, const char* who, F&& f) {
-  if (dtype == IGN_F32) return f(float{});
-  return dispatch_label(dtype, who, f);
+// every voxel of one box of the cutout, every channel, set to v
+template <typename T>
+__global__ void __launch_bounds__(256)
+    k_fill_box(T* __restrict__ out, uint64_t X, uint64_t Y, uint64_t Z, uint64_t x0, uint64_t y0, uint64_t z0,
+               uint64_t bx, uint64_t by, uint64_t bz, uint64_t n, T v) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t x = i % bx, y = (i / bx) % by, q = i / (bx * by), z = q % bz, c = q / bz;
+    out[(x0 + x) + X * ((y0 + y) + Y * ((z0 + z) + Z * c))] = v;
+  }
 }
 
 // the background as a T: `bits` holds the value's own bit pattern, zero-extended
@@ -145,6 +151,25 @@ int ign_chunks_cut_dev(ign_ctx* ctx, const void* cutout, int dtype, uint64_t X, 
     using T = decltype(t);
     IGN_LAUNCH(ctx, k_chunks_cut<T>, g, 256, 0, (const T*)cutout, X, Y, Z, nc, (const CutRow*)dr, n_rows,
                bg_value<T>(background), (char*)packed, all_bg);
+    return IGN_OK;
+  });
+}
+
+int ign_fill_box_dev(ign_ctx* ctx, void* cutout, int dtype, uint64_t X, uint64_t Y, uint64_t Z, uint64_t nc,
+                     uint64_t x0, uint64_t y0, uint64_t z0, uint64_t bx, uint64_t by, uint64_t bz, uint64_t value) {
+  IGN_TRY(activate(ctx));
+  IGN_REQUIRE(x0 <= X && bx <= X - x0 && y0 <= Y && by <= Y - y0 && z0 <= Z && bz <= Z - z0, IGN_ERR_INVALID,
+              "fill_box: box (%llu, %llu, %llu) + (%llu, %llu, %llu) lies outside the %llu x %llu x %llu cutout",
+              (unsigned long long)x0, (unsigned long long)y0, (unsigned long long)z0, (unsigned long long)bx,
+              (unsigned long long)by, (unsigned long long)bz, (unsigned long long)X, (unsigned long long)Y,
+              (unsigned long long)Z);
+  const uint64_t n = bx * by * bz * nc;
+  IGN_REQUIRE(n == 0 || cutout, IGN_ERR_INVALID, "fill_box: null cutout");
+  return dispatch_chunk(dtype, "fill_box", [&](auto t) -> int {
+    using T = decltype(t);
+    if (n == 0) return IGN_OK;
+    const unsigned grid = (unsigned)std::min<uint64_t>(blocks_for(n, 256), (uint64_t)ctx->sm_count * 32);
+    IGN_LAUNCH(ctx, k_fill_box<T>, grid, 256, 0, (T*)cutout, X, Y, Z, x0, y0, z0, bx, by, bz, n, bg_value<T>(value));
     return IGN_OK;
   });
 }

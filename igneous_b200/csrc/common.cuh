@@ -65,6 +65,14 @@ int dispatch_label(int dtype, const char* who, F&& f) {
   return IGN_ERR_UNSUPPORTED;
 }
 
+// f(T{}) with T the element type of dtype: the label types, and float for IGN_F32 (whose comparisons
+// then follow float rules, as numpy's do)
+template <typename F>
+int dispatch_chunk(int dtype, const char* who, F&& f) {
+  if (dtype == IGN_F32) return f(float{});
+  return dispatch_label(dtype, who, f);
+}
+
 }  // namespace ign
 
 constexpr int IGN_TIMER_SLOTS = 64;  // CUDA event pairs per context: timers and cross-stream marks

@@ -152,6 +152,14 @@ class Bbox:
   def astype(self, dtype):
     return Bbox(self.minpt.astype(dtype), self.maxpt.astype(dtype), dtype=dtype)
 
+  def round_to_chunk_size(self, chunk_size, offset=(0, 0, 0)):
+    """minpt and maxpt each moved to the nearest chunk boundary (cloudvolume's rule as recalled: np.round
+    of the chunk count, computed in float64, so a half goes to the even multiple)"""
+    cs, off = np.asarray(chunk_size, dtype=np.float64)[:3], np.asarray(offset)[:3]
+    lo = np.round((self.minpt - off) / cs) * cs + off
+    hi = np.round((self.maxpt - off) / cs) * cs + off
+    return Bbox(lo.astype(int), hi.astype(int))
+
   def expand_to_chunk_size(self, chunk_size, offset=(0, 0, 0)):
     cs, off = np.asarray(chunk_size)[:3], np.asarray(offset)[:3]
     lo = np.floor((self.minpt - off) / cs) * cs + off
@@ -223,6 +231,15 @@ class DeviceCutout:
   @property
   def nbytes(self):
     return self.size * self.dtype.itemsize
+
+  def fill(self, box, value):
+    """Set every voxel of `box` (a Bbox relative to the cutout), every channel, to `value` on the device."""
+    from . import _shim
+    bits = np.asarray(value).astype(self.dtype).reshape(1).view(np.dtype("u%d" % self.dtype.itemsize))[0]
+    X, Y, Z, nc = self.shape
+    _shim.check(self.ctx.lib.ign_fill_box_dev(self.ctx.handle, self.ptr, _shim.dtype_code(self.dtype), X, Y, Z, nc,
+                                              *(int(v) for v in box.minpt), *(int(v) for v in box.size3()),
+                                              int(bits)))
 
   def to_host(self):
     out = np.empty(self.shape, dtype=self.dtype, order="F")
@@ -440,6 +457,9 @@ class _Meta:
   def bounds(self, mip):
     return self._cv.bounds_at(mip)
 
+  def voxels(self, mip):
+    return self._cv.volume_size_at(mip).rectVolume()
+
   def add_resolution(self, *args, **kwargs):
     return self._cv.add_resolution(*args, **kwargs)
 
@@ -531,7 +551,8 @@ class CloudVolume:
   """file:// Precomputed subset of cloudvolume.CloudVolume."""
 
   def __init__(self, cloudpath, mip=0, fill_missing=False, bounded=True, info=None, compress="gzip",
-               delete_black_uploads=False, background_color=0, parallel=1, progress=False, **kwargs):
+               delete_black_uploads=False, background_color=0, parallel=1, progress=False, non_aligned_writes=False,
+               **kwargs):
     self.cloudpath = cloudpath
     self.path = _strip(cloudpath)
     self.fill_missing = bool(fill_missing)
@@ -539,6 +560,7 @@ class CloudVolume:
     self.compress = compress
     self.delete_black_uploads = delete_black_uploads
     self.background_color = background_color
+    self.non_aligned_writes = bool(non_aligned_writes)
     self.cf = CloudFiles(cloudpath)
     self.provenance = _Provenance()
     self.mesh = _MeshMeta()
@@ -638,6 +660,9 @@ class CloudVolume:
 
   # current-mip properties, as on cloudvolume.CloudVolume
   resolution = property(lambda self: self.resolution_at(self._mip))
+  downsample_ratio = property(lambda self: Vec(*(np.asarray(self.resolution_at(self._mip), dtype=np.float64)
+                                                 / np.asarray(self.resolution_at(0), dtype=np.float64)),
+                                               dtype=np.float64))
   chunk_size = property(lambda self: self.chunk_size_at(self._mip))
   volume_size = property(lambda self: self.volume_size_at(self._mip))
   voxel_offset = property(lambda self: self.voxel_offset_at(self._mip))
@@ -904,9 +929,11 @@ class CloudVolume:
       out[tuple(slice(d, d + z) for d, z in zip(dst, size))] = chunk[tuple(slice(a, a + z) for a, z in zip(src, size))]
     return out
 
-  def _pieces(self, bbox, mip):
+  def _pieces(self, bbox, mip, fill_missing=None):
     """(bbox, the chunk files under it) for a read: (chunk shape, file bytes, corner in the chunk, box size,
-    corner in the cutout) per chunk that is present; a missing chunk raises unless fill_missing"""
+    corner in the cutout) per chunk that is present; a missing chunk raises unless fill_missing (None: the
+    volume's setting)"""
+    fill_missing = self.fill_missing if fill_missing is None else fill_missing
     bbox = self._to_bbox(bbox)
     if self.bounded and not (np.all(bbox.minpt >= self.bounds_at(mip).minpt) and np.all(bbox.maxpt <= self.bounds_at(mip).maxpt)):
       raise OutOfBoundsError("%r is outside %r" % (bbox, self.bounds_at(mip)))
@@ -918,20 +945,20 @@ class CloudVolume:
       if inter.subvoxel():
         continue
       if data is None:
-        if not self.fill_missing:
+        if not fill_missing:
           raise EmptyVolumeException(self._chunk_name(mip, c))
         continue
       pieces.append(([int(v) for v in c.size3()], data, [int(v) for v in inter.minpt - c.minpt],
                      [int(v) for v in inter.size3()], [int(v) for v in inter.minpt - bbox.minpt]))
     return bbox, pieces
 
-  def download_dev(self, bbox, mip=None, ctx=None):
+  def download_dev(self, bbox, mip=None, ctx=None, fill_missing=None):
     """Cutout as a DeviceCutout: the chunk files are read (unsharded files or shard reads), sent to
     the device in one copy, decoded in one batched call and placed in one launch.  Voxels outside
-    the volume, and missing chunks under fill_missing, are 0."""
+    the volume, and missing chunks under fill_missing (None: the volume's setting), are 0."""
     from . import _shim
     mip = self._mip if mip is None else mip
-    bbox, pieces = self._pieces(bbox, mip)
+    bbox, pieces = self._pieces(bbox, mip, fill_missing)
     ctx = ctx or _shim.default_context()
     out = DeviceCutout.empty(tuple(int(v) for v in bbox.size3()) + (self.num_channels,), self.dtype, ctx)
     ctx.memset(out.buf, 0, out.nbytes)
@@ -944,10 +971,28 @@ class CloudVolume:
   def __setitem__(self, key, img):
     self.upload_dev(self._to_bbox(key), img, mip=self._mip)
 
+  def _write_region(self, bbox, mip):
+    """The chunk-aligned region a write of `bbox` at `mip` covers: bbox itself when it is chunk aligned;
+    otherwise, under non_aligned_writes, bbox expanded to the chunk grid and clamped to the bounds, and
+    without it a ValueError."""
+    for c in self._chunks(mip, bbox):
+      inter = Bbox.intersection(c, bbox)
+      if inter.subvoxel() or inter == c:
+        continue
+      if not self.non_aligned_writes:
+        raise ValueError("writes must be chunk aligned: %r vs chunk %r" % (bbox, c))
+      vb = self.bounds_at(mip)
+      if not (np.all(bbox.minpt >= vb.minpt) and np.all(bbox.maxpt <= vb.maxpt)):
+        raise OutOfBoundsError("a non-aligned write of %r reaches outside %r" % (bbox, vb))
+      return Bbox.clamp(bbox.expand_to_chunk_size(self.chunk_size_at(mip), self.voxel_offset_at(mip)), vb)
+    return bbox
+
   def upload_dev(self, bbox, img, mip=None):
-    """Write a chunk-aligned cutout (a DeviceCutout, or a host array that is sent over first): one
-    cut, one batched encode and one D2H, then one file per chunk.  Under delete_black_uploads the
-    chunks that hold only background_color are deleted instead."""
+    """Write a cutout (a DeviceCutout, or a host array that is sent over first): one cut, one batched
+    encode and one D2H, then one file per chunk.  Under delete_black_uploads the chunks that hold only
+    background_color are deleted instead.  A box off the chunk grid raises ValueError unless
+    non_aligned_writes is set; then the chunk-aligned region around it is read (missing chunks as 0),
+    the cutout is placed into it on the device and the region is written."""
     mip = self._mip if mip is None else mip
     bbox = self._to_bbox(bbox)
     shape = img.shape if isinstance(img, DeviceCutout) else np.shape(img)
@@ -955,14 +1000,10 @@ class CloudVolume:
       raise ValueError("image %r does not fit %r" % (tuple(shape), bbox))
     if self._sharding(mip) is not None:
       raise NotImplementedError("writes to a sharded scale go through image.make_shard (whole shards only)")
-    boxes = []
-    for c in self._chunks(mip, bbox):
-      inter = Bbox.intersection(c, bbox)
-      if inter.subvoxel():
-        continue
-      if not (inter == c):
-        raise ValueError("writes must be chunk aligned: %r vs chunk %r" % (bbox, c))
-      boxes.append(c)
+    region = self._write_region(bbox, mip)
+    if not (region == bbox):
+      img, bbox = self._placed(img, bbox, region, mip), region
+    boxes = [c for c in self._chunks(mip, bbox) if not Bbox.intersection(c, bbox).subvoxel()]
     files, black = self._chunk_files(img, [c - bbox.minpt for c in boxes], mip)
     # jpeg files are already entropy coded: stored without gzip, as CloudVolume stores jpeg chunks
     compress = None if self._encoding(mip) == "jpeg" else self.compress
@@ -972,6 +1013,27 @@ class CloudVolume:
         self.cf.delete(name)
         continue
       self.cf.put(name, data, compress=compress)
+
+  def _placed(self, img, bbox, region, mip):
+    """`region` read from the layer (missing chunks as 0) with img placed at bbox, as a DeviceCutout"""
+    from . import _shim
+    src = self._device_cutout(img)
+    out = self.download_dev(region, mip=mip, ctx=src.ctx, fill_missing=True)
+    X, Y, Z, nc = out.shape
+    size = [int(v) for v in bbox.size3()]
+    row = np.array(size + [0, 0, 0, 0] + size + [int(v) for v in bbox.minpt - region.minpt], dtype=np.uint64)
+    _shim.check(out.ctx.lib.ign_chunks_place_dev(out.ctx.handle, src.ptr, _shim.dtype_code(out.dtype), nc,
+                                                 _shim.ptr(row), 1, out.ptr, X, Y, Z))
+    return out
+
+  def delete(self, bbox, mip=None):
+    """Delete the chunk files at `mip` that lie wholly inside `bbox` (cloudvolume's delete)."""
+    mip = self._mip if mip is None else mip
+    if self._sharding(mip) is not None:
+      raise NotImplementedError("deleting from a sharded scale would rewrite whole shards; only unsharded "
+                                "scales are supported")
+    bbox = self._to_bbox(bbox)
+    self.cf.delete([self._chunk_name(mip, c) for c in self._chunks(mip, bbox) if Bbox.intersection(c, bbox) == c])
 
 
 # --------------------------------------------------------------------- queue

@@ -1,7 +1,8 @@
 """create_downsampling_tasks, create_image_shard_downsample_tasks, the transfer creators, the
-contrast / CLAHE / quantize creators, the three CCL task creators and create_voxel_counting_tasks
-(igneous/task_creation/image.py:170-345, 507-637, 639-770, 815-1133, 1247-1618, 1726-1936): same
-signatures, same info / provenance side effects, tasks from igneous_b200.tasks."""
+contrast / CLAHE / quantize creators, the three CCL task creators, create_voxel_counting_tasks, the
+blackout / touch / deletion creators and compute_rois (igneous/task_creation/image.py:76-171, 170-345,
+507-637, 639-770, 772-813, 815-1133, 1247-1618, 1726-1936, 1995-2058): same signatures, same info /
+provenance side effects, tasks from igneous_b200.tasks."""
 import copy
 import math
 from functools import partial, reduce
@@ -9,10 +10,12 @@ from time import strftime
 
 import numpy as np
 
-from .. import downsample_scales, fastremap, sharding, shards
+from .. import _shim, downsample_scales, fastremap, rois, sharding, shards, tinybrain
 from .._compat import Bbox, CloudVolume, CloudFiles, InfoUnavailableError, Vec, min2
 from ..tasks import (DownsampleTask, TransferTask, ImageShardTransferTask, ImageShardDownsampleTask, CCLFacesTask, CCLEquivalancesTask, RelabelCCLTask,
-                     QuantizeTask, CLAHETask, ContrastNormalizationTask, LuminanceLevelsTask, CountVoxelsTask)
+                     QuantizeTask, CLAHETask, ContrastNormalizationTask, LuminanceLevelsTask, CountVoxelsTask,
+                     BlackoutTask, TouchTask, DeleteTask)
+from ..tasks.image import layer_value, refuse_sharded
 from ..types import DownsampleMethods
 from .common import FinelyDividedTaskIterator, get_bounds, operator_contact
 
@@ -673,3 +676,150 @@ def create_voxel_counting_tasks(cloudpath, mip, fill_missing=False, agglomerate=
            shape=shape.tolist(), fill_missing=fill_missing, agglomerate=agglomerate, timestamp=timestamp)
 
   return CountVoxelsTaskIterator(bounds, shape)
+
+
+# ------------------------------------------------------------ blackout, touch, delete, rois
+# task_creation/image.py:76-171, 772-813 and 1995-2058.
+
+def create_blackout_tasks(cloudpath, bounds, mip=0, shape=(2048, 2048, 64), value=0, non_aligned_writes=False):
+  """Paint `bounds` (given at mip 0) with `value` at `mip` (task_creation/image.py:76-123).  The bounds are
+  moved to `mip`, expanded to the chunk grid unless non_aligned_writes, and clamped to the mip's bounds.
+  A value the dtype cannot hold raises ValueError and a sharded scale NotImplementedError, before any task.
+  As in the reference, on_finish appends the provenance entry to the volume in memory and does not commit
+  it: the layer's provenance file is left as it was, so a run leaves the same files as the reference's."""
+  vol = CloudVolume(cloudpath, mip=mip)
+  layer_value(vol.dtype, value)
+  refuse_sharded(vol, [mip], "create_blackout_tasks")
+  shape = Vec(*shape)
+  bounds = Bbox.create(bounds)
+  bounds = vol.bbox_to_mip(bounds, mip=0, to_mip=mip)
+  if not non_aligned_writes:
+    bounds = bounds.expand_to_chunk_size(vol.chunk_size, vol.voxel_offset)
+  bounds = Bbox.clamp(bounds, vol.mip_bounds(mip))
+
+  class BlackoutTaskIterator(FinelyDividedTaskIterator):
+    def task(self, shape, offset):
+      return partial(BlackoutTask, cloudpath=cloudpath, mip=mip, shape=shape.clone(), offset=offset.clone(),
+                     value=value, non_aligned_writes=non_aligned_writes)
+
+    def on_finish(self):
+      vol.provenance.processing.append({
+        "method": {"task": "BlackoutTask", "cloudpath": cloudpath, "mip": mip,
+                   "non_aligned_writes": non_aligned_writes, "value": value, "shape": shape.tolist(),
+                   "bounds": [bounds.minpt.tolist(), bounds.maxpt.tolist()]},
+        "by": operator_contact(), "date": strftime("%Y-%m-%d %H:%M %Z")})
+
+  return BlackoutTaskIterator(bounds, shape)
+
+
+def create_touch_tasks(cloudpath, mip=0, shape=(2048, 2048, 64), bounds=None):
+  """Read every chunk of a layer at `mip` to find missing or corrupt files (task_creation/image.py:125-171).
+  As in the reference `bounds` is read at mip 0 and moved to `mip`, the default (the volume's bounds at
+  `mip`) included, and each task's shape is clamped to the volume's far edge."""
+  vol = CloudVolume(cloudpath, mip=mip)
+  shape = Vec(*shape)
+  if bounds is None:
+    bounds = vol.bounds.clone()
+  bounds = Bbox.create(bounds)
+  bounds = vol.bbox_to_mip(bounds, mip=0, to_mip=mip)
+  bounds = Bbox.clamp(bounds, vol.mip_bounds(mip))
+
+  class TouchTaskIterator(FinelyDividedTaskIterator):
+    def task(self, shape, offset):
+      bounded_shape = min2(shape, vol.bounds.maxpt - offset)
+      return partial(TouchTask, cloudpath=cloudpath, shape=bounded_shape.clone(), offset=offset.clone(), mip=mip)
+
+    def on_finish(self):
+      vol.provenance.processing.append({
+        "method": {"task": "TouchTask", "mip": mip, "shape": shape.tolist(),
+                   "bounds": [bounds.minpt.tolist(), bounds.maxpt.tolist()]},
+        "by": operator_contact(), "date": strftime("%Y-%m-%d %H:%M %Z")})
+      vol.commit_provenance()
+
+  return TouchTaskIterator(bounds, shape)
+
+
+def create_deletion_tasks(layer_path, mip=0, num_mips=5, shape=None, bounds=None):
+  """Delete a layer's chunks from `mip` up through mip + num_mips (`igneous image rm`,
+  task_creation/image.py:772-813).  The default shape is the chunk size at `mip` times 2^num_mips in x
+  and y; `bounds` (a Bbox at `mip`, default its bounds) is used as given, and each task's shape is
+  clamped to it.  A sharded scale in that range raises NotImplementedError before any task."""
+  vol = CloudVolume(layer_path, max_redirects=0)
+  refuse_sharded(vol, range(mip, min(vol.available_mips[-1], mip + num_mips) + 1), "create_deletion_tasks")
+  if shape is None:
+    shape = vol.meta.chunk_size(mip)[:3]
+    shape.x *= 2 ** num_mips
+    shape.y *= 2 ** num_mips
+  else:
+    shape = Vec(*shape)
+  if not bounds:
+    bounds = vol.mip_bounds(mip).clone()
+
+  class DeleteTaskIterator(FinelyDividedTaskIterator):
+    def task(self, shape, offset):
+      bounded_shape = min2(shape, bounds.maxpt - offset)
+      return partial(DeleteTask, layer_path=layer_path, shape=bounded_shape.clone(), offset=offset.clone(),
+                     mip=mip, num_mips=num_mips)
+
+    def on_finish(self):
+      pvol = CloudVolume(layer_path, max_redirects=0)
+      pvol.provenance.processing.append({
+        "method": {"task": "DeleteTask", "mip": mip, "num_mips": num_mips, "shape": shape.tolist()},
+        "by": operator_contact(), "date": strftime("%Y-%m-%d %H:%M %Z")})
+      pvol.commit_provenance()
+
+  return DeleteTaskIterator(bounds, shape)
+
+
+def compute_rois(cloudpath, progress=False, suppress_faint_voxels=0, dust_threshold=10, max_axial_length=512,
+                 z_step=None):
+  """The bounding boxes of the non-empty parts of a layer, recorded in info["scales"][0]["rois"] and
+  returned (`igneous image roi`, task_creation/image.py:1995-2058); the rules are DESIGN.md §5k's.
+  The top mip is read in z slabs of z_step (default: all of z) with missing chunks as 0.  A slab whose xy
+  area exceeds max_axial_length^2 is pooled by (2, 2, 1) ceil(log2(area / max_axial_length^2)) times
+  (averaging, mode pooling for segmentation), thresholded (> suppress_faint_voxels) and split into
+  26-connected components, those of fewer than dust_threshold voxels dropped; each box, in the order of
+  its component's first voxel, is scaled by the downsample ratio (and 2^pooled mips in x and y), shifted
+  by the slab's z and has 1 taken off its maximum.  All of that runs on the device and only the boxes come
+  back.  Signed integer layers raise NotImplementedError before anything is read.  The reference's
+  quirks are kept: the boxes are relative to the top mip's cutout in x and y (its
+  voxel offset is not added), the slab's z is added at the top mip's scale after the scaling, and a top
+  mip of more than 8e9 voxels prints a warning."""
+  cv = CloudVolume(cloudpath, progress=progress, fill_missing=True)
+  _shim.require_unsigned(cv.dtype, "compute_rois")  # the threshold kernel compares unsigned
+  cv.mip = len(cv.scales) - 1  # the reference sets the top scale's resolution, which names this mip
+  cv.meta.rois = None
+  if cv.meta.voxels(cv.mip) > int(8e9):
+    print("Warning: lowest resolution is larger than 8 gigavoxels. Consider additional downsampling.")
+  bounds = cv.bounds
+  if z_step is None:
+    z_step = bounds.size3()[2]
+  more_mips = 0
+  max_size = max_axial_length ** 2
+  bboxes = []
+  method = "mode" if cv.layer_type == "segmentation" else "average"
+  for z in range(int(bounds.minpt.z), int(bounds.maxpt.z), int(z_step)):
+    upper = min(z + int(z_step), int(bounds.maxpt.z))
+    slab = Bbox((bounds.minpt.x, bounds.minpt.y, z), (bounds.maxpt.x, bounds.maxpt.y, upper))
+    img = rois.channel0(cv.download_dev(slab, mip=cv.mip))
+    sxy = img.shape[0] * img.shape[1]
+    if sxy > max_size:
+      more_mips = int(np.ceil(np.log2(sxy / max_size)))
+      if more_mips > 0:
+        img = tinybrain.downsample_dev(img, method, (2, 2, 1), more_mips)[-1]
+      else:
+        more_mips = 0
+    boxes = rois.component_boxes_dev(rois.threshold_dev(img, suppress_faint_voxels), dust_threshold)
+    del img
+    factor3 = cv.downsample_ratio
+    factor3.x *= 2 ** more_mips
+    factor3.y *= 2 ** more_mips
+    for row in boxes:
+      bbx = Bbox(row[1:4].astype(np.int64), row[4:7].astype(np.int64) + 1) * factor3
+      bbx.minpt.z += z
+      bbx.maxpt.z += z
+      bbx.maxpt -= 1
+      bboxes.append(bbx.astype(int))
+  cv.scales[0]["rois"] = [bbx.to_list() for bbx in bboxes]
+  cv.commit_info()
+  return bboxes

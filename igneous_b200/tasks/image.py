@@ -1,9 +1,10 @@
-"""DownsampleTask / TransferTask with the pooling done on the GPU.
+"""DownsampleTask / TransferTask with the pooling done on the GPU, and the other image tasks.
 
 Same names, arguments and side effects as igneous/tasks/image/image.py:
   downsample_method_to_fn :37-55, downsample_and_upload :57-100,
   TransferTask :434-516, DownsampleTask :518-549, ImageShardTransferTask :595-670.
   ImageShardDownsampleTask :672-843, CountVoxelsTask :845-880.
+  DeleteTask :103-122, BlackoutTask :124-135, TouchTask :137-143.
   QuantizeTask :145-162, CLAHETask :164-209, ContrastNormalizationTask :211-343,
   LuminanceLevelsTask :345-432 (per-voxel work in igneous_b200.contrast).
 Only the library behind `fn(image, factors[0], num_mips=...)` (:91) changes:
@@ -275,6 +276,93 @@ def CountVoxelsTask(cloudpath, shape, offset, mip=0, fill_missing=False, agglome
   voxel_counts = {str(int(segid)): int(ct) for segid, ct in zip(uniq, cts)}
   cf = CloudFiles(cloudpath)
   cf.put_json(cf.join(cv.key, "stats", "voxel_counts", "%s.json" % bbox.to_filename()), voxel_counts)
+
+
+# ------------------------------------------------------------ blackout, touch, delete
+# image.py:103-143: edit and check a layer in place.
+
+def layer_value(dtype, value):
+  """`value` as a scalar of the layer's dtype; a value the dtype cannot hold (out of range, a fraction for
+  an integer dtype, a finite number that overflows float32) raises ValueError."""
+  dt = np.dtype(dtype)
+  if dt.kind in "ui":
+    try:
+      iv = int(value)
+      exact = iv == value
+    except (TypeError, ValueError, OverflowError):
+      exact = False
+    if not exact or not (np.iinfo(dt).min <= iv <= np.iinfo(dt).max):
+      raise ValueError("%r is not a %s value" % (value, dt))
+    return dt.type(iv)
+  with np.errstate(over="ignore"):
+    typed = dt.type(value)
+  if math.isfinite(float(value)) and not np.isfinite(typed):
+    raise ValueError("%r is not a %s value" % (value, dt))
+  return typed
+
+
+def refuse_sharded(vol, mips, what):
+  if any(vol._sharding(m) is not None for m in mips):
+    raise NotImplementedError("%s: sharded scales are not supported (a shard holds many chunks and would "
+                              "have to be rewritten whole)" % what)
+
+
+@queueable
+def BlackoutTask(cloudpath, mip, shape, offset, value=0, non_aligned_writes=False):
+  """Write `value` over the box, clamped to the volume at `mip` (image.py:124-135).  As in the reference
+  the box is not clamped to the creator's bounds: the last task of each axis paints up to the next
+  multiple of the task shape past them, or the volume's edge.  The box is filled
+  on the device: a chunk-aligned box in a fresh cutout; with non_aligned_writes, a box off the chunk
+  grid inside the chunk-aligned region read around it (missing chunks as 0), so the voxels of the edge
+  chunks outside the box keep their values.  A value the layer's dtype cannot hold raises ValueError, a
+  sharded scale NotImplementedError, and a box off the grid without non_aligned_writes the storage's
+  ValueError, each before anything is written."""
+  shape, offset, mip = Vec(*shape), Vec(*offset), int(mip)
+  vol = CloudVolume(cloudpath, mip, non_aligned_writes=non_aligned_writes)
+  bounds = Bbox.clamp(Bbox(offset, shape + offset), vol.bounds)
+  value = layer_value(vol.dtype, value)
+  refuse_sharded(vol, [mip], "BlackoutTask")
+  region = vol._write_region(bounds, mip)
+  if bounds.subvoxel():
+    return
+  if region == bounds:
+    img = DeviceCutout.empty(tuple(int(v) for v in bounds.size3()) + (vol.num_channels,), vol.dtype)
+  else:
+    img = vol.download_dev(region, mip=mip, fill_missing=True)
+  img.fill(bounds - region.minpt, value)
+  vol.upload_dev(region, img, mip=mip)
+
+
+@queueable
+def TouchTask(cloudpath, mip, shape, offset):
+  """Read the box, clamped to the volume at `mip`, and discard it (image.py:137-143): a missing chunk
+  raises EmptyVolumeException and a corrupt one its codec's error.  The chunks are decoded on the
+  device (download_dev)."""
+  shape, offset, mip = Vec(*shape), Vec(*offset), int(mip)
+  vol = CloudVolume(cloudpath, mip, fill_missing=False)
+  bounds = Bbox.clamp(Bbox(offset, shape + offset), vol.bounds)
+  vol.download_dev(bounds, mip=mip)
+
+
+@queueable
+def DeleteTask(layer_path, shape, offset, mip=0, num_mips=5):
+  """Delete a block of a layer at every mip from `mip` to min(top mip, mip + num_mips) (image.py:103-122):
+  at each the box is mapped to that mip, rounded to the nearest chunk boundaries
+  (Bbox.round_to_chunk_size) and clamped to the bounds, and the chunk files inside it are deleted.
+  A sharded scale in that range raises NotImplementedError before anything is deleted."""
+  shape, offset, mip = Vec(*shape), Vec(*offset), int(mip)
+  vol = CloudVolume(layer_path, mip=mip, max_redirects=0)
+  highres_bbox = Bbox(offset, offset + shape)
+  top_mip = min(vol.available_mips[-1], mip + num_mips)
+  refuse_sharded(vol, range(mip, top_mip + 1), "DeleteTask")
+  for mip_i in range(mip, top_mip + 1):
+    vol.mip = mip_i
+    bbox = vol.bbox_to_mip(highres_bbox, mip, mip_i)
+    bbox = bbox.round_to_chunk_size(vol.chunk_size, offset=vol.bounds.minpt)
+    bbox = Bbox.clamp(bbox, vol.bounds)
+    if bbox.volume() == 0:
+      continue
+    vol.delete(bbox)
 
 
 def _shard_chunks(vol, cutout, box, mip):

@@ -648,6 +648,34 @@ IGN_API int ign_chunks_place_dev(ign_ctx* ctx, const void* packed, int dtype, ui
 IGN_API int ign_chunks_cut_dev(ign_ctx* ctx, const void* cutout, int dtype, uint64_t X, uint64_t Y, uint64_t Z,
                                uint64_t nc, const uint64_t* rows, uint64_t n_rows, uint64_t background,
                                void* packed, uint32_t* all_bg);
+/* ign_fill_box_dev: every voxel of the box [x0, x0+bx) x [y0, y0+by) x [z0, z0+bz), every channel, of an
+ * F-order [X, Y, Z, nc] device cutout is set to `value` (the value's bit pattern, zero-extended, as for
+ * ign_chunks_cut_dev's background).  BlackoutTask's write (igneous/tasks/image/image.py:124-135).
+ * dtype: IGN_U8 / U16 / U32 / U64 / F32.  A box outside the cutout -> IGN_ERR_INVALID.  64-bit indexing. */
+IGN_API int ign_fill_box_dev(ign_ctx* ctx, void* cutout, int dtype, uint64_t X, uint64_t Y, uint64_t Z, uint64_t nc,
+                             uint64_t x0, uint64_t y0, uint64_t z0, uint64_t bx, uint64_t by, uint64_t bz,
+                             uint64_t value);
+
+/* ------------------------------------------------------- regions of interest
+ * compute_rois (igneous/task_creation/image.py:1995-2058) per z slab of the top mip:
+ *   np.greater(img, suppress_faint_voxels); cc3d.connected_components (26-connected); cc3d.dust;
+ *   cc3d.statistics(...)["bounding_boxes"].
+ * ign_threshold_dev: out[i] = in[i] > t (u8 0 / 1), n voxels, 64-bit indexing.  Integer dtypes
+ *   (IGN_U8 / U16 / U32 / U64) compare as unsigned 64-bit integers, so every t >= 0 is exact; for
+ *   IGN_F32 the low 32 bits of t are the float32 threshold's bit pattern (NaN is never greater).
+ * ign_mask_boxes_dev: the 26-connected components of the non-zero voxels of an F-order (sx, sy, sz) u8
+ *   mask, fewer than 2^32 - 1 voxels (more -> IGN_ERR_UNSUPPORTED).  Components of fewer than
+ *   dust_threshold voxels are dropped.  *n = the number kept; when *n <= capacity, rows (HOST, capacity
+ *   rows of IGN_BOX_ROW uint32 words) receives per kept component
+ *     {voxel count, min x, min y, min z, max x, max y, max z}   (maxima inclusive)
+ *   in the order of each component's first voxel in F order (cc3d's numbering), copied from the device
+ *   before the call returns.  A capacity of ceil(sx/2) * ceil(sy/2) * ceil(sz/2) rows always suffices
+ *   (26-connected components cannot be denser); with less and *n > capacity, rows is not written.  The
+ *   stream is synchronised three times: for the component count, the kept count and the rows. */
+#define IGN_BOX_ROW 7
+IGN_API int ign_threshold_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint64_t t, uint8_t* out);
+IGN_API int ign_mask_boxes_dev(ign_ctx* ctx, const uint8_t* mask, uint64_t sx, uint64_t sy, uint64_t sz,
+                               uint64_t dust_threshold, uint32_t* rows, uint64_t capacity, uint64_t* n);
 
 /* ------------------------------------------------------------------ jpeg codec
  * The Precomputed `jpeg` chunk encoding of uint8 image layers, which CloudVolume applies on the host
