@@ -17,9 +17,11 @@ _TASK_NAMES = ("DownsampleTask", "TransferTask", "ImageShardTransferTask", "Imag
                "downsample_method_to_fn", "threshold_image", "blackout_non_face_rails", "DisjointSet",
                "QuantizeTask", "CLAHETask", "ContrastNormalizationTask", "LuminanceLevelsTask",
                "SpatialIndexTask", "CountVoxelsTask", "SkeletonTask", "UnshardedSkeletonMergeTask",
-               "BlackoutTask", "TouchTask", "DeleteTask")
+               "BlackoutTask", "TouchTask", "DeleteTask", "ShardedFromUnshardedSkeletonMergeTask")
+# creators whose task is in _TASK_NAMES and that have no other root-level name in the reference
+_CREATION_NAMES = ("create_sharded_skeletons_from_unsharded_tasks",)
 _COMPAT_NAMES = ("CloudVolume", "EmptyVolumeException", "LocalTaskQueue", "RegisteredTask", "queueable")
-__all__ = ["Mesher", "__version__"] + list(_TASK_NAMES) + list(_COMPAT_NAMES)
+__all__ = ["Mesher", "__version__"] + list(_TASK_NAMES) + list(_CREATION_NAMES) + list(_COMPAT_NAMES)
 
 
 def __getattr__(name):
@@ -29,6 +31,9 @@ def __getattr__(name):
   if name in _TASK_NAMES:
     from . import tasks
     return getattr(tasks, name)
+  if name in _CREATION_NAMES:
+    from . import task_creation
+    return getattr(task_creation, name)
   if name in _COMPAT_NAMES:
     from . import _compat
     return getattr(_compat, name)

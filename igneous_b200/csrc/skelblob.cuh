@@ -1,6 +1,6 @@
 // skelblob.cuh -- the neuroglancer precomputed skeleton encoder of ign_skeleton_export_dev (skeleton.cu) and
-// ign_skeleton_merge_dev (skelmerge.cu), sm_90a: the only code under csrc/ that knows the blob layout
-// (DESIGN.md §5g).  The caller numbers its final vertices label-major, sorts its edges as keys (lo << 32) | hi
+// ign_skeleton_merge_dev (skelmerge.cu), and the blob layout ign_skeleton_restrip_dev (labelshard.cu) reads,
+// sm_90a: the only code under csrc/ that knows the blob layout (DESIGN.md §5g).  The caller numbers its final vertices label-major, sorts its edges as keys (lo << 32) | hi
 // of those numbers, and describes its G rows with a source, a device functor with
 //   vstart(g), g <= G      the first final vertex of row g (vstart(G) is the vertex count)
 //   label(g)               column 0 of the table
@@ -26,8 +26,13 @@ __device__ __forceinline__ uint64_t sb_lower(const uint64_t* __restrict__ a, uin
   return lo;
 }
 
+// a blob: uint32 nv, ne, float32 vertices[nv][3], uint32 edges[ne][2], then one section per vertex attribute,
+// each nv values; sb_head_bytes is where the first attribute section starts
+__device__ __forceinline__ uint64_t sb_head_bytes(uint64_t nv, uint64_t ne) { return 8 + 12 * nv + 8 * ne; }
+
+// the blob of the encoder below: radius float32, then vertex_types uint8 when vt
 __device__ __forceinline__ uint64_t sb_blob_bytes(uint64_t nv, uint64_t ne, int vt) {
-  return 8 + 16 * nv + 8 * ne + (vt ? nv : 0);
+  return sb_head_bytes(nv, ne) + (vt ? 5 : 4) * nv;
 }
 
 template <class Src>
@@ -84,8 +89,8 @@ __global__ void __launch_bounds__(256) k_sb_verts(Src src, uint64_t G, uint64_t 
   vert[0] = c[0];
   vert[1] = c[1];
   vert[2] = c[2];
-  ((float*)(blobs + o + 8 + 12 * nv + 8 * ne))[i] = r;
-  if (vt) blobs[o + 8 + 16 * nv + 8 * ne + i] = t;
+  ((float*)(blobs + o + sb_head_bytes(nv, ne)))[i] = r;
+  if (vt) blobs[o + sb_head_bytes(nv, ne) + 4 * nv + i] = t;
 }
 
 template <class Src>

@@ -1,5 +1,6 @@
 """neuroglancer_uint64_sharded_v1 for image chunks: the container either side of
-ImageShardDownsampleTask (igneous/tasks/image/image.py:672-843).
+ImageShardDownsampleTask (igneous/tasks/image/image.py:672-843).  LabelShardingSpecification is the same
+container keyed by label with the murmurhash3_x86_128 hash, for skeleton layers (DESIGN.md §5l).
 
 The reference gets all of this from cloudvolume (`ShardingSpecification`,
 `create_sharded_image_info`, `image.make_shard[_chunks]`), which is not installed
@@ -101,43 +102,24 @@ class ShardingSpecification:
   # ---- writer
   def synthesize_shard(self, chunks):
     """{chunk id: encoded chunk bytes} (all of one shard) -> the bytes of the shard file."""
-    by_mini = {}
-    shard_no = None
-    for cid in chunks:
-      s, m = self.locate(cid)
-      if shard_no is None:
-        shard_no = s
-      elif s != shard_no:
-        raise ValueError("chunks of shards %x and %x in one synthesize_shard call" % (shard_no, s))
-      by_mini.setdefault(m, []).append(int(cid))
-    payload, pos = [], 0
-    indices = {}
-    for m in sorted(by_mini):
-      ids = sorted(by_mini[m])
-      table = np.zeros((3, len(ids)), dtype="<u8")
-      prev_id, prev_end = 0, 0
-      for i, cid in enumerate(ids):
-        blob = chunks[cid]
-        if self.data_encoding == "gzip":
-          blob = gzip.compress(blob, compresslevel=6, mtime=0)
-        table[0, i] = cid - prev_id
-        table[1, i] = pos - prev_end if i else pos
-        table[2, i] = len(blob)
-        payload.append(blob)
-        pos += len(blob)
-        prev_id, prev_end = cid, pos
-      raw = table.tobytes(order="C")
-      indices[m] = gzip.compress(raw, compresslevel=6, mtime=0) if self.minishard_index_encoding == "gzip" else raw
-    shard_index = np.zeros((1 << self.minishard_bits, 2), dtype="<u8")
-    tail = []
-    for m in range(1 << self.minishard_bits):
-      if m in indices:
-        shard_index[m] = (pos, pos + len(indices[m]))
-        tail.append(indices[m])
-        pos += len(indices[m])
-      else:
-        shard_index[m] = (pos, pos)  # empty minishard
-    return shard_index.tobytes(order="C") + b"".join(payload) + b"".join(tail)
+    keys = list(chunks)
+    ids = np.fromiter((int(c) for c in keys), dtype=np.uint64, count=len(keys))
+    shards, minis = self.locate_many(ids)
+    if len(ids) and np.any(shards != shards[0]):
+      other = shards[np.argmax(shards != shards[0])]
+      raise ValueError("chunks of shards %x and %x in one synthesize_shard call" % (int(shards[0]), int(other)))
+    order = np.lexsort((ids, minis))
+    blobs = [chunks[keys[i]] for i in order]
+    if self.data_encoding == "gzip":
+      blobs = [gzip.compress(b, compresslevel=6, mtime=0) for b in blobs]
+    return pack_shard(self.minishard_bits, self.minishard_index_encoding, minis[order], ids[order], blobs)
+
+  def locate_many(self, chunk_ids):
+    """-> (shard numbers, minishard numbers) of a uint64 array of chunk ids"""
+    h = np.asarray(chunk_ids, dtype=np.uint64) >> np.uint64(self.preshift_bits)
+    mini = h & np.uint64((1 << self.minishard_bits) - 1)
+    shard = (h >> np.uint64(self.minishard_bits)) & np.uint64((1 << self.shard_bits) - 1)
+    return shard, mini
 
   # ---- reader
   def minishard_table(self, shard_bytes, minishard):
@@ -176,6 +158,105 @@ class ShardingSpecification:
     for m in range(1 << self.minishard_bits):
       out.extend(int(v) for v in self.minishard_table(shard_bytes, m)[0])
     return sorted(out)
+
+
+_U32 = np.uint64(0xFFFFFFFF)
+
+
+def _rotl32(x, r):
+  return ((x << np.uint64(r)) | (x >> np.uint64(32 - r))) & _U32
+
+
+def _fmix32(h):
+  h ^= h >> np.uint64(16)
+  h = (h * np.uint64(0x85EBCA6B)) & _U32
+  h ^= h >> np.uint64(13)
+  h = (h * np.uint64(0xC2B2AE35)) & _U32
+  return h ^ (h >> np.uint64(16))
+
+
+def murmurhash3_x86_128_u64(keys):
+  """MurmurHash3_x86_128 with seed 0 of the 8 little-endian bytes of each uint64 key, low 64 bits (h1 | h2 << 32).
+  Vectorised; 32-bit words are held in uint64 and masked after every product (DESIGN.md §5l)."""
+  keys = np.asarray(keys, dtype=np.uint64)
+  c1, c2, c3 = np.uint64(0x239B961B), np.uint64(0xAB0E9789), np.uint64(0x38B34AE5)
+  k1, k2 = keys & _U32, keys >> np.uint64(32)
+  # an 8-byte key has no 16-byte block: bytes 4..7 are tail word k2, bytes 0..3 tail word k1
+  h2 = (_rotl32((k2 * c2) & _U32, 16) * c3) & _U32
+  h1 = (_rotl32((k1 * c1) & _U32, 15) * c2) & _U32
+  h3 = np.zeros_like(keys)
+  h4 = np.zeros_like(keys)
+  h1, h2, h3, h4 = (h ^ np.uint64(8) for h in (h1, h2, h3, h4))  # the length
+  h1 = (h1 + h2 + h3 + h4) & _U32
+  h2, h3, h4 = ((h + h1) & _U32 for h in (h2, h3, h4))
+  h1, h2, h3, h4 = (_fmix32(h) for h in (h1, h2, h3, h4))
+  h1 = (h1 + h2 + h3 + h4) & _U32
+  h2 = (h2 + h1) & _U32
+  return h1 | (h2 << np.uint64(32))
+
+
+class LabelShardingSpecification(ShardingSpecification):
+  """The `sharding` member of a skeleton (or mesh) info: neuroglancer_uint64_sharded_v1 keyed by label with
+  the murmurhash3_x86_128 hash (DESIGN.md §5l).  The container is the image shards' own; only the hash
+  differs: h = murmur(label >> preshift_bits), minishard = h & (2^minishard_bits - 1),
+  shard = (h >> minishard_bits) & (2^shard_bits - 1)."""
+
+  HASH = "murmurhash3_x86_128"
+
+  def __init__(self, spec):
+    spec = dict(spec)
+    if spec.get("hash", self.HASH) != self.HASH:
+      raise ValueError("LabelShardingSpecification: hash %r (only %r)" % (spec.get("hash"), self.HASH))
+    super().__init__(dict(spec, hash="identity"))
+    self.hash = self.HASH
+    if not (0 <= self.preshift_bits < 64 and 0 <= self.minishard_bits and 0 <= self.shard_bits
+            and self.minishard_bits + self.shard_bits <= 64):
+      raise ValueError("LabelShardingSpecification: preshift_bits %d, minishard_bits %d, shard_bits %d"
+                       % (self.preshift_bits, self.minishard_bits, self.shard_bits))
+
+  def locate_many(self, labels):
+    h = murmurhash3_x86_128_u64(np.asarray(labels, dtype=np.uint64) >> np.uint64(self.preshift_bits))
+    mini = h & np.uint64((1 << self.minishard_bits) - 1)
+    shard = (h >> np.uint64(self.minishard_bits)) & np.uint64((1 << self.shard_bits) - 1) \
+        if self.minishard_bits < 64 else np.zeros_like(h)
+    return shard, mini
+
+  def locate(self, label):
+    """-> (shard number, minishard number)"""
+    shard, mini = self.locate_many(np.array([int(label)], dtype=np.uint64))
+    return int(shard[0]), int(mini[0])
+
+
+def pack_shard(minishard_bits, minishard_index_encoding, minis, ids, blobs):
+  """The bytes of a shard file whose entries are already in (minishard, id) order: minis and ids the
+  minishard and id of each entry, blobs its payload as stored (already data-encoded).  The payloads go back to
+  back after the shard index, then each non-empty minishard's index ([3, n] u64le: delta-coded ids,
+  delta-coded starts, sizes), encoded with minishard_index_encoding, in minishard order."""
+  minis = np.asarray(minis, dtype=np.uint64)
+  ids = np.asarray(ids, dtype=np.uint64)
+  sizes = np.fromiter((len(b) for b in blobs), dtype=np.uint64, count=len(blobs))
+  starts = np.zeros(len(blobs), dtype=np.uint64)
+  if len(blobs):
+    np.cumsum(sizes[:-1], out=starts[1:])
+  pos = int(sizes.sum())
+  shard_index = np.zeros((1 << minishard_bits, 2), dtype="<u8")
+  tail = []
+  bounds = np.searchsorted(minis, np.arange((1 << minishard_bits) + 1, dtype=np.uint64))
+  for m in range(1 << minishard_bits):
+    a, b = int(bounds[m]), int(bounds[m + 1])
+    if a == b:
+      shard_index[m] = (pos, pos)  # empty minishard
+      continue
+    table = np.zeros((3, b - a), dtype="<u8")
+    table[0, 0], table[0, 1:] = ids[a], np.diff(ids[a:b])
+    table[1, 0] = starts[a]  # every later payload starts where the previous one ends
+    table[2] = sizes[a:b]
+    raw = table.tobytes(order="C")
+    raw = gzip.compress(raw, compresslevel=6, mtime=0) if minishard_index_encoding == "gzip" else raw
+    shard_index[m] = (pos, pos + len(raw))
+    tail.append(raw)
+    pos += len(raw)
+  return shard_index.tobytes(order="C") + b"".join(bytes(b) for b in blobs) + b"".join(tail)
 
 
 def create_sharded_image_info(dataset_size, chunk_size, encoding, dtype, uncompressed_shard_bytesize=int(3.5e9),

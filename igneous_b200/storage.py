@@ -410,10 +410,12 @@ class _SkeletonMeta:
 
 
 class _SkeletonSource:
-  """cv.skeleton: meta, path, spatial_index (cv.mesh's) and get(segid) of unsharded precomputed skeletons."""
+  """cv.skeleton: meta, path, spatial_index (cv.mesh's) and get(segid) of precomputed skeletons, unsharded or
+  in hashed shards (the info's `sharding`)."""
 
   def __init__(self, cv):
-    subdir = cv.info.get("skeletons", "skeletons")  # cloudvolume's default directory, as recalled
+    # CloudVolume(skel_dir=...), else the layer's, else cloudvolume's default directory, as recalled
+    subdir = cv.skel_dir or cv.info.get("skeletons", "skeletons")
     self._cv = cv
     self.meta = _SkeletonMeta(cv, subdir)
     self.path = cv.cf.join(cv.cloudpath, subdir)
@@ -424,7 +426,10 @@ class _SkeletonSource:
     if isinstance(segid, (list, tuple)):
       return [self.get(s) for s in segid]
     from .kimimaro import split_blobs
-    data = self._cv.cf.get("%s/%d" % (self.meta.subdir, int(segid)))
+    if self.meta.info.get("sharding"):
+      data = self._sharded(int(segid))
+    else:
+      data = self._cv.cf.get("%s/%d" % (self.meta.subdir, int(segid)))
     if data is None:
       raise FileNotFoundError("no skeleton %d in %s" % (int(segid), self.path))
     buf = np.frombuffer(bytearray(data), dtype=np.uint8)  # writable: the Skeleton's arrays are views into it
@@ -434,6 +439,13 @@ class _SkeletonSource:
       raise ValueError("skeleton %d: %d bytes, the info's attributes describe %d" % (int(segid), buf.size,
                                                                                       blobs[0].size))
     return skeletons[0]
+
+  def _sharded(self, segid):
+    """the blob of segid from its shard file, or None"""
+    from .sharding import LabelShardingSpecification
+    spec = LabelShardingSpecification(self.meta.info["sharding"])
+    shard = self._cv.cf.get("%s/%s" % (self.meta.subdir, spec.shard_filename(spec.locate(segid)[0])))
+    return None if shard is None else spec.read_chunk(shard, segid)
 
 
 class _Meta:
@@ -552,8 +564,9 @@ class CloudVolume:
 
   def __init__(self, cloudpath, mip=0, fill_missing=False, bounded=True, info=None, compress="gzip",
                delete_black_uploads=False, background_color=0, parallel=1, progress=False, non_aligned_writes=False,
-               **kwargs):
+               skel_dir=None, **kwargs):
     self.cloudpath = cloudpath
+    self.skel_dir = skel_dir
     self.path = _strip(cloudpath)
     self.fill_missing = bool(fill_missing)
     self.bounded = bounded

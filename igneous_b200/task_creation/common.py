@@ -107,3 +107,34 @@ def spatial_index_tasks(cloudpath, shape, mip, fill_missing, compress, subdir, k
       vol.commit_provenance()
 
   return SpatialIndexTaskIterator(vol.bounds, shape)
+
+
+def compute_shard_params_for_hashed(num_labels, shard_index_bytes=2 ** 13, minishard_index_bytes=2 ** 15, min_shards=1):
+  """(shard_bits, minishard_bits, preshift_bits) for labels spread evenly by a hash
+  (igneous/task_creation/common.py:140-213).  A shard index of shard_index_bytes holds
+  shard_index_bytes / 16 minishards; a minishard index of minishard_index_bytes holds
+  minishard_index_bytes / 24 labels.  Enough minishard and shard bits are taken for num_labels to fit:
+  a full shard index once the labels fill more than one shard, then whole shards; a shard less than 55%
+  used gives one shard bit back.  At least round(log2(min_shards)) shard bits are kept, taken from the
+  minishard bits.  Preshift is 0: hashed labels have no locality to keep."""
+  assert min_shards >= 1
+  if num_labels <= 0:
+    return (0, 0, 0)
+  minishards_per_shard = shard_index_bytes / 16
+  labels_per_minishard = minishard_index_bytes / 24
+  labels_per_shard = minishards_per_shard * labels_per_minishard
+  if num_labels >= labels_per_shard:
+    minishard_bits = int(np.ceil(np.log2(minishards_per_shard)))
+    shard_bits = int(np.ceil(np.log2(num_labels / (labels_per_minishard * 2 ** minishard_bits))))
+  elif num_labels >= labels_per_minishard:
+    minishard_bits, shard_bits = int(np.ceil(np.log2(num_labels / labels_per_minishard))), 0
+  else:
+    minishard_bits, shard_bits = 0, 0
+  if num_labels / (labels_per_shard * 2 ** shard_bits) <= 0.55:
+    shard_bits -= 1
+  shard_bits = max(shard_bits, 0)
+  want = int(np.round(np.log2(min_shards)))
+  if want > shard_bits:
+    minishard_bits -= want - shard_bits
+    shard_bits = want
+  return (int(shard_bits), int(max(minishard_bits, 0)), 0)

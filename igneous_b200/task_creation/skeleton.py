@@ -1,13 +1,19 @@
 """create_skeletonizing_tasks (igneous/task_creation/skeleton.py:68-388),
-create_unsharded_skeleton_merge_tasks (:535-591) and create_spatial_index_skeleton_tasks (:795-867)."""
+create_unsharded_skeleton_merge_tasks (:535-591), create_sharded_skeletons_from_unsharded_tasks (:659-753) and
+create_spatial_index_skeleton_tasks (:795-867)."""
+import copy
+import re
+from functools import partial
 from time import strftime
 
 import numpy as np
 
+from .. import labelshard
 from .._compat import CloudVolume, CloudFiles, Vec
-from ..tasks import SkeletonTask, UnshardedSkeletonMergeTask
-from ..tasks.skeleton import refuse
-from .common import FinelyDividedTaskIterator, operator_contact, spatial_index_tasks
+from ..sharding import LabelShardingSpecification
+from ..tasks import SkeletonTask, UnshardedSkeletonMergeTask, ShardedFromUnshardedSkeletonMergeTask
+from ..tasks.skeleton import refuse, refuse_same_directory
+from .common import FinelyDividedTaskIterator, compute_shard_params_for_hashed, operator_contact, spatial_index_tasks
 
 
 def create_skeletonizing_tasks(cloudpath, mip, shape=Vec(512, 512, 512), teasar_params={"scale": 10, "const": 10},
@@ -132,3 +138,68 @@ def create_spatial_index_skeleton_tasks(cloudpath, shape=(448, 448, 448), mip=0,
   """Rebuild the spatial index of a skeleton directory (default: the layer's, else skeletons_mip_{mip}),
   or build one over a different grid than the skeleton tasks used."""
   return spatial_index_tasks(cloudpath, shape, mip, fill_missing, compress, skel_dir, "skeletons")
+
+
+# a source skeleton file: the whole name is the label's digits, optionally with a compression suffix (chosen:
+# the reference's re.search would also take the trailing digits of "{segid}:{bbox}" fragment names)
+LABEL_FILE = re.compile(r"(\d+)(\.gz|\.br|\.zstd)?")
+
+
+def create_sharded_skeletons_from_unsharded_tasks(src, dest, shard_index_bytes=2 ** 13, minishard_index_bytes=2 ** 15,
+                                                  min_shards=1, minishard_index_encoding="gzip",
+                                                  data_encoding="gzip", skel_dir=None):
+  """ShardedFromUnshardedSkeletonMergeTasks that turn the unsharded skeletons of src into a sharded
+  (murmurhash3_x86_128) skeleton layer at dest (igneous/task_creation/skeleton.py:659-753).  The destination
+  skeleton info is the source's with only its float32 and float64 vertex_attributes and a `sharding` from
+  compute_shard_params_for_hashed; every label is hashed on the device, each shard's labels go to a gzipped
+  `{shard}.labels` JSON list in (minishard, label) order, the provenance is appended, and one task is
+  returned per non-empty shard, in shard order.  A destination that is the source's skeleton directory raises
+  ValueError, and a source skeleton stored with brotli or zstd NotImplementedError, before anything is
+  written (DESIGN.md §5l)."""
+  cv_src = CloudVolume(src)
+  cv_src.mip = cv_src.skeleton.meta.mip
+  cv_dest = CloudVolume(dest, skel_dir=skel_dir)
+  refuse_same_directory("create_sharded_skeletons_from_unsharded_tasks", cv_src, cv_dest)
+  labels = []
+  for name in CloudFiles(cv_src.skeleton.path).list():
+    m = LABEL_FILE.fullmatch(name)
+    if m is None:
+      continue
+    if m.group(2) in (".br", ".zstd"):
+      raise NotImplementedError("create_sharded_skeletons_from_unsharded_tasks: %s is stored with %s; only raw "
+                                "and gzip skeletons are read" % (name, m.group(2)[1:]))
+    if int(m.group(1)) >= 1 << 64:
+      raise ValueError("create_sharded_skeletons_from_unsharded_tasks: %s is not a uint64 label" % name)
+    labels.append(int(m.group(1)))
+
+  shard_bits, minishard_bits, preshift_bits = compute_shard_params_for_hashed(
+    num_labels=len(labels), shard_index_bytes=int(shard_index_bytes),
+    minishard_index_bytes=int(minishard_index_bytes), min_shards=int(min_shards))
+  spec = LabelShardingSpecification({
+    "@type": "neuroglancer_uint64_sharded_v1", "preshift_bits": preshift_bits, "hash": "murmurhash3_x86_128",
+    "minishard_bits": minishard_bits, "shard_bits": shard_bits,
+    "minishard_index_encoding": minishard_index_encoding, "data_encoding": data_encoding})
+  info = copy.deepcopy(cv_src.skeleton.meta.info)
+  info["vertex_attributes"] = [a for a in info.get("vertex_attributes") or []
+                               if a["data_type"] in ("float32", "float64")]
+  info["sharding"] = spec.to_dict()
+  ordered, _, starts, shards = labelshard.shard_hash(np.array(labels, dtype=np.uint64), preshift_bits,
+                                                     minishard_bits, shard_bits)
+  starts = starts.tolist()
+
+  cv_dest.skeleton.meta.info = info
+  cv_dest.skeleton.meta.commit_info()
+  cf = CloudFiles(cv_dest.skeleton.path)
+  cf.put_jsons((("%d.labels" % s, ordered[a:b].tolist()) for s, a, b in zip(shards.tolist(), starts[:-1], starts[1:])),
+               compress="gzip", cache_control="no-cache")
+  cv_dest.provenance.processing.append({
+    "method": {
+      "task": "ShardedFromUnshardedSkeletonMergeTask", "src": src, "dest": dest, "preshift_bits": preshift_bits,
+      "minishard_bits": minishard_bits, "shard_bits": shard_bits, "skel_dir": skel_dir,
+    },
+    "by": operator_contact(),
+    "date": strftime("%Y-%m-%d %H:%M %Z"),
+  })
+  cv_dest.commit_provenance()
+  return [partial(ShardedFromUnshardedSkeletonMergeTask, src=src, dest=dest, shard_no=str(s), skel_dir=skel_dir)
+          for s in shards.tolist()]

@@ -5,4 +5,4 @@ from .ccl import (CCLFacesTask, CCLEquivalancesTask, RelabelCCLTask, create_rela
                   clean_intermediate_files, threshold_image, blackout_non_face_rails, DisjointSet)
 from .mesh import MeshTask
 from .spatial_index import SpatialIndexTask
-from .skeleton import SkeletonTask, UnshardedSkeletonMergeTask
+from .skeleton import SkeletonTask, UnshardedSkeletonMergeTask, ShardedFromUnshardedSkeletonMergeTask

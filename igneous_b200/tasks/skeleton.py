@@ -8,8 +8,11 @@ to dataset coordinates, encodes each skeleton in the precomputed format and boxe
 device renumbers, and the export keys skeletons by original label.
 
 UnshardedSkeletonMergeTask mirrors igneous/tasks/skeleton.py:810-916; its fuse and kimimaro.postprocess run on
-the device (igneous_b200.kimimaro.merge_fragments, DESIGN.md §5h).
+the device (igneous_b200.kimimaro.merge_fragments, DESIGN.md §5h).  ShardedFromUnshardedSkeletonMergeTask
+mirrors :1074-1130: it packs finished unsharded skeletons into one hashed shard (DESIGN.md §5l).
 """
+import gzip
+import os
 import pickle
 import re
 import time
@@ -17,8 +20,9 @@ from collections import defaultdict
 
 import numpy as np
 
-from .. import fastremap, kimimaro
-from .._compat import CloudVolume, CloudFiles, Bbox, Vec, RegisteredTask
+from .. import fastremap, kimimaro, labelshard
+from .._compat import CloudVolume, CloudFiles, Bbox, Vec, RegisteredTask, queueable
+from ..sharding import LabelShardingSpecification, pack_shard
 
 # seconds per phase of the last execute() in this process, host clock (diagnostic)
 last_phase_seconds = {}
@@ -199,3 +203,86 @@ class UnshardedSkeletonMergeTask(RegisteredTask):
       cf.delete(filenames)
     last_phase_seconds.update(list=t1 - t0, unpickle=t2 - t1, merge=t3 - t2, writes=time.perf_counter() - t3)
     return merged
+
+
+def _skeleton_dir(vol):
+  """the skeleton directory of a volume as a comparable path (file:// resolved on disk)"""
+  path = vol.skeleton.path
+  if path.startswith("file://"):
+    return os.path.realpath(path[len("file://"):])
+  return path.rstrip("/")
+
+
+def refuse_same_directory(who, cv_src, cv_dest):
+  if _skeleton_dir(cv_src) == _skeleton_dir(cv_dest):
+    raise ValueError("%s: the destination skeleton directory %s is the source's; pass another dest or skel_dir"
+                     % (who, cv_dest.skeleton.path))
+
+
+@queueable
+def ShardedFromUnshardedSkeletonMergeTask(src, dest, shard_no, cache_control=False, skel_dir=None, progress=False):
+  """Write shard `shard_no` of a sharded skeleton layer from the unsharded skeletons of src
+  (igneous/tasks/skeleton.py:1097-1130).  The labels are `{shard_no}.labels` of the destination skeleton
+  directory (written by create_sharded_skeletons_from_unsharded_tasks); each one's skeleton is read from the
+  source directory, the labels are ordered on the device, and every skeleton loses its integer vertex
+  attributes in one device pass (DESIGN.md §5l).  Raw data with raw minishard indices leaves the device as
+  the finished shard file; otherwise the host compresses each skeleton (gzip data) and builds the indices
+  (gzip indices).  An empty label list writes nothing."""
+  last_phase_seconds.clear()
+  t0 = time.perf_counter()
+  cv_src = CloudVolume(src)
+  if skel_dir is None and "skeletons" in cv_src.info:
+    skel_dir = cv_src.info["skeletons"]
+  cv_dest = CloudVolume(dest, skel_dir=skel_dir, progress=progress)
+  refuse_same_directory("ShardedFromUnshardedSkeletonMergeTask", cv_src, cv_dest)
+  sharding = cv_dest.skeleton.meta.info.get("sharding")
+  if not sharding:
+    raise ValueError("ShardedFromUnshardedSkeletonMergeTask: %s/info has no sharding" % cv_dest.skeleton.path)
+  spec = LabelShardingSpecification(sharding)
+  cf_dest = CloudFiles(cv_dest.skeleton.path)
+  labels = cf_dest.get_json("%s.labels" % shard_no)
+  if labels is None:
+    raise FileNotFoundError("ShardedFromUnshardedSkeletonMergeTask: no %s.labels in %s"
+                            % (shard_no, cv_dest.skeleton.path))
+  if len(labels) == 0:
+    return
+  labels = np.asarray([int(l) for l in labels], dtype=np.uint64)
+  if np.unique(labels).size != labels.size:
+    raise ValueError("ShardedFromUnshardedSkeletonMergeTask: %s.labels lists a label twice" % shard_no)
+  labels, locations, _, shards = labelshard.shard_hash(labels, spec.preshift_bits, spec.minishard_bits,
+                                                       spec.shard_bits)
+  if shards.size != 1 or int(shards[0]) != int(shard_no):
+    wrong = int(labels[np.argmax((locations >> np.uint64(spec.minishard_bits)) != np.uint64(int(shard_no)))]) \
+        if spec.minishard_bits < 64 else int(labels[0])
+    raise ValueError("ShardedFromUnshardedSkeletonMergeTask: label %d of %s.labels is not in shard %s"
+                     % (wrong, shard_no, shard_no))
+  t1 = time.perf_counter()
+  cf_src = CloudFiles(cv_src.skeleton.path)
+  names = [str(l) for l in labels.tolist()]
+  contents = cf_src.get(names, return_dict=True)
+  blobs = []
+  for name in names:
+    if contents.get(name) is None:
+      raise FileNotFoundError("ShardedFromUnshardedSkeletonMergeTask: label %s of %s.labels has no skeleton in %s"
+                              % (name, shard_no, cv_src.skeleton.path))
+    blobs.append(contents[name])
+  del contents
+  t2 = time.perf_counter()
+  attributes = cv_src.skeleton.meta.info.get("vertex_attributes") or []
+  if spec.data_encoding == "raw" and spec.minishard_index_encoding == "raw":
+    data = labelshard.restrip(blobs, attributes, locations, labels, spec.minishard_bits)
+    t3 = t4 = time.perf_counter()
+  else:
+    buf, offs = labelshard.restrip(blobs, attributes)
+    t3 = time.perf_counter()
+    offs = offs.tolist()
+    stored = [buf[a:b].tobytes() for a, b in zip(offs[:-1], offs[1:])]
+    if spec.data_encoding == "gzip":
+      stored = [gzip.compress(b, compresslevel=6, mtime=0) for b in stored]
+    data = pack_shard(spec.minishard_bits, spec.minishard_index_encoding,
+                      locations & np.uint64((1 << spec.minishard_bits) - 1), labels, stored)
+    t4 = time.perf_counter()
+  cf_dest.put(spec.shard_filename(int(shard_no)), data, compress=None, content_type="application/octet-stream",
+              cache_control="no-cache")
+  last_phase_seconds.update(labels=t1 - t0, read=t2 - t1, device=t3 - t2, gzip=t4 - t3,
+                            write=time.perf_counter() - t4)

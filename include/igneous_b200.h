@@ -511,6 +511,42 @@ IGN_API int ign_skeleton_merge_dev(ign_ctx* ctx, uint64_t n_labels, const uint64
                                    uint64_t* nbytes);
 IGN_API int ign_skeleton_merge_capacity(uint64_t n_labels, uint64_t n_vertices, uint64_t n_edges, uint64_t* bytes);
 
+/* ------------------------------------------------------------- label shards
+ * neuroglancer_uint64_sharded_v1 with the murmurhash3_x86_128 hash, for skeleton layers
+ * (ShardedFromUnshardedSkeletonMergeTask, create_sharded_skeletons_from_unsharded_tasks,
+ * igneous/tasks/skeleton.py:1074-1130); the rule is DESIGN.md §5l.  Every array is a DEVICE array unless
+ * marked HOST.
+ * ign_shard_hash_dev: h = MurmurHash3_x86_128 (seed 0) of the 8 little-endian bytes of label >> preshift_bits,
+ *   low 64 bits; location = h & (2^(minishard_bits + shard_bits) - 1), that is (shard << minishard_bits) |
+ *   minishard.  Out: labels_out the n labels sorted by (shard, minishard, label) (equal labels stay
+ *   together), locations_out the location of each, and the runs of equal shards: *n_runs of them, run r
+ *   starting at run_start_out[r] (run_start_out[*n_runs] = n) with shard run_shard_out[r].  run_start_out has
+ *   room for min(n, 2^shard_bits) + 1 entries, run_shard_out for min(n, 2^shard_bits).  preshift_bits above 63
+ *   or minishard_bits + shard_bits above 64 -> IGN_ERR_INVALID; n of 2^31 or more -> IGN_ERR_OVERFLOW.  The
+ *   host synchronises once.
+ * ign_skeleton_restrip_dev: n precomputed skeleton blobs packed in blobs, blob i the bytes
+ *   [offsets[i], offsets[i + 1]).  attrs (HOST uint32 [n_attrs][2], n_attrs <= 32): the source's vertex
+ *   attributes in blob order, each (bytes per vertex, keep).  Out: each blob with only the kept attribute
+ *   sections, in the same order, blob i at out_offsets[i] of out (packed, no padding; out_offsets has n + 1
+ *   entries), *nbytes = out_offsets[n].  A blob shorter than 8 bytes or whose length is not 8 + 12 nv + 8 ne +
+ *   (sum of bytes per vertex) nv -> IGN_ERR_INVALID naming its row (the lowest), before anything is written
+ *   to out; a capacity below the output -> IGN_ERR_INVALID.  The host synchronises once.
+ * ign_shard_assemble_dev: the shard file of n payloads already at payload = shard + 16 * 2^minishard_bits,
+ *   payload i at bytes [offsets[i], offsets[i + 1]) of it, rows in (minishard, label) order: locations
+ *   the location of each row (its minishard = the low minishard_bits), labels its label.  Writes the shard
+ *   index at shard[0..16 * 2^minishard_bits) and the raw minishard indices after the payloads; *nbytes = the
+ *   file's length.  minishard_bits above 32 or a capacity below the file -> IGN_ERR_INVALID.  Rows out of
+ *   (minishard, label) order are not detected.  The host synchronises once. */
+IGN_API int ign_shard_hash_dev(ign_ctx* ctx, const uint64_t* labels, uint64_t n, int preshift_bits,
+                               int minishard_bits, int shard_bits, uint64_t* labels_out, uint64_t* locations_out,
+                               uint64_t* run_start_out, uint64_t* run_shard_out, uint64_t* n_runs);
+IGN_API int ign_skeleton_restrip_dev(ign_ctx* ctx, const uint8_t* blobs, const uint64_t* offsets, uint64_t n,
+                                     const uint32_t* attrs, int n_attrs, uint8_t* out, uint64_t capacity,
+                                     uint64_t* out_offsets, uint64_t* nbytes);
+IGN_API int ign_shard_assemble_dev(ign_ctx* ctx, const uint64_t* locations, const uint64_t* labels,
+                                   const uint64_t* offsets, uint64_t n, int minishard_bits, uint8_t* shard,
+                                   uint64_t capacity, uint64_t* nbytes);
+
 /* ------------------------------------------------------- cross-sectional area
  * kimimaro.cross_sectional_area (igneous/tasks/skeleton.py:219-226, :400-475); the rule is DESIGN.md §5i.
  * ign_cross_section_normals: HOST arrays.  n_vertices vertices (below 2^32, else IGN_ERR_UNSUPPORTED) of any
