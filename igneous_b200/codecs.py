@@ -44,15 +44,11 @@ def cseg_encode(labels, block_size=(8, 8, 8), ctx=None):
   bx, by, bz = (int(v) for v in block_size)
   args = [ctx.handle, _shim.ptr(arr), _shim.dtype_code(arr.dtype), sx, sy, sz, sc, bx, by, bz]
   n = c.c_uint64(0)
-  gx, gy, gz = -(-sx // bx), -(-sy // by), -(-sz // bz)
-  # worst case: every voxel its own table entry
-  cap = sc * (1 + 2 * gx * gy * gz + (arr.dtype.itemsize // 4 + 1) * gx * gy * gz * bx * by * bz)
-  cap = int(min(cap, 1 << 26))
+  # the worst case, capped at the longest stream the format allows: per channel its offset word and at
+  # most 0xFFFFFF + 1024 words (the encoder refuses longer channels before it looks at the capacity)
+  cap = min(cseg_capacity_words([(sx, sy, sz)], sc, arr.dtype, block_size), sc * (0xFFFFFF + 1024 + 1))
   out = np.empty(cap, dtype=np.uint32)
   _shim.check(ctx.lib.ign_cseg_encode(*args, _shim.ptr(out), cap, c.byref(n)))
-  if n.value > cap:  # does not happen for 24-bit addressable chunks; kept for safety
-    out = np.empty(int(n.value), dtype=np.uint32)
-    _shim.check(ctx.lib.ign_cseg_encode(*args, _shim.ptr(out), n.value, c.byref(n)))
   return out[:int(n.value)].tobytes()
 
 

@@ -13,15 +13,22 @@
 // packed indices; bits in {0,1,2,4,8,16,32}; offsets in u32 words from the channel start.
 // The emission order of oracle/igneous_oracle.c::orc_cseg_encode_* (block raster order, a
 // table is emitted by the FIRST block that uses it) is reproduced exactly, so the streams are
-// byte-identical:
-//   1  k_cseg_scan<T, false>  one warp per block: the distinct values are extracted in
-//      ascending order (repeated warp minimum) -> n, smallest / largest value, 64-bit hash
+// byte-identical.
+//
+// One encoder and one decoder serve every entry point; a single chunk is a batch of one.  N chunks
+// x sc channels are S = N*sc segments, one channel stream each, and all their blocks one global
+// block range (segment-major, raster order inside a segment):
+//   1  k_cb_scan<T, false>  one warp per block: the distinct values are extracted in ascending
+//      order (repeated warp minimum) -> n, smallest / largest value, 64-bit hash (segment included)
 //   2  radix sort of (hash, block) -> the first block of every run of equal hashes is the owner
-//      candidate; k_cseg_verify compares each block's table with its candidate's.  Equal hashes
-//      do not prove equal tables: after a mismatch k_cseg_resolve recomputes every owner by
-//      content, so the owner is always the first block with an identical table
-//   3  exclusive scan of the per-block sizes -> offsets
-//   4  k_cseg_scan<T, true>   the same extraction again, now writing indices, tables, headers
+//      candidate; k_cb_verify compares each block's segment and table with its candidate's.  Equal
+//      hashes do not prove equal tables: after a mismatch k_cb_resolve recomputes every owner by
+//      content, so the owner is always the first block of its segment with an identical table
+//   3  exclusive scan of the per-block sizes (k_cb_sizes) -> offsets; k_cb_segments places every
+//      segment and checks the format's 24-bit table offsets.  Segment s = (chunk i, channel c)
+//      starts at word scan[b0_s] + 2*b0_s + sc*(i + 1) of the concatenated chunk files (chunk i's
+//      sc-word channel table precedes its channels)
+//   4  k_cb_scan<T, true>   the same extraction again, now writing indices, tables, headers
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
@@ -107,81 +114,6 @@ __device__ bool cs_same_table(const T* __restrict__ in, const CsegDims& d, uint6
   return true;
 }
 
-// One warp per block.  WRITE = false: n[b], hash[b] and the smallest / largest value lo[b], hi[b].
-// WRITE = true: the stream.  hash_mask keeps only some bits of the hash (IGN_CSEG_HASH_BITS, a test
-// knob that forces collisions); the hash only groups candidates, k_cseg_verify decides by content.
-template <typename T, bool WRITE, int CS_PER_LANE>  // CS_PER_LANE * 32 >= voxels per block
-__global__ void __launch_bounds__(128)
-    k_cseg_scan(const T* __restrict__ in, CsegDims d, uint64_t nblock, uint32_t* __restrict__ info_n,
-                unsigned long long* __restrict__ hash, unsigned long long hash_mask, unsigned long long* __restrict__ lo,
-                unsigned long long* __restrict__ hi, const uint32_t* __restrict__ enc_off,
-                const uint32_t* __restrict__ tab_off, const uint32_t* __restrict__ owner, uint32_t* __restrict__ out) {
-  constexpr int WORDS = sizeof(T) / 4;
-  const uint32_t lane = threadIdx.x & 31u;
-  const uint64_t b = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5;
-  if (b >= nblock) return;
-  uint64_t val[CS_PER_LANE];
-  uint32_t idx[CS_PER_LANE] = {};
-  const uint32_t have = cs_load<T, CS_PER_LANE>(in, d, b, lane, val);  // bit k: slot k is inside the volume
-  uint32_t todo = have;                                                 // bit k: slot k not classified yet
-  uint32_t n = 0;
-  uint64_t h = 0x9E3779B97F4A7C15ull, first = 0, m = 0;
-  const uint32_t toff = WRITE ? tab_off[b] : 0u;
-  const bool own = WRITE ? (owner[b] == (uint32_t)b) : false;
-  while (__any_sync(CS_FULL, todo != 0)) {
-    m = cs_warp_min<CS_PER_LANE>(val, todo);
-#pragma unroll
-    for (int k = 0; k < CS_PER_LANE; k++)
-      if (((todo >> k) & 1u) && val[k] == m) {
-        idx[k] = n;
-        todo &= ~(1u << k);
-      }
-    if (WRITE) {
-      if (own && lane == 0) {
-        out[toff + n * WORDS] = (uint32_t)m;
-        if (WORDS == 2) out[toff + n * WORDS + 1] = (uint32_t)(m >> 32);
-      }
-    } else {
-      if (n == 0) first = m;
-      h = mix64(h ^ m);
-    }
-    n++;
-  }
-  const uint32_t bits = cs_bits(n);
-  if (!WRITE) {
-    if (lane == 0) {
-      info_n[b] = n;
-      hash[b] = mix64(h + n) & hash_mask;
-      lo[b] = first;
-      hi[b] = m;
-    }
-    return;
-  }
-  // ---- packed indices: word w of the block holds positions [w*32/bits, (w+1)*32/bits)
-  const uint32_t eoff = enc_off[b];
-  if (bits) {
-    const uint32_t per = 32 / bits;             // values per word
-    const uint32_t nwords = (bits * d.bvox + 31) / 32;
-    // every lane contributes its values with atomicOr-free packing: values of one word sit in
-    // `per` consecutive positions, i.e. in `per` consecutive lanes (or the same lane for per > 32)
-#pragma unroll
-    for (int k = 0; k < CS_PER_LANE; k++) {
-      const uint32_t p = lane + 32 * k;
-      if (32 * k >= d.bvox) break;
-      const uint32_t v = ((have >> k) & 1u) ? idx[k] : 0u;
-      uint32_t word = v << ((p % per) * bits);
-      // OR-reduce over the aligned group of `per` lanes (per is a power of two <= 32)
-      for (uint32_t s = 1; s < per; s <<= 1) word |= __shfl_xor_sync(CS_FULL, word, s);
-      if (p < d.bvox && (p % per) == 0 && p / per < nwords) out[eoff + p / per] = word;
-    }
-  }
-  if (lane == 0) {
-    // header: blocks are in raster order at the start of the channel
-    out[2 * b] = toff | (bits << 24);
-    out[2 * b + 1] = eoff;
-  }
-}
-
 __global__ void __launch_bounds__(256) k_iota32(uint32_t* p, uint32_t n) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = i;
@@ -199,77 +131,6 @@ __global__ void __launch_bounds__(256)
                  uint32_t* __restrict__ owner) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) owner[sblock[i]] = sblock[headpos[i]];  // headpos: inclusive max-scan of the head positions
-}
-
-// One warp per block: does the block's table equal the one of the head of its hash run?  Tables
-// of at most two values are fixed by (n, lo, hi); longer ones are compared value by value.  Any
-// mismatch raises *collided and the owners are recomputed by k_cseg_resolve.
-template <typename T, int CS_PER_LANE>
-__global__ void __launch_bounds__(128)
-    k_cseg_verify(const T* __restrict__ in, CsegDims d, uint32_t nblock, const uint32_t* __restrict__ n,
-                  const unsigned long long* __restrict__ lo, const unsigned long long* __restrict__ hi,
-                  const uint32_t* __restrict__ owner, uint32_t* __restrict__ collided) {
-  const uint32_t lane = threadIdx.x & 31u;
-  const uint32_t b = (uint32_t)((blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5);
-  if (b >= nblock) return;
-  const uint32_t o = owner[b];
-  if (o == b) return;
-  bool same = n[o] == n[b] && lo[o] == lo[b] && hi[o] == hi[b];
-  if (same && n[b] > 2) same = cs_same_table<T, CS_PER_LANE>(in, d, o, b, n[b], lane);
-  if (!same && lane == 0) *collided = 1;
-}
-
-// The path taken after a hash collision: one warp per sorted position i.  The owner of block
-// sblock[i] is the first block of its hash run (ascending block order) with an equal table,
-// possibly itself.  Quadratic in the run length; 64-bit hashes of distinct tables rarely meet.
-template <typename T, int CS_PER_LANE>
-__global__ void __launch_bounds__(128)
-    k_cseg_resolve(const T* __restrict__ in, CsegDims d, uint32_t nblock, const uint32_t* __restrict__ n,
-                   const unsigned long long* __restrict__ lo, const unsigned long long* __restrict__ hi,
-                   const uint32_t* __restrict__ sblock, const uint32_t* __restrict__ headpos, uint32_t* __restrict__ owner) {
-  const uint32_t lane = threadIdx.x & 31u;
-  const uint32_t i = (uint32_t)((blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5);
-  if (i >= nblock) return;
-  const uint32_t b = sblock[i];
-  const uint32_t nb = n[b];
-  const unsigned long long lob = lo[b], hib = hi[b];
-  uint32_t own = b;
-  for (uint32_t base = headpos[i]; base < i && own == b; base += 32) {
-    const uint32_t j = base + lane;
-    const uint32_t c = j < i ? sblock[j] : 0u;
-    uint32_t cand = __ballot_sync(CS_FULL, j < i && n[c] == nb && lo[c] == lob && hi[c] == hib);
-    while (cand) {
-      const uint32_t cb = __shfl_sync(CS_FULL, c, __ffs(cand) - 1);
-      if (nb <= 2 || cs_same_table<T, CS_PER_LANE>(in, d, cb, b, nb, lane)) {
-        own = cb;
-        break;
-      }
-      cand &= cand - 1;
-    }
-  }
-  if (lane == 0) owner[b] = own;
-}
-
-template <int WORDS>
-__global__ void __launch_bounds__(256)
-    k_cseg_sizes(const uint32_t* __restrict__ n, const uint32_t* __restrict__ owner, uint32_t nblock, uint32_t bvox,
-                 uint32_t* __restrict__ size) {
-  const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= nblock) return;
-  const uint32_t bits = cs_bits(n[b]);
-  size[b] = (bits * bvox + 31) / 32 + (owner[b] == b ? n[b] * WORDS : 0u);
-}
-
-// offsets from the channel start: indices at 2*nblock + scan[b]; own tables right after them
-__global__ void __launch_bounds__(256)
-    k_cseg_offsets(const uint32_t* __restrict__ n, const uint32_t* __restrict__ owner, const uint32_t* __restrict__ scan,
-                   uint32_t nblock, uint32_t bvox, uint32_t* __restrict__ enc_off, uint32_t* __restrict__ tab_off) {
-  const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= nblock) return;
-  enc_off[b] = 2 * nblock + scan[b];
-  const uint32_t o = owner[b];
-  const uint32_t obits = cs_bits(n[o]);
-  tab_off[b] = 2 * nblock + scan[o] + (obits * bvox + 31) / 32;
 }
 
 // value of voxel (x, y, z) in block b of one channel stream of nwords words; false: malformed stream
@@ -297,19 +158,6 @@ __device__ __forceinline__ bool cs_decode_voxel(const uint32_t* __restrict__ in,
   return true;
 }
 
-template <typename T>
-__global__ void __launch_bounds__(256)
-    k_cseg_decode(const uint32_t* __restrict__ in, uint64_t nwords, CsegDims d, T* __restrict__ out, uint32_t* err) {
-  const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  const uint64_t n = (uint64_t)d.sx * d.sy * d.sz;
-  if (i >= n) return;
-  const uint32_t x = (uint32_t)(i % d.sx), y = (uint32_t)((i / d.sx) % d.sy), z = (uint32_t)(i / ((uint64_t)d.sx * d.sy));
-  const uint64_t b = (x / d.bx) + (uint64_t)d.gx * ((y / d.by) + (uint64_t)d.gy * (z / d.bz));
-  uint64_t v;
-  if (!cs_decode_voxel<T>(in, nwords, d, x, y, z, b, &v)) { *err = 1; return; }
-  out[i] = (T)v;
-}
-
 static int cseg_dims(uint64_t sx, uint64_t sy, uint64_t sz, uint32_t bx, uint32_t by, uint32_t bz, CsegDims* d) {
   IGN_REQUIRE(sx && sy && sz && bx && by && bz, IGN_ERR_INVALID, "cseg: empty chunk or block");
   IGN_REQUIRE((uint64_t)bx * by * bz <= CS_MAX_BVOX, IGN_ERR_UNSUPPORTED, "cseg: blocks of more than %d voxels are not supported", CS_MAX_BVOX);
@@ -324,124 +172,7 @@ static int cseg_dims(uint64_t sx, uint64_t sy, uint64_t sz, uint32_t bx, uint32_
   return IGN_OK;
 }
 
-// cub temporary bytes of one channel of nb blocks
-static size_t cseg_tmp_bytes(uint32_t nb) {
-  size_t sortb = 0, scanb = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, sortb, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                  (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)nb);
-  cub::DeviceScan::ExclusiveSum(nullptr, scanb, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)nb + 1);
-  {
-    size_t mb = 0;
-    cub::DeviceScan::InclusiveScan(nullptr, mb, (const uint32_t*)nullptr, (uint32_t*)nullptr, cub::Max(), (int)nb);
-    if (mb > scanb) scanb = mb;
-  }
-  return (sortb > scanb ? sortb : scanb) + 256;
-}
-
-// one channel; out_dev may be NULL (size query).  *n_words = words of the channel stream.
-template <typename T>
-static int cseg_encode_channel(ign_ctx* ctx, const T* in, const CsegDims& d, uint32_t* out_dev, uint64_t cap_words,
-                               uint64_t* n_words) {
-  constexpr int WORDS = sizeof(T) / 4;
-  const uint32_t nb = d.gx * d.gy * d.gz;
-  const size_t tmpb = cseg_tmp_bytes(nb);
-  unsigned long long hash_mask = ~0ull;
-  if (const char* e = getenv("IGN_CSEG_HASH_BITS")) {
-    const int k = atoi(e);
-    hash_mask = k >= 64 ? ~0ull : k <= 0 ? 0ull : (1ull << k) - 1;
-  }
-  ScratchFrame f(ctx);
-  unsigned long long *hash, *shash, *lo, *hi;
-  uint32_t *n, *blk, *sblk, *owner, *size, *scan, *enc_off, *tab_off, *collided;
-  void* tmp;
-  IGN_TRY(f.take(&hash, nb));
-  IGN_TRY(f.take(&shash, nb));
-  IGN_TRY(f.take(&lo, nb));
-  IGN_TRY(f.take(&hi, nb));
-  IGN_TRY(f.take(&n, (size_t)nb + 1));
-  IGN_TRY(f.take(&blk, (size_t)nb + 1));
-  IGN_TRY(f.take(&sblk, (size_t)nb + 1));
-  IGN_TRY(f.take(&owner, (size_t)nb + 1));
-  IGN_TRY(f.take(&size, (size_t)nb + 1));
-  IGN_TRY(f.take(&scan, (size_t)nb + 1));
-  IGN_TRY(f.take(&enc_off, (size_t)nb + 1));
-  IGN_TRY(f.take(&tab_off, (size_t)nb + 1));
-  IGN_TRY(f.take(&collided, 1));
-  IGN_TRY(f.take(&tmp, tmpb));
-#define CS_LAUNCH_PL(kernel, ...)                                                      \
-  do {                                                                                 \
-    if (d.bvox <= 512) IGN_LAUNCH(ctx, (kernel<T, 16>), gw, 128, 0, __VA_ARGS__);     \
-    else IGN_LAUNCH(ctx, (kernel<T, 32>), gw, 128, 0, __VA_ARGS__);                    \
-  } while (0)
-  const unsigned gw = blocks_for((uint64_t)nb * 32, 128);
-  if (d.bvox <= 512)
-    IGN_LAUNCH(ctx, (k_cseg_scan<T, false, 16>), gw, 128, 0, in, d, (uint64_t)nb, n, hash, hash_mask, lo, hi,
-               (const uint32_t*)nullptr, (const uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr);
-  else
-    IGN_LAUNCH(ctx, (k_cseg_scan<T, false, 32>), gw, 128, 0, in, d, (uint64_t)nb, n, hash, hash_mask, lo, hi,
-               (const uint32_t*)nullptr, (const uint32_t*)nullptr, (const uint32_t*)nullptr, (uint32_t*)nullptr);
-  IGN_LAUNCH(ctx, k_iota32, blocks_for(nb, 256), 256, 0, blk, nb);
-  {
-    size_t tb = tmpb;
-    IGN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, hash, shash, blk, sblk, (int)nb, 0, 64, ctx->stream));
-    ctx->launches += 9;
-  }
-  IGN_LAUNCH(ctx, k_cseg_heads, blocks_for(nb, 256), 256, 0, shash, nb, enc_off);  // enc_off / tab_off: free until the offsets pass
-  {
-    size_t tb = tmpb;
-    IGN_CUDA(cub::DeviceScan::InclusiveScan(tmp, tb, enc_off, tab_off, cub::Max(), (int)nb, ctx->stream));
-    ctx->launches += 2;
-  }
-  IGN_LAUNCH(ctx, k_cseg_owner, blocks_for(nb, 256), 256, 0, tab_off, sblk, nb, owner);
-  IGN_CUDA(cudaMemsetAsync(collided, 0, 4, ctx->stream));
-  CS_LAUNCH_PL(k_cseg_verify, in, d, nb, n, (const unsigned long long*)lo, (const unsigned long long*)hi,
-               (const uint32_t*)owner, collided);
-  // the collision flag comes back with `total`; only after a collision is there a second round trip
-  uint32_t total = 0, hcollided = 0;
-  for (int pass = 0;; pass++) {
-    IGN_LAUNCH(ctx, (k_cseg_sizes<WORDS>), blocks_for(nb, 256), 256, 0, n, owner, nb, d.bvox, size);
-    IGN_CUDA(cudaMemsetAsync(size + nb, 0, 4, ctx->stream));
-    {
-      size_t tb = tmpb;
-      IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, size, scan, (int)nb + 1, ctx->stream));
-      ctx->launches += 2;
-    }
-    IGN_TRY(small_d2h(ctx, &total, scan + nb, 4));
-    if (pass == 0) IGN_TRY(small_d2h(ctx, &hcollided, collided, 4));
-    IGN_TRY(small_sync(ctx));
-    if (pass > 0 || hcollided == 0) break;
-    CS_LAUNCH_PL(k_cseg_resolve, in, d, nb, n, (const unsigned long long*)lo, (const unsigned long long*)hi,
-                 (const uint32_t*)sblk, (const uint32_t*)tab_off, owner);
-  }
-  const uint64_t words = 2ull * nb + total;
-  *n_words = words;
-  if (words > 0xFFFFFFull + 1024) {
-    set_error("cseg: the encoded chunk (%llu words) exceeds the format's 24-bit table offsets", (unsigned long long)words);
-    return IGN_ERR_OVERFLOW;
-  }
-  if (out_dev != nullptr && words <= cap_words) {
-    IGN_LAUNCH(ctx, k_cseg_offsets, blocks_for(nb, 256), 256, 0, n, owner, scan, nb, d.bvox, enc_off, tab_off);
-    if (d.bvox <= 512)
-      IGN_LAUNCH(ctx, (k_cseg_scan<T, true, 16>), gw, 128, 0, in, d, (uint64_t)nb, (uint32_t*)nullptr, (unsigned long long*)nullptr,
-                 hash_mask, (unsigned long long*)nullptr, (unsigned long long*)nullptr, enc_off, tab_off, owner, out_dev);
-    else
-      IGN_LAUNCH(ctx, (k_cseg_scan<T, true, 32>), gw, 128, 0, in, d, (uint64_t)nb, (uint32_t*)nullptr, (unsigned long long*)nullptr,
-                 hash_mask, (unsigned long long*)nullptr, (unsigned long long*)nullptr, enc_off, tab_off, owner, out_dev);
-  }
-  return IGN_OK;
-#undef CS_LAUNCH_PL
-}
-
-
-// ------------------------------------------------------------------ batches
-// N chunks x sc channels are S = N*sc segments, one channel stream each, and all their blocks one
-// global block range (segment-major, raster order inside a segment).  The passes of the one-chunk
-// encoder above run once over that range: a table's owner is still the first block OF ITS SEGMENT
-// with an identical table (the segment joins the hash, and verify / resolve compare it), so every
-// chunk's stream is the one cseg_encode_channel writes for it.  One exclusive scan over all blocks
-// places every segment: segment s = (chunk i, channel c) starts at word
-//   scan[b0_s] + 2*b0_s + sc*(i + 1)
-// of the concatenated chunk files (chunk i's sc-word channel table precedes its channels).
+// one segment: channel c of chunk i
 struct CsegSeg {
   CsegDims d;
   uint64_t in_off;    // element offset of the channel in the packed chunks
@@ -459,9 +190,13 @@ __device__ __forceinline__ uint64_t cb_find(const CsegSeg* __restrict__ segs, ui
   return lo;
 }
 
-// k_cb_scan and k_cb_resolve hold their segment's dims in registers, where the one-chunk kernels read
-// them from the parameter bank; under __launch_bounds__(128) ptxas spilled a few of them (16 / 40
-// bytes).  An explicit register cap lets it keep everything in registers.  Both launch 128 threads.
+// One warp per block.  WRITE = false: n[g], the block's segment, hash[g] and the smallest / largest
+// value lo[g], hi[g].  WRITE = true: the stream.  hash_mask keeps only some bits of the hash
+// (IGN_CSEG_HASH_BITS, a test knob that forces collisions); the hash only groups candidates,
+// k_cb_verify decides by content.
+// k_cb_scan and k_cb_resolve hold their segment's dims in registers; under __launch_bounds__(128)
+// ptxas spilled a few of them (16 / 40 bytes).  An explicit register cap lets it keep everything in
+// registers.  Both launch 128 threads.
 template <typename T, bool WRITE, int CS_PER_LANE>
 __global__ void __maxnreg__(128)
     k_cb_scan(const T* __restrict__ in, const CsegSeg* __restrict__ segs, uint64_t nseg, uint64_t nblock, uint64_t sc,
@@ -526,9 +261,12 @@ __global__ void __maxnreg__(128)
     }
     return;
   }
+  // packed indices: word w of the block holds positions [w*32/bits, (w+1)*32/bits)
   if (bits) {
-    const uint32_t per = 32 / bits;
+    const uint32_t per = 32 / bits;  // values per word
     const uint32_t nwords = (bits * d.bvox + 31) / 32;
+    // the values of one word sit in `per` consecutive positions, i.e. in `per` consecutive lanes:
+    // OR-reduce over that aligned group of lanes (per is a power of two <= 32)
 #pragma unroll
     for (int k = 0; k < CS_PER_LANE; k++) {
       const uint32_t p = lane + 32 * k;
@@ -608,11 +346,12 @@ __global__ void __launch_bounds__(256)
   size[g] = (cs_bits(n[g]) * bvox + 31) / 32 + (owner[g] == g ? n[g] * WORDS : 0u);
 }
 
-// one thread per segment: its stream length (-> *too_long past the format's 24-bit offsets), its
-// entry in its chunk's channel table, and (channel 0) the chunk's word offset in the output
+// one thread per segment: its stream length (-> *too_long past the format's 24-bit offsets); with out
+// set, also its entry in its chunk's channel table, (channel 0) the chunk's word offset in the output and
+// (the last segment) the end of the output
 __global__ void __launch_bounds__(256)
     k_cb_segments(const CsegSeg* __restrict__ segs, uint64_t nseg, uint64_t sc, const unsigned long long* __restrict__ scan,
-                  uint32_t* __restrict__ too_long, uint32_t* __restrict__ out, unsigned long long* __restrict__ chunk_off) {
+                  uint32_t* __restrict__ too_long, uint32_t* __restrict__ out, unsigned long long* __restrict__ offsets) {
   const uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (s >= nseg) return;
   const CsegSeg& S = segs[s];
@@ -620,9 +359,11 @@ __global__ void __launch_bounds__(256)
   const uint64_t start = scan[S.b0] + 2 * S.b0 + sc * (S.chunk + 1);
   const uint64_t words = 2 * nb + scan[S.b0 + nb] - scan[S.b0];
   if (words > 0xFFFFFFull + 1024) atomicMax(too_long, 1u);
+  if (!out) return;
   const uint64_t cstart = scan[segs[s - S.chan].b0] + 2 * segs[s - S.chan].b0 + sc * S.chunk;  // chunk i's first word
-  if (out) out[cstart + S.chan] = (uint32_t)(start - cstart);
-  if (S.chan == 0) chunk_off[S.chunk] = cstart;
+  out[cstart + S.chan] = (uint32_t)(start - cstart);
+  if (S.chan == 0) offsets[S.chunk] = cstart;
+  if (s == nseg - 1) offsets[S.chunk + 1] = start + words;
 }
 
 template <typename T>
@@ -695,7 +436,7 @@ static int cseg_encode_batch(ign_ctx* ctx, const T* in, const std::vector<CsegSe
   const size_t tmpb = std::max(sortb, std::max(scanb, maxb)) + 256;
   ScratchFrame f(ctx);
   CsegSeg* segs;
-  unsigned long long *hash, *shash, *lo, *hi, *scan, *chunk_off;
+  unsigned long long *hash, *shash, *lo, *hi, *scan;
   unsigned long long* size;
   uint32_t *cnt, *bseg, *blk, *sblk, *owner, *headpos, *runhead, *flags;
   void* tmp;
@@ -705,7 +446,6 @@ static int cseg_encode_batch(ign_ctx* ctx, const T* in, const std::vector<CsegSe
   IGN_TRY(f.take(&lo, nb));
   IGN_TRY(f.take(&hi, nb));
   IGN_TRY(f.take(&scan, (size_t)nb + 1));
-  IGN_TRY(f.take(&chunk_off, n + 1));
   IGN_TRY(f.take(&cnt, (size_t)nb + 1));
   IGN_TRY(f.take(&bseg, (size_t)nb + 1));
   IGN_TRY(f.take(&blk, (size_t)nb + 1));
@@ -716,7 +456,7 @@ static int cseg_encode_batch(ign_ctx* ctx, const T* in, const std::vector<CsegSe
   IGN_TRY(f.take(&runhead, (size_t)nb + 1));
   IGN_TRY(f.take(&flags, 2));  // [collided, too_long]
   IGN_TRY(f.take(&tmp, tmpb));
-  IGN_CUDA(cudaMemcpyAsync(segs, hsegs.data(), nseg * sizeof(CsegSeg), cudaMemcpyHostToDevice, ctx->stream));
+  IGN_TRY(small_h2d(ctx, segs, hsegs.data(), nseg * sizeof(CsegSeg)));
   IGN_CUDA(cudaMemsetAsync(flags, 0, 8, ctx->stream));
   const unsigned gw = blocks_for((uint64_t)nb * 32, 128);
   const bool wide = bvox > 512;
@@ -746,38 +486,39 @@ static int cseg_encode_batch(ign_ctx* ctx, const T* in, const std::vector<CsegSe
   IGN_LAUNCH(ctx, k_cseg_owner, blocks_for(nb, 256), 256, 0, runhead, sblk, nb, owner);
   CB_LAUNCH_PL(k_cb_verify, in, (const CsegSeg*)segs, nb, (const uint32_t*)bseg, (const uint32_t*)cnt,
                (const unsigned long long*)lo, (const unsigned long long*)hi, (const uint32_t*)owner, flags);
+  // the collision flag comes back with the total; only after a collision is there a second round trip
   uint32_t hflags[2] = {0, 0};
-  IGN_TRY(small_d2h(ctx, hflags, flags, 4));
-  IGN_TRY(small_sync(ctx));
-  if (hflags[0])
+  unsigned long long total_data = 0;
+  for (int pass = 0;; pass++) {
+    IGN_LAUNCH(ctx, (k_cb_sizes<WORDS>), blocks_for(nb, 256), 256, 0, (const CsegSeg*)segs, (const uint32_t*)bseg,
+               (const uint32_t*)cnt, (const uint32_t*)owner, nb, size);
+    IGN_CUDA(cudaMemsetAsync(size + nb, 0, 8, ctx->stream));
+    {
+      size_t tb = tmpb;
+      IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, size, scan, (int)nb + 1, ctx->stream));
+      ctx->launches += 2;
+    }
+    // the sizes pass: the 24-bit check, nothing written yet
+    IGN_LAUNCH(ctx, k_cb_segments, blocks_for(nseg, 256), 256, 0, (const CsegSeg*)segs, nseg, sc,
+               (const unsigned long long*)scan, flags + 1, (uint32_t*)nullptr, (unsigned long long*)nullptr);
+    IGN_TRY(small_d2h(ctx, &total_data, scan + nb, 8));
+    IGN_TRY(small_d2h(ctx, hflags, flags, 8));
+    IGN_TRY(small_sync(ctx));
+    if (pass > 0 || hflags[0] == 0) break;
     CB_LAUNCH_PL(k_cb_resolve, in, (const CsegSeg*)segs, nb, (const uint32_t*)bseg, (const uint32_t*)cnt,
                  (const unsigned long long*)lo, (const unsigned long long*)hi, (const uint32_t*)sblk,
                  (const uint32_t*)runhead, owner);
-#undef CB_LAUNCH_PL
-  IGN_LAUNCH(ctx, (k_cb_sizes<WORDS>), blocks_for(nb, 256), 256, 0, (const CsegSeg*)segs, (const uint32_t*)bseg,
-             (const uint32_t*)cnt, (const uint32_t*)owner, nb, size);
-  IGN_CUDA(cudaMemsetAsync(size + nb, 0, 8, ctx->stream));
-  {
-    size_t tb = tmpb;
-    IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, size, scan, (int)nb + 1, ctx->stream));
-    ctx->launches += 2;
+    IGN_CUDA(cudaMemsetAsync(flags + 1, 0, 4, ctx->stream));  // too_long again, from the resolved sizes
   }
-  // the sizes pass: chunk offsets and the 24-bit check, nothing written yet
-  IGN_LAUNCH(ctx, k_cb_segments, blocks_for(nseg, 256), 256, 0, (const CsegSeg*)segs, nseg, sc,
-             (const unsigned long long*)scan, flags + 1, (uint32_t*)nullptr, chunk_off);
-  unsigned long long total_data = 0;
-  IGN_TRY(small_d2h(ctx, &total_data, scan + nb, 8));
-  IGN_TRY(small_d2h(ctx, hflags + 1, flags + 1, 4));
-  IGN_TRY(small_sync(ctx));
+#undef CB_LAUNCH_PL
   const uint64_t total = total_data + 2ull * nb + sc * n;
   *n_words = total;
   IGN_REQUIRE(hflags[1] == 0, IGN_ERR_OVERFLOW,
-              "cseg batch: a chunk's channel stream exceeds the format's 24-bit table offsets");
-  IGN_REQUIRE(total <= cap_words, IGN_ERR_OVERFLOW, "cseg batch: %llu words needed, the output holds %llu",
+              "cseg: a chunk's channel stream exceeds the format's 24-bit table offsets");
+  IGN_REQUIRE(total <= cap_words, IGN_ERR_OVERFLOW, "cseg: %llu words needed, the output holds %llu",
               (unsigned long long)total, (unsigned long long)cap_words);
-  IGN_CUDA(cudaMemcpyAsync(chunk_off + n, &total, 8, cudaMemcpyHostToDevice, ctx->stream));
   IGN_LAUNCH(ctx, k_cb_segments, blocks_for(nseg, 256), 256, 0, (const CsegSeg*)segs, nseg, sc,
-             (const unsigned long long*)scan, flags + 1, out, chunk_off);
+             (const unsigned long long*)scan, flags + 1, out, (unsigned long long*)offsets);
   if (!wide)
     IGN_LAUNCH(ctx, (k_cb_scan<T, true, 16>), gw, 128, 0, in, (const CsegSeg*)segs, nseg, nblock, sc, cnt,
                (uint32_t*)nullptr, (unsigned long long*)nullptr, hash_mask, (unsigned long long*)nullptr,
@@ -786,7 +527,43 @@ static int cseg_encode_batch(ign_ctx* ctx, const T* in, const std::vector<CsegSe
     IGN_LAUNCH(ctx, (k_cb_scan<T, true, 32>), gw, 128, 0, in, (const CsegSeg*)segs, nseg, nblock, sc, cnt,
                (uint32_t*)nullptr, (unsigned long long*)nullptr, hash_mask, (unsigned long long*)nullptr,
                (unsigned long long*)nullptr, (const unsigned long long*)scan, (const uint32_t*)owner, out);
-  IGN_CUDA(cudaMemcpyAsync(offsets, chunk_off, (n + 1) * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+  return IGN_OK;
+}
+
+// n streams, stream i at streams[word_offsets[i] .. word_offsets[i+1]) (offsets on the host), of the
+// chunks of shapes[i] (host n x 3) -> the packed chunks in out
+static int cseg_decode_batch(ign_ctx* ctx, const uint32_t* streams, const uint64_t* word_offsets, uint64_t n_streams,
+                             int dtype, const uint32_t* shapes, uint64_t sc, uint32_t bx, uint32_t by, uint32_t bz,
+                             void* out) {
+  for (uint64_t i = 0; i < n_streams; i++)
+    IGN_REQUIRE(word_offsets[i] <= word_offsets[i + 1], IGN_ERR_INVALID, "cseg: stream %llu has a negative length",
+                (unsigned long long)i);
+  std::vector<CsegSeg> hsegs;
+  uint64_t nblock = 0, most = 0;
+  IGN_TRY(cb_segments(shapes, n_streams, sc, bx, by, bz, hsegs, &nblock));
+  for (const CsegSeg& S : hsegs) most = std::max(most, (uint64_t)S.d.sx * S.d.sy * S.d.sz);
+  ScratchFrame f(ctx);
+  CsegSeg* segs;
+  unsigned long long* woff;
+  uint32_t* bad;
+  IGN_TRY(f.take(&segs, hsegs.size()));
+  IGN_TRY(f.take(&woff, n_streams + 1));
+  IGN_TRY(f.take(&bad, 1));
+  IGN_CUDA(cudaMemcpyAsync(segs, hsegs.data(), hsegs.size() * sizeof(CsegSeg), cudaMemcpyHostToDevice, ctx->stream));
+  IGN_CUDA(cudaMemcpyAsync(woff, word_offsets, (n_streams + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
+  IGN_CUDA(cudaMemsetAsync(bad, 0xFF, 4, ctx->stream));
+  const uint64_t gx = std::min<uint64_t>(blocks_for(most, 256), 1024);
+  const dim3 grid((unsigned)gx, (unsigned)std::min<uint64_t>(hsegs.size(), 65535));
+  if (dtype == IGN_U32)
+    IGN_LAUNCH(ctx, k_cb_decode<uint32_t>, grid, 256, 0, streams, (const unsigned long long*)woff, (const CsegSeg*)segs,
+               (uint64_t)hsegs.size(), sc, (uint32_t*)out, bad);
+  else
+    IGN_LAUNCH(ctx, k_cb_decode<uint64_t>, grid, 256, 0, streams, (const unsigned long long*)woff, (const CsegSeg*)segs,
+               (uint64_t)hsegs.size(), sc, (uint64_t*)out, bad);
+  uint32_t hbad = 0;
+  IGN_TRY(small_d2h(ctx, &hbad, bad, 4));
+  IGN_TRY(small_sync(ctx));
+  IGN_REQUIRE(hbad == 0xFFFFFFFFu, IGN_ERR_INVALID, "cseg: stream %u is malformed", hbad);
   return IGN_OK;
 }
 
@@ -800,25 +577,24 @@ int ign_cseg_encode_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx
                         uint64_t sc, uint32_t bx, uint32_t by, uint32_t bz, uint32_t* out, uint64_t cap_words,
                         uint64_t* n_words) {
   IGN_TRY(activate(ctx));
-  IGN_REQUIRE(labels && n_words && sc >= 1, IGN_ERR_INVALID, "null argument");
+  IGN_REQUIRE(labels && out && n_words && sc >= 1, IGN_ERR_INVALID, "null argument");
   IGN_REQUIRE(dtype == IGN_U32 || dtype == IGN_U64, IGN_ERR_UNSUPPORTED, "compressed_segmentation holds uint32 / uint64 labels");
   CsegDims d;
   IGN_TRY(cseg_dims(sx, sy, sz, bx, by, bz, &d));
-  const uint64_t n = sx * sy * sz;
-  uint64_t at = sc;  // the channel offset table comes first
-  std::vector<uint32_t> chan_off(sc, 0);
-  for (uint64_t c = 0; c < sc; c++) {
-    chan_off[c] = (uint32_t)at;
-    uint64_t w = 0;
-    uint32_t* dst = (out && at < cap_words) ? out + at : nullptr;
-    const uint64_t room = (out && at < cap_words) ? cap_words - at : 0;
-    if (dtype == IGN_U32) IGN_TRY(cseg_encode_channel<uint32_t>(ctx, (const uint32_t*)labels + c * n, d, dst, room, &w));
-    else IGN_TRY(cseg_encode_channel<uint64_t>(ctx, (const uint64_t*)labels + c * n, d, dst, room, &w));
-    at += w;
-  }
-  *n_words = at;
-  if (out && at <= cap_words) IGN_TRY(small_h2d(ctx, out, chan_off.data(), sc * 4));
-  if (out) IGN_CUDA(cudaStreamSynchronize(ctx->stream));
+  const uint32_t shape[3] = {d.sx, d.sy, d.sz};
+  std::vector<CsegSeg> segs;
+  uint64_t nblock = 0;
+  IGN_TRY(cb_segments(shape, 1, sc, bx, by, bz, segs, &nblock));
+  ScratchFrame f(ctx);
+  uint64_t* offsets;  // {0, *n_words}
+  IGN_TRY(f.take(&offsets, 2));
+  if (dtype == IGN_U32)
+    IGN_TRY(cseg_encode_batch<uint32_t>(ctx, (const uint32_t*)labels, segs, nblock, 1, sc, d.bvox, out, cap_words,
+                                        offsets, n_words));
+  else
+    IGN_TRY(cseg_encode_batch<uint64_t>(ctx, (const uint64_t*)labels, segs, nblock, 1, sc, d.bvox, out, cap_words,
+                                        offsets, n_words));
+  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   return IGN_OK;
 }
 
@@ -829,27 +605,9 @@ int ign_cseg_decode_dev(ign_ctx* ctx, const uint32_t* in, uint64_t n_words, int 
   IGN_REQUIRE(dtype == IGN_U32 || dtype == IGN_U64, IGN_ERR_UNSUPPORTED, "compressed_segmentation holds uint32 / uint64 labels");
   CsegDims d;
   IGN_TRY(cseg_dims(sx, sy, sz, bx, by, bz, &d));
-  const uint64_t n = sx * sy * sz;
-  std::vector<uint32_t> chan_off(sc, 0);
-  IGN_CUDA(cudaMemcpyAsync(chan_off.data(), in, sc * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  ScratchFrame f(ctx);
-  uint32_t* err;
-  IGN_TRY(f.take(&err, 64));
-  IGN_CUDA(cudaMemsetAsync(err, 0, 4, ctx->stream));
-  for (uint64_t c = 0; c < sc; c++) {
-    const uint64_t base = chan_off[c];
-    IGN_REQUIRE(base <= n_words, IGN_ERR_INVALID, "cseg: channel offset outside the stream");
-    if (dtype == IGN_U32)
-      IGN_LAUNCH(ctx, (k_cseg_decode<uint32_t>), blocks_for(n, 256), 256, 0, in + base, n_words - base, d, (uint32_t*)out + c * n, err);
-    else
-      IGN_LAUNCH(ctx, (k_cseg_decode<uint64_t>), blocks_for(n, 256), 256, 0, in + base, n_words - base, d, (uint64_t*)out + c * n, err);
-  }
-  uint32_t herr = 0;
-  IGN_CUDA(cudaMemcpyAsync(&herr, err, 4, cudaMemcpyDeviceToHost, ctx->stream));
-  IGN_CUDA(cudaStreamSynchronize(ctx->stream));
-  IGN_REQUIRE(herr == 0, IGN_ERR_INVALID, "cseg: malformed stream");
-  return IGN_OK;
+  const uint32_t shape[3] = {d.sx, d.sy, d.sz};
+  const uint64_t word_offsets[2] = {0, n_words};
+  return cseg_decode_batch(ctx, in, word_offsets, 1, dtype, shape, sc, bx, by, bz, out);
 }
 
 int ign_cseg_encode_batch_dev(ign_ctx* ctx, const void* chunks, int dtype, uint64_t n_chunks, const uint32_t* shapes,
@@ -880,40 +638,11 @@ int ign_cseg_decode_batch_dev(ign_ctx* ctx, const uint32_t* streams, const uint6
               "cseg batch: null argument");
   IGN_REQUIRE(dtype == IGN_U32 || dtype == IGN_U64, IGN_ERR_UNSUPPORTED, "compressed_segmentation holds uint32 / uint64 labels");
   if (n_streams == 0) return IGN_OK;
-  for (uint64_t i = 0; i < n_streams; i++)
-    IGN_REQUIRE(word_offsets[i] <= word_offsets[i + 1], IGN_ERR_INVALID, "cseg batch: stream %llu has a negative length",
-                (unsigned long long)i);
-  std::vector<CsegSeg> hsegs;
-  uint64_t nblock = 0, most = 0;
-  IGN_TRY(cb_segments(shapes, n_streams, sc, bx, by, bz, hsegs, &nblock));
-  for (const CsegSeg& S : hsegs) most = std::max(most, (uint64_t)S.d.sx * S.d.sy * S.d.sz);
-  ScratchFrame f(ctx);
-  CsegSeg* segs;
-  unsigned long long* woff;
-  uint32_t* bad;
-  IGN_TRY(f.take(&segs, hsegs.size()));
-  IGN_TRY(f.take(&woff, n_streams + 1));
-  IGN_TRY(f.take(&bad, 1));
-  IGN_CUDA(cudaMemcpyAsync(segs, hsegs.data(), hsegs.size() * sizeof(CsegSeg), cudaMemcpyHostToDevice, ctx->stream));
-  IGN_CUDA(cudaMemcpyAsync(woff, word_offsets, (n_streams + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
-  IGN_CUDA(cudaMemsetAsync(bad, 0xFF, 4, ctx->stream));
-  const uint64_t gx = std::min<uint64_t>(blocks_for(most, 256), 1024);
-  const dim3 grid((unsigned)gx, (unsigned)std::min<uint64_t>(hsegs.size(), 65535));
-  if (dtype == IGN_U32)
-    IGN_LAUNCH(ctx, k_cb_decode<uint32_t>, grid, 256, 0, streams, (const unsigned long long*)woff, (const CsegSeg*)segs,
-               (uint64_t)hsegs.size(), sc, (uint32_t*)out, bad);
-  else
-    IGN_LAUNCH(ctx, k_cb_decode<uint64_t>, grid, 256, 0, streams, (const unsigned long long*)woff, (const CsegSeg*)segs,
-               (uint64_t)hsegs.size(), sc, (uint64_t*)out, bad);
-  uint32_t hbad = 0;
-  IGN_TRY(small_d2h(ctx, &hbad, bad, 4));
-  IGN_TRY(small_sync(ctx));
-  IGN_REQUIRE(hbad == 0xFFFFFFFFu, IGN_ERR_INVALID, "cseg batch: stream %u is malformed", hbad);
-  return IGN_OK;
+  return cseg_decode_batch(ctx, streams, word_offsets, n_streams, dtype, shapes, sc, bx, by, bz, out);
 }
 
-// host-buffer wrappers: encode returns the words needed in *n_words (call with out == NULL first, or
-// with a capacity of sc + 2*blocks + 3*voxels words, the worst case)
+// host-buffer wrappers: encode needs room for the whole stream; the worst case is sc + 2*blocks +
+// (label words + 1)*voxels words, and a shorter out fails with *n_words = the words needed
 int ign_cseg_encode(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz, uint64_t sc,
                     uint32_t bx, uint32_t by, uint32_t bz, uint32_t* out, uint64_t cap_words, uint64_t* n_words) {
   CsegDims dims;
@@ -921,7 +650,7 @@ int ign_cseg_encode(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, ui
   std::vector<HostBuf> bufs = {{labels, nullptr, sx * sy * sz * sc * dtype_size(dtype)}, {nullptr, out, cap_words * 4}};
   return staged(ctx, bufs, [&](void* const* d) -> int {
     IGN_TRY(ign_cseg_encode_dev(ctx, d[0], dtype, sx, sy, sz, sc, bx, by, bz, (uint32_t*)d[1], cap_words, n_words));
-    bufs[1].bytes = *n_words <= cap_words ? *n_words * 4 : 0;
+    bufs[1].bytes = *n_words * 4;
     return IGN_OK;
   });
 }

@@ -632,8 +632,9 @@ IGN_API int ign_mesh_free(ign_mesher* m);
  * (igneous/tasks/image/image.py:95-100 `vol[new_bounds] = mipped`, ccl.py:346-356 RelabelCCLTask's
  * output, igneous/task_creation/common.py:215-236 set_encoding).  labels: Fortran order [x,y,z,c],
  * uint32 / uint64; block (bx,by,bz) is (8,8,8) in every Precomputed layer.  The stream is the
- * uint32 word sequence of the file.  encode: *n_words = words needed; nothing is written when
- * out is NULL or cap_words is too small.  One call = one chunk (24-bit table offsets). */
+ * uint32 word sequence of the file.  encode: *n_words = words of the stream; when they are more
+ * than cap_words nothing is written and the call fails with IGN_ERR_OVERFLOW (*n_words still
+ * reports the need).  One call = one chunk (24-bit table offsets). */
 IGN_API int ign_cseg_encode(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy, uint64_t sz,
                             uint64_t sc, uint32_t bx, uint32_t by, uint32_t bz, uint32_t* out,
                             uint64_t cap_words, uint64_t* n_words);
@@ -654,7 +655,7 @@ IGN_API int ign_cseg_decode_dev(ign_ctx* ctx, const uint32_t* in, uint64_t n_wor
  * i as out[offsets[i] : offsets[i+1]] in words; *n_words = words of all files.  One size pass for the
  * whole batch; when the files need more than cap_words words nothing is written and the call fails
  * with IGN_ERR_OVERFLOW (*n_words still reports the need).  Every file is byte-identical to what
- * ign_cseg_encode writes for that chunk alone.
+ * the CPU oracle's encoder (oracle/igneous_oracle.c::orc_cseg_encode_*) writes for that chunk alone.
  * decode: stream i is streams[word_offsets[i] : word_offsets[i+1]] (word_offsets on the host); a
  * malformed stream fails the call with IGN_ERR_INVALID, and the message names the first such index. */
 IGN_API int ign_cseg_encode_batch_dev(ign_ctx* ctx, const void* chunks, int dtype, uint64_t n_chunks,

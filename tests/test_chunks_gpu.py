@@ -1,5 +1,5 @@
 """ign_chunks_place_dev / ign_chunks_cut_dev against numpy slicing, and the compressed_segmentation
-batch entries against the one-chunk ign_cseg_encode / ign_cseg_decode, chunk by chunk."""
+batch entries against the CPU oracle's encoder and decoder, chunk by chunk."""
 import ctypes as c
 
 import numpy as np
@@ -123,7 +123,7 @@ def _mixed_chunks(dtype, sc, rng):
 @pytest.mark.parametrize("dtype", [np.uint32, np.uint64])
 @pytest.mark.parametrize("block", [(8, 8, 8), (4, 4, 2)])
 @pytest.mark.parametrize("sc", [1, 2])
-def test_cseg_batch_equals_one_chunk_codec(ctx, dtype, block, sc):
+def test_cseg_batch_equals_oracle(ctx, oracle, dtype, block, sc):
   from igneous_b200 import codecs
   from igneous_b200.storage import DeviceCutout, _upload_bytes
   chunks = _mixed_chunks(dtype, sc, np.random.default_rng(3))
@@ -131,7 +131,7 @@ def test_cseg_batch_equals_one_chunk_codec(ctx, dtype, block, sc):
   shapes = [ch.shape[:3] for ch in chunks]
   files = codecs.cseg_encode_batch_dev(packed, dtype, shapes, sc, block, ctx)
   for ch, f in zip(chunks, files):
-    assert f == codecs.cseg_encode(ch, block)
+    assert f == oracle.cseg_encode(ch, block).tobytes()
   streams, offs = _upload_bytes(ctx, files)
   out = DeviceCutout.empty((sum(int(np.prod(ch.shape)) for ch in chunks),), dtype, ctx)
   codecs.cseg_decode_batch_dev(streams, offs, dtype, shapes, sc, block, out.buf, ctx)
@@ -140,11 +140,11 @@ def test_cseg_batch_equals_one_chunk_codec(ctx, dtype, block, sc):
     n = int(np.prod(ch.shape))
     got = flat[at:at + n].reshape(ch.shape, order="F")
     assert np.array_equal(got, ch)
-    assert np.array_equal(got, codecs.cseg_decode(f, ch.shape, dtype, block))
+    assert np.array_equal(got, oracle.cseg_decode(np.frombuffer(f, np.uint32), ch.shape, dtype, block))
     at += n
 
 
-def test_cseg_batch_hash_collisions(ctx, monkeypatch):
+def test_cseg_batch_hash_collisions(ctx, oracle, monkeypatch):
   """IGN_CSEG_HASH_BITS=2 makes most tables share a hash, across chunks too: owners are still found by
   content inside each chunk's channel"""
   from igneous_b200 import codecs
@@ -155,16 +155,16 @@ def test_cseg_batch_hash_collisions(ctx, monkeypatch):
   files = codecs.cseg_encode_batch_dev(packed, np.uint64, [ch.shape[:3] for ch in chunks], 2, (8, 8, 8), ctx)
   monkeypatch.delenv("IGN_CSEG_HASH_BITS")
   for ch, f in zip(chunks, files):
-    assert f == codecs.cseg_encode(ch, (8, 8, 8))
+    assert f == oracle.cseg_encode(ch, (8, 8, 8)).tobytes()
 
 
-def test_cseg_batch_refusals(ctx):
+def test_cseg_batch_refusals(ctx, oracle):
   from igneous_b200 import _shim, codecs
   from igneous_b200.storage import _upload_bytes
   chunks = _mixed_chunks(np.uint32, 1, np.random.default_rng(1))[:3]
   shapes = np.ascontiguousarray(np.array([ch.shape[:3] for ch in chunks], dtype=np.uint32))
   packed, _ = _upload_bytes(ctx, [ch.tobytes(order="F") for ch in chunks])
-  need = sum(len(codecs.cseg_encode(ch)) for ch in chunks) // 4
+  need = sum(len(oracle.cseg_encode(ch)) for ch in chunks)
   out, offs, nw = ctx.alloc(need * 4), ctx.alloc(32), c.c_uint64(0)
   with pytest.raises(_shim.IgneousB200Error, match="words needed"):
     _shim.check(ctx.lib.ign_cseg_encode_batch_dev(ctx.handle, _shim.ptr(packed), _shim.IGN_U32, 3, _shim.ptr(shapes),
@@ -175,7 +175,7 @@ def test_cseg_batch_refusals(ctx):
   with pytest.raises(NotImplementedError):
     _shim.check(ctx.lib.ign_cseg_encode_batch_dev(ctx.handle, _shim.ptr(packed), _shim.IGN_U16, 3, _shim.ptr(shapes),
                                                   1, 8, 8, 8, _shim.ptr(out), need, _shim.ptr(offs), c.byref(nw)))
-  files = [codecs.cseg_encode(ch) for ch in chunks]
+  files = [oracle.cseg_encode(ch).tobytes() for ch in chunks]
   files[1] = files[1][:len(files[1]) // 8 * 4]  # truncated to half its words
   streams, boffs = _upload_bytes(ctx, files)
   dec = ctx.alloc(sum(ch.nbytes for ch in chunks))

@@ -43,6 +43,21 @@ def test_cseg_multichannel_and_block_sizes(ctx, oracle):
     assert np.array_equal(codecs.cseg_decode(got.tobytes(), v.shape, np.uint32, bs), v)
 
 
+def test_cseg_encode_capacity(ctx, oracle):
+  """an output one word short fails and reports the words needed; the exact size takes the stream"""
+  import ctypes as c
+  from igneous_b200 import _shim
+  v = np.asfortranarray(_vols(oracle, np.uint32)[0])
+  want = oracle.cseg_encode(v)
+  args = [ctx.handle, _shim.ptr(v), _shim.IGN_U32, *v.shape, 1, 8, 8, 8]
+  out, n = np.zeros(len(want), np.uint32), c.c_uint64(0)
+  with pytest.raises(_shim.IgneousB200Error, match="words needed"):
+    _shim.check(ctx.lib.ign_cseg_encode(*args, _shim.ptr(out), len(want) - 1, c.byref(n)))
+  assert n.value == len(want)
+  _shim.check(ctx.lib.ign_cseg_encode(*args, _shim.ptr(out), len(want), c.byref(n)))
+  assert n.value == len(want) and np.array_equal(out, want)
+
+
 def test_cseg_rejects_malformed_and_unsupported(ctx):
   from igneous_b200 import codecs, _shim
   with pytest.raises(NotImplementedError):
