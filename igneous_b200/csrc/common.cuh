@@ -212,6 +212,17 @@ int small_sync(ign_ctx* ctx);
 // profiled launch: like IGN_LAUNCH, plus an event pair when profiling is on
 int prof_begin(ign_ctx* ctx, int cls);
 void prof_end(ign_ctx* ctx, int slot);
+// event pair around the work a scope enqueues on ctx->stream (end() closes it early)
+struct ProfSpan {
+  ign_ctx* ctx;
+  int slot;
+  ProfSpan(ign_ctx* c, int cls) : ctx(c), slot(prof_begin(c, cls)) {}
+  void end() {
+    prof_end(ctx, slot);
+    slot = -1;
+  }
+  ~ProfSpan() { end(); }
+};
 #define IGN_LAUNCH_PROF(ctx, cls, kernel, grid, block, smem, ...)                 \
   do {                                                                           \
     const int _slot = ign::prof_begin((ctx), (cls));                             \

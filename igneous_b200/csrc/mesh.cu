@@ -6,19 +6,24 @@
 //   renumber   labels -> dense 1..K (shares remap.cu's hash table kernels)
 //   count      one thread per 2x2x2 cube (x fastest, corners through L1): for
 //              every distinct non-zero corner label the 256-case table gives a
-//              triangle count; warp-reduced, one atomicAdd per warp.
-//   emit       same walk; a warp prefix-sum + ONE atomicAdd per warp reserves a
-//              contiguous slice of the compacted triangle buffer
-//              (warp-aggregated atomics); records are 64-bit keys
-//              [label | cube | t] + the 8-bit case index.
-//   sort       radix sort of the keys -> per label, cube raster order
-//              (deterministic whatever order the atomics resolved in).
-//   weld       3 vertex keys [label | z | y | x] (half-voxel lattice) per
-//              triangle, radix sorted; heads of runs are the unique vertices;
-//              an exclusive scan ranks them; faces index them per label.
+//              triangle count; one total per CTA.  A pass over the lattice
+//              edges counts vertex records (below) per warp.
+//   emit       an exclusive scan of the totals gives each CTA (warp) its base;
+//              its records go to base + in-CTA (in-warp) prefix, so they land in
+//              raster order with no atomics: (label, cube<<11 | case<<3 | t).
+//   sort       stable radix sort on the label bits alone -> (label, cube, t).
+//   weld       a vertex of label L sits on every lattice edge with one endpoint
+//              L != 0 and the other != L (every case of mc_table.h uses exactly
+//              the edges whose endpoint bits differ).  Edges are enumerated in
+//              raster order of the half-voxel lattice, one record per non-zero
+//              side, and stably sorted on the label: that is the unique vertex
+//              order (label, z2, y2, x2).  Per-warp record masks give each
+//              face corner the emission index of its vertex record, and the
+//              sort's inverse permutation its vertex id.
 // Roofline: HBM-bound streaming over the label volume for count/emit
 // (algorithmic bytes = sizeof(label) per voxel); the sorts are bound by the
 // surface size, not the volume.
+#include <cub/block/block_scan.cuh>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
@@ -32,10 +37,10 @@
 namespace ign {
 
 constexpr unsigned MFULL = 0xFFFFFFFFu;
-constexpr int TRI_T_BITS = 3, TRI_CUBE_BITS = 30;
 constexpr int V_COORD_BITS = 11;
 constexpr int V_LABEL_SHIFT = 3 * V_COORD_BITS;  // 33
-constexpr int TRI_LABEL_SHIFT = TRI_T_BITS + TRI_CUBE_BITS;  // 33
+constexpr int TRI_CASE_SHIFT = 3, TRI_CUBE_SHIFT = 11;  // triangle record: cube << 11 | case << 3 | t
+using BlockScan256 = cub::BlockScan<uint32_t, 256>;
 
 __constant__ int8_t c_edge_mid[12][3] = {{1, 0, 0}, {2, 1, 0}, {1, 2, 0}, {0, 1, 0},
                                          {1, 0, 2}, {2, 1, 2}, {1, 2, 2}, {0, 1, 2},
@@ -46,6 +51,36 @@ struct McTables {
   uint8_t ntri[256];
 };
 __constant__ McTables c_mc;
+
+// Lattice edges in raster order of the half-voxel lattice (z2, y2, x2): per plane z, the x-edges
+// then the y-edges of each row y, then the plane's z-edges in (y, x) order.  An edge's slot in that
+// order is its id (< 3 * 1023^3 < 2^32); slots of edges that leave the volume hold no vertex.
+struct Lattice {
+  uint32_t sx, sy, sz;
+  __device__ __forceinline__ uint32_t plane() const { return 3 * sx * sy; }
+  // slot -> lower endpoint voxel and direction (0 x, 1 y, 2 z)
+  __device__ __forceinline__ void edge(uint32_t g, uint32_t& x, uint32_t& y, uint32_t& z, uint32_t& dir) const {
+    z = g / plane();
+    uint32_t r = g - z * plane();
+    if (r < 2 * sx * sy) {
+      y = r / (2 * sx);
+      r -= y * 2 * sx;
+      dir = r >= sx;
+      x = r - dir * sx;
+    } else {
+      r -= 2 * sx * sy;
+      dir = 2;
+      y = r / sx;
+      x = r - y * sx;
+    }
+  }
+  // half-voxel coordinates of an edge midpoint -> slot
+  __device__ __forceinline__ uint32_t slot(uint32_t X2, uint32_t Y2, uint32_t Z2) const {
+    const uint32_t base = (Z2 >> 1) * plane();
+    if (Z2 & 1) return base + 2 * sx * sy + (Y2 >> 1) * sx + (X2 >> 1);
+    return base + (Y2 >> 1) * 2 * sx + ((Y2 & 1) ? sx : 0) + (X2 >> 1);
+  }
+};
 
 // corner k of Bourke's numbering -> offset (dx,dy,dz)
 __device__ __forceinline__ void cube_corners(const uint32_t* __restrict__ lab, uint32_t sx,
@@ -60,19 +95,18 @@ __device__ __forceinline__ void cube_corners(const uint32_t* __restrict__ lab, u
   c[7] = lab[base + sx + sxy];
 }
 
-// EMIT=false: count triangles; EMIT=true: write records
+// EMIT=false: triangles per CTA into cta[blockIdx.x]; EMIT=true: records at the CTA's scanned base
 template <bool EMIT>
 __global__ void __launch_bounds__(256)
     k_mc(const uint32_t* __restrict__ lab, uint32_t sx, uint32_t sy, uint32_t sz,
-         unsigned long long* total, uint64_t* __restrict__ keys, uint8_t* __restrict__ cases,
-         uint64_t capacity) {
+         unsigned long long* __restrict__ cta, uint32_t* __restrict__ tlabel, uint64_t* __restrict__ trec) {
   __shared__ uint8_t s_ntri[256];
+  __shared__ typename BlockScan256::TempStorage s_scan;
   for (int i = threadIdx.x; i < 256; i += blockDim.x) s_ntri[i] = c_mc.ntri[i];
   __syncthreads();
   const uint32_t cx = sx - 1, cy = sy - 1, cz = sz - 1;
   const uint64_t ncubes = (uint64_t)cx * cy * cz;
   const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  const uint32_t lane = threadIdx.x & 31;
   uint32_t mine = 0;
   uint32_t c[8];
   uint32_t x = 0, y = 0, z = 0;
@@ -103,107 +137,141 @@ __global__ void __launch_bounds__(256)
       mine += s_ntri[idxs[k]];
     }
   }
+  uint32_t pre, total;
+  BlockScan256(s_scan).ExclusiveSum(mine, pre, total);
   if (!EMIT) {
-    uint32_t s = mine;
-    for (int d = 16; d > 0; d >>= 1) s += __shfl_down_sync(MFULL, s, d);
-    if (lane == 0 && s) atomicAdd(total, (unsigned long long)s);
+    if (threadIdx.x == 0) cta[blockIdx.x] = total;
     return;
   }
-  // warp-aggregated reservation
-  uint32_t incl = mine;
-  for (int d = 1; d < 32; d <<= 1) {
-    const uint32_t v = __shfl_up_sync(MFULL, incl, d);
-    if (lane >= d) incl += v;
-  }
-  const uint32_t warp_total = __shfl_sync(MFULL, incl, 31);
-  if (warp_total == 0) return;
-  unsigned long long base = 0;
-  if (lane == 31) base = atomicAdd(total, (unsigned long long)warp_total);
-  base = __shfl_sync(MFULL, base, 31);
-  uint64_t pos = base + (incl - mine);
-  if (active) {
-    const uint64_t cube = (uint64_t)t;
+  if (!active) return;
+  uint64_t pos = cta[blockIdx.x] + pre;
+  const uint64_t cube = (uint64_t)t;
 #pragma unroll
-    for (int k = 0; k < 8; k++) {
-      const uint32_t n = s_ntri[idxs[k]];
-      for (uint32_t tt = 0; tt < n; tt++) {
-        if (pos < capacity) {
-          keys[pos] = ((uint64_t)c[k] << TRI_LABEL_SHIFT) | (cube << TRI_T_BITS) | tt;
-          cases[pos] = idxs[k];
-        }
-        pos++;
-      }
+  for (int k = 0; k < 8; k++) {
+    const uint32_t n = s_ntri[idxs[k]];
+    for (uint32_t tt = 0; tt < n; tt++) {
+      tlabel[pos] = c[k];
+      trec[pos] = (cube << TRI_CUBE_SHIFT) | ((uint64_t)idxs[k] << TRI_CASE_SHIFT) | tt;
+      pos++;
     }
   }
 }
 
-// triangle records (sorted) -> 3 vertex keys each
+// Vertex records are counted per warp of 32 edge slots: bit j of the warp's mask is set when slot j
+// holds at least one record, bit 32 + j when it holds two.  With the scanned warp bases that gives the
+// emission index of any record without storing one per edge.
+__device__ __forceinline__ uint64_t record_index(const uint64_t* __restrict__ wmask,
+                                                 const unsigned long long* __restrict__ wbase, uint32_t g) {
+  const uint64_t mk = wmask[g >> 5];
+  const uint32_t below = (1u << (g & 31)) - 1;
+  return wbase[g >> 5] + __popc((uint32_t)mk & below) + __popc((uint32_t)(mk >> 32) & below);
+}
+
+// EMIT=false: masks and record counts per warp; EMIT=true: (label, edge slot) records at the warp's
+// scanned base, the side of the lower endpoint first
+template <bool EMIT>
 __global__ void __launch_bounds__(256)
-    k_tri_vertices(const uint64_t* __restrict__ keys, const uint8_t* __restrict__ cases, uint64_t T,
-                   uint32_t cx, uint32_t cy, uint64_t* __restrict__ vkeys,
-                   uint32_t* __restrict__ corner) {
+    k_edges(const uint32_t* __restrict__ lab, Lattice lt, uint64_t* __restrict__ wmask,
+            unsigned long long* __restrict__ wcount, uint32_t* __restrict__ vlabel, uint32_t* __restrict__ vedge) {
+  const uint64_t nslots = 3ull * lt.sx * lt.sy * lt.sz;
+  const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  uint32_t a = 0, b = 0, mine = 0;
+  if (t < nslots) {
+    uint32_t x, y, z, dir;
+    lt.edge((uint32_t)t, x, y, z, dir);
+    const bool inside = dir == 0 ? x + 1 < lt.sx : dir == 1 ? y + 1 < lt.sy : z + 1 < lt.sz;
+    if (inside) {
+      const uint64_t i = ((uint64_t)z * lt.sy + y) * lt.sx + x;
+      a = lab[i];
+      b = lab[i + (dir == 0 ? 1ull : dir == 1 ? (uint64_t)lt.sx : (uint64_t)lt.sx * lt.sy)];
+      if (a != b) mine = (a != 0) + (b != 0);
+    }
+  }
+  const uint32_t m1 = __ballot_sync(MFULL, mine >= 1), m2 = __ballot_sync(MFULL, mine == 2);
+  if (!EMIT) {
+    if ((threadIdx.x & 31) == 0) {
+      wmask[t >> 5] = m1 | ((uint64_t)m2 << 32);
+      wcount[t >> 5] = __popc(m1) + __popc(m2);
+    }
+    return;
+  }
+  if (!mine) return;
+  uint64_t pos = record_index(wmask, wcount, (uint32_t)t);
+  if (a) {
+    vlabel[pos] = a;
+    vedge[pos] = (uint32_t)t;
+    pos++;
+  }
+  if (b) {
+    vlabel[pos] = b;
+    vedge[pos] = (uint32_t)t;
+  }
+}
+
+// emission index of the record of label L on edge slot g, whose lower endpoint is labelled a
+__device__ __forceinline__ uint64_t side_index(const uint64_t* __restrict__ wmask,
+                                               const unsigned long long* __restrict__ wbase, uint32_t g,
+                                               uint32_t a, uint32_t L) {
+  return record_index(wmask, wbase, g) + (L != a && a != 0);
+}
+
+// sorted vertex records -> packed vertex keys [label | z2 | y2 | x2], and the sorted position of
+// every record by its emission index
+__global__ void __launch_bounds__(256)
+    k_vertex_keys(const uint32_t* __restrict__ lab, Lattice lt, const uint64_t* __restrict__ wmask,
+                  const unsigned long long* __restrict__ wbase, const uint32_t* __restrict__ vlabel,
+                  const uint32_t* __restrict__ vedge, uint64_t U, uint64_t* __restrict__ uniq_vkeys,
+                  uint32_t* __restrict__ sorted_pos) {
+  const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (i >= U) return;
+  const uint32_t L = vlabel[i], g = vedge[i];
+  uint32_t x, y, z, dir;
+  lt.edge(g, x, y, z, dir);
+  const uint64_t vx = 2 * x + (dir == 0), vy = 2 * y + (dir == 1), vz = 2 * z + (dir == 2);
+  uniq_vkeys[i] = ((uint64_t)L << V_LABEL_SHIFT) | (vz << (2 * V_COORD_BITS)) | (vy << V_COORD_BITS) | vx;
+  const uint32_t a = lab[((uint64_t)z * lt.sy + y) * lt.sx + x];
+  sorted_pos[side_index(wmask, wbase, g, a, L)] = (uint32_t)i;
+}
+
+// sorted triangle records -> faces as vertex ids local to the label
+__global__ void __launch_bounds__(256)
+    k_faces(const uint32_t* __restrict__ lab, Lattice lt, const uint32_t* __restrict__ tlabel,
+            const uint64_t* __restrict__ trec, uint64_t T, const uint64_t* __restrict__ wmask,
+            const unsigned long long* __restrict__ wbase, const uint32_t* __restrict__ sorted_pos,
+            const uint32_t* __restrict__ vert_off, uint32_t* __restrict__ faces) {
   const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (t >= T) return;
-  const uint64_t key = keys[t];
-  const uint64_t label = key >> TRI_LABEL_SHIFT;
-  const uint64_t cube = (key >> TRI_T_BITS) & ((1ull << TRI_CUBE_BITS) - 1);
-  const uint32_t tt = (uint32_t)(key & ((1u << TRI_T_BITS) - 1));
-  const uint32_t x = (uint32_t)(cube % cx), y = (uint32_t)((cube / cx) % cy),
-                 z = (uint32_t)(cube / ((uint64_t)cx * cy));
-  const int8_t* row = c_mc.tri[cases[t]];
+  const uint32_t L = tlabel[t];
+  const uint64_t rec = trec[t];
+  const uint32_t cube = (uint32_t)(rec >> TRI_CUBE_SHIFT);
+  const uint32_t cs = (uint32_t)(rec >> TRI_CASE_SHIFT) & 255u, tt = (uint32_t)rec & 7u;
+  const uint32_t cx = lt.sx - 1, cy = lt.sy - 1;
+  const uint32_t x = cube % cx, y = (cube / cx) % cy, z = cube / (cx * cy);
+  const int8_t* row = c_mc.tri[cs];
+  const uint32_t off = vert_off[L];
 #pragma unroll
   for (int v = 0; v < 3; v++) {
     // table winds clockwise seen from outside for "bit = inside"; reverse it so
     // that normals point out of the label (oracle.marching_cubes flip=True)
     const int e = row[3 * tt + (2 - v)];
-    const uint64_t vx = 2 * x + c_edge_mid[e][0], vy = 2 * y + c_edge_mid[e][1],
-                   vz = 2 * z + c_edge_mid[e][2];
-    vkeys[3 * t + v] = (label << V_LABEL_SHIFT) | (vz << (2 * V_COORD_BITS)) | (vy << V_COORD_BITS) | vx;
-    corner[3 * t + v] = (uint32_t)(3 * t + v);
+    const uint32_t X2 = 2 * x + c_edge_mid[e][0], Y2 = 2 * y + c_edge_mid[e][1], Z2 = 2 * z + c_edge_mid[e][2];
+    const uint32_t a = lab[((uint64_t)(Z2 >> 1) * lt.sy + (Y2 >> 1)) * lt.sx + (X2 >> 1)];
+    faces[3 * t + v] = sorted_pos[side_index(wmask, wbase, lt.slot(X2, Y2, Z2), a, L)] - off;
   }
 }
 
-// boundaries in a sorted array of keys -> per-label [start) markers
+// boundaries in a sorted array of labels -> per-label [start) markers
 __global__ void __launch_bounds__(256)
-    k_label_starts(const uint64_t* __restrict__ keys, uint64_t n, int shift,
-                   uint32_t* __restrict__ start /* [K+2], prefilled with n */) {
+    k_label_starts(const uint32_t* __restrict__ labels, uint64_t n, uint32_t* __restrict__ start /* [K+2], prefilled with n */) {
   const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const uint64_t label = keys[i] >> shift;
-  if (i == 0 || (keys[i - 1] >> shift) != label) start[label] = (uint32_t)i;
+  const uint32_t label = labels[i];
+  if (i == 0 || labels[i - 1] != label) start[label] = (uint32_t)i;
 }
 
 __global__ void __launch_bounds__(256) k_fill_u32(uint32_t* a, uint32_t value, uint32_t n) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) a[i] = value;
-}
-
-__global__ void __launch_bounds__(256)
-    k_vertex_heads(const uint64_t* __restrict__ vkeys_sorted, uint64_t n, uint32_t* __restrict__ heads) {
-  const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  if (i < n) heads[i] = (i == 0 || vkeys_sorted[i - 1] != vkeys_sorted[i]) ? 1u : 0u;
-}
-
-// heads + exclusive scan -> unique vertex list and global vertex id per corner
-__global__ void __launch_bounds__(256)
-    k_vertex_assign(const uint64_t* __restrict__ vkeys_sorted, const uint32_t* __restrict__ corner_sorted,
-                    const uint32_t* __restrict__ heads, const uint32_t* __restrict__ rank, uint64_t n,
-                    uint64_t* __restrict__ uniq_vkeys, uint32_t* __restrict__ face_global) {
-  const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint32_t id = rank[i] + heads[i] - 1;  // inclusive rank - 1
-  if (heads[i]) uniq_vkeys[id] = vkeys_sorted[i];
-  face_global[corner_sorted[i]] = id;
-}
-
-// global vertex ids -> ids local to the label
-__global__ void __launch_bounds__(256)
-    k_faces_local(const uint64_t* __restrict__ tri_keys, const uint32_t* __restrict__ vert_off,
-                  uint64_t T, uint32_t* __restrict__ faces) {
-  const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  if (i >= 3 * T) return;
-  const uint64_t label = tri_keys[i / 3] >> TRI_LABEL_SHIFT;
-  faces[i] -= vert_off[label];
 }
 
 __global__ void __launch_bounds__(256)
@@ -286,6 +354,7 @@ int ign_mesh_begin_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx,
   IGN_TRY(activate(ctx));
   IGN_REQUIRE(labels && out, IGN_ERR_INVALID, "null argument");
   *out = nullptr;
+  ProfSpan prof(ctx, IGN_PROF_MC);
   IGN_REQUIRE(sx >= 1 && sy >= 1 && sz >= 1, IGN_ERR_INVALID, "empty volume");
   IGN_REQUIRE(sx <= 1023 && sy <= 1023 && sz <= 1023, IGN_ERR_UNSUPPORTED,
               "mesher: task of %llux%llux%llu exceeds the 1023^3 limit of the packed vertex format",
@@ -335,81 +404,84 @@ int ign_mesh_begin_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx,
   }
   IGN_REQUIRE(K < (1ull << 31), IGN_ERR_OVERFLOW, "mesher: too many labels");
 
-  // ---- count
-  unsigned long long* d_total;
-  IGN_TRY(f.take(&d_total, 32));
-  const uint64_t ncubes = (sx - 1) * (sy - 1) * (sz - 1);
-  const unsigned grid = blocks_for(ncubes, 256);
-  unsigned long long T = 0;
-  IGN_CUDA(cudaMemsetAsync(d_total, 0, 8, ctx->stream));
-  IGN_LAUNCH(ctx, (k_mc<false>), grid, 256, 0, d_lab, (uint32_t)sx, (uint32_t)sy, (uint32_t)sz, d_total,
-             (uint64_t*)nullptr, (uint8_t*)nullptr, 0ull);
-  IGN_TRY(small_d2h(ctx, &T, d_total, 8));
+  // ---- count: triangles per CTA of cubes, vertex records per warp of edge slots.  An exclusive scan
+  // of each (one slot past the end, zeroed) gives every CTA's or warp's base and, last, the total.
+  const Lattice lt{(uint32_t)sx, (uint32_t)sy, (uint32_t)sz};
+  const uint64_t ncubes = (sx - 1) * (sy - 1) * (sz - 1), nwarps = (3 * n + 31) / 32;
+  const unsigned grid = blocks_for(ncubes, 256), egrid = blocks_for(3 * n, 256);
+  unsigned long long *tcnt, *tbase, *wcnt, *wbase;
+  uint64_t* wmask;
+  IGN_TRY(f.take(&tcnt, grid + 1));
+  IGN_TRY(f.take(&tbase, grid + 1));
+  IGN_TRY(f.take(&wcnt, nwarps + 1));
+  IGN_TRY(f.take(&wbase, nwarps + 1));
+  IGN_TRY(f.take(&wmask, nwarps));
+  size_t scanb = 0, sortt = 0, sortv = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, scanb, tcnt, tbase, (int64_t)nwarps + 1);
+  void* scan_tmp;
+  IGN_TRY(f.take(&scan_tmp, scanb));
+  IGN_CUDA(cudaMemsetAsync(tcnt + grid, 0, 8, ctx->stream));
+  IGN_CUDA(cudaMemsetAsync(wcnt + nwarps, 0, 8, ctx->stream));
+  IGN_LAUNCH(ctx, (k_mc<false>), grid, 256, 0, d_lab, (uint32_t)sx, (uint32_t)sy, (uint32_t)sz, tcnt,
+             (uint32_t*)nullptr, (uint64_t*)nullptr);
+  IGN_LAUNCH(ctx, (k_edges<false>), egrid, 256, 0, d_lab, lt, wmask, wcnt, (uint32_t*)nullptr, (uint32_t*)nullptr);
+  size_t tb = scanb;
+  IGN_CUDA(cub::DeviceScan::ExclusiveSum(scan_tmp, tb, tcnt, tbase, (int64_t)grid + 1, ctx->stream));
+  tb = scanb;
+  IGN_CUDA(cub::DeviceScan::ExclusiveSum(scan_tmp, tb, wcnt, wbase, (int64_t)nwarps + 1, ctx->stream));
+  ctx->launches += 4;
+  unsigned long long tot[2];
+  IGN_TRY(small_d2h(ctx, &tot[0], tbase + grid, 8));
+  IGN_TRY(small_d2h(ctx, &tot[1], wbase + nwarps, 8));
   IGN_TRY(small_sync(ctx));
+  const unsigned long long T = tot[0], U = tot[1];
   m->T = T;
   if (T == 0) {
     guard.m = nullptr;
     *out = m;
     return IGN_OK;
   }
-  // the sorts and the scan below take int item counts: 3T corners must fit an int
+  // the sorts take int item counts: 3T corners must fit an int (and U <= 3T: every vertex is a corner)
   IGN_REQUIRE(3 * T <= (unsigned long long)INT_MAX, IGN_ERR_OVERFLOW,
               "mesher: %llu triangles exceed 2^31 - 1 corners; split the volume into tasks", T);
+  m->U = U;
 
-  // ---- emit + sort + weld buffers
-  size_t sort1 = 0, sort2 = 0, scanb = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, sort1, (const uint64_t*)nullptr, (uint64_t*)nullptr,
-                                  (const uint8_t*)nullptr, (uint8_t*)nullptr, (int)T);
-  cub::DeviceRadixSort::SortPairs(nullptr, sort2, (const uint64_t*)nullptr, (uint64_t*)nullptr,
-                                  (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)(3 * T));
-  cub::DeviceScan::ExclusiveSum(nullptr, scanb, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)(3 * T));
-  size_t tmp_bytes = sort1 > sort2 ? sort1 : sort2;
-  if (scanb > tmp_bytes) tmp_bytes = scanb;
-  uint64_t *keys, *keys_s, *vkeys, *vkeys_s;
-  uint8_t *cases, *cases_s;
-  uint32_t *corner, *corner_s, *heads, *rank, *d_tri_off, *d_vert_off;
+  // ---- emit + sort buffers
+  cub::DeviceRadixSort::SortPairs(nullptr, sortt, (const uint32_t*)nullptr, (uint32_t*)nullptr,
+                                  (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)T);
+  cub::DeviceRadixSort::SortPairs(nullptr, sortv, (const uint32_t*)nullptr, (uint32_t*)nullptr,
+                                  (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)U);
+  const size_t tmp_bytes = sortt > sortv ? sortt : sortv;
+  uint32_t *tlabel, *tlabel_s, *vlabel, *vlabel_s, *vedge, *vedge_s, *sorted_pos, *d_tri_off, *d_vert_off;
+  uint64_t *trec, *trec_s;
   void* tmp;
-  IGN_TRY(f.take(&keys, T));
-  IGN_TRY(f.take(&keys_s, T));
-  IGN_TRY(f.take(&cases, T));
-  IGN_TRY(f.take(&cases_s, T));
-  IGN_TRY(f.take(&vkeys, 3 * T));
-  IGN_TRY(f.take(&vkeys_s, 3 * T));
-  IGN_TRY(f.take(&corner, 3 * T));
-  IGN_TRY(f.take(&corner_s, 3 * T));
-  IGN_TRY(f.take(&heads, 3 * T));
-  IGN_TRY(f.take(&rank, 3 * T));
+  IGN_TRY(f.take(&tlabel, T));
+  IGN_TRY(f.take(&tlabel_s, T));
+  IGN_TRY(f.take(&trec, T));
+  IGN_TRY(f.take(&trec_s, T));
+  IGN_TRY(f.take(&vlabel, U));
+  IGN_TRY(f.take(&vlabel_s, U));
+  IGN_TRY(f.take(&vedge, U));
+  IGN_TRY(f.take(&vedge_s, U));
+  IGN_TRY(f.take(&sorted_pos, U));
   IGN_TRY(f.take(&d_tri_off, K + 2));
   IGN_TRY(f.take(&d_vert_off, K + 2));
   IGN_TRY(f.take(&tmp, tmp_bytes));
 
-  // ---- emit + sort
-  IGN_CUDA(cudaMemsetAsync(d_total, 0, 8, ctx->stream));
-  IGN_LAUNCH(ctx, (k_mc<true>), grid, 256, 0, d_lab, (uint32_t)sx, (uint32_t)sy, (uint32_t)sz, d_total, keys,
-             cases, (uint64_t)T);
+  // ---- emit in raster order; a stable sort on the label bits then gives (label, cube, t) and
+  // (label, z2, y2, x2)
   const int label_bits = bits_for(K);
-  size_t tb = tmp_bytes;
-  IGN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, keys, keys_s, cases, cases_s, (int)T, 0,
-                                           TRI_LABEL_SHIFT + label_bits, ctx->stream));
-  ctx->launches += 4;
-
-  // ---- weld
-  IGN_LAUNCH(ctx, k_tri_vertices, blocks_for(T, 256), 256, 0, keys_s, cases_s, (uint64_t)T, (uint32_t)(sx - 1),
-             (uint32_t)(sy - 1), vkeys, corner);
+  IGN_LAUNCH(ctx, (k_mc<true>), grid, 256, 0, d_lab, (uint32_t)sx, (uint32_t)sy, (uint32_t)sz, tbase, tlabel,
+             trec);
   tb = tmp_bytes;
-  IGN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, vkeys, vkeys_s, corner, corner_s, (int)(3 * T), 0,
-                                           V_LABEL_SHIFT + label_bits, ctx->stream));
-  ctx->launches += 4;
-  IGN_LAUNCH(ctx, k_vertex_heads, blocks_for(3 * T, 256), 256, 0, vkeys_s, (uint64_t)(3 * T), heads);
-  tb = tmp_bytes;
-  IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, heads, rank, (int)(3 * T), ctx->stream));
+  IGN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, tlabel, tlabel_s, trec, trec_s, (int)T, 0, label_bits,
+                                           ctx->stream));
   ctx->launches += 2;
-  uint32_t last[2];
-  IGN_TRY(small_d2h(ctx, &last[0], rank + (3 * T - 1), 4));
-  IGN_TRY(small_d2h(ctx, &last[1], heads + (3 * T - 1), 4));
-  IGN_TRY(small_sync(ctx));
-  const uint64_t U = (uint64_t)last[0] + last[1];
-  m->U = U;
+  IGN_LAUNCH(ctx, (k_edges<true>), egrid, 256, 0, d_lab, lt, wmask, wbase, vlabel, vedge);
+  tb = tmp_bytes;
+  IGN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, vlabel, vlabel_s, vedge, vedge_s, (int)U, 0, label_bits,
+                                           ctx->stream));
+  ctx->launches += 2;
   {
     const size_t fbytes = align_up(3 * T * 4, 256), vbytes = align_up(U * 12, 256);  // 12: float3 after simplify
     if (!ctx->mesh_pool_busy) {
@@ -431,14 +503,14 @@ int ign_mesh_begin_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx,
       IGN_CUDA(cudaMalloc((void**)&m->d_uniq_vkeys, U * 12));  // 12: float3 positions after simplification
     }
   }
-  IGN_LAUNCH(ctx, k_vertex_assign, blocks_for(3 * T, 256), 256, 0, vkeys_s, corner_s, heads, rank,
-             (uint64_t)(3 * T), m->d_uniq_vkeys, m->d_faces);
+  IGN_LAUNCH(ctx, k_vertex_keys, blocks_for(U, 256), 256, 0, d_lab, lt, wmask, wbase, vlabel_s, vedge_s,
+             (uint64_t)U, m->d_uniq_vkeys, sorted_pos);
 
   // ---- per-label offsets (labels are 1..K; slot K+1 is the end sentinel)
   IGN_LAUNCH(ctx, k_fill_u32, blocks_for(K + 2, 256), 256, 0, d_tri_off, (uint32_t)T, (uint32_t)(K + 2));
   IGN_LAUNCH(ctx, k_fill_u32, blocks_for(K + 2, 256), 256, 0, d_vert_off, (uint32_t)U, (uint32_t)(K + 2));
-  IGN_LAUNCH(ctx, k_label_starts, blocks_for(T, 256), 256, 0, keys_s, (uint64_t)T, TRI_LABEL_SHIFT, d_tri_off);
-  IGN_LAUNCH(ctx, k_label_starts, blocks_for(U, 256), 256, 0, m->d_uniq_vkeys, U, V_LABEL_SHIFT, d_vert_off);
+  IGN_LAUNCH(ctx, k_label_starts, blocks_for(T, 256), 256, 0, tlabel_s, (uint64_t)T, d_tri_off);
+  IGN_LAUNCH(ctx, k_label_starts, blocks_for(U, 256), 256, 0, vlabel_s, (uint64_t)U, d_vert_off);
   IGN_TRY(small_d2h(ctx, m->tri_off.data(), d_tri_off, (K + 2) * 4));
   IGN_TRY(small_d2h(ctx, m->vert_off.data(), d_vert_off, (K + 2) * 4));
   IGN_TRY(small_sync(ctx));
@@ -448,7 +520,8 @@ int ign_mesh_begin_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx,
     if (m->vert_off[l] > m->vert_off[l + 1]) m->vert_off[l] = m->vert_off[l + 1];
   }
   IGN_TRY(small_h2d(ctx, d_vert_off, m->vert_off.data(), (K + 2) * 4));
-  IGN_LAUNCH(ctx, k_faces_local, blocks_for(3 * T, 256), 256, 0, keys_s, d_vert_off, (uint64_t)T, m->d_faces);
+  IGN_LAUNCH(ctx, k_faces, blocks_for(T, 256), 256, 0, d_lab, lt, tlabel_s, trec_s, (uint64_t)T, wmask, wbase,
+             sorted_pos, d_vert_off, m->d_faces);
   IGN_CUDA(cudaStreamSynchronize(ctx->stream));
   for (uint64_t l = 1; l <= K; l++)
     if (m->tri_off[l + 1] > m->tri_off[l]) m->present.push_back(m->ids[l - 1]);

@@ -31,7 +31,6 @@
 // All arithmetic is double precision WITHOUT fused multiply-add (this file is
 // compiled with -fmad=false) so that oracle/igneous_oracle.c::orc_simplify
 // reproduces it bit for bit.
-#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include <stdlib.h>
@@ -211,13 +210,14 @@ __global__ void __launch_bounds__(256)
   vn[i] = 0;
 }
 
-// faces: local ids + per-label vertex base -> global ids; flabel by offsets search
+// faces: local ids + per-label vertex base -> global ids; flabel by offsets search; every corner
+// (node 3f+k) appended to its vertex's incidence list (vn zeroed by k_simp_init_verts)
 __global__ void __launch_bounds__(256)
     k_simp_init_faces(const uint32_t* __restrict__ faces_local, const uint32_t* __restrict__ tri_off,
                       const uint32_t* __restrict__ vert_off, uint32_t K, uint64_t T,
                       uint32_t* __restrict__ face, uint32_t* __restrict__ flabel,
-                      uint8_t* __restrict__ falive, uint32_t* __restrict__ node_vertex,
-                      uint32_t* __restrict__ node_id) {
+                      uint8_t* __restrict__ falive, uint32_t* __restrict__ vf, uint32_t* __restrict__ vn,
+                      uint32_t* overflow) {
   const uint64_t f = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   if (f >= T) return;
   // largest l in [1,K] with tri_off[l] <= f
@@ -232,29 +232,29 @@ __global__ void __launch_bounds__(256)
   for (int k = 0; k < 3; k++) {
     const uint32_t g = faces_local[3 * f + k] + vert_off[lo];
     face[3 * f + k] = g;
-    node_vertex[3 * f + k] = g;
-    node_id[3 * f + k] = (uint32_t)(3 * f + k);
+    const uint32_t c = atomicAdd(&vn[g], 1u);
+    if (c < S_VCAP) vf[(uint64_t)g * S_VCAP + c] = (uint32_t)(3 * f + k);
+    else *overflow = 1;
   }
 }
 
-// sorted (vertex, node) pairs -> per-vertex arrays in ascending node order
+// each vertex's incidence list into ascending node order (the order k_simp_quadrics sums in)
 __global__ void __launch_bounds__(256)
-    k_simp_link(const uint32_t* __restrict__ sv, const uint32_t* __restrict__ sh, uint64_t n,
-                uint32_t* __restrict__ vf, uint32_t* __restrict__ vn, uint32_t* overflow) {
-  const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint32_t v = sv[i];
-  if (i > 0 && sv[i - 1] == v) return;  // the first pair of a run writes the whole run
-  uint32_t c = 0;
-  for (uint64_t j = i; j < n && sv[j] == v; j++) {
-    if (c < S_VCAP) vf[(uint64_t)v * S_VCAP + c] = sh[j];
-    c++;
+    k_simp_vf_sort(uint64_t U, uint32_t* __restrict__ vf, uint32_t* __restrict__ vn) {
+  const uint64_t v = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  if (v >= U) return;
+  uint32_t n = vn[v];
+  if (n > S_VCAP) {  // flagged by k_simp_init_faces
+    n = S_VCAP;
+    vn[v] = n;
   }
-  if (c > S_VCAP) {
-    *overflow = 1;
-    c = S_VCAP;
+  uint32_t* l = vf + v * S_VCAP;
+  for (uint32_t i = 1; i < n; i++) {
+    const uint32_t h = l[i];
+    uint32_t j = i;
+    for (; j > 0 && l[j - 1] > h; j--) l[j] = l[j - 1];
+    l[j] = h;
   }
-  vn[v] = c;
 }
 
 __global__ void __launch_bounds__(128) k_simp_quadrics(Simp s) {
@@ -1687,18 +1687,17 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
     m->d_pos_f = nullptr;
     return IGN_OK;
   }
-  size_t sortb = 0, scanb = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, sortb, (const uint32_t*)nullptr, (uint32_t*)nullptr,
-                                  (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)(3 * T));
+  ProfSpan prof(ctx, IGN_PROF_MC);  // the simplifier's setup, up to the label launches
+  size_t scanb = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, scanb, (const uint32_t*)nullptr, (uint32_t*)nullptr,
-                                (int)(3 * T));
-  const size_t tmpb = (sortb > scanb ? sortb : scanb) + 256;
+                                (int)(U > T ? U : T));
+  const size_t tmpb = scanb + 256;
   ScratchFrame f(ctx);
   Simp s;
   s.U = U;
   s.T = T;
-  uint32_t *node_v, *node_h, *vscan, *vflag32, *d_target, *d_tri_off, *d_vert_off, *d_new_tri_off, *d_new_vert_off;
-  uint32_t *d_order, *flags, *gl_f[2], *gl_v[2], *sorted_v, *sorted_h, *d_mq;
+  uint32_t *fscan, *fflag, *vscan, *vflag32, *d_target, *d_tri_off, *d_vert_off, *d_new_tri_off, *d_new_vert_off;
+  uint32_t *d_order, *flags, *gl_f[2], *gl_v[2], *d_mq;
   uint16_t* finv;
   uint8_t *fstate, *vflag, *vlose;
   unsigned long long* key1;
@@ -1708,8 +1707,8 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   IGN_TRY(f.take(&s.Q, U * 10));
   IGN_TRY(f.take(&s.face, 3 * T));
   IGN_TRY(f.take(&s.vf, U * S_VCAP));
-  IGN_TRY(f.take(&node_v, 3 * T));  // reused as face scan later
-  IGN_TRY(f.take(&node_h, 3 * T));
+  IGN_TRY(f.take(&fscan, T));
+  IGN_TRY(f.take(&fflag, T));
   IGN_TRY(f.take(&s.flabel, T));
   IGN_TRY(f.take(&s.falive, T));
   IGN_TRY(f.take(&fstate, T));
@@ -1739,8 +1738,6 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   IGN_TRY(f.take(&d_mq, (size_t)SL_MREC * K * (SL_NCLASS - 1)));
   IGN_TRY(f.take(&finv, T));
   IGN_TRY(f.take(&tmp, tmpb));
-  IGN_TRY(f.take(&sorted_v, 3 * T));
-  IGN_TRY(f.take(&sorted_h, 3 * T));
   s.tri_off = d_tri_off;
 
   std::vector<uint32_t> target(K + 2, 0);
@@ -1777,19 +1774,10 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   IGN_TRY(small_h2d(ctx, d_order, order.data(), K * 4));
   IGN_LAUNCH(ctx, k_simp_init_verts, blocks_for(U, 256), 256, 0, m->d_uniq_vkeys, U, (double)resolution[0],
              (double)resolution[1], (double)resolution[2], s.pos, s.valive, s.vbound, s.vn);
-  IGN_LAUNCH(ctx, k_simp_init_faces, blocks_for(T, 256), 256, 0, m->d_faces, d_tri_off, d_vert_off, (uint32_t)K, T,
-             s.face, s.flabel, s.falive, node_v, node_h);
-  {
-    int bits = 1;
-    while (bits < 32 && (1ull << bits) < U) bits++;
-    size_t tb = tmpb;
-    IGN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, node_v, sorted_v, node_h, sorted_h, (int)(3 * T), 0, bits,
-                                             ctx->stream));
-    ctx->launches += 3;
-  }
   IGN_CUDA(cudaMemsetAsync(flags, 0, 32 * 4, ctx->stream));
-  IGN_LAUNCH(ctx, k_simp_link, blocks_for(3 * T, 256), 256, 0, sorted_v, sorted_h, (uint64_t)(3 * T), s.vf, s.vn,
-             flags + 12);
+  IGN_LAUNCH(ctx, k_simp_init_faces, blocks_for(T, 256), 256, 0, m->d_faces, d_tri_off, d_vert_off, (uint32_t)K, T,
+             s.face, s.flabel, s.falive, s.vf, s.vn, flags + 12);
+  IGN_LAUNCH(ctx, k_simp_vf_sort, blocks_for(U, 256), 256, 0, U, s.vf, s.vn);
   IGN_LAUNCH(ctx, k_simp_quadrics, blocks_for(U, 128), 128, 0, s);
   IGN_LAUNCH(ctx, k_simp_boundary, blocks_for(3 * T, 256), 256, 0, s);
   const double max_err2 = (double)max_error * (double)max_error;
@@ -1828,6 +1816,7 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   const char* group_env = getenv("IGN_SIMP_GROUP");
   const int group = group_env ? atoi(group_env) : 0;
   A.group_min = group == 16 || group == 32 ? (uint32_t)group : 8u;
+  prof.end();
   {
     const int slot = prof_begin(ctx, IGN_PROF_SIMP);
     // default: one CTA per label (SMs are handed back to the block scheduler after every label, so
@@ -1912,8 +1901,6 @@ extern "C" int ign_mesh_simplify(ign_mesher* m, const float resolution[3], int r
   }
 
   // ---- compaction
-  uint32_t* fscan = node_v;   // 3T u32 >= T
-  uint32_t* fflag = node_h;
   size_t tb = tmpb;
   IGN_LAUNCH(ctx, k_simp_flags_u32, blocks_for(U, 256), 256, 0, s.valive, U, vflag32);
   IGN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, vflag32, vscan, (int)U, ctx->stream));
