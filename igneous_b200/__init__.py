@@ -17,9 +17,13 @@ _TASK_NAMES = ("DownsampleTask", "TransferTask", "ImageShardTransferTask", "Imag
                "downsample_method_to_fn", "threshold_image", "blackout_non_face_rails", "DisjointSet",
                "QuantizeTask", "CLAHETask", "ContrastNormalizationTask", "LuminanceLevelsTask",
                "SpatialIndexTask", "CountVoxelsTask", "SkeletonTask", "UnshardedSkeletonMergeTask",
-               "BlackoutTask", "TouchTask", "DeleteTask", "ShardedFromUnshardedSkeletonMergeTask")
+               "BlackoutTask", "TouchTask", "DeleteTask", "ShardedFromUnshardedSkeletonMergeTask",
+               "MeshManifestPrefixTask", "MeshManifestFilesystemTask", "TransferMeshFilesTask", "DeleteMeshFilesTask",
+               "TransferSkeletonFilesTask", "DeleteSkeletonFilesTask")
 # creators whose task is in _TASK_NAMES and that have no other root-level name in the reference
-_CREATION_NAMES = ("create_sharded_skeletons_from_unsharded_tasks",)
+_CREATION_NAMES = ("create_sharded_skeletons_from_unsharded_tasks", "create_mesh_manifest_tasks",
+                   "create_mesh_deletion_tasks", "create_xfer_meshes_tasks", "create_skeleton_deletion_tasks",
+                   "create_xfer_skeleton_tasks")
 _COMPAT_NAMES = ("CloudVolume", "EmptyVolumeException", "LocalTaskQueue", "RegisteredTask", "queueable")
 __all__ = ["Mesher", "__version__"] + list(_TASK_NAMES) + list(_CREATION_NAMES) + list(_COMPAT_NAMES)
 

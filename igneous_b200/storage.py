@@ -17,6 +17,7 @@ import gzip
 import json
 import os
 import re
+import shutil
 
 import numpy as np
 
@@ -355,6 +356,17 @@ class CloudFiles:
           out.append(rel)
     return sorted(set(out))
 
+  def transfer_to(self, cf_dest, paths, **kwargs):
+    """Copy the stored files of `paths` (keys as list() gives them) to the same keys under cf_dest, byte for
+    byte: a file stored with a compression suffix keeps its suffix and its compressed stream."""
+    for key in list(paths):
+      path, ext = self._find(key)
+      if path is None:
+        continue
+      dest = cf_dest._abs(key) + ext
+      os.makedirs(os.path.dirname(dest), exist_ok=True)
+      shutil.copyfile(path, dest)
+
   def delete(self, keys):
     if isinstance(keys, str):
       keys = [keys]
@@ -378,7 +390,26 @@ class _SpatialIndex:
 
 
 class _MeshMeta:
+  """cv.mesh.meta: the mesh directory's info ({dir}/info, {} when the file is absent), the directory's path
+  and whether its meshes are sharded."""
+
+  def __init__(self, cv, subdir):
+    self.subdir = subdir
+    self.info = cv.cf.get_json(subdir + "/info") or {}
+    self.layerpath = cv.join(cv.cloudpath, subdir)
+
+  def is_sharded(self):
+    return self.info.get("sharding") is not None
+
+
+class _MeshSource:
+  """cv.mesh: meta and spatial_index of the mesh directory (CloudVolume(mesh_dir=...), else the layer's
+  info['mesh'], else `mesh`, as recalled of cloudvolume)."""
+
   spatial_index = _SpatialIndex()
+
+  def __init__(self, cv):
+    self.meta = _MeshMeta(cv, cv.mesh_dir or cv.info.get("mesh", "mesh"))
 
 
 # cloudvolume's default skeleton info, as recalled (unpinned): identity transform, radius then vertex_types
@@ -394,11 +425,15 @@ DEFAULT_SKELETON_INFO = {
 
 class _SkeletonMeta:
   """cv.skeleton.meta: the skeleton directory's info ({info['skeletons']}/info, cloudvolume's default
-  when the file is absent) and commit_info()."""
+  when the file is absent), the directory's path, whether it is sharded, and commit_info()."""
 
   def __init__(self, cv, subdir):
     self._cv, self.subdir = cv, subdir
     self.info = cv.cf.get_json(subdir + "/info") or copy.deepcopy(DEFAULT_SKELETON_INFO)
+    self.layerpath = cv.join(cv.cloudpath, subdir)
+
+  def is_sharded(self):
+    return self.info.get("sharding") is not None
 
   @property
   def mip(self):
@@ -419,7 +454,7 @@ class _SkeletonSource:
     self._cv = cv
     self.meta = _SkeletonMeta(cv, subdir)
     self.path = cv.cf.join(cv.cloudpath, subdir)
-    self.spatial_index = cv.mesh.spatial_index
+    self.spatial_index = _MeshSource.spatial_index
 
   def get(self, segid):
     """The skeleton {dir}/{segid} decoded per meta.info['vertex_attributes'] (a list of ids -> a list)."""
@@ -564,9 +599,10 @@ class CloudVolume:
 
   def __init__(self, cloudpath, mip=0, fill_missing=False, bounded=True, info=None, compress="gzip",
                delete_black_uploads=False, background_color=0, parallel=1, progress=False, non_aligned_writes=False,
-               skel_dir=None, **kwargs):
+               skel_dir=None, mesh_dir=None, **kwargs):
     self.cloudpath = cloudpath
     self.skel_dir = skel_dir
+    self.mesh_dir = mesh_dir
     self.path = _strip(cloudpath)
     self.fill_missing = bool(fill_missing)
     self.bounded = bounded
@@ -576,7 +612,7 @@ class CloudVolume:
     self.non_aligned_writes = bool(non_aligned_writes)
     self.cf = CloudFiles(cloudpath)
     self.provenance = _Provenance()
-    self.mesh = _MeshMeta()
+    self._mesh = None
     self._skeleton = None
     if info is not None:
       self.info = copy.deepcopy(info)
@@ -596,6 +632,13 @@ class CloudVolume:
   @property
   def image(self):
     return _ImageSource(self)
+
+  @property
+  def mesh(self):
+    """the mesh source, read on first use (its info file and directory follow mesh_dir or info['mesh'])"""
+    if self._mesh is None:
+      self._mesh = _MeshSource(self)
+    return self._mesh
 
   @property
   def skeleton(self):

@@ -1,6 +1,7 @@
 """Grid enumeration shared by the task creators
 (igneous/task_creation/common.py:11-104)."""
 import copy
+import itertools
 import os
 import subprocess
 from functools import partial
@@ -138,3 +139,37 @@ def compute_shard_params_for_hashed(num_labels, shard_index_bytes=2 ** 13, minis
     minishard_bits -= want - shard_bits
     shard_bits = want
   return (int(shard_bits), int(max(minishard_bits, 0)), 0)
+
+
+def deletion_prefixes(who, magnitude):
+  """the prefixes of the unsharded mesh and skeleton deletions: "0" (spatial index files from 0), "1:" ...
+  "{10^(m-1) - 1}:", then 10^(m-1) ... 10^m - 1.  magnitude 0 has none (the reference's range(1, 0.1)
+  fails), so it raises ValueError."""
+  magnitude = int(magnitude)
+  if magnitude < 1:
+    raise ValueError("%s: magnitude must be at least 1 (got %d)" % (who, magnitude))
+  start, end = 10 ** (magnitude - 1), 10 ** magnitude
+  return ["0"] + [str(p) + ":" for p in range(1, start)] + [str(p) for p in range(start, end)]
+
+
+def xfer_destination_dir(who, cf_dest, subdir, key):
+  """the directory a mesh or skeleton transfer writes to: subdir, else the destination info's `key`.
+  ValueError when the destination has no info (its tasks could not open it) or neither names a directory."""
+  info = cf_dest.get_json("info")
+  if info is None:
+    raise ValueError("%s: %s has no info file" % (who, cf_dest.cloudpath))
+  if not subdir:
+    subdir = info.get(key)
+  if not subdir:
+    raise ValueError("%s: pass the destination directory or give %s/info a `%s`" % (who, cf_dest.cloudpath, key))
+  return subdir
+
+
+def xfer_prefixes(magnitude, sharded, suffix):
+  """every string of `magnitude` characters over 0-9 (and a-f when sharded), then every shorter one
+  followed by `suffix`"""
+  alphabet = [str(i) for i in range(10)] + (list("abcdef") if sharded else [])
+  prefixes = ["".join(x) for x in itertools.product(alphabet, repeat=int(magnitude))]
+  for i in range(1, int(magnitude)):
+    prefixes += ["".join(x) + suffix for x in itertools.product(alphabet, repeat=i)]
+  return prefixes

@@ -1,10 +1,13 @@
-"""create_meshing_tasks (igneous/task_creation/mesh.py:158-267) and
-create_spatial_index_mesh_tasks (:363-435)."""
+"""create_meshing_tasks (igneous/task_creation/mesh.py:158-267), create_spatial_index_mesh_tasks (:363-435),
+create_mesh_manifest_tasks (:54-89), create_mesh_deletion_tasks (:91-155) and create_xfer_meshes_tasks
+(:548-588)."""
+from functools import partial
 from time import strftime
 
 from .._compat import CloudVolume, CloudFiles, Vec
-from ..tasks import MeshTask
-from .common import FinelyDividedTaskIterator, operator_contact, spatial_index_tasks
+from ..tasks import MeshTask, MeshManifestPrefixTask, MeshManifestFilesystemTask, TransferMeshFilesTask, DeleteMeshFilesTask
+from .common import (FinelyDividedTaskIterator, deletion_prefixes, operator_contact, spatial_index_tasks,
+                     xfer_destination_dir, xfer_prefixes)
 
 
 def create_meshing_tasks(layer_path, mip, shape=(448, 448, 448), simplification=True,
@@ -56,3 +59,61 @@ def create_spatial_index_mesh_tasks(cloudpath, shape=(448, 448, 448), mip=0, fil
   """Rebuild the spatial index of a mesh directory (default: the layer's, else mesh_mip_{mip}_err_40),
   or build one over a different grid than the mesh tasks used."""
   return spatial_index_tasks(cloudpath, shape, mip, fill_missing, compress, mesh_dir, "mesh")
+
+
+def create_mesh_manifest_tasks(layer_path, magnitude=3, mesh_dir=None):
+  """Tasks that write each label's legacy manifest {mesh_dir}/{segid}:0 from its fragments.  A file://
+  layer gets one MeshManifestFilesystemTask; any other protocol 10^m - 1 MeshManifestPrefixTasks over the
+  prefixes "1:" ... "{10^(m-1) - 1}:", then 10^(m-1) ... 10^m - 1, each of which also takes the longer labels
+  that start with it (DESIGN.md §5m)."""
+  assert int(magnitude) == magnitude
+  assert magnitude > 0
+  if "://" not in layer_path or layer_path.startswith("file://"):
+    return [partial(MeshManifestFilesystemTask, layer_path=layer_path, mesh_dir=mesh_dir)]
+  start, end = int(10 ** (magnitude - 1)), int(10 ** magnitude)
+
+  class MeshManifestTaskIterator:
+    def __len__(self):
+      return end - 1
+
+    def __iter__(self):
+      for prefix in [str(p) + ":" for p in range(1, start)] + [str(p) for p in range(start, end)]:
+        yield partial(MeshManifestPrefixTask, layer_path=layer_path, prefix=prefix, mesh_dir=mesh_dir)
+
+  return MeshManifestTaskIterator()
+
+
+def create_mesh_deletion_tasks(layer_path, magnitude=3, mesh_dir=None):
+  """Tasks that delete the mesh directory's files.  The directory's info is deleted here, while the tasks
+  are made, and the provenance is appended.  A sharded directory gets one task over every file; otherwise
+  10^m tasks: "0", "1:" ... "{10^(m-1) - 1}:", then 10^(m-1) ... 10^m - 1 (DESIGN.md §5m lists the spatial
+  index files these leave).  magnitude=0 raises ValueError before anything is deleted."""
+  assert int(magnitude) == magnitude
+  assert magnitude >= 0
+  prefixes = deletion_prefixes("create_mesh_deletion_tasks", magnitude)
+  cv = CloudVolume(layer_path, mesh_dir=mesh_dir)
+  CloudFiles(cv.mesh.meta.layerpath).delete("info")
+  if cv.mesh.meta.is_sharded():
+    prefixes = [""]
+  cv.provenance.processing.append({
+    "method": {"task": "DeleteMeshFilesTask", "layer_path": layer_path, "mesh_dir": mesh_dir},
+    "by": operator_contact(),
+    "date": strftime("%Y-%m-%d %H:%M %Z"),
+  })
+  cv.commit_provenance()
+  return [partial(DeleteMeshFilesTask, cloudpath=layer_path, prefix=p, mesh_dir=mesh_dir) for p in prefixes]
+
+
+def create_xfer_meshes_tasks(src, dest, mesh_dir=None, magnitude=2):
+  """Tasks that copy src's mesh files, byte for byte, to dest's mesh directory (mesh_dir, else dest's
+  info['mesh']), after writing src's mesh info there.  The prefixes are every string of `magnitude` digits
+  (hex digits for a sharded source), then every shorter one followed by ":0" (unsharded) or "." (sharded);
+  DESIGN.md §5m lists the files they miss.  A dest without an info file, or with neither mesh_dir nor a
+  `mesh` in its info, raises ValueError before anything is written."""
+  cv_src = CloudVolume(src)
+  cf_dest = CloudFiles(dest)
+  mesh_dir = xfer_destination_dir("create_xfer_meshes_tasks", cf_dest, mesh_dir, "mesh")
+  cf_dest.put_json("%s/info" % mesh_dir, cv_src.mesh.meta.info)
+  sharded = cv_src.mesh.meta.is_sharded()
+  prefixes = xfer_prefixes(magnitude, sharded, "." if sharded else ":0")
+  return [partial(TransferMeshFilesTask, src=src, dest=dest, prefix=p, mesh_dir=mesh_dir) for p in prefixes]

@@ -1,6 +1,7 @@
 """create_skeletonizing_tasks (igneous/task_creation/skeleton.py:68-388),
-create_unsharded_skeleton_merge_tasks (:535-591), create_sharded_skeletons_from_unsharded_tasks (:659-753) and
-create_spatial_index_skeleton_tasks (:795-867)."""
+create_unsharded_skeleton_merge_tasks (:535-591), create_sharded_skeletons_from_unsharded_tasks (:659-753),
+create_spatial_index_skeleton_tasks (:795-867), create_skeleton_deletion_tasks (:593-657) and
+create_xfer_skeleton_tasks (:756-793)."""
 import copy
 import re
 from functools import partial
@@ -11,9 +12,11 @@ import numpy as np
 from .. import labelshard
 from .._compat import CloudVolume, CloudFiles, Vec
 from ..sharding import LabelShardingSpecification
-from ..tasks import SkeletonTask, UnshardedSkeletonMergeTask, ShardedFromUnshardedSkeletonMergeTask
+from ..tasks import (SkeletonTask, UnshardedSkeletonMergeTask, ShardedFromUnshardedSkeletonMergeTask,
+                     DeleteSkeletonFilesTask, TransferSkeletonFilesTask)
 from ..tasks.skeleton import refuse, refuse_same_directory
-from .common import FinelyDividedTaskIterator, compute_shard_params_for_hashed, operator_contact, spatial_index_tasks
+from .common import (FinelyDividedTaskIterator, compute_shard_params_for_hashed, deletion_prefixes, operator_contact,
+                     spatial_index_tasks, xfer_destination_dir, xfer_prefixes)
 
 
 def create_skeletonizing_tasks(cloudpath, mip, shape=Vec(512, 512, 512), teasar_params={"scale": 10, "const": 10},
@@ -203,3 +206,38 @@ def create_sharded_skeletons_from_unsharded_tasks(src, dest, shard_index_bytes=2
   cv_dest.commit_provenance()
   return [partial(ShardedFromUnshardedSkeletonMergeTask, src=src, dest=dest, shard_no=str(s), skel_dir=skel_dir)
           for s in shards.tolist()]
+
+
+def create_skeleton_deletion_tasks(cloudpath, magnitude=2, skel_dir=None):
+  """Tasks that delete the skeleton directory's files.  The directory's info is deleted here, while the
+  tasks are made, and the provenance is appended.  A sharded directory gets one task over every file;
+  otherwise 10^m tasks: "0", "1:" ... "{10^(m-1) - 1}:", then 10^(m-1) ... 10^m - 1 (DESIGN.md §5m lists the
+  files these leave).  magnitude=0 raises ValueError before anything is deleted."""
+  assert int(magnitude) == magnitude
+  assert magnitude >= 0
+  prefixes = deletion_prefixes("create_skeleton_deletion_tasks", magnitude)
+  cv = CloudVolume(cloudpath, skel_dir=skel_dir)
+  CloudFiles(cv.skeleton.meta.layerpath).delete("info")
+  if cv.skeleton.meta.is_sharded():
+    prefixes = [""]
+  cv.provenance.processing.append({
+    "method": {"task": "DeleteSkeletonFilesTask", "cloudpath": cloudpath, "skel_dir": skel_dir},
+    "by": operator_contact(),
+    "date": strftime("%Y-%m-%d %H:%M %Z"),
+  })
+  cv.commit_provenance()
+  return [partial(DeleteSkeletonFilesTask, cloudpath=cloudpath, prefix=p, skel_dir=skel_dir) for p in prefixes]
+
+
+def create_xfer_skeleton_tasks(src, dest, skel_dir=None, magnitude=2):
+  """Tasks that copy src's skeleton files, byte for byte, to dest's skeleton directory (skel_dir, else
+  dest's info['skeletons']), after writing src's skeleton info there.  The prefixes are every string of
+  `magnitude` digits (hex digits for a sharded source), then every shorter one, which overlap the longer ones.
+  A dest without an info file, or with neither skel_dir nor a `skeletons` in its info, raises ValueError before
+  anything is written."""
+  cv_src = CloudVolume(src)
+  cf_dest = CloudFiles(dest)
+  skel_dir = xfer_destination_dir("create_xfer_skeleton_tasks", cf_dest, skel_dir, "skeletons")
+  cf_dest.put_json("%s/info" % skel_dir, cv_src.skeleton.meta.info)
+  prefixes = xfer_prefixes(magnitude, cv_src.skeleton.meta.is_sharded(), "")
+  return [partial(TransferSkeletonFilesTask, src=src, dest=dest, prefix=p, skel_dir=skel_dir) for p in prefixes]

@@ -5,11 +5,18 @@ path (MeshTask.__init__ options :98-129, execute :140-265,
 _handle_dataset_boundary :267-303, _remove_dust :313-322, _remap :357-369,
 fill_holes :211-243, compute_meshes :371-383, _create_mesh_binary :432-450, uploads :399-464).
 zmesh / fastremap / fastmorph are replaced by igneous_b200.zmesh / .fastremap / .fastmorph.
+
+The manifest, transfer and deletion tasks (:624-749) only list, group, copy and delete files; they have no
+device work (DESIGN.md §5m).
 """
+import os
+import re
+from collections import defaultdict
+
 import numpy as np
 
 from .. import fastmorph, fastremap, zmesh
-from .._compat import CloudVolume, CloudFiles, Bbox, Vec, RegisteredTask
+from .._compat import CloudVolume, CloudFiles, Bbox, Vec, RegisteredTask, queueable
 
 _DEFAULTS = {
   "cache_control": None, "draco_compression_level": 1, "draco_create_metadata": False,
@@ -184,3 +191,72 @@ class MeshTask(RegisteredTask):
     cf.put_json("%s/%s.spatial" % (self._mesh_dir, phys.to_filename(self._volume.mesh.spatial_index.precision)),
                 {str(k): v for k, v in mesh_bboxes.items()}, compress=self.options["compress"],
                 cache_control=False)  # mesh.py:452-464
+
+
+# a fragment "{segid}:{lod}:{bbox}"; a manifest "{segid}:{lod}", the info and .spatial files never match
+FRAGMENT = re.compile(r"(\d+):(\d+):")
+
+
+def _manifest_dir(who, cf, mesh_dir):
+  """mesh_dir, else the layer info's `mesh`; ValueError when neither names one"""
+  if mesh_dir is not None:
+    return mesh_dir
+  info = cf.get_json("info")
+  if info is None or "mesh" not in info:
+    raise ValueError("%s: pass mesh_dir or give %s/info a `mesh` directory" % (who, cf.cloudpath))
+  return info["mesh"]
+
+
+def _put_manifests(cf, mesh_dir, lod, names):
+  """{mesh_dir}/{segid}:{lod} -> {"fragments": [...]} for the names of lod's fragments, grouped by segid in
+  the order they come, stored uncompressed"""
+  segids = defaultdict(list)
+  for name in names:
+    m = FRAGMENT.search(name)
+    if m is None or int(m.group(2)) != lod:
+      continue
+    segids[int(m.group(1))].append(name)
+  cf.put_jsons(("%s/%d:%d" % (mesh_dir, segid, lod), {"fragments": frags}) for segid, frags in segids.items())
+
+
+@queueable
+def MeshManifestPrefixTask(layer_path, prefix, lod=0, mesh_dir=None):
+  """Write the manifest of every label with a lod fragment whose name starts with `prefix` in the mesh
+  directory (igneous/tasks/mesh/mesh.py:672-724).  Names are the listing's, without a storage suffix, so
+  neuroglancer requests the fragments by them."""
+  cf = CloudFiles(layer_path)
+  mesh_dir = _manifest_dir("MeshManifestPrefixTask", cf, mesh_dir)
+  names = (os.path.basename(n) for n in cf.list(prefix=cf.join(mesh_dir, prefix)))
+  _put_manifests(cf, mesh_dir, int(lod), names)
+
+
+@queueable
+def MeshManifestFilesystemTask(layer_path, lod=0, mesh_dir=None):
+  """MeshManifestPrefixTask over one scan of a file:// mesh directory (igneous/tasks/mesh/mesh.py:624-670):
+  regular files only, each name without its extension (1:0:0-64_0-64_0-64.gz -> 1:0:0-64_0-64_0-64)."""
+  cf = CloudFiles(layer_path)
+  mesh_dir = _manifest_dir("MeshManifestFilesystemTask", cf, mesh_dir)
+  path = layer_path[len("file://"):] if layer_path.startswith("file://") else layer_path
+  if "://" in path:
+    raise ValueError("MeshManifestFilesystemTask: %s is not a file:// path" % layer_path)
+  with os.scandir(os.path.join(path, mesh_dir)) as entries:
+    names = [os.path.splitext(e.name)[0] for e in entries if e.is_file()]
+  _put_manifests(cf, mesh_dir, int(lod), names)
+
+
+@queueable
+def TransferMeshFilesTask(src, dest, prefix, mesh_dir=None):
+  """Copy the stored files whose names start with `prefix` from src's mesh directory to dest's (mesh_dir,
+  else dest's info), byte for byte (igneous/tasks/mesh/mesh.py:726-739)."""
+  cv_src = CloudVolume(src)
+  cv_dest = CloudVolume(dest, mesh_dir=mesh_dir)
+  cf_src = CloudFiles(cv_src.mesh.meta.layerpath)
+  cf_src.transfer_to(CloudFiles(cv_dest.mesh.meta.layerpath), paths=cf_src.list(prefix=prefix))
+
+
+@queueable
+def DeleteMeshFilesTask(cloudpath, prefix, mesh_dir=None):
+  """Delete the files whose names start with `prefix` in the mesh directory (igneous/tasks/mesh/mesh.py:741-749)."""
+  cv = CloudVolume(cloudpath, mesh_dir=mesh_dir)
+  cf = CloudFiles(cv.mesh.meta.layerpath)
+  cf.delete(cf.list(prefix=prefix))

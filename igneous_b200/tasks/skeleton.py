@@ -10,6 +10,8 @@ device renumbers, and the export keys skeletons by original label.
 UnshardedSkeletonMergeTask mirrors igneous/tasks/skeleton.py:810-916; its fuse and kimimaro.postprocess run on
 the device (igneous_b200.kimimaro.merge_fragments, DESIGN.md §5h).  ShardedFromUnshardedSkeletonMergeTask
 mirrors :1074-1130: it packs finished unsharded skeletons into one hashed shard (DESIGN.md §5l).
+TransferSkeletonFilesTask and DeleteSkeletonFilesTask (:1133-1156) copy and delete files; they have no device
+work (DESIGN.md §5m).
 """
 import gzip
 import os
@@ -286,3 +288,21 @@ def ShardedFromUnshardedSkeletonMergeTask(src, dest, shard_no, cache_control=Fal
               cache_control="no-cache")
   last_phase_seconds.update(labels=t1 - t0, read=t2 - t1, device=t3 - t2, gzip=t4 - t3,
                             write=time.perf_counter() - t4)
+
+
+@queueable
+def DeleteSkeletonFilesTask(cloudpath, prefix, skel_dir=None):
+  """Delete the files whose names start with `prefix` in the skeleton directory (igneous/tasks/skeleton.py:1133-1141)."""
+  cv = CloudVolume(cloudpath, skel_dir=skel_dir)
+  cf = CloudFiles(cv.skeleton.meta.layerpath)
+  cf.delete(cf.list(prefix=prefix))
+
+
+@queueable
+def TransferSkeletonFilesTask(src, dest, prefix, skel_dir=None):
+  """Copy the stored files whose names start with `prefix` from src's skeleton directory to dest's (skel_dir,
+  else dest's info), byte for byte (igneous/tasks/skeleton.py:1144-1156)."""
+  cv_src = CloudVolume(src)
+  cv_dest = CloudVolume(dest, skel_dir=skel_dir)
+  cf_src = CloudFiles(cv_src.skeleton.meta.layerpath)
+  cf_src.transfer_to(CloudFiles(cv_dest.skeleton.meta.layerpath), paths=cf_src.list(prefix=prefix))
