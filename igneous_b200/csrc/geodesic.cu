@@ -446,7 +446,7 @@ __global__ void __launch_bounds__(256) k_teasar_pdrf(const T* __restrict__ lab, 
 
 
 // ---------------------------------------------------------------------------------------------------
-// TEASAR (DESIGN.md §5f): objects, the path loop and its compaction.  Objects are u32 ids 1..K.
+// TEASAR (DESIGN.md §5f): border targets, the path loop and its compaction.  Objects are u32 ids 1..K.
 
 constexpr uint32_t NONE32 = 0xFFFFFFFFu;
 constexpr uint64_t NONE64 = ~0ull;
@@ -467,37 +467,6 @@ struct TpCtl {
 constexpr size_t TP_ROUND_BYTES = 16;
 
 thread_local uint64_t g_tp_stats[4];  // rounds, paths, voxels invalidated, host synchronisations
-
-__global__ void __launch_bounds__(256) k_obj_seeds(const uint64_t* __restrict__ idx, uint64_t k, uint64_t* src,
-                                                   unsigned long long* ns) {
-  const uint64_t l = 1 + blockIdx.x * 256ull + threadIdx.x;
-  if (l <= k && idx[l] != NONE64) src[atomicAdd(ns, 1ull)] = idx[l];
-}
-
-// reached voxels of the pending labels become the object of their label's seed (seed index + 1)
-__global__ void __launch_bounds__(256) k_obj_claim(uint32_t* __restrict__ pending, const float* __restrict__ dist,
-                                                   const uint64_t* __restrict__ idx, uint64_t n,
-                                                   uint32_t* __restrict__ key) {
-  for (uint64_t i = blockIdx.x * 256ull + threadIdx.x; i < n; i += (uint64_t)gridDim.x * 256) {
-    const uint32_t l = pending[i];
-    if (l && isfinite(dist[i])) {
-      key[i] = (uint32_t)idx[l] + 1;
-      pending[i] = 0;
-    }
-  }
-}
-
-__global__ void __launch_bounds__(256) k_obj_count(const uint32_t* __restrict__ obj, uint64_t n, uint32_t* count) {
-  for (uint64_t i = blockIdx.x * 256ull + threadIdx.x; i < n; i += (uint64_t)gridDim.x * 256)
-    if (obj[i]) atomicAdd(count + obj[i], 1u);
-}
-
-__global__ void __launch_bounds__(256) k_obj_dust(const uint32_t* obj, const uint32_t* __restrict__ count, uint64_t n,
-                                                  uint64_t dust, uint32_t* out) {  // in place
-
-  for (uint64_t i = blockIdx.x * 256ull + threadIdx.x; i < n; i += (uint64_t)gridDim.x * 256)
-    out[i] = obj[i] && count[obj[i]] >= dust ? obj[i] : 0;
-}
 
 // the last target of each object (in the order given) replaces its root; targets off every object are ignored
 __global__ void __launch_bounds__(256) k_tg_last(const uint32_t* __restrict__ obj, uint64_t n,
@@ -823,62 +792,6 @@ int ign_teasar_pdrf_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t n,
   });
 }
 
-int ign_teasar_objects_dev(ign_ctx* ctx, const uint32_t* labels, uint64_t sx, uint64_t sy, uint64_t sz,
-                           uint64_t max_label, int connectivity, uint64_t dust_threshold, uint32_t* objects_out,
-                           uint64_t* n_objects) {
-  IGN_TRY(activate(ctx));
-  IGN_TRY(geo_check(IGN_U32, sx, sy, sz, connectivity, nullptr, true, true));
-  IGN_REQUIRE(n_objects && max_label < (1ull << 32), IGN_ERR_INVALID, "teasar_objects: null count or max_label >= 2^32");
-  const uint64_t n = sx * sy * sz;
-  *n_objects = 0;
-  if (n == 0) return IGN_OK;
-  IGN_REQUIRE(labels && objects_out, IGN_ERR_INVALID, "teasar_objects: null buffer");
-  const float one[3] = {1.f, 1.f, 1.f};
-  const Nbrs nb = make_nbrs(connectivity, one);
-  ScratchFrame f(ctx);
-  uint32_t *pending, *count;
-  float *zero, *dist, *vmax;
-  uint64_t *idx, *src;
-  unsigned long long* ns;
-  IGN_TRY(f.take(&pending, n));
-  IGN_TRY(f.take(&zero, n));
-  IGN_TRY(f.take(&dist, n));
-  IGN_TRY(f.take(&idx, max_label + 1));
-  IGN_TRY(f.take(&vmax, max_label + 1));
-  IGN_TRY(f.take(&src, max_label + 1));
-  IGN_TRY(f.take(&ns, 1));
-  IGN_CUDA(cudaMemcpyAsync(pending, labels, n * 4, cudaMemcpyDeviceToDevice, ctx->stream));
-  IGN_CUDA(cudaMemsetAsync(zero, 0, n * 4, ctx->stream));
-  IGN_CUDA(cudaMemsetAsync(objects_out, 0, n * 4, ctx->stream));
-  const unsigned vgrid = (unsigned)std::min<uint64_t>(blocks_for(n, 256), (uint64_t)ctx->sm_count * 16);
-  // one solve per part of the most-split label: seed every label with a pending voxel at its first one
-  // (the argmax of a zero field), claim what the seeds reach, repeat; each round claims at least a voxel
-  for (uint64_t r = 0;; ++r) {
-    IGN_REQUIRE(r <= n, IGN_ERR_INVALID, "teasar_objects: not done after %llu rounds", (unsigned long long)r);
-    IGN_TRY(ign_label_argmax_dev(ctx, pending, IGN_U32, n, zero, max_label, idx, vmax));
-    IGN_CUDA(cudaMemsetAsync(ns, 0, 8, ctx->stream));
-    IGN_LAUNCH(ctx, k_obj_seeds, blocks_for(max_label, 256) + 1, 256, 0, idx, max_label, src, ns);
-    unsigned long long hns = 0;
-    IGN_TRY(small_d2h(ctx, &hns, ns, 8));
-    IGN_TRY(small_sync(ctx));
-    if (hns == 0) break;
-    IGN_TRY((geo_run<uint32_t, false>(ctx, pending, sx, sy, sz, nb, nullptr, src, hns, dist, nullptr)));
-    IGN_LAUNCH(ctx, k_obj_claim, vgrid, 256, 0, pending, dist, idx, n, objects_out);
-  }
-  // object ids by first voxel in F order, dust dropped, ids again 1..K
-  uint64_t k = 0;
-  IGN_TRY(ign_renumber_dev(ctx, objects_out, IGN_U32, n, pending, nullptr, 0, &k));
-  if (dust_threshold > 1 && k) {
-    IGN_TRY(f.take(&count, k + 1));
-    IGN_CUDA(cudaMemsetAsync(count, 0, (k + 1) * 4, ctx->stream));
-    IGN_LAUNCH(ctx, k_obj_count, vgrid, 256, 0, pending, n, count);
-    IGN_LAUNCH(ctx, k_obj_dust, vgrid, 256, 0, pending, count, n, dust_threshold, pending);
-  }
-  IGN_TRY(ign_renumber_dev(ctx, pending, IGN_U32, n, objects_out, nullptr, 0, &k));
-  *n_objects = k;
-  return IGN_OK;
-}
-
 int ign_teasar_border_targets_dev(ign_ctx* ctx, const uint32_t* objects, uint64_t sx, uint64_t sy, uint64_t sz,
                                   uint64_t n_objects, const float anisotropy[3], uint64_t* targets_out,
                                   uint64_t capacity, uint64_t* count) {
@@ -905,7 +818,7 @@ int ign_teasar_border_targets_dev(ign_ctx* ctx, const uint32_t* objects, uint64_
     IGN_LAUNCH(ctx, k_face_extract, grid, 256, 0, objects, face, sx, sy, sz, p0, np, plane);
     // the 8-connected parts of each object in the plane (connectivity 18 on an extent-1 axis), by first voxel
     uint64_t nparts = 0;
-    IGN_TRY(ign_teasar_objects_dev(ctx, plane, p0, p1, 1, n_objects, 18, 0, parts, &nparts));
+    IGN_TRY(ign_label_parts_dev(ctx, plane, IGN_U32, p0, p1, 1, 18, 0, parts, nullptr, 0, &nparts));
     if (!nparts) continue;
     IGN_REQUIRE(total + nparts <= capacity, IGN_ERR_OVERFLOW, "teasar_border_targets: more than %llu targets",
                 (unsigned long long)capacity);

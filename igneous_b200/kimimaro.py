@@ -212,8 +212,8 @@ def export_skeletons(all_labels, offset=(0.0, 0.0, 0.0), vertex_types=True, teas
                                       drop.size, 1))
     obj = alloc(n * 4)
     m = ctypes.c_uint64(0)
-    _shim.check(lib.ign_teasar_objects_dev(h, ptr(lab), *vol.shape, K, 26, int(dust_threshold), ptr(obj),
-                                           ctypes.byref(m)))
+    _shim.check(lib.ign_label_parts_dev(h, ptr(lab), _shim.IGN_U32, *vol.shape, 26, int(dust_threshold), ptr(obj),
+                                        None, 0, ctypes.byref(m)))
     M = int(m.value)
     phase("upload_objects")
     if M == 0:

@@ -61,8 +61,8 @@ def component_boxes_dev(mask, dust_threshold):
   # 2^32 - 1 voxels or more is refused by the call before it writes, so it gets none
   cap = (X + 1) // 2 * ((Y + 1) // 2) * ((Z + 1) // 2) if X * Y * Z < 2 ** 32 - 1 else 0
   rows = np.empty((cap, 7), dtype=np.uint32)
-  _shim.check(ctx.lib.ign_mask_boxes_dev(ctx.handle, mask.ptr, X, Y, Z, max(int(dust_threshold), 0), _shim.ptr(rows), cap,
-                                         _shim.ptr(n)))
+  _shim.check(ctx.lib.ign_label_parts_dev(ctx.handle, mask.ptr, _shim.IGN_U8, X, Y, Z, 26, max(int(dust_threshold), 0),
+                                          None, _shim.ptr(rows), cap, _shim.ptr(n)))
   return rows[:int(n[0])].copy()
 
 

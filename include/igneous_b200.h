@@ -419,9 +419,8 @@ IGN_API int ign_teasar_pdrf_dev(ign_ctx* ctx, const void* labels, int dtype, uin
                                 uint64_t max_label, float scale, int exponent, float* out);
 /* TEASAR skeletons (kimimaro.skeletonize as recalled, parity unpinned; DESIGN.md §5f).  Every array is a
  * DEVICE array; volumes are (sx, sy, sz) F-order with fewer than 2^32 - 1 voxels.
- * ign_teasar_objects_dev: labels u32 1..max_label (renumbered) -> objects_out u32 1..*n_objects, the parts of
- *   each label joined under `connectivity` (6 / 18 / 26), numbered by first voxel in linear order; parts of
- *   fewer than dust_threshold voxels are 0.  One geodesic solve per part of the most-split label.
+ * kimimaro.skeletonize takes its objects from ign_label_parts_dev at connectivity 26, so a volume of 2^32 - 1
+ *   voxels or more is refused there with IGN_ERR_UNSUPPORTED, before the solver's IGN_ERR_OVERFLOW.
  * ign_teasar_border_targets_dev: kimimaro's fix_borders targets (as recalled): for each face in the order
  *   x = 0, x = sx - 1, y = 0, y = sy - 1, z = 0, z = sz - 1, the 8-connected parts of each object in the
  *   face plane, ordered by first voxel in the plane's F order, and per part the voxel of greatest 2-D edt
@@ -441,9 +440,6 @@ IGN_API int ign_teasar_pdrf_dev(ign_ctx* ctx, const void* labels, int dtype, uin
  *   naming it.  The host synchronises once per round (plus the solver's own synchronisations).
  * ign_teasar_last_stats: diagnostic only; this thread's last paths call: [0] rounds, [1] paths, [2] box
  *   voxels visited by the invalidation, [3] host synchronisations. */
-IGN_API int ign_teasar_objects_dev(ign_ctx* ctx, const uint32_t* labels, uint64_t sx, uint64_t sy, uint64_t sz,
-                                   uint64_t max_label, int connectivity, uint64_t dust_threshold,
-                                   uint32_t* objects_out, uint64_t* n_objects);
 IGN_API int ign_teasar_border_targets_dev(ign_ctx* ctx, const uint32_t* objects, uint64_t sx, uint64_t sy,
                                           uint64_t sz, uint64_t n_objects, const float anisotropy[3],
                                           uint64_t* targets_out, uint64_t capacity, uint64_t* count);
@@ -700,19 +696,25 @@ IGN_API int ign_fill_box_dev(ign_ctx* ctx, void* cutout, int dtype, uint64_t X, 
  * ign_threshold_dev: out[i] = in[i] > t (u8 0 / 1), n voxels, 64-bit indexing.  Integer dtypes
  *   (IGN_U8 / U16 / U32 / U64) compare as unsigned 64-bit integers, so every t >= 0 is exact; for
  *   IGN_F32 the low 32 bits of t are the float32 threshold's bit pattern (NaN is never greater).
- * ign_mask_boxes_dev: the 26-connected components of the non-zero voxels of an F-order (sx, sy, sz) u8
- *   mask, fewer than 2^32 - 1 voxels (more -> IGN_ERR_UNSUPPORTED).  Components of fewer than
- *   dust_threshold voxels are dropped.  *n = the number kept; when *n <= capacity, rows (HOST, capacity
- *   rows of IGN_BOX_ROW uint32 words) receives per kept component
+ * ign_label_parts_dev: the connected parts of an F-order (sx, sy, sz) volume of labels (IGN_U8 / U16 / U32 /
+ *   U64; any other dtype -> IGN_ERR_UNSUPPORTED) of fewer than 2^32 - 1 voxels (more -> IGN_ERR_UNSUPPORTED).
+ *   Two neighbours under `connectivity` (6 / 18 / 26; anything else -> IGN_ERR_INVALID) join when they hold
+ *   the same non-zero label.  Parts are numbered by first voxel in F order (cc3d's numbering); parts of fewer
+ *   than dust_threshold voxels are dropped and the others keep their order.  *n = the number kept.
+ *   parts_out (DEVICE, sx * sy * sz words, may be NULL): each voxel's kept part 1..*n, 0 on label 0 and dust.
+ *   rows (HOST, capacity rows of IGN_BOX_ROW uint32 words; NULL only with capacity 0): when *n <= capacity,
+ *   it receives per kept part
  *     {voxel count, min x, min y, min z, max x, max y, max z}   (maxima inclusive)
- *   in the order of each component's first voxel in F order (cc3d's numbering), copied from the device
- *   before the call returns.  A capacity of ceil(sx/2) * ceil(sy/2) * ceil(sz/2) rows always suffices
- *   (26-connected components cannot be denser); with less and *n > capacity, rows is not written.  The
- *   stream is synchronised three times: for the component count, the kept count and the rows. */
+ *   in part order, copied from the device before the call returns; with *n > capacity it is not written.
+ *   For a 0 / 1 mask at connectivity 26 a capacity of ceil(sx/2) * ceil(sy/2) * ceil(sz/2) rows always
+ *   suffices (its parts cannot be denser).  The stream is synchronised for the part count, the kept count
+ *   and, when rows are written, once more.  compute_rois uses it on a u8 mask at 26, kimimaro.skeletonize for its
+ *   objects and ign_teasar_border_targets_dev for the parts of each face plane (18 on an extent-1 axis). */
 #define IGN_BOX_ROW 7
 IGN_API int ign_threshold_dev(ign_ctx* ctx, const void* in, int dtype, uint64_t n, uint64_t t, uint8_t* out);
-IGN_API int ign_mask_boxes_dev(ign_ctx* ctx, const uint8_t* mask, uint64_t sx, uint64_t sy, uint64_t sz,
-                               uint64_t dust_threshold, uint32_t* rows, uint64_t capacity, uint64_t* n);
+IGN_API int ign_label_parts_dev(ign_ctx* ctx, const void* labels, int dtype, uint64_t sx, uint64_t sy,
+                                uint64_t sz, int connectivity, uint64_t dust_threshold, uint32_t* parts_out,
+                                uint32_t* rows, uint64_t capacity, uint64_t* n);
 
 /* ------------------------------------------------------------------ jpeg codec
  * The Precomputed `jpeg` chunk encoding of uint8 image layers, which CloudVolume applies on the host

@@ -124,7 +124,7 @@ def test_empty_layer(ctx, oracle, tmp_path):
   assert _check(path, top, True, z0, oracle) == []
 
 
-def test_mask_boxes_kernel(ctx):
+def test_component_boxes_kernel(ctx):
   """many components, 26-connected, with their voxel counts, in one call"""
   from igneous_b200 import rois
   from igneous_b200.storage import DeviceCutout

@@ -7,7 +7,7 @@ teasar_params scale 4, const 500; and a 449^3 volume of 120 random capsule trees
 with scale 1.5, const 50, where objects need many paths and rounds.  Anisotropy (16, 16, 40), dust_threshold
 1000, fix_borders on, both fix_branching modes.  Per workload: median and min seconds of the whole call over
 the timed reps after one warm-up, the time of each phase of the last rep (kimimaro.last_phase_seconds), the
-object split alone (ign_teasar_objects_dev), and the loop's rounds, paths, box voxels visited and host
+object split alone (ign_label_parts_dev), and the loop's rounds, paths, box voxels visited and host
 synchronisations.  The CPU baseline is the serial C checker of the loop alone (one host core) on the fields
 of a 256^3 cutout, against the loop phase of the GPU call on the same cutout.  Prints one JSON line per measurement with the card's name, power
 limit, SM clock and throttle reasons read before and after."""
@@ -66,8 +66,8 @@ def objects_ms(ctx, vol, reps):
   _shim.check(ctx.lib.ign_renumber_dev(ctx.handle, _shim.ptr(raw), U32, n, _shim.ptr(lab), None, 0, c.byref(k)))
 
   def run():
-    _shim.check(ctx.lib.ign_teasar_objects_dev(ctx.handle, _shim.ptr(lab), *vol.shape, k.value, 26, 1000,
-                                               _shim.ptr(obj), c.byref(m)))
+    _shim.check(ctx.lib.ign_label_parts_dev(ctx.handle, _shim.ptr(lab), U32, *vol.shape, 26, 1000, _shim.ptr(obj),
+                                            None, 0, c.byref(m)))
     ctx.sync()
   ms = timed(run, reps)[0] * 1e3
   for b in (raw, lab, obj):
